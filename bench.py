@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/s of the batched humanoid-imitation rollout (BASELINE.json metric) on N B200s.
+"""bench.py -- env-steps/s of the batched humanoid-imitation rollout (BASELINE.json metric) on N H100s.
 
-A "step" is one lock-step control step of every environment: observation normaliser -> policy MLP forward (tcgen05) ->
+A "step" is one lock-step control step of every environment: observation normaliser -> policy MLP forward (wgmma) ->
 Gaussian sample -> fused physics(15 substeps)+task kernel -> transition written to the HBM rollout buffer -> re-seeding of
 finished episodes; the whole step is one call of the C-ABI loop (uhc_rollout) = one CUDA-graph launch.  Workload at N=1 = BASELINE.json configs[1]: 4096 SMPL-neutral humanoids imitating one AMASS-shaped clip,
 policy rollout only.  N>1: weak scaling, 4096 envs per GPU, no data-path collective (the rollout has none).
 
   python bench.py --gpus 1 --steps 20 --warmup 3
+  python bench.py --gpus 1 --steps 20 --warmup 3 --dump-outputs DIR   # + the last timed step's outputs as DIR/<name>.npy
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference          # the reference's CPU path: oracle port (fp64 C) on all host cores
 """
@@ -161,7 +162,7 @@ def workload_config(n):
     return {"workload": f"{ENVS_PER_GPU} SMPL-neutral humanoids per GPU imitating one {CLIP_FRAMES}-frame AMASS-shaped clip, policy rollout only "
                         "(obs normaliser + 657-2048-1024-512-105 gelu policy + physics/task step), uhc_implicit_shape hyper-parameters",
             "envs_per_gpu": ENVS_PER_GPU, "global_envs": ENVS_PER_GPU * n, "parallelism": f"env-sharded x{n}, no data-path collective",
-            "l2": "flushed (256 MiB write) between timed steps", "policy_gemm": "tcgen05 bf16 operands, fp32 accumulate",
+            "l2": "flushed (256 MiB write) between timed steps", "policy_gemm": "wgmma bf16 operands, fp32 accumulate",
             "physics": "fp32, 15 substeps/step, primal Newton contact solve"}
 
 
@@ -214,6 +215,14 @@ class ClockSampler:
                 "samples": len(sel), "where": where, "reasons": sorted(reasons)}
 
 
+def dump_outputs(d, **arrays):
+    """DIR/<name>.npy for each array (float32; float64 stays float64), so that two builds can be compared output for output"""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy()
+        np.save(os.path.join(d, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
+
+
 # ------------------------------------------------------------------------------------------------ GPU arm
 def run_gpu(args):
     import ctypes as C
@@ -255,6 +264,10 @@ def run_gpu(args):
         dist.barrier()
     t_wall1 = time.time()
     clk = clocks.stop(t_wall0, t_wall1) if clocks else None
+    if args.dump_outputs and rank == 0:                  # what the last timed step handed its caller, before anything else runs
+        r = (K - 1) % R
+        dump_outputs(args.dump_outputs, next_obs=agent.obs, states=buf.states[r], actions=buf.actions[r], rewards=buf.rewards[r], masks=buf.masks[r],
+                     exps=buf.exps[r], logp=buf.logp[r], fails=buf.fails[r])
     total_ms = sum(a.elapsed_time(b) for a, b in ev)
     ms = C.c_float(0)
     kms, kern_src = [], "CUDA events around k_env_step recorded inside the timed graph replays (external event-record nodes on the launching stream)"
@@ -323,22 +336,15 @@ def run_gpu(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     achieved = BYTES_PER_ENV_STEP * E / (kern_ms * 1e-3) / 1e9
     traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "r02_env_step_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("how")
-        except Exception:
-            pass
     cb = cpu_baseline(steps=6, warmup=1) if (world == 1 and not os.environ.get("UHC_BENCH_SKIP_CPU")) else None   # (skipped under ncu)
     line = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=K, warmup=W, ms_per_step=total_ms / K, higher_is_better=True,
                 scaling="weak", vs_baseline=None, dtype="f32", data="synthetic", config=workload_config(world),
                 roofline=dict(bound="hbm", achieved=achieved, peak=peak, unit="GB/s", frac=achieved / peak, traffic=traffic, traffic_source=traffic_src,
                               kernel="k_env_step<float>", kernel_ms=kern_ms, kernel_ms_source=kern_src, kernel_share_of_step=kern_ms / (total_ms / K),
-                              peak_source="MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s",
+                              peak_source="MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet 3350 GB/s",
                               note="algorithmic bytes 6396 B/env-step (SURVEY 8d); the step is latency/issue bound, not HBM bound -- see DESIGN.md"),
                 e2e=dict(value=e2e_val, unit=UNIT, h2d_bytes_per_step=E * 657 * 4, d2h_bytes_per_step=E * (657 + 105 + 1 + 1 + 1) * 4, steps=Ke,
                          path="pinned host obs -> device, BatchedAgent.rollout (uhc_rollout, 1 step), next obs / action / reward / mask / fail -> pinned host, one sync"),
@@ -414,6 +420,12 @@ def run_train(args):
         for key in phases:
             phases[key] += out.get(key, 0)
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:                  # the last iteration's results: the updated nets and the rollout they were trained on
+        g = torch.Generator(device="cpu").manual_seed(0)
+        rows = torch.randperm(T * E, generator=g)[:4096].to(agent.dev)       # a fixed sample of the transitions (the whole buffer is 1.3 GB)
+        dump_outputs(args.dump_outputs, policy_params=agent.policy.flat, value_params=agent.value.flat,
+                     states=buf.states.reshape(T * E, -1)[rows], actions=buf.actions.reshape(T * E, -1)[rows], rewards=buf.rewards.reshape(-1)[rows],
+                     masks=buf.masks.reshape(-1)[rows], fails=buf.fails.reshape(-1)[rows], running_state=agent.running_state.stats)
     if world > 1:
         dist.barrier()
     t_wall1 = time.time()
@@ -445,7 +457,7 @@ def run_train(args):
     N = T * E
     npar = agent.policy.flat.numel() + agent.value.flat.numel()
     flops_update = TRAIN_EPOCHS * 6.0 * (sum(w.numel() for w in agent.policy.W) + sum(w.numel() for w in agent.value.W)) * N
-    peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    peak = float(peaks.get("bf16_tflops_sustained", 989.0))
     ach = flops_update / (phases["epochs_ms"] / K * 1e-3) / 1e12
     line = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=K, warmup=W, ms_per_step=total_ms / K, higher_is_better=True, scaling="weak",
                 vs_baseline=None, dtype="f32 physics / bf16 tensor-core operands, fp32 accumulate + fp32 master weights", data="synthetic",
@@ -462,8 +474,8 @@ def run_train(args):
                             allreduce_calls_per_iter=phases["allreduce_calls"] / K,
                             allreduce_busbw_GBps=(phases["allreduce_bytes"] * 2 * (world - 1) / world / (phases["allreduce_ms"] * 1e-3) / 1e9) if phases["allreduce_ms"] > 0 else None),
                 replicas_identical=same, parameters=npar,
-                roofline=dict(bound="tensor", kernel="k_linear_tc2 (CTA-pair tcgen05 GEMMs: forward, dX with the activation backward fused, split-K dW of both nets)", achieved=ach, peak=peak, unit="TFLOP/s", frac=ach / peak, traffic=None,
-                              peak_source="MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1400 TFLOP/s",
+                roofline=dict(bound="tensor", kernel="k_linear_tc (wgmma GEMMs: forward, dX with the activation backward fused, split-K dW of both nets)", achieved=ach, peak=peak, unit="TFLOP/s", frac=ach / peak, traffic=None,
+                              peak_source="MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet 989 TFLOP/s (dense bf16)",
                               note="6 x parameters x N flop per epoch over the measured time of the 10 epochs (includes the loss, head activation-gradient, weight-transpose, Adam and bf16 weight-refresh kernels)"),
                 e2e=dict(value=value, unit=UNIT, h2d_bytes_per_step=0, d2h_bytes_per_step=16,
                          note="the training iteration has no host inputs (observations, rollout buffer and weights are device resident); the host reads back the two loss scalars"),
@@ -482,6 +494,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="rollout", choices=["rollout", "train"],
                     help="rollout (default, the headline: BASELINE configs[1]) or train (configs[2] at N=1, configs[3]/[4] shapes at N>1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32 / float64, < 64 MB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* uhc_b200.h -- C ABI of the B200 humanoid-imitation engine (libuhc_b200.so).
+/* uhc_b200.h -- C ABI of the batched (H100) humanoid-imitation engine (libuhc_b200.so).
  *
  * The reference (ZhengyiLuo/UHC) exposes NO native interface: its boundary is duck-typed Python over mujoco-py.
  * Each entry point below names the reference Python call it replaces (file:line under the reference tree); the

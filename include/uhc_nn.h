@@ -20,7 +20,7 @@ int uhc_linear_forward(const float *x, const float *W, const float *b, float *y,
 int uhc_linear_backward(const float *x, const float *W, const float *dz, float *dx_or_null, float *dW, float *db, int M, int N, int K, void *stream);
 int uhc_act_backward(const float *dh, const float *z, float *dz, long n, int act, void *stream);
 
-/* tensor-core forward of the same layer for the rollout path (tcgen05, bf16 operands, fp32 accumulate): see mlp_tcgen05.cu.
+/* tensor-core forward of the same layer for the rollout path (wgmma, bf16 operands, fp32 accumulate): see mlp_wgmma.cu.
  * x_bf16 [M][Kp], W_bf16 [N][Kp] with Kp a multiple of 64 (zero padded); y_bf16 [M][Np] (next layer's input) and/or y_f32 [M][N]. */
 int uhc_linear_forward_tc(const void *x_bf16, const void *W_bf16, const float *b, void *y_bf16_or_null, float *y_f32_or_null,
                           int M, int N, int Kp, int ldy_bf16, int act, void *stream);
@@ -34,8 +34,8 @@ int uhc_linear_forward_tc_train(const void *x_bf16, const void *W_bf16, const fl
  * epilogue through the TMA engine.  Needs the TMA-store path (uhc_tc_tma_store_enabled(); UHC_TC_TMA_STORE=0 in the environment turns it off). */
 int uhc_linear_forward_tc_train_t(const void *x_bf16, const void *W_bf16, const float *b, void *y_bf16, void *yT_bf16, int ld_yT, float *z_f32_or_null,
                                   int M, int N, int Kp, int ldy_bf16, int act, void *stream);
-/* plain fp32 product y[M][ld_y] = x W^T with an explicit row pitch ld_y >= N (floats, multiple of 4) on the CTA-pair split-K path; -2 when the shape is not
- * eligible (M, N >= 256 and Kp >= 16384 are required) */
+/* plain fp32 product y[M][ld_y] = x W^T with an explicit row pitch ld_y >= N (floats, multiple of 4, 16-byte aligned output) through the TMA engine, split-K
+ * where the output has few tiles; -2 when the arguments are not eligible (or the TMA-store path is off) */
 int uhc_linear_forward_tc_f32_pitched(const void *x_bf16, const void *W_bf16, float *y_f32, int ld_y, int M, int N, int Kp, void *stream);
 int uhc_tc_tma_store_enabled(void);
 /* backward through one Linear and the PREVIOUS layer's activation in one kernel: dz_prev = (dz W) * act'(z_prev), emitted as bf16 [M][ld_dz] and transposed

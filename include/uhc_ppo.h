@@ -10,7 +10,7 @@
  * optimisation step, issued on the caller's ncclComm_t from a side stream so it overlaps the other net's forward / backward; the
  * global-batch statistics (advantage moments and count, selected-row count, the ranks' ZFilter increments) ride in the tail of the first one.
  *
- * Every GEMM runs on the tcgen05 kernel (bf16 operands, fp32 accumulate; mlp_tcgen05.cu); parameters, gradients and Adam moments are fp32.
+ * Every GEMM runs on the wgmma kernel (bf16 operands, fp32 accumulate; mlp_wgmma.cu); parameters, gradients and Adam moments are fp32.
  * All pointers are device pointers unless marked host.  Functions return 0 on success; uhc_ppo_last_error() describes the last failure.
  */
 #ifndef UHC_PPO_H

@@ -1,4 +1,4 @@
-"""Import-compatible shim: the B200 engine replaces MuJoCo 2.1.0 / mujoco-py on the hot path.  scripts/train_uhc.py imports
+"""Import-compatible shim: the batched engine replaces MuJoCo 2.1.0 / mujoco-py on the hot path.  scripts/train_uhc.py imports
 `load_model_from_path, MjSim` only under --render; both explain themselves when used."""
 
 

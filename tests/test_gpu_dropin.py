@@ -99,33 +99,3 @@ def test_single_env_facade_matches_engine_and_oracle(tmp_path, monkeypatch, gold
         assert np.abs(env.data.qpos - oe.d.qpos).max() < 1e-4 and len(env.model.actuator_names) == 69
     env.fail_safe()
     assert np.abs(env.get_humanoid_qpos() - env.get_expert_qpos()).max() < 1e-6
-
-
-def test_reference_script_files_run_against_this_package(tmp_path):
-    """When a checkout of the reference is available ($UHC_REFERENCE, default /root/reference) its OWN script files are executed
-    (scripts/train_uhc.py, then scripts/eval_uhc.py --mode stats) with cwd = a scratch copy of this repo's config/assets layout, so that
-    `sys.path.append(os.getcwd())` (train_uhc.py:24) resolves `uhc` to this package.  Skipped where the reference is absent (the GPU box)."""
-    import subprocess
-    import sys
-    import yaml
-    ref = os.environ.get("UHC_REFERENCE", "/root/reference")
-    if not os.path.exists(os.path.join(ref, "scripts", "train_uhc.py")):
-        pytest.skip("no reference checkout on this machine")
-    root = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
-    for d in ("uhc", "uhc_b200", "mujoco_py", "assets"):
-        if os.path.exists(os.path.join(root, d)):
-            os.symlink(os.path.join(root, d), tmp_path / d)
-    os.makedirs(tmp_path / "config")
-    base = yaml.safe_load(open(os.path.join(root, "config", "uhc_b200_default.yml")))
-    base.update(policy_hsize=[128, 64], value_hsize=[128, 64], min_batch_size=1024, num_optim_epoch=2, num_envs=64, save_n_epochs=2, num_epoch=2)
-    base["data_specs"]["file_path"] = write_synthetic_pkl(str(tmp_path / "sample_data" / "clips.pkl"))
-    base["data_specs"]["t_max"] = 40
-    yaml.safe_dump(base, open(tmp_path / "config" / "refscript.yml", "w"))
-    env = dict(os.environ, PYTHONPATH=str(tmp_path), WANDB_MODE="disabled")
-    r = subprocess.run([sys.executable, os.path.join(ref, "scripts", "train_uhc.py"), "--cfg", "refscript", "--no_log"], cwd=tmp_path, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and "training done!" in r.stdout, r.stderr[-3000:]
-    assert os.path.exists(tmp_path / "results" / "motion_im" / "refscript" / "models" / "iter_0002.p")
-    r = subprocess.run([sys.executable, os.path.join(ref, "scripts", "eval_uhc.py"), "--cfg", "refscript", "--epoch", "2", "--mode", "stats"], cwd=tmp_path,
-                       env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-3000:]

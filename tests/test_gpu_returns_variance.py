@@ -1,5 +1,5 @@
 """GPU: "returns within stochastic variance" (BASELINE north_star).  The same stochastic policy (same weights, same observation normaliser, same noise
-scale) rolled out on the product path -- fp32 physics kernel, tcgen05 bf16 policy forward, device Gaussian sampler, 1024 envs -- and on the reference-pinned
+scale) rolled out on the product path -- fp32 physics kernel, wgmma bf16 policy forward, device Gaussian sampler, 1024 envs -- and on the reference-pinned
 fp64 oracle env with an fp64 numpy policy (48 envs): episode returns, episode lengths and the failure rate must agree within their sampling error."""
 import os
 

@@ -83,19 +83,14 @@ def test_supported_variant_accepts_the_shipped_configs_and_names_what_it_refuses
         assert supported_variant(_cfg_view(d)) == "implicit"
 
 
-def test_reference_yaml_coverage():
-    """how many of the reference's own config files the drop-in accepts (needs the reference checkout; the count is what DESIGN.md section 5 quotes)"""
-    import glob
-    import pytest
-    import yaml
+def test_reference_yaml_coverage(golden_dir):
+    """how many of the reference's own config files the drop-in accepts (the count is what DESIGN.md section 5 quotes); the keys supported_variant reads
+    from each of the reference's yaml files are stored in tests/golden/reference_yaml_keys.json (tools/make_golden.py gen_yaml_keys)"""
+    import json
     from uhc.agents.agent_copycat import supported_variant
-    root = os.environ.get("UHC_REFERENCE", "/root/reference")
-    files = sorted(glob.glob(os.path.join(root, "config", "**", "*.yml"), recursive=True))
-    if not files:
-        pytest.skip("reference checkout not present")
+    files = json.load(open(os.path.join(golden_dir, "reference_yaml_keys.json")))
     accepted = 0
-    for f in files:
-        d = yaml.safe_load(open(f)) or {}
+    for f, d in sorted(files.items()):
         if d.get("agent_name", "agent_copycat") != "agent_copycat":
             continue
         try:

@@ -389,6 +389,47 @@ def gen_math():
     print("math goldens ok", out["mul_doctest"])
 
 
+YAML_KEYS = ("agent_name", "obs_v", "actor_type", "reward_id", "fix_std", "residual_force", "obs_vel", "obs_coord", "obs_phase", "has_shape", "env_term_body",
+             "residual_force_mode", "residual_force_bodies", "residual_force_torque", "residual_force_bodies_num", "residual_contact_only",
+             "residual_contact_projection", "env_init_noise")
+
+
+def gen_yaml_keys():
+    """reference_yaml_keys.json: for every yaml file under the reference's config/, the keys supported_variant (uhc/agents/agent_copycat.py) reads"""
+    import glob
+    import json
+    import yaml
+    root = os.path.join(H.REF, "config")
+    out = {}
+    for f in sorted(glob.glob(os.path.join(root, "**", "*.yml"), recursive=True)):
+        d = yaml.safe_load(open(f)) or {}
+        out[os.path.relpath(f, root)] = {k: d[k] for k in YAML_KEYS if k in d}
+    json.dump(out, open(os.path.join(OUT, "reference_yaml_keys.json"), "w"), sort_keys=True, separators=(",", ":"))
+
+
+def gen_zfilter_pickle():
+    """zfilter_reference.npz: the reference's ZFilter (uhc/khrylib/utils/zfilter.py) pushed the 40 rows of tests/test_checkpoint_compat.py one by one and
+    pickled as agent_copycat.py:190-201 saves it (`pickle_ref`), and the reference class applied to this repo's ZFilter of the same rows (`y_ref`)"""
+    import io
+    import pickle
+    import subprocess
+    import tempfile
+    x = np.random.RandomState(1).normal(0.5, 3.0, (40, 657))
+    ours = ("import sys, pickle, numpy as np\nsys.path.insert(0, %r)\nfrom uhc.khrylib.utils.zfilter import ZFilter\nx = np.load(sys.argv[1])\n"
+            "z = ZFilter.from_stats(40, x.mean(0), ((x - x.mean(0)) ** 2).sum(0), clip=5.0)\npickle.dump({'running_state': z}, open(sys.argv[2], 'wb'))\n") % H.ROOT
+    ref = ("import sys, pickle, numpy as np\nsys.path.insert(0, %r)\nfrom uhc.khrylib.utils import zfilter\nx = np.load(sys.argv[1])\n"
+           "rs = pickle.loads(open(sys.argv[2], 'rb').read())['running_state']\ny = rs(x[0], update=False)\n"
+           "z = zfilter.ZFilter((657,), clip=5)\nfor r in x: z(r)\nsys.stdout.buffer.write(pickle.dumps({'y': y, 'p': pickle.dumps({'running_state': z})}))\n") % H.REF
+    with tempfile.TemporaryDirectory() as d:
+        np.save(os.path.join(d, "x.npy"), x)
+        env = {k: v for k, v in os.environ.items() if k != "PYTHONPATH"}
+        args = [os.path.join(d, "x.npy"), os.path.join(d, "ours.p")]
+        subprocess.run([sys.executable, "-c", ours] + args, cwd=d, env=env, check=True)
+        r = subprocess.run([sys.executable, "-c", ref] + args, capture_output=True, cwd=d, env=env, check=True)
+    res = pickle.load(io.BytesIO(r.stdout))
+    np.savez_compressed(os.path.join(OUT, "zfilter_reference.npz"), y_ref=res["y"], pickle_ref=np.frombuffer(res["p"], np.uint8))
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     H.install()
@@ -451,6 +492,10 @@ def main():
         gen_metrics()
     if "sampler" in what:
         gen_sampler(H.make_cfg())
+    if "yaml_keys" in what:
+        gen_yaml_keys()
+    if "zfilter" in what:
+        gen_zfilter_pickle()
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""AgentCopycat with the reference's surface (uhc/agents/agent_copycat.py:51-605) on the batched B200 engine.
+"""AgentCopycat with the reference's surface (uhc/agents/agent_copycat.py:51-605) on the batched engine.
 
   AgentCopycat(cfg, dtype, device, training=True, checkpoint_epoch=0)
   .optimize_policy(epoch)   per_epoch_update -> sample -> update_params -> checkpoint / eval every save_n_epochs -> log   (:326-352)
@@ -51,7 +51,7 @@ def supported_variant(cfg):
     naming the key: of the reference's 115 yaml files 86 pass (tests/test_shim_cpu.py counts them); the others use explicit residual forces with contact gating /
     projection / body subsets (10), the six-term world_rfc_implicit_v2 / _v3 rewards (8), obs_v 0 / 4 (6), a trained log_std (2), ..."""
     assert cfg.obs_v in (1, 2, 3, 5, 6) and cfg.actor_type in ("gauss", "mcp") and cfg.reward_id in reward_func, \
-        "the B200 engine implements obs_v 1 | 2 | 3 | 5 | 6, the gauss and mcp actors, world_rfc_implicit (_v1_mul) / world_rfc_explicit (obs_v 0/4, reward v2/v3: SURVEY.md section 8f, next)"
+        "the batched engine implements obs_v 1 | 2 | 3 | 5 | 6, the gauss and mcp actors, world_rfc_implicit (_v1_mul) / world_rfc_explicit (obs_v 0/4, reward v2/v3: SURVEY.md section 8f, next)"
     assert cfg.get("obs_vel", "full") == "full" and cfg.get("obs_coord", "root") == "root" and not cfg.get("obs_phase", False), "obs_vel full / obs_coord root / no phase only"
     if cfg.obs_v == 1:
         assert not cfg.get("has_shape", False), "obs_v 1 carries no shape vector (has_shape: false in config/release/uhc_implicit.yml)"
@@ -78,7 +78,7 @@ class AgentCopycat:
         self.epoch, self.max_freq = 0, 50
         dev_index = device.index if getattr(device, "type", "cpu") == "cuda" and device.index is not None else int(getattr(cfg, "gpu_index", 0) or 0)
         if not torch.cuda.is_available():
-            raise RuntimeError("the B200 engine needs a CUDA device (the reference's CPU sampling path is replaced, not kept as a fallback)")
+            raise RuntimeError("the batched engine needs a CUDA device (the reference's CPU sampling path is replaced, not kept as a fallback)")
         self.model_tables = HumanoidModel()
         # data (setup_data_loader :128-134)
         self.data_loader = DatasetAMASSSingle(cfg.data_specs, data_mode="train", model=self.model_tables)

@@ -1,5 +1,5 @@
 """HumanoidEnv: single-environment facade with the reference's env surface (uhc/envs/humanoid_im.py:50, khrylib
-mujoco_env.py:95-113) over one environment of the batched B200 engine.  Used by evaluation / debugging code that wants the
+mujoco_env.py:95-113) over one environment of the batched engine.  Used by evaluation / debugging code that wants the
 classic gym-style loop; training uses uhc_b200.agent.BatchedAgent (thousands of envs in lock-step).
 
     env = HumanoidEnv(cfg, init_expert, data_specs, mode)     # init_expert: a dataset sample dict (pose_aa, trans, beta, gender, ...)
@@ -23,7 +23,7 @@ class _RobotShim:
     smpl_model = "smpl"
 
     def export_vis_string(self):
-        raise NotImplementedError("the B200 engine has no MuJoCo XML to export; rendering is out of scope")
+        raise NotImplementedError("the batched engine has no MuJoCo XML to export; rendering is out of scope")
 
 
 class _ModelShim:
@@ -182,7 +182,7 @@ class HumanoidEnv:
         return st["xpos"][0] + _quat_rot(st["qpos"][3:7]).dot(self.model_tables.ipos[0])
 
     def render(self, *a, **k):
-        raise NotImplementedError("rendering needs MuJoCo; the B200 engine has no viewer")
+        raise NotImplementedError("rendering needs MuJoCo; the batched engine has no viewer")
 
     def calc_body_diff(self):
         cur = self.engine.get_state(0)["xpos"]

@@ -3,4 +3,4 @@
 
 class MjViewer:
     def __init__(self, sim=None):
-        raise NotImplementedError("MjViewer (GL rendering) is not part of the B200 engine")
+        raise NotImplementedError("MjViewer (GL rendering) is not part of the batched engine")

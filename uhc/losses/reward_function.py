@@ -1,4 +1,4 @@
-"""Reward registry (uhc/losses/reward_function.py:823-833).  On the B200 engine the imitation reward is fused into the step
+"""Reward registry (uhc/losses/reward_function.py:823-833).  On the batched engine the imitation reward is fused into the step
 kernel (sim_core.h diff_and_reward, restating world_rfc_implicit_reward :12-88 and, with residual_force_mode = explicit,
 world_rfc_explicit_reward :253-341, and with reward_id world_rfc_implicit_v1_mul the product form :174-250); the callable keeps the reference signature
 `reward(env, state, action, info) -> (reward, c_info[5])` and returns what the kernel computed for the step just taken."""

@@ -1,12 +1,12 @@
-"""Builds libuhc_b200.so (CUDA, sm_100a) in-tree.  nvcc cross-compiles without a GPU."""
+"""Builds libuhc_b200.so (CUDA, sm_90a) in-tree.  nvcc cross-compiles without a GPU."""
 import os
 import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "libuhc_b200.so")
-SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_tcgen05.cu", "rollout.cu", "ppo_update.cu"]
+SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_wgmma.cu", "rollout.cu", "ppo_update.cu"]
 DEPS = ["sim_core.h", "env_step.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 

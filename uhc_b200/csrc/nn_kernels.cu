@@ -5,8 +5,8 @@
 //   a14 Value              uhc/khrylib/rl/core/critic.py:15-18
 //   a15 estimate_advantages uhc/khrylib/rl/core/common.py:5-25
 //   a16 update_policy/ppo_loss/update_value/clip grad  uhc/khrylib/rl/agents/agent_ppo.py:16-65, agent_pg.py:18-25; torch.optim.Adam
-// This file holds the fp32 SIMT GEMM (all three layouts) and every streaming kernel; the tcgen05 tensor-core GEMM used
-// for the rollout-time forward lives in mlp_tcgen05.cu.
+// This file holds the fp32 SIMT GEMM (all three layouts) and every streaming kernel; the wgmma tensor-core GEMM used
+// for the rollout-time forward lives in mlp_wgmma.cu.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -346,7 +346,7 @@ int uhc_linear_backward(const float *x, const float *W, const float *dz, float *
     return 0;
 }
 int uhc_act_backward(const float *dh, const float *z, float *dz, long n, int act, void *stream) {
-    k_act_bwd<<<1184, 256, 0, (cudaStream_t)stream>>>(dh, z, dz, (size_t)n, act); CKN(cudaGetLastError()); return 0;
+    k_act_bwd<<<1056, 256, 0, (cudaStream_t)stream>>>(dh, z, dz, (size_t)n, act); CKN(cudaGetLastError()); return 0;
 }
 int uhc_gaussian_sample(const float *mean, const float *log_std, const unsigned char *mean_action, float *action, float *logp, int M, int A,
                         unsigned long long seed, unsigned long long step, void *stream) {
@@ -378,7 +378,7 @@ int uhc_sqsum(const float *x, long n, double *out_acc, void *stream) {
 int uhc_adam_step(float *p, const float *g, float *m, float *v, long n, float lr, float beta1, float beta2, float eps, int step,
                   const double *sqnorm_or_null, float max_norm, void *stream) {
     const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-    k_adam<<<1184, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (size_t)n, lr, beta1, beta2, eps, bc1, bc2, sqnorm_or_null, max_norm);
+    k_adam<<<1056, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (size_t)n, lr, beta1, beta2, eps, bc1, bc2, sqnorm_or_null, max_norm);
     CKN(cudaGetLastError()); return 0;
 }
 int uhc_gae(const float *rew, const float *mask, const float *val, const float *last_val, float gamma, float tau, float *adv, float *ret, int T, int E,

@@ -417,7 +417,7 @@ int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_stat
     CKU(uhc_gae(rewards, masks, t->vb.out, t->last_v, cfg->gamma, cfg->tau, t->adv, t->ret, T, E, st), "gae");
     CKU(uhc_adv_moments(t->adv, M, t->mom, st), "advantage moments");
     CKP(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
-    ++g_launches; k_count_selected<<<296, 256, 0, st>>>(exps, (size_t)M, t->cnt); CKP(cudaGetLastError());
+    ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CKP(cudaGetLastError());
     float *tail = val.gfull + val.nflat;
     if (!comm) {
         CKU(uhc_adv_normalize(t->adv, M, t->mom, nullptr, st), "advantage normalisation");
@@ -448,7 +448,7 @@ int uhc_ppo_update_policy(UhcPpoTrainer *t, const float *states, const float *ac
     CKP(cudaMemcpyAsync(t->adv, advantages, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CKP(cudaMemcpyAsync(t->ret, returns, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CKP(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
-    ++g_launches; k_count_selected<<<296, 256, 0, st>>>(exps, (size_t)M, t->cnt); CKP(cudaGetLastError());
+    ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CKP(cudaGetLastError());
     ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CKP(cudaGetLastError());      // (a sharded caller passes world = 1 per shard or pre-scales exps)
     return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, nullptr, nullptr, world > 1 ? nccl_comm : nullptr, world, false,
                       false, losses_out, st);

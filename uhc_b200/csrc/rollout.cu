@@ -4,7 +4,7 @@
 //   state -> running_state -> policy_net.select_action -> env.step -> custom_reward -> memory.push(state, action, mask, reward, exp))
 // by T lock-step control steps of all E device-resident environments.  One control step is
 //   k_zfilter_partial, _merge, _count, k_zfilter_apply_bf16   obs -> normalised state (buffer row, fp32) + bf16 K-padded copy      (a12)
-//   4 x k_linear_tc                                           policy MLP on tensor cores (tcgen05 / TMEM / TMA, mlp_tcgen05.cu)      (a13)
+//   4 x k_linear_tc                                           policy MLP on tensor cores (wgmma / TMA, mlp_wgmma.cu)                (a13)
 //   k_gauss_sample_dev                                        action + log-prob into the buffer row                                  (a13)
 //   k_env_step                                                15 physics substeps + obs + reward + termination + in-kernel re-seeding (a1-a10)
 //   k_rollout_post                                            mask / fail / exp rows, device step counter += 1                        (a11)
@@ -181,7 +181,7 @@ int enqueue_policy(RolloutCtx *c, const float *obs, const Policy *pol, double *z
     const int E = c->E, D = m0->dims[0], P = pol->nprim, A = m0->dims[m0->nlayers];
     int n = 0;
     if (update_filter) { CKC(uhc_zfilter_ws(obs, nullptr, E, D, zstats, zclip, 1, c->d_zws, st), "zfilter update"); n += 3; }
-    k_zfilter_apply_bf16<<<1184, 256, 0, st>>>(obs, state_out, (unsigned short *)c->ns[0].acts[0], E, D, m0->kp[0], zstats, zclip);
+    k_zfilter_apply_bf16<<<1056, 256, 0, st>>>(obs, state_out, (unsigned short *)c->ns[0].acts[0], E, D, m0->kp[0], zstats, zclip);
     CKR(cudaGetLastError()); n++;
     for (int j = 0; j < (P > 0 ? P + 1 : 1); j++) {
         const UhcMlp *m = &pol->nets[j];

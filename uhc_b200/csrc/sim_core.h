@@ -1,6 +1,6 @@
 // sim_core.h -- the per-humanoid physics + imitation-task step, one WARP per environment.
 //
-// Product code (CUDA, sm_100a).  Everything in this header is written in an SPMD "phase" style:
+// Product code (CUDA, sm_90a).  Everything in this header is written in an SPMD "phase" style:
 //     LANES_BEGIN ... per-lane code, no cross-lane dependency inside ... LANES_END   (= __syncwarp())
 // so that the very same source can also be compiled by g++ as a lane-loop emulation (tests/emu, -DUHC_EMU) and be
 // debugged on a CPU-only box.  The emulation is test infrastructure; the C-ABI library only ever launches the CUDA build.
@@ -247,24 +247,12 @@ template <class R> UHC_DEV void sym6_mul(const R *K, const R *x, R *y) {
 }
 
 // ------------------------------------------------------------------------------------------------ packed pairs
-// Two Reals handled by one instruction where the hardware has it: sm_100 issues fp32 pairs as FFMA2 / FMUL2 / FADD2 and loads
-// them from shared memory as one 64-bit access; doubles (and the host emulation) fall back to component-wise arithmetic.
+// Two Reals handled together: loaded from shared memory as one 64-bit access, arithmetic component-wise (sm_90 has no packed fp32 instructions).
 template <class R> struct alignas(2 * sizeof(R)) Pr { R x, y; };
 template <class R> UHC_DEV Pr<R> pbc(R s) { Pr<R> r; r.x = s; r.y = s; return r; }
 template <class R> UHC_DEV Pr<R> pfma(Pr<R> a, Pr<R> b, Pr<R> c) { Pr<R> r; r.x = a.x * b.x + c.x; r.y = a.y * b.y + c.y; return r; }
 template <class R> UHC_DEV Pr<R> pmul(Pr<R> a, Pr<R> b) { Pr<R> r; r.x = a.x * b.x; r.y = a.y * b.y; return r; }
 template <class R> UHC_DEV Pr<R> padd(Pr<R> a, Pr<R> b) { Pr<R> r; r.x = a.x + b.x; r.y = a.y + b.y; return r; }
-#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ >= 1000
-template <> UHC_DEV Pr<float> pfma<float>(Pr<float> a, Pr<float> b, Pr<float> c) {
-    const float2 t = __ffma2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y), make_float2(c.x, c.y)); Pr<float> r; r.x = t.x; r.y = t.y; return r;
-}
-template <> UHC_DEV Pr<float> pmul<float>(Pr<float> a, Pr<float> b) {
-    const float2 t = __fmul2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y)); Pr<float> r; r.x = t.x; r.y = t.y; return r;
-}
-template <> UHC_DEV Pr<float> padd<float>(Pr<float> a, Pr<float> b) {
-    const float2 t = __fadd2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y)); Pr<float> r; r.x = t.x; r.y = t.y; return r;
-}
-#endif
 // 6-vectors as three pairs
 template <class R> UHC_DEV R pdot6(const Pr<R> *a, const Pr<R> *b) { Pr<R> t = pmul(a[0], b[0]); t = pfma(a[1], b[1], t); t = pfma(a[2], b[2], t); return t.x + t.y; }
 template <class R> UHC_DEV void paxpy6(R s, const Pr<R> *x, Pr<R> *y) { const Pr<R> ss = pbc(s); y[0] = pfma(ss, x[0], y[0]); y[1] = pfma(ss, x[1], y[1]); y[2] = pfma(ss, x[2], y[2]); }
@@ -1289,10 +1277,8 @@ UHC_DEV void integrate(const Model<Real> &m, Work<Real> &w) {
 enum { PH_PD = 0, PH_SMOOTH = 1, PH_NEWTON = 2 };
 // The warps of a CTA are re-aligned at points every warp passes exactly once per substep: they then run the same code at
 // the same time and share instruction-cache lines (the per-substep code is ~3x the 32 KB instruction cache).
-// Measured (E = 4096): whole-CTA alignment 1.25 M env-steps/s, groups of 4 / 3 / 2 warps 1.23 / 1.20 / 1.16 M, none 0.95 M;
-// every 2nd / 3rd substep only 1.06 / 1.00 M; aligning each Newton iteration too 1.06 M.  Re-measured on the final kernel (1.57 M):
-// without the barrier before the Newton phase 1.53 M, without the one at the substep start 1.57 M (neutral), without both 1.52 M.
-// Round-2 kernel (profiles/r02_env_step_sync_groups.txt): groups of 2 / 3 / 4 warps 1.46 / 1.53 / 1.64 M, the whole 7-warp CTA 1.74 M, one 14-warp CTA per SM 1.70 M.
+// Aligning the whole CTA was faster than groups of 2 / 3 / 4 warps, than aligning every 2nd / 3rd substep or each Newton iteration, and than one
+// 14-warp CTA per SM (measured on the GPU the kernel was first tuned on; not re-measured on the H100).
 // The barrier is a NAMED barrier with an explicit thread count (w.sync_threads = 32 x the warps of the CTA that own a valid
 // environment): warps without work leave the kernel before the substep loop and are simply not counted.
 #if !defined(UHC_EMU) && !defined(UHC_NO_CTA_SYNC)

@@ -1,5 +1,5 @@
 // step_kernel.cu -- CUDA kernels + C ABI (include/uhc_b200.h) for the batched humanoid env: one warp per environment,
-// working set in shared memory, state records in HBM.  sm_100a.
+// working set in shared memory, state records in HBM.  sm_90a.
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -205,8 +205,8 @@ template <class Real> static int build_view(UhcEngine *e, EngineView<Real> &ev, 
 
 constexpr int EPB_F = UHC_EPB_F, EPB_D = 2;
 template <class Real, int EPB> constexpr size_t step_smem() { return EPB * sizeof(Work<Real>) + 2 * NV * 4 * sizeof(Real) + (MAXLEVEL + 1) * LVL_G * sizeof(int) + 32 * sizeof(LaneTopo); }  // environments (warps) per block
-// the fp32 step kernel is tuned for UHC_MIN_CTAS resident blocks per SM (sm_100: 228 KiB of shared memory per SM, 1 KiB reserved per block, ~1 KiB static here):
-// a few hundred bytes more in Work / LaneTopo silently halve the residency (measured: 1.27 -> 0.88 M env-steps/s), so it is a compile-time error
+// the fp32 step kernel is tuned for UHC_MIN_CTAS resident blocks per SM (sm_90: 228 KiB of shared memory per SM, 1 KiB reserved per block, ~1 KiB static here):
+// a few hundred bytes more in Work / LaneTopo silently halve the residency, so it is a compile-time error
 static_assert(EPB_F != 7 || UHC_MIN_CTAS * (step_smem<float, EPB_F>() + 1024 + 1088) <= 228 * 1024, "k_env_step<float>: the work sets of UHC_MIN_CTAS blocks no longer fit one SM");
 
 extern "C" {
@@ -220,7 +220,7 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
     e->E = num_envs; e->device = device; e->precision = precision; e->launches = 0; e->nshape = model->nshape > 0 ? model->nshape : 1;
     int rc = precision == 32 ? build_view<float>(e, e->evf, model, cfg) : build_view<double>(e, e->evd, model, cfg);
     if (rc) { delete e; return rc; }
-    {   // work-sorted warp slots: opt-in (UHC_SORT_ENVS=1).  Measured at 4096 envs: 1.52 M env-steps/s sorted vs 1.57 M with the identity
+    {   // work-sorted warp slots: opt-in (UHC_SORT_ENVS=1).  At 4096 envs sorting was slower than the identity
         // mapping -- the previous step's iteration total does not predict the per-substep imbalance well enough to pay for itself
         const char *se = getenv("UHC_SORT_ENVS");
         if (se && se[0] == '1' && num_envs > 2 * EPB_F) { CK(cudaMalloc((void **)&e->d_order, (size_t)num_envs * sizeof(int))); e->allocs.push_back(e->d_order); }

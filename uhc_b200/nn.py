@@ -372,7 +372,7 @@ def _pad64(n):
 
 
 class TCTrainer:
-    """Tensor-core (tcgen05, bf16 operands / fp32 accumulate) forward + backward of an MLPNet for the PPO update:
+    """Tensor-core (wgmma, bf16 operands / fp32 accumulate) forward + backward of an MLPNet for the PPO update:
     forward stores bf16 activations and fp32 pre-activations; dX = dZ W and dW = dZ^T X run on the same TN GEMM kernel using
     transposed bf16 copies; dz = dh * act'(z), its transpose and the bias gradient come from one fused kernel."""
 
@@ -666,7 +666,7 @@ def zfilter_from_sums(sums, D):
 def ppo_update(policy, value, log_std, opt_p, opt_v, states, actions, returns, advantages, exps, clip_eps=0.2, epochs=10, grad_clip=40.0,
                use_tc=False, comm=None):
     """AgentPPO.update_policy (agent_ppo.py:16-51), full batch: per epoch one value step then one clipped-surrogate policy step.
-    use_tc=False: fp32 SIMT GEMMs (parity path); use_tc=True: tcgen05 bf16/fp32-accumulate GEMMs for forward, dX and dW (production)."""
+    use_tc=False: fp32 SIMT GEMMs (parity path); use_tc=True: wgmma bf16/fp32-accumulate GEMMs for forward, dX and dW (production)."""
     if use_tc:
         tp = getattr(policy, "_tc_trainer", None) or TCTrainer(policy)
         tv = getattr(value, "_tc_trainer", None) or TCTrainer(value)
