@@ -123,12 +123,27 @@ struct Work {
     Real Ib[NB][10];              // per-body rigid inertia about O, world axes (of the last forward pass)
     alignas(16) Real S[NV + 6][6];   // motion subspaces; rows NV.. are the unit vectors of the solve's virtual dofs
     // ---- derived pose (vector stores to the record), the rest of the working set
-    alignas(16) Real xpos[NB][3]; Real xipos[NB][3], xquat[NB][4], xmat[NB][9];
+    alignas(16) Real xpos[NB][3]; Real xipos[NB][3], xmat[NB][9];
     Real act[ACT_DIM + 3];
-    alignas(16) Real aU[NV + 6][6];   // articulated-body sweep: columns of  U D^-1  per 3-dof block (U = IA S, D = S^T U + arm)
-    Real au[NV + 6];                // D^-1 u per block
-    Real fs[NV + 1], as_[NV + 1], a[NV + 1], g[NV + 1], p[NV + 1], Mp[NV + 1], tau[NV + 1];   // Mp: the solve's joint-space diagonal
-    alignas(16) Real Vb[NB][6], Ab[NB][6], Fb[NB][6];
+    // The articulated-body sweep's scratch is only live inside one aba_solve; it shares its bytes with vectors that are dead across every
+    // aba_solve of a substep (1.8 KB less per env, so 16 work sets fit one SM):
+    //   Vb  kin_rne_forward -> constraint_setup (the smooth solve only runs when there is no constraint, so none runs in between)
+    //   Fb  body-wrench scratch of kin_rne_forward / project_force, rfc_explicit, newton_init, newton_advance (never held across a solve)
+    //   fs  smooth phase -> newton_init (same argument as Vb)
+    //   xquat  world_quat after the last solve of the step / of the reset -> observation, store_state
+    union {
+        struct {
+            alignas(16) Real aU[NV + 6][6];   // columns of  U D^-1  per 3-dof block (U = IA S, D = S^T U + arm)
+            Real au[NV + 6];                // D^-1 u per block
+        };
+        struct {
+            alignas(16) Real xquat[NB][4];
+            alignas(16) Real Vb[NB][6], Fb[NB][6];
+            Real fs[NV + 1];
+        };
+    };
+    Real as_[NV + 1], a[NV + 1], g[NV + 1], p[NV + 1], Mp[NV + 1], tau[NV + 1];   // Mp: the solve's joint-space diagonal
+    alignas(16) Real Ab[NB][6];
     // contacts
     int cbody[MAXCON]; Real cr[MAXCON][3], cdist[MAXCON], cD[MAXCON], caref[MAXCON][4], cres[MAXCON][4], cjp[MAXCON][4];
     int bcon_adr[NB + 1];
@@ -136,8 +151,8 @@ struct Work {
     int nlim;                     // joint-limit rows of this substep (hinges past their range); their data rides in tau (sign * D) and as_ (residual)
     int con_overflow;             // a candidate body's contacts did not fit MAXCON in some substep of this step (the env is failed, never silently truncated)
     alignas(8) unsigned long long mbar;   // mbarrier of this warp's bulk-async state load
-    int sync_threads;             // threads taking part in the CTA-level substep alignment barrier (32 x warps that own a valid env)
-    int sync_id;                  // named barrier of this warp's alignment group (1 = the whole CTA; UHC_SYNC_SPLIT builds use one barrier per group)
+    int sync_threads;             // threads taking part in the substep alignment barrier of this warp's group (32 x its warps that own a valid env)
+    int sync_id;                  // named barrier of this warp's alignment group (1 + group index; SYNC_GROUP warps per group)
     // this env's model view (shape variant) and config: kept here so that the non-inlined phases read them from shared memory
     // instead of a per-thread local-memory copy
     alignas(8) Model<Real> mdl;
@@ -1277,9 +1292,10 @@ UHC_DEV void integrate(const Model<Real> &m, Work<Real> &w) {
 enum { PH_PD = 0, PH_SMOOTH = 1, PH_NEWTON = 2 };
 // The warps of a CTA are re-aligned at points every warp passes exactly once per substep: they then run the same code at
 // the same time and share instruction-cache lines (the per-substep code is ~3x the 32 KB instruction cache).
-// Aligning the whole CTA was faster than groups of 2 / 3 / 4 warps, than aligning every 2nd / 3rd substep or each Newton iteration, and than one
-// 14-warp CTA per SM (measured on the GPU the kernel was first tuned on; not re-measured on the H100).
-// The barrier is a NAMED barrier with an explicit thread count (w.sync_threads = 32 x the warps of the CTA that own a valid
+// The fp32 kernel runs one 16-warp CTA per SM aligned as two groups of 8 warps (one named barrier each): on an H100 at 4096 envs that
+// was ~1 % faster than two 8-warp CTAs per SM aligned as a whole (k_env_step 3.06 vs 3.08 ms).  On the GPU the kernel was first tuned
+// on, aligning 7 warps was faster than groups of 2 / 3 / 4 warps and than aligning every 2nd / 3rd substep or each Newton iteration.
+// The barrier is a NAMED barrier with an explicit thread count (w.sync_threads = 32 x the warps of the group that own a valid
 // environment): warps without work leave the kernel before the substep loop and are simply not counted.
 #if !defined(UHC_EMU) && !defined(UHC_NO_CTA_SYNC)
 #define UHC_CTA_SYNC(on) do { if (on) asm volatile("bar.sync %0, %1;" :: "r"(w.sync_id), "r"(w.sync_threads) : "memory"); } while (0)

@@ -7,9 +7,6 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_b200.h"
-#ifndef UHC_EPB_F
-#define UHC_EPB_F 7
-#endif
 #include "env_step.h"
 
 using namespace uhc;
@@ -32,28 +29,25 @@ __device__ __forceinline__ void stage_tables(EngineView<Real> &ev, unsigned char
     ev.model.dof_f = s_dof; ev.model.dof_lim = s_lim; ev.model.lvl_pack = s_lvl; ev.model.topo_s = s_topo;
 }
 
-#ifndef UHC_MIN_CTAS
-#define UHC_MIN_CTAS 2
-#endif
+// warps per substep alignment group (sim_core.h, UHC_CTA_SYNC): the fp32 kernel's 16-warp CTA is two groups, the fp64 kernel's one
+constexpr int SYNC_GROUP = 8;
 #ifdef UHC_MAXNREG     /* experiment knob: cap registers without changing the CTA shape */
 #define UHC_STEP_BOUNDS(EPB, Real) __maxnreg__(UHC_MAXNREG)
 #else
-#define UHC_STEP_BOUNDS(EPB, Real) __launch_bounds__(32 * EPB, (sizeof(Real) == 4 && EPB <= 7 ? UHC_MIN_CTAS : 1))
+#define UHC_STEP_BOUNDS(EPB, Real) __launch_bounds__(32 * EPB, 1)
 #endif
 template <class Real, int EPB>
 __global__ void UHC_STEP_BOUNDS(EPB, Real)
 k_env_step(EngineView<Real> ev, const float *__restrict__ act, float *__restrict__ obs, float *__restrict__ rew, float *__restrict__ cinfo,
            int *__restrict__ fail, int *__restrict__ end, float *__restrict__ pct, float *__restrict__ torque, const int *__restrict__ order) {
     extern __shared__ __align__(16) unsigned char smem[];
-#ifndef UHC_SYNC_SPLIT
-#define UHC_SYNC_SPLIT EPB            /* warps per alignment group (experiment knob; measured: the whole CTA is best) */
-#endif
-    __shared__ int s_nvalid[8];
-    const int warp = threadIdx.x >> 5, slot = blockIdx.x * EPB + warp, grp = warp / (UHC_SYNC_SPLIT);
-    if (threadIdx.x < 8) s_nvalid[threadIdx.x] = 0;
+    constexpr int NGRP = (EPB + SYNC_GROUP - 1) / SYNC_GROUP;
+    __shared__ int s_nvalid[NGRP];
+    const int warp = threadIdx.x >> 5, slot = blockIdx.x * EPB + warp, grp = warp / SYNC_GROUP;
+    if (threadIdx.x < NGRP) s_nvalid[threadIdx.x] = 0;
     stage_tables<Real, EPB>(ev, smem);
-    // the warps of a CTA wait for each other every substep: `order` groups environments that needed a similar number of solver
-    // iterations in the previous step into the same CTA (k_order_envs), outputs stay indexed by the environment id
+    // the warps of an alignment group wait for each other every substep: `order` groups environments that needed a similar number of
+    // solver iterations in the previous step into the same CTA (k_order_envs), outputs stay indexed by the environment id
     const int env = slot < ev.num_envs ? (order ? order[slot] : slot) : -1;
     const bool valid = env >= 0 && env_record_valid(ev, env);
     if (valid && (threadIdx.x & 31) == 0) atomicAdd(&s_nvalid[grp], 1);
@@ -203,11 +197,13 @@ template <class Real> static int build_view(UhcEngine *e, EngineView<Real> &ev, 
     return 0;
 }
 
-constexpr int EPB_F = UHC_EPB_F, EPB_D = 2;
-template <class Real, int EPB> constexpr size_t step_smem() { return EPB * sizeof(Work<Real>) + 2 * NV * 4 * sizeof(Real) + (MAXLEVEL + 1) * LVL_G * sizeof(int) + 32 * sizeof(LaneTopo); }  // environments (warps) per block
-// the fp32 step kernel is tuned for UHC_MIN_CTAS resident blocks per SM (sm_90: 228 KiB of shared memory per SM, 1 KiB reserved per block, ~1 KiB static here):
-// a few hundred bytes more in Work / LaneTopo silently halve the residency, so it is a compile-time error
-static_assert(EPB_F != 7 || UHC_MIN_CTAS * (step_smem<float, EPB_F>() + 1024 + 1088) <= 228 * 1024, "k_env_step<float>: the work sets of UHC_MIN_CTAS blocks no longer fit one SM");
+// environments (warps) per block.  fp32: one 16-warp CTA per SM, so 132 SMs hold 2112 envs and 4096 envs run in two full waves
+// (at 14 per SM they took three, the last one a 58-CTA tail)
+constexpr int EPB_F = 16, EPB_D = 2;
+template <class Real, int EPB> constexpr size_t step_smem() { return EPB * sizeof(Work<Real>) + 2 * NV * 4 * sizeof(Real) + (MAXLEVEL + 1) * LVL_G * sizeof(int) + 32 * sizeof(LaneTopo); }
+// sm_90: 228 KiB of shared memory per SM, 1 KiB of it reserved per block, 32 B of static shared memory here (64 allowed).  A few hundred bytes
+// more in Work / LaneTopo and the 16-warp block no longer launches, so it is a compile-time error
+static_assert(step_smem<float, EPB_F>() + 1024 + 64 <= 228 * 1024, "k_env_step<float>: the 16 work sets of a block no longer fit one SM");
 
 extern "C" {
 
@@ -230,7 +226,7 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
         CK(cudaFuncSetAttribute(k_env_reset<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         int resident = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, k_env_step<float, EPB_F>, 32 * EPB_F, step_smem<float, EPB_F>()));
-        if (EPB_F == 7 && resident < UHC_MIN_CTAS) { g_err = "uhc_engine_create: k_env_step<float> reaches only " + std::to_string(resident) + " resident block(s) per SM (built for " + std::to_string(UHC_MIN_CTAS) + ")"; delete e; return -3; }
+        if (resident < 1) { g_err = "uhc_engine_create: k_env_step<float> with " + std::to_string(EPB_F) + " envs per block does not fit one SM"; delete e; return -3; }
     } else {
         CK(cudaFuncSetAttribute(k_env_step<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
         CK(cudaFuncSetAttribute(k_env_reset<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
