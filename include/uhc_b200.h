@@ -88,6 +88,26 @@ int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg);
 /* Expert tables for C clips (replaces HumanoidEnv.load_expert's per-episode recompute, humanoid_im.py:182-215):
  * frames_host = concatenated [sum(len)][UHC_EX_SIZE] doubles, shape_host = [C][17] (beta16, gender). */
 int uhc_load_clips(UhcEngine *e, int nclips, const int *clip_len, const double *frames_host, const double *shape_host);
+/* Expert tables built on the device from raw motion (the opt-in alternative to building them on the host with
+ * uhc_b200/motion_lib.py and calling uhc_load_clips; same table, same contract).  rows_host = concatenated [sum(len)][row width]
+ * doubles of one kind:
+ *   UHC_MOTION_SMPL  pose_aa (pose_dim = 72, or 156 for SMPL-H: columns 66:72 are read as zero) then trans (3): smpl_to_qpose
+ *                    (smpl_mujoco.py:543-607) then qpos_fk;
+ *   UHC_MOTION_QPOS  qpos (pose_dim = 76): qpos_fk only (torch_smpl_humanoid.py:155-261).
+ * The FK uses shape variant fk_model_host[c] of the engine's model for clip c (NULL = variant 0).  The records are computed in fp64 and
+ * stored in the engine's precision.  The rows reach the device through a pinned staging buffer in chunks of whole clips of up to
+ * chunk_frames frames (0 = 32768; a longer clip is a chunk of its own), so the device scratch is bounded by the chunk.  As after
+ * uhc_load_clips: every env record is invalidated, the sampling weights return to the sample_keys rule and the clip models to
+ * variant 0.  Clips shorter than 2 frames and arguments out of range are rejected (-2) with the previous table left loaded. */
+#define UHC_MOTION_SMPL 0   /* rows: pose_aa (72 | 156) then trans (3) */
+#define UHC_MOTION_QPOS 1   /* rows: qpos (76) */
+int uhc_load_motions(UhcEngine *e, int nclips, const int *clip_len_host, int kind, int pose_dim, const double *rows_host,
+                     const double *shape_host, const int *fk_model_host, int chunk_frames);
+/* rows first .. first + n - 1 of clip `clip` of the loaded table, as doubles: out_host = [n][UHC_EX_SIZE] */
+int uhc_get_clip_frames(UhcEngine *e, int clip, int first, int n, double *out_host);
+/* device time of the last uhc_load_motions, from CUDA events (ms): out2[0] = its kernels, out2[1] = its host-to-device row copies */
+int uhc_load_motions_time(const UhcEngine *e, float *out2);
+
 /* body-shape variant of every clip (index into the model's shape variants); the reference rebuilds the robot per clip from
  * its beta/gender (humanoid_im.py:154-180).  Call after uhc_load_clips; default = variant 0 for every clip. */
 int uhc_set_clip_models(UhcEngine *e, int nclips, const int *clip_model);

@@ -100,7 +100,7 @@ class AgentCopycat:
             sync = make_nccl_grad_sync(world)
         rfc_mode = supported_variant(cfg)       # refuses (AssertionError) what the batched engine does not implement instead of accepting it silently (ADVICE r1)
         self.agent = BatchedAgent(
-            self.num_envs, self.data_loader.experts, self.data_loader.shapes, device=dev_index, seed=cfg.seed, policy_hsize=cfg.policy_hsize,
+            self.num_envs, self.data_loader.motions if self._device_tables(self.data_loader) else self.data_loader.experts, self.data_loader.shapes, device=dev_index, seed=cfg.seed, policy_hsize=cfg.policy_hsize,
             value_hsize=cfg.value_hsize, htype=cfg.policy_htype, log_std=cfg.log_std, policy_lr=cfg.policy_lr, value_lr=cfg.value_lr,
             gamma=cfg.gamma, tau=cfg.tau, clip_epsilon=cfg.clip_epsilon, num_optim_epoch=cfg.num_optim_epoch, grad_clip=40.0,
             t_min=cfg.data_specs.get("t_min", 90), t_max=cfg.data_specs.get("t_max", -1), rank=rank, world=world, grad_sync=sync,
@@ -209,8 +209,9 @@ class AgentCopycat:
         E = self.num_envs
         for loader in self.test_data_loaders:
             n = loader.get_len()
+            device_tables = self._device_tables(loader)
             if loader is not self.data_loader:
-                eng.load_clips(loader.experts, loader.shapes)      # invalidates every env record: only the envs reset below are stepped
+                self._load_tables(loader)      # invalidates every env record: only the envs reset below are stepped
             eng.set_cfg(**self._env_cfg(test=True))
             res = {}
             for c0 in range(0, n, E):
@@ -223,6 +224,15 @@ class AgentCopycat:
                 alive = np.ones(len(ids), bool); fail_any = np.zeros(len(ids), bool)
                 rsum = np.zeros(len(ids)); last_t = np.zeros(len(ids), np.int64)
                 traj = [dict(pred=[], pred_jpos=[], t=[]) for _ in ids]
+                gt = {}
+
+                def expert(i):
+                    """expert table of clip c0 + i: the host-built one, or the device-built one read back once (in the engine's precision)"""
+                    if not device_tables:
+                        return loader.experts[clips[i]]
+                    if i not in gt:
+                        gt[i] = eng.clip_frames(clips[i])
+                    return gt[i]
                 det = torch.ones(E, dtype=torch.uint8, device=obs.device)
                 for t in range(int(lens.max()) - 1):
                     s = self.running_state(obs, update=False)
@@ -240,9 +250,9 @@ class AgentCopycat:
                     fail_any[failed] = True
                     if len(failed):
                         if cfg.fail_safe:
-                            tt = [min(int(last_t[i]), loader.experts[clips[i]]["len"] - 1) for i in failed]
-                            eng.set_states(ids[failed], np.stack([loader.experts[clips[i]]["qpos"][k] for i, k in zip(failed, tt)]),
-                                           np.stack([loader.experts[clips[i]]["qvel"][k] for i, k in zip(failed, tt)]))
+                            tt = [min(int(last_t[i]), expert(i)["len"] - 1) for i in failed]
+                            eng.set_states(ids[failed], np.stack([expert(i)["qpos"][k] for i, k in zip(failed, tt)]),
+                                           np.stack([expert(i)["qvel"][k] for i, k in zip(failed, tt)]))
                         else:
                             alive[failed] = False
                     alive[live[e[live]]] = False
@@ -250,7 +260,7 @@ class AgentCopycat:
                         break
                 for i in ids:
                     k = loader.data_keys[c0 + i]
-                    ex = loader.experts[clips[i]]
+                    ex = expert(i)
                     tt = np.minimum(np.array(traj[i]["t"], dtype=np.int64), ex["len"] - 1)
                     percent = float(last_t[i]) / float(max(lens[i] - 1, 1))
                     r_i = {"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
@@ -264,7 +274,7 @@ class AgentCopycat:
                     if k in self.freq_dict:      # eval outcome feeds the failure-weighted sampler like a training episode ([percent, fr_start])
                         self.freq_dict[k] = (self.freq_dict[k] + [[1.0 if m["succ"][0] else min(percent, 0.999), 0]])[-self.max_freq:]
             if loader is not self.data_loader:
-                eng.load_clips(self.data_loader.experts, self.data_loader.shapes)
+                self._load_tables(self.data_loader)
             eng.set_cfg(**self._env_cfg(test=False))
             self.agent.obs = None
             names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
@@ -279,6 +289,17 @@ class AgentCopycat:
                 joblib.dump(res, path)
         self._push_clip_weights()
         return res_dicts
+
+    @staticmethod
+    def _device_tables(loader):
+        """data_specs.expert_tables: device -- the loader keeps the raw motion and the engine builds the expert tables on the GPU"""
+        return getattr(loader, "expert_tables", "host") == "device"
+
+    def _load_tables(self, loader):
+        if self._device_tables(loader):
+            self.agent.engine.load_motions(loader.motions, loader.shapes)
+        else:
+            self.agent.engine.load_clips(loader.experts, loader.shapes)
 
     def _env_cfg(self, test):
         cfg = self.cfg

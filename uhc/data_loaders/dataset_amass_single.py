@@ -1,6 +1,7 @@
 """DatasetAMASSSingle of the reference (uhc/data_loaders/dataset_amass_single.py:27-253): same pickle schema
 {key: {pose_aa, pose_6d, trans, beta, gender, ...}}, same filtering (len >= t_min + 1), same sampling rules; in addition it
-precomputes the expert tables of every clip once (uhc_b200.motion_lib) instead of once per episode."""
+precomputes the expert tables of every clip once (uhc_b200.motion_lib) instead of once per episode, or, with
+data_specs.expert_tables: device, hands the raw motion to the engine, which builds them on the GPU."""
 import random
 
 import joblib
@@ -43,8 +44,14 @@ class DatasetAMASSSingle:
             self.sample_keys += [(k, [-1])] * reps
         self.seq_len = len(self.data_keys)
         self.curr_key = ""
-        # expert tables of every clip, once (humanoid_im.py:182-215 does this per episode)
-        self.experts = [motion_lib.make_expert(self.data["pose_aa"][k], self.data["trans"][k], model) for k in self.data_keys]
+        # expert tables of every clip, once (humanoid_im.py:182-215 does this per episode).  data_specs.expert_tables: "host" (default)
+        # builds them here; "device" keeps only the raw motion (self.motions) and the engine builds the tables on the GPU (Engine.load_motions)
+        self.expert_tables = data_specs.get("expert_tables", "host")
+        assert self.expert_tables in ("host", "device"), "data_specs.expert_tables: host | device"
+        if self.expert_tables == "device":
+            self.motions = motion_lib.MotionSet([{"pose_aa": self.data["pose_aa"][k], "trans": self.data["trans"][k]} for k in self.data_keys])
+        else:
+            self.experts = [motion_lib.make_expert(self.data["pose_aa"][k], self.data["trans"][k], model) for k in self.data_keys]
         self.shapes = [np.concatenate([self.data["beta"][k][0], [self.data["gender"][k][0]]]) for k in self.data_keys]
 
     def get_len(self):

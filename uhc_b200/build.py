@@ -1,11 +1,14 @@
 """Builds libuhc_b200.so (CUDA, sm_90a) in-tree.  nvcc cross-compiles without a GPU."""
 import os
 import subprocess
+import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "libuhc_b200.so")
 SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_wgmma.cu", "rollout.cu", "ppo_update.cu"]
-DEPS = ["sim_core.h", "env_step.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h"]
+# compiled on their own without multiply-add contraction: the motion library restates numpy's fp64 arithmetic operation for operation
+NO_FMA_SRCS = ["motion_lib.cu"]
+DEPS = ["sim_core.h", "env_step.h", "motion_core.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
@@ -13,12 +16,24 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
 def build(force=False, verbose=False):
     csrc = os.path.join(HERE, "csrc")
     srcs = [os.path.join(csrc, s) for s in SRCS]
-    deps = srcs + [os.path.join(csrc, d) for d in DEPS] + [os.path.abspath(__file__)]
+    nofma = [os.path.join(csrc, s) for s in NO_FMA_SRCS]
+    deps = srcs + nofma + [os.path.join(csrc, d) for d in DEPS] + [os.path.abspath(__file__)]
     if not force and os.path.exists(SO) and os.path.getmtime(SO) >= max(os.path.getmtime(d) for d in deps if os.path.exists(d)):
         return SO
     flags = [f for f in NVCC_FLAGS if f != "--use_fast_math=false"] + os.environ.get("UHC_NVCC_EXTRA", "").split()
-    cmd = ["nvcc"] + flags + ["-o", SO] + srcs + ["-ldl"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
+    with tempfile.TemporaryDirectory() as tmp:
+        objs = []
+        for s in nofma:
+            o = os.path.join(tmp, os.path.basename(s) + ".o")
+            cmd = ["nvcc"] + [f for f in flags if f != "-shared"] + ["-fmad=false", "-c", "-o", o, s]
+            r = subprocess.run(cmd, capture_output=True, text=True)
+            if verbose or r.returncode:
+                print(r.stdout[-6000:], r.stderr[-12000:])
+            if r.returncode:
+                raise RuntimeError("nvcc failed")
+            objs.append(o)
+        cmd = ["nvcc"] + flags + ["-o", SO] + srcs + objs + ["-ldl"]
+        r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or r.returncode:
         print(r.stdout[-6000:], r.stderr[-12000:])
     if r.returncode:

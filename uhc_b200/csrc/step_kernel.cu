@@ -8,6 +8,7 @@
 #include <vector>
 #include "../../include/uhc_b200.h"
 #include "env_step.h"
+#include "motion_core.h"
 
 using namespace uhc;
 
@@ -135,6 +136,9 @@ struct UhcEngine {
     std::vector<float> clip_w;            // clip sampling weights behind clip_cdf (uhc_set_clip_weights), empty = sample_keys rule
     int *d_order = nullptr;   // warp slot -> environment (work-sorted each step), null = identity
     std::vector<int> clip_len_h;   // host copy of the clip lengths (argument validation)
+    std::vector<int> clip_adr_h;   // host copy of the first frame of every clip
+    motion::MotionModel mo_model;  // FK tables of the device motion library (uhc_load_motions); mo_model.body = fp64 offsets / ipos on the device
+    float mo_ms[2] = {0.f, 0.f};   // kernel / row-copy time of the last uhc_load_motions (CUDA events, ms)
 };
 
 template <class T> static int dev_copy(UhcEngine *e, T **dst, const T *src, size_t n) {
@@ -216,6 +220,13 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
     e->E = num_envs; e->device = device; e->precision = precision; e->launches = 0; e->nshape = model->nshape > 0 ? model->nshape : 1;
     int rc = precision == 32 ? build_view<float>(e, e->evf, model, cfg) : build_view<double>(e, e->evd, model, cfg);
     if (rc) { delete e; return rc; }
+    {   // the motion library's FK reads the bone offsets / com positions of every shape variant in fp64, whatever the engine's precision
+        std::vector<double> body((size_t)e->nshape * NB * motion::BODY6);
+        motion::motion_body_table(model->body_f, BODYF, e->nshape, body.data());
+        double *d_body;
+        if (dev_copy(e, &d_body, body.data(), body.size())) { delete e; return -1; }
+        motion::motion_model_init(e->mo_model, model->parent, model->ee, d_body);
+    }
     {   // work-sorted warp slots: opt-in (UHC_SORT_ENVS=1).  At 4096 envs sorting was slower than the identity
         // mapping -- the previous step's iteration total does not predict the per-substep imbalance well enough to pay for itself
         const char *se = getenv("UHC_SORT_ENVS");
@@ -287,17 +298,16 @@ int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
     return 0;
 }
 
-int uhc_load_clips(UhcEngine *e, int nclips, const int *clip_len, const double *frames_host, const double *shape_host) {
-    if (!e || nclips <= 0 || !clip_len || !frames_host || !shape_host) { g_err = "uhc_load_clips: bad argument"; return -2; }
-    CK(cudaSetDevice(e->device));
-    CK(cudaDeviceSynchronize());
+// replaces the clip table (shared by uhc_load_clips and uhc_load_motions): clip addresses, sampling CDF back to the sample_keys rule,
+// clip models back to variant 0, every env record invalidated, shapes uploaded; d_expert is allocated (uninitialised) for the caller
+static int new_clip_table(UhcEngine *e, int nclips, const int *clip_len, const double *shape_host) {
     std::vector<int> adr(nclips + 1, 0);
-    for (int i = 0; i < nclips; i++) { if (clip_len[i] < 2) { g_err = "uhc_load_clips: clip shorter than 2 frames"; return -2; } adr[i + 1] = adr[i] + clip_len[i]; }
+    for (int i = 0; i < nclips; i++) adr[i + 1] = adr[i] + clip_len[i];
     const size_t nf = (size_t)adr[nclips] * EX_SIZE, ns = (size_t)nclips * 17;
     if (e->d_expert) { cudaFree(e->d_expert); cudaFree(e->d_shape); cudaFree(e->d_clip_adr); cudaFree(e->d_clip_cdf); e->d_expert = e->d_shape = nullptr; e->d_clip_adr = nullptr; e->d_clip_cdf = nullptr; }
     CK(cudaMalloc((void **)&e->d_clip_adr, (nclips + 1) * sizeof(int)));
     CK(cudaMemcpy(e->d_clip_adr, adr.data(), (nclips + 1) * sizeof(int), cudaMemcpyHostToDevice));
-    e->num_clips = nclips; e->clip_len_h.assign(clip_len, clip_len + nclips); e->clip_w.clear();
+    e->num_clips = nclips; e->clip_len_h.assign(clip_len, clip_len + nclips); e->clip_adr_h = adr; e->clip_w.clear();
     e->evf.cfg.num_clips = nclips; e->evd.cfg.num_clips = nclips;
     if (upload_clip_cdf(e)) return -1;
     if (e->d_clip_model) { cudaFree(e->d_clip_model); e->d_clip_model = nullptr; }
@@ -306,17 +316,133 @@ int uhc_load_clips(UhcEngine *e, int nclips, const int *clip_len, const double *
     // until uhc_env_reset gives it a slice of the new table
     CK(cudaMemset(e->precision == 32 ? e->evf.istate : e->evd.istate, 0, (size_t)e->E * SI_SIZE * sizeof(int)));
     if (e->precision == 32) {
-        std::vector<float> f(nf), s(ns);
-        for (size_t i = 0; i < nf; i++) f[i] = (float)frames_host[i];
+        std::vector<float> s(ns);
         for (size_t i = 0; i < ns; i++) s[i] = (float)shape_host[i];
         CK(cudaMalloc(&e->d_expert, nf * 4)); CK(cudaMalloc(&e->d_shape, ns * 4));
-        CK(cudaMemcpy(e->d_expert, f.data(), nf * 4, cudaMemcpyHostToDevice)); CK(cudaMemcpy(e->d_shape, s.data(), ns * 4, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(e->d_shape, s.data(), ns * 4, cudaMemcpyHostToDevice));
         e->evf.expert = (const float *)e->d_expert; e->evf.clip_shape = (const float *)e->d_shape; e->evf.clip_adr = e->d_clip_adr;
     } else {
         CK(cudaMalloc(&e->d_expert, nf * 8)); CK(cudaMalloc(&e->d_shape, ns * 8));
-        CK(cudaMemcpy(e->d_expert, frames_host, nf * 8, cudaMemcpyHostToDevice)); CK(cudaMemcpy(e->d_shape, shape_host, ns * 8, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(e->d_shape, shape_host, ns * 8, cudaMemcpyHostToDevice));
         e->evd.expert = (const double *)e->d_expert; e->evd.clip_shape = (const double *)e->d_shape; e->evd.clip_adr = e->d_clip_adr;
     }
+    return 0;
+}
+
+int uhc_load_clips(UhcEngine *e, int nclips, const int *clip_len, const double *frames_host, const double *shape_host) {
+    if (!e || nclips <= 0 || !clip_len || !frames_host || !shape_host) { g_err = "uhc_load_clips: bad argument"; return -2; }
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());
+    size_t nframes = 0;
+    for (int i = 0; i < nclips; i++) { if (clip_len[i] < 2) { g_err = "uhc_load_clips: clip shorter than 2 frames"; return -2; } nframes += clip_len[i]; }
+    if (new_clip_table(e, nclips, clip_len, shape_host)) return -1;
+    const size_t nf = nframes * EX_SIZE;
+    if (e->precision == 32) {
+        std::vector<float> f(nf);
+        for (size_t i = 0; i < nf; i++) f[i] = (float)frames_host[i];
+        CK(cudaMemcpy(e->d_expert, f.data(), nf * 4, cudaMemcpyHostToDevice));
+    } else {
+        CK(cudaMemcpy(e->d_expert, frames_host, nf * 8, cudaMemcpyHostToDevice));
+    }
+    return 0;
+}
+
+// pinned / device staging of uhc_load_motions: two buffers, so the host fills one chunk while the device copies and expands the other
+struct MotionStaging {
+    double *h[2] = {nullptr, nullptr}, *d[2] = {nullptr, nullptr}; int *d_fk = nullptr;
+    cudaEvent_t ev[2][3] = {};   // per buffer: copy start, kernel start, kernel end
+    ~MotionStaging() {
+        for (int s = 0; s < 2; s++) {
+            if (h[s]) cudaFreeHost(h[s]);
+            if (d[s]) cudaFree(d[s]);
+            for (int k = 0; k < 3; k++) if (ev[s][k]) cudaEventDestroy(ev[s][k]);
+        }
+        if (d_fk) cudaFree(d_fk);
+    }
+};
+static void add_elapsed(float *acc, cudaEvent_t a, cudaEvent_t b) { float ms = 0.f; if (cudaEventElapsedTime(&ms, a, b) == cudaSuccess) *acc += ms; }
+
+int uhc_load_motions(UhcEngine *e, int nclips, const int *clip_len, int kind, int pose_dim, const double *rows_host, const double *shape_host,
+                     const int *fk_model, int chunk_frames) {
+    if (!e || nclips <= 0 || !clip_len || !rows_host || !shape_host) { g_err = "uhc_load_motions: bad argument"; return -2; }
+    if (kind != UHC_MOTION_SMPL && kind != UHC_MOTION_QPOS) { g_err = "uhc_load_motions: kind must be UHC_MOTION_SMPL or UHC_MOTION_QPOS"; return -2; }
+    if (kind == UHC_MOTION_SMPL ? (pose_dim != 72 && pose_dim != 156) : pose_dim != NQ) { g_err = "uhc_load_motions: pose_dim must be 72 or 156 (UHC_MOTION_SMPL) or 76 (UHC_MOTION_QPOS)"; return -2; }
+    if (chunk_frames < 0) { g_err = "uhc_load_motions: chunk_frames < 0"; return -2; }
+    long long total = 0;
+    for (int i = 0; i < nclips; i++) {
+        if (clip_len[i] < 2) { g_err = "uhc_load_motions: clip shorter than 2 frames"; return -2; }
+        total += clip_len[i];
+        if (fk_model && (fk_model[i] < 0 || fk_model[i] >= e->nshape)) { g_err = "uhc_load_motions: fk_model index out of range"; return -2; }
+    }
+    if (total > 0x7fffffffLL) { g_err = "uhc_load_motions: more than 2^31 - 1 frames"; return -2; }
+    const int row_w = kind == UHC_MOTION_SMPL ? pose_dim + 3 : NQ;
+    const int cap = chunk_frames > 0 ? chunk_frames : 32768;
+    // chunks of whole clips, each of at most `cap` frames unless a single clip is longer
+    std::vector<int> cut(1, 0); size_t rows_max = 0;
+    {
+        long long n = 0;
+        for (int i = 0; i < nclips; i++) {
+            if (n > 0 && n + clip_len[i] > cap) { cut.push_back(i); rows_max = (size_t)n > rows_max ? (size_t)n : rows_max; n = 0; }
+            n += clip_len[i];
+        }
+        cut.push_back(nclips); rows_max = (size_t)n > rows_max ? (size_t)n : rows_max;
+    }
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());
+    MotionStaging st;
+    const size_t stage_bytes = rows_max * row_w * sizeof(double);
+    for (int s = 0; s < 2; s++) {
+        CK(cudaHostAlloc((void **)&st.h[s], stage_bytes, cudaHostAllocDefault)); CK(cudaMalloc((void **)&st.d[s], stage_bytes));
+        for (int k = 0; k < 3; k++) CK(cudaEventCreate(&st.ev[s][k]));
+    }
+    if (fk_model) { CK(cudaMalloc((void **)&st.d_fk, nclips * sizeof(int))); CK(cudaMemcpy(st.d_fk, fk_model, nclips * sizeof(int), cudaMemcpyHostToDevice)); }
+    if (new_clip_table(e, nclips, clip_len, shape_host)) return -1;
+    e->mo_ms[0] = e->mo_ms[1] = 0.f;
+    const int nchunk = (int)cut.size() - 1;
+    for (int k = 0; k < nchunk; k++) {
+        const int s = k & 1, c0 = cut[k], c1 = cut[k + 1];
+        const int f0 = e->clip_adr_h[c0], nf = e->clip_adr_h[c1] - f0;
+        if (k >= 2) {   // buffer s was last used by chunk k - 2: wait for its kernel, then take its timings
+            CK(cudaEventSynchronize(st.ev[s][2]));
+            add_elapsed(&e->mo_ms[1], st.ev[s][0], st.ev[s][1]); add_elapsed(&e->mo_ms[0], st.ev[s][1], st.ev[s][2]);
+        }
+        memcpy(st.h[s], rows_host + (size_t)f0 * row_w, (size_t)nf * row_w * sizeof(double));
+        CK(cudaEventRecord(st.ev[s][0], 0));
+        CK(cudaMemcpyAsync(st.d[s], st.h[s], (size_t)nf * row_w * sizeof(double), cudaMemcpyHostToDevice, 0));
+        CK(cudaEventRecord(st.ev[s][1], 0));
+        CK(e->precision == 32 ? motion::launch_motion_frames<float>(e->mo_model, kind, pose_dim, st.d[s], e->d_clip_adr, st.d_fk, c0, c1, nf, (float *)e->d_expert, 0)
+                              : motion::launch_motion_frames<double>(e->mo_model, kind, pose_dim, st.d[s], e->d_clip_adr, st.d_fk, c0, c1, nf, (double *)e->d_expert, 0));
+        CK(cudaEventRecord(st.ev[s][2], 0));
+        e->launches++;
+    }
+    CK(cudaDeviceSynchronize());
+    for (int k = nchunk > 2 ? nchunk - 2 : 0; k < nchunk; k++) {
+        const int s = k & 1;
+        add_elapsed(&e->mo_ms[1], st.ev[s][0], st.ev[s][1]); add_elapsed(&e->mo_ms[0], st.ev[s][1], st.ev[s][2]);
+    }
+    return 0;
+}
+
+int uhc_get_clip_frames(UhcEngine *e, int clip, int first, int n, double *out_host) {
+    if (!e || !out_host || clip < 0 || clip >= e->num_clips || first < 0 || n < 0 || first + n > e->clip_len_h[clip]) { g_err = "uhc_get_clip_frames: bad argument"; return -2; }
+    if (!e->d_expert) { g_err = "uhc_get_clip_frames: no clips loaded"; return -3; }
+    if (n == 0) return 0;
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());
+    const size_t off = ((size_t)e->clip_adr_h[clip] + first) * EX_SIZE, cnt = (size_t)n * EX_SIZE;
+    if (e->precision == 32) {
+        std::vector<float> f(cnt);
+        CK(cudaMemcpy(f.data(), (const float *)e->d_expert + off, cnt * 4, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < cnt; i++) out_host[i] = (double)f[i];
+    } else {
+        CK(cudaMemcpy(out_host, (const double *)e->d_expert + off, cnt * 8, cudaMemcpyDeviceToHost));
+    }
+    return 0;
+}
+
+int uhc_load_motions_time(const UhcEngine *e, float *out2) {
+    if (!e || !out2) { g_err = "uhc_load_motions_time: bad argument"; return -2; }
+    out2[0] = e->mo_ms[0]; out2[1] = e->mo_ms[1];
     return 0;
 }
 

@@ -79,6 +79,19 @@ def pack_expert(ex):
     return out
 
 
+def unpack_expert(rec):
+    """[T][576] frame records -> dict with the fields of motion_lib.qpos_fk (the inverse of pack_expert)"""
+    rec = np.asarray(rec, dtype=np.float64)
+    T, ex, o = len(rec), {}, 0
+    for k, n in EXPERT_FIELDS:
+        ex[k] = rec[:, o:o + n].copy()
+        o += n
+    ex["body_com"] = rec[:, 502:574].copy()
+    ex["height_lb"] = ex["qpos"][:, 2].min() if T else np.nan
+    ex["len"] = T
+    return ex
+
+
 _lib = None
 
 
@@ -175,6 +188,39 @@ class Engine:
         self.clip_len = lens
         if clip_models is not None:
             _chk(self.lib.uhc_set_clip_models(self.h, C.c_int(len(experts)), _ip(clip_models)))
+
+    def load_motions(self, motions, shapes=None, clip_models=None, fk_models=None, chunk_frames=0):
+        """Expert tables built on the GPU (uhc_load_motions) from a motion_lib.MotionSet: the same table load_clips gets from
+        [motion_lib.make_expert | qpos_fk per clip], without building it on the host.  fk_models: shape variant per clip used by the FK
+        (None: variant 0, as make_expert's default model); clip_models: the simulated body per clip (uhc_set_clip_models); chunk_frames:
+        frames per host-to-device chunk (0: the library's default)."""
+        n = len(motions)
+        lens = np.ascontiguousarray(motions.lens, np.int32)
+        rows = np.ascontiguousarray(motions.rows, np.float64)
+        shp = np.zeros((n, 17)) if shapes is None else np.asarray(shapes, dtype=np.float64).reshape(n, 17)
+        shp = np.ascontiguousarray(shp)
+        fk = None if fk_models is None else np.ascontiguousarray(fk_models, np.int32).reshape(n)
+        _chk(self.lib.uhc_load_motions(self.h, C.c_int(n), _ip(lens), C.c_int(motions.kind), C.c_int(motions.pose_dim),
+                                       rows.ctypes.data_as(C.POINTER(C.c_double)), shp.ctypes.data_as(C.POINTER(C.c_double)),
+                                       None if fk is None else _ip(fk), C.c_int(int(chunk_frames))))
+        self.clip_len = lens.copy()
+        if clip_models is not None:
+            _chk(self.lib.uhc_set_clip_models(self.h, C.c_int(n), _ip(clip_models)))
+
+    @property
+    def load_motions_time(self):
+        """device time of the last load_motions from CUDA events (ms): its kernels and its host-to-device row copies"""
+        out = np.zeros(2, np.float32)
+        _chk(self.lib.uhc_load_motions_time(self.h, out.ctypes.data_as(C.POINTER(C.c_float))))
+        return dict(kernel_ms=float(out[0]), copy_ms=float(out[1]))
+
+    def clip_frames(self, clip, first=0, n=None):
+        """rows first .. first + n - 1 of a loaded clip (uhc_get_clip_frames), in the engine's precision, as a dict with the field
+        names and shapes of motion_lib.qpos_fk (height_lb and len are those of the rows read)."""
+        n = int(self.clip_len[clip]) - first if n is None else int(n)
+        out = np.zeros((n, EX_SIZE))
+        _chk(self.lib.uhc_get_clip_frames(self.h, C.c_int(int(clip)), C.c_int(int(first)), C.c_int(n), out.ctypes.data_as(C.POINTER(C.c_double))))
+        return unpack_expert(out)
 
     def _stream(self):
         return C.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)

@@ -128,6 +128,44 @@ def make_expert(pose_aa, trans, model=None):
     return qpos_fk(smpl_to_qpos(pose_aa, trans, m), m)
 
 
+class MotionSet:
+    """Raw motion of a dataset, for Engine.load_motions: the expert tables are built on the GPU from it (uhc_b200/csrc/motion_lib.cu),
+    so the host never holds them.  clips: list of {pose_aa [T][72 | 156], trans [T][3] (None: the default height)} or of {qpos [T][76]}
+    dicts, all of one kind.  Keeps the concatenated rows [sum T][pose_dim + 3 | 76] (fp64) and the clip lengths.  A set that mixes 72- and
+    156-wide poses is stored 72 wide with the SMPL-H conversion applied (columns 66:72 zeroed), which smpl_to_qpos would do per clip."""
+    SMPL, QPOS = 0, 1          # include/uhc_b200.h UHC_MOTION_SMPL / UHC_MOTION_QPOS
+
+    def __init__(self, clips):
+        clips = list(clips)
+        assert clips, "MotionSet: no clips"
+        if all("qpos" in c and "pose_aa" not in c for c in clips):
+            self.kind, self.pose_dim = self.QPOS, 76
+            rows = [np.asarray(c["qpos"], dtype=np.float64).reshape(-1, 76) for c in clips]
+        else:
+            assert all("pose_aa" in c for c in clips), "MotionSet: every clip needs pose_aa (+ trans), or every clip qpos"
+            poses = [np.asarray(c["pose_aa"], dtype=np.float64) for c in clips]
+            poses = [p.reshape(p.shape[0], -1) for p in poses]
+            widths = {p.shape[1] for p in poses}
+            assert widths <= {72, 156}, "MotionSet: pose_aa rows are 72 (SMPL) or 156 (SMPL-H) wide"
+            if len(widths) > 1:
+                poses = [p if p.shape[1] == 72 else np.concatenate([p[:, :66], np.zeros((len(p), 6))], 1) for p in poses]
+            self.kind, self.pose_dim = self.SMPL, poses[0].shape[1]
+            rows = []
+            for p, c in zip(poses, clips):
+                tr = c.get("trans")
+                tr = np.tile([0.0, 0.0, 0.91437225], (len(p), 1)) if tr is None else np.asarray(tr, dtype=np.float64).reshape(len(p), 3)
+                rows.append(np.concatenate([p, tr], 1))
+        self.lens = np.array([len(r) for r in rows], np.int32)
+        self.rows = np.ascontiguousarray(np.concatenate(rows))
+
+    def __len__(self):
+        return len(self.lens)
+
+    @property
+    def num_frames(self):
+        return int(self.lens.sum())
+
+
 def synthetic_clip(T, rng, model=None, kind="normal"):
     """AMASS-shaped synthetic motion (SURVEY.md section 8d config 5): 30 fps, joint angles = sum of 3 low-frequency sinusoids
     (amplitude <= 0.5 rad, f <= 1.5 Hz), slow root walk; `kind` sets the root-height profile."""
