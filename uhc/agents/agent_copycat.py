@@ -202,8 +202,9 @@ class AgentCopycat:
         (smpl_eval.compute_metrics: mpjpe / pa-mpjpe / accel / vel / root distance, restated in uhc_b200/metrics.py); fail_safe re-seats a
         failed humanoid on the expert pose with one batched set_state (humanoid_im.py:902-905)."""
         import torch
-        from uhc_b200.metrics import compute_metrics
+        from uhc_b200.metrics import compute_metrics, metrics_from_frames
         cfg = self.cfg
+        on_device = bool(cfg.get("eval_on_device", False))     # opt-in: BatchedAgent.evaluate (uhc_eval_run) instead of the host loop below
         res_dicts = []
         eng = self.agent.engine
         E = self.num_envs
@@ -217,10 +218,17 @@ class AgentCopycat:
             for c0 in range(0, n, E):
                 ids = np.arange(min(E, n - c0), dtype=np.int32)
                 clips = (c0 + ids).astype(np.int32)
+                lens = eng.clip_len[clips]
+                if on_device:                                      # the same roll-out as the loop below, as CUDA-graph replays with the metrics on the device
+                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32)
+                    last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
+                    rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
+                    self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec,
+                                       lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs))
+                    continue
                 if len(ids) < E:                                   # idle envs: park them on clip c0 so every record is valid (their outputs are ignored)
                     eng.reset(np.arange(len(ids), E, dtype=np.int32), np.full(E - len(ids), c0, np.int32), 0, None)
                 obs = eng.reset(ids, clips, 0, None)
-                lens = eng.clip_len[clips]
                 alive = np.ones(len(ids), bool); fail_any = np.zeros(len(ids), bool)
                 rsum = np.zeros(len(ids)); last_t = np.zeros(len(ids), np.int64)
                 traj = [dict(pred=[], pred_jpos=[], t=[]) for _ in ids]
@@ -258,21 +266,12 @@ class AgentCopycat:
                     alive[live[e[live]]] = False
                     if not alive.any():
                         break
-                for i in ids:
-                    k = loader.data_keys[c0 + i]
+                def host_metrics(i, pct, fs):
                     ex = expert(i)
                     tt = np.minimum(np.array(traj[i]["t"], dtype=np.int64), ex["len"] - 1)
-                    percent = float(last_t[i]) / float(max(lens[i] - 1, 1))
-                    r_i = {"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
-                           "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": 1.0 if (percent >= 1.0 and not fail_any[i]) else min(percent, 0.999),
-                           "fail_safe": bool(fail_any[i] and cfg.fail_safe)}
-                    m = compute_metrics(r_i) if len(tt) >= 3 else {"succ": np.array([False])}
-                    m["succ"] = np.array([bool(m["succ"][0]) and not fail_any[i]])
-                    m["reward"] = rsum[i] / max(lens[i] - 1, 1)
-                    m["percent"] = percent
-                    res[k] = m
-                    if k in self.freq_dict:      # eval outcome feeds the failure-weighted sampler like a training episode ([percent, fr_start])
-                        self.freq_dict[k] = (self.freq_dict[k] + [[1.0 if m["succ"][0] else min(percent, 0.999), 0]])[-self.max_freq:]
+                    return compute_metrics({"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
+                                            "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": pct, "fail_safe": fs})
+                self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics)
             if loader is not self.data_loader:
                 self._load_tables(self.data_loader)
             eng.set_cfg(**self._env_cfg(test=False))
@@ -289,6 +288,22 @@ class AgentCopycat:
                 joblib.dump(res, path)
         self._push_clip_weights()
         return res_dicts
+
+    def _eval_results(self, res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec, metrics_of):
+        """res[key] of every clip of one evaluation chunk, from either roll-out: the percent / succ rules of eval_seq, the reward
+        average, and the eval outcome fed to the failure-weighted sampler.  metrics_of(i, percent, fail_safe) -> compute_metrics' dict."""
+        cfg = self.cfg
+        for i in ids:
+            k = loader.data_keys[c0 + i]
+            percent = float(last_t[i]) / float(max(lens[i] - 1, 1))
+            pct = 1.0 if (percent >= 1.0 and not fail_any[i]) else min(percent, 0.999)
+            m = metrics_of(i, pct, bool(fail_any[i] and cfg.fail_safe)) if nrec[i] >= 3 else {"succ": np.array([False])}
+            m["succ"] = np.array([bool(m["succ"][0]) and not fail_any[i]])
+            m["reward"] = rsum[i] / max(lens[i] - 1, 1)
+            m["percent"] = percent
+            res[k] = m
+            if k in self.freq_dict:      # eval outcome feeds the failure-weighted sampler like a training episode ([percent, fr_start])
+                self.freq_dict[k] = (self.freq_dict[k] + [[1.0 if m["succ"][0] else min(percent, 0.999), 0]])[-self.max_freq:]
 
     @staticmethod
     def _device_tables(loader):

@@ -348,6 +348,24 @@ class BatchedAgent:
             out.update(allreduce_ms=ms, allreduce_bytes=by, allreduce_calls=calls)
         return out
 
+    def evaluate(self, clips, fail_safe, window=32, record_states=False):
+        """deterministic roll-out of every listed clip from frame 0 on the device (Engine.eval_run, one call per chunk of E clips) under
+        the engine's current cfg.  Returns one dict per clip: frames = [nframes][6] per-frame rows (uhc_b200/metrics.py
+        metrics_from_frames), last_t, fail_any, reward_sum (and states = [nframes][148] when record_states)."""
+        mcp = self.actor_type == "mcp"
+        pol = nn.mcp_struct(self.policy) if mcp else nn.mlp_struct(self.policy)
+        clips = np.asarray(clips, dtype=np.int32).reshape(-1)
+        out = []
+        for c0 in range(0, len(clips), self.E):
+            r = self.engine.eval_run(clips[c0:c0 + self.E], pol, self.log_std, self.running_state.stats, self.running_state.clip, fail_safe, window, record_states)
+            for i, nf in enumerate(r["nframes"]):
+                d = dict(frames=r["frames"][i, :nf].copy(), last_t=int(r["last_t"][i]), fail_any=bool(r["fail_any"][i]), reward_sum=float(r["reward_sum"][i]))
+                if record_states:
+                    d["states"] = r["states"][i, :nf].copy()
+                out.append(d)
+        self.obs = None       # every env was reset onto an evaluation clip
+        return out
+
     def optimize_policy(self, T):
         buf, log = self.sample(T)
         log.update(self.update_params(buf))

@@ -1,0 +1,269 @@
+// eval.cu -- the device evaluation behind the C ABI (include/uhc_eval.h): deterministic roll-outs of whole clips, fail_safe and the
+// per-frame imitation metrics, as CUDA-graph replays.
+//
+// Replaces one iteration of the chunk loop of AgentCopycat.eval_policy (uhc/agents/agent_copycat.py, kept as the default and as the
+// reference of tests/test_gpu_eval.py).  One control step is
+//   k_zfilter_apply_bf16, the policy GEMMs (+ mixture head), k_gauss_sample_dev   uhc_policy_forward's kernels, mean action, no ZFilter update
+//   k_env_step                                                                   uhc_env_step under the engine's current (test-mode) cfg
+//   k_eval_frame                                                                 per env still alive: the frame's metrics into a window buffer,
+//                                                                                the reward sum, fail / end, the fail_safe flag
+//   k_eval_reseat (fail_safe only)                                               uhc_env_set_state_batch's re-seat of the flagged envs
+// `window` steps are captured once per argument set into a CUDA graph; after each replay one 2-D copy moves the window's frame rows
+// into the caller's (pinned) array and one 4-byte copy returns the number of envs still alive, the host loop's early exit.
+//
+// Compiled on its own with -fmad=false (uhc_b200/build.py) like motion_lib.cu: k_eval_frame restates numpy's fp64 arithmetic
+// (eval_core.h) without contracted multiply-adds.  The policy and physics kernels it replays are compiled with the rest of the library.
+#include <cuda_runtime.h>
+#include <string.h>
+#include <string>
+#include <vector>
+#include "../../include/uhc_eval.h"
+#include "eval_core.h"
+#include "eval_glue.h"
+#include "sim_core.h"
+
+using namespace uhc;
+
+static thread_local std::string g_ev_err;
+#define CKE(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_ev_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
+
+namespace {
+
+constexpr int NCOL = evalm::EV_N, NSTATE = UHC_EVAL_STATE, RING = 2 * 144;   // ring per env: pred xpos72 + gt wbpos72 of the two previous frames
+static_assert(NCOL == UHC_EVAL_NCOL, "eval_core.h and uhc_eval.h disagree on the frame columns");
+
+// one thread per env i < n: the recorded frame of this step (host loop: get_states of the live envs, traj append, rsum += r,
+// fail -> set_states or alive = False, end -> alive = False)
+template <class Real>
+__global__ void __launch_bounds__(128) k_eval_frame(const Real *__restrict__ state, const int *__restrict__ istate, const Real *__restrict__ expert,
+                                                    const int *__restrict__ clip_adr, const float *__restrict__ rew, const int *__restrict__ fail,
+                                                    const int *__restrict__ end, int n, int nrec_max, int fail_safe, int window, int slot,
+                                                    UhcEvalClip *__restrict__ clips, int *__restrict__ alive, int *__restrict__ reseat,
+                                                    double *__restrict__ ring, double *__restrict__ win, double *__restrict__ win_states,
+                                                    int *__restrict__ alive_count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    reseat[i] = 0;
+    if (alive[i]) {
+        UhcEvalClip c = clips[i];
+        const int k = c.frames;
+        if (k >= nrec_max) alive[i] = 0;       // the host loop's step limit, max(len) - 1: only the tail of the last window steps past it
+        else {
+            const int *is = istate + (size_t)i * SI_SIZE;
+            const int cur_t = is[SI_CUR_T], clip = is[SI_CLIP];
+            const int a0 = clip_adr[clip], len = clip_adr[clip + 1] - a0;
+            const Real *gt = expert + ((size_t)a0 + (cur_t < len - 1 ? cur_t : len - 1)) * EX_SIZE;
+            const Real *st = state + (size_t)i * ST_SIZE;
+            double pq[7], gq[7], pj[72], gj[72];
+            for (int j = 0; j < 7; j++) { pq[j] = (double)st[ST_Q + j]; gq[j] = (double)gt[EX_QPOS + j]; }
+            for (int j = 0; j < 72; j++) { pj[j] = (double)st[ST_XPOS + j]; gj[j] = (double)gt[EX_WBPOS + j]; }
+            double *r = ring + (size_t)i * RING;
+            double *cur = r + (k & 1) * 144, *prev = r + ((k + 1) & 1) * 144;     // prev: frame k - 1; cur (before it is overwritten): frame k - 2
+            double out[NCOL];
+            evalm::eval_frame(pq, gq, pj, gj, k >= 1 ? prev : nullptr, k >= 1 ? prev + 72 : nullptr, k >= 2 ? cur : nullptr, k >= 2 ? cur + 72 : nullptr, out);
+            for (int j = 0; j < 72; j++) { cur[j] = pj[j]; cur[72 + j] = gj[j]; }
+            double *w = win + ((size_t)i * window + slot) * NCOL;
+            for (int j = 0; j < NCOL; j++) w[j] = out[j];
+            if (win_states) {
+                double *ws = win_states + ((size_t)i * window + slot) * NSTATE;
+                for (int j = 0; j < 76; j++) ws[j] = (double)st[ST_Q + j];
+                for (int j = 0; j < 72; j++) ws[76 + j] = pj[j];
+            }
+            c.frames = k + 1; c.last_t = cur_t; c.reward_sum += (double)rew[i];
+            const bool f = fail[i] != 0, d = end[i] != 0;
+            if (f) { c.fail_any = 1; if (fail_safe) reseat[i] = 1; else alive[i] = 0; }
+            if (d) alive[i] = 0;
+            clips[i] = c;
+        }
+    }
+    if (alive_count && alive[i]) atomicAdd(alive_count, 1);
+}
+
+__global__ void k_eval_init(int n, UhcEvalClip *__restrict__ clips, int *__restrict__ alive, int *__restrict__ reseat, unsigned char *__restrict__ ones, int E) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) { UhcEvalClip c; c.frames = 0; c.last_t = 0; c.fail_any = 0; c.reserved = 0; c.reward_sum = 0.0; clips[i] = c; alive[i] = 1; reseat[i] = 0; }
+    if (i < E) ones[i] = 1;
+}
+
+struct EvalKey {
+    int n, nrec_max, window, fail_safe, states, nprim; float zclip; unsigned long long scratch_gen, eval_gen, view_gen;
+    UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; const float *log_std; const double *zstats;
+    bool operator==(const EvalKey &o) const { return memcmp(this, &o, sizeof(EvalKey)) == 0; }
+};
+struct EvalCtx {
+    UhcEngine *eng = nullptr;
+    int E = 0, n_cap = 0, win_cap = 0, states_cap = 0;
+    unsigned long long gen = 0;                   // bumped when the scratch below is reallocated
+    UhcEvalClip *d_clips = nullptr; int *d_alive = nullptr, *d_reseat = nullptr, *d_count = nullptr; unsigned char *d_ones = nullptr;
+    double *d_ring = nullptr, *d_win = nullptr, *d_wstates = nullptr;
+    int *h_count = nullptr;                       // pinned
+    cudaEvent_t ev = nullptr;
+    std::vector<int> ids, clip0, start, len;      // reset arguments (kept: no allocation in the steady state)
+    std::vector<std::pair<EvalKey, cudaGraphExec_t>> graphs;
+};
+std::vector<EvalCtx *> g_ev;
+
+EvalCtx *ev_ctx(UhcEngine *e) {
+    for (EvalCtx *c : g_ev) if (c->eng == e) return c;
+    EvalCtx *c = new EvalCtx(); c->eng = e; c->E = uhc_num_envs(e);
+    g_ev.push_back(c);
+    return c;
+}
+void drop_graphs(EvalCtx *c) { for (auto &g : c->graphs) cudaGraphExecDestroy(g.second); c->graphs.clear(); }
+
+// per-env arrays sized by E once; the window buffers grow with n * window (and the state record with it when requested)
+int ensure(EvalCtx *c, int n, int window, bool states) {
+    const size_t E = c->E;
+    if (!c->d_clips) {
+        CKE(cudaMalloc((void **)&c->d_clips, E * sizeof(UhcEvalClip))); CKE(cudaMalloc((void **)&c->d_alive, E * 4)); CKE(cudaMalloc((void **)&c->d_reseat, E * 4));
+        CKE(cudaMalloc((void **)&c->d_count, 4)); CKE(cudaMalloc((void **)&c->d_ones, E)); CKE(cudaMalloc((void **)&c->d_ring, E * RING * sizeof(double)));
+        CKE(cudaHostAlloc((void **)&c->h_count, 4, cudaHostAllocDefault)); CKE(cudaEventCreateWithFlags(&c->ev, cudaEventDisableTiming));
+        c->gen++;
+    }
+    const int need = n * window;
+    if (need > c->win_cap) {
+        if (c->d_win) cudaFree(c->d_win);
+        CKE(cudaMalloc((void **)&c->d_win, (size_t)need * NCOL * sizeof(double))); c->win_cap = need; c->gen++;
+    }
+    if (states && need > c->states_cap) {
+        if (c->d_wstates) cudaFree(c->d_wstates);
+        CKE(cudaMalloc((void **)&c->d_wstates, (size_t)need * NSTATE * sizeof(double))); c->states_cap = need; c->gen++;
+    }
+    return 0;
+}
+
+int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
+                   int n, int nrec_max, int fail_safe, int window, bool states, cudaStream_t st) {
+    std::string err;
+    for (int s = 0; s < window; s++) {
+        int rc = evalx::policy_enqueue(c->eng, mlp, mcp, R.obs, log_std, zstats, zclip, c->d_ones, R.act, st, &err);
+        if (rc) { g_ev_err = err; return rc; }
+        if (uhc_env_step(c->eng, R.act, R.obs, R.rew, R.cinfo, R.fail, R.end, R.pct, nullptr, st)) { g_ev_err = std::string("env step: ") + uhc_last_error(); return -1; }
+        const bool last = s == window - 1;
+        if (last) CKE(cudaMemsetAsync(c->d_count, 0, 4, st));
+        if (R.precision == 32)
+            k_eval_frame<float><<<(n + 127) / 128, 128, 0, st>>>((const float *)R.state, R.istate, (const float *)R.expert, R.clip_adr, R.rew, R.fail, R.end, n, nrec_max,
+                                                                fail_safe, window, s, c->d_clips, c->d_alive, c->d_reseat, c->d_ring, c->d_win,
+                                                                states ? c->d_wstates : nullptr, last ? c->d_count : nullptr);
+        else
+            k_eval_frame<double><<<(n + 127) / 128, 128, 0, st>>>((const double *)R.state, R.istate, (const double *)R.expert, R.clip_adr, R.rew, R.fail, R.end, n, nrec_max,
+                                                                 fail_safe, window, s, c->d_clips, c->d_alive, c->d_reseat, c->d_ring, c->d_win,
+                                                                 states ? c->d_wstates : nullptr, last ? c->d_count : nullptr);
+        CKE(cudaGetLastError());
+        if (fail_safe) CKE(evalx::launch_reseat(c->eng, n, c->d_reseat, st));
+    }
+    return 0;
+}
+
+int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats,
+             float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host, void *stream) {
+    const char *who = mcp ? "uhc_eval_run_mcp" : "uhc_eval_run";
+    if (!e || !clip_host || (!mlp && !mcp) || !log_std || !zfilter_stats || !frames_host || !clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
+    evalx::EngineRefs R; evalx::engine_refs(e, &R);
+    if (n < 1 || n > R.E) { g_ev_err = std::string(who) + ": n must be 1 .. E"; return -2; }
+    if (window < 1) { g_ev_err = std::string(who) + ": window < 1"; return -2; }
+    if (R.num_clips <= 0) { g_ev_err = std::string(who) + ": no clips loaded"; return -2; }
+    int max_len = 0;
+    for (int i = 0; i < n; i++) {
+        if (clip_host[i] < 0 || clip_host[i] >= R.num_clips) { g_ev_err = std::string(who) + ": clip index out of range"; return -2; }
+        max_len = R.clip_len_h[clip_host[i]] > max_len ? R.clip_len_h[clip_host[i]] : max_len;
+    }
+    unsigned long long sgen = 0; std::string err;
+    int rc = evalx::policy_prepare(e, mlp, mcp, &sgen, &err);
+    if (rc) { g_ev_err = err; return rc; }
+    EvalCtx *c = ev_ctx(e);
+    const bool states = states_host != nullptr;
+    if (ensure(c, n, window, states)) return -1;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int nrec_max = max_len - 1;
+    // reset: idle envs parked on the chunk's first clip, then envs 0..n-1 on their clips from frame 0 (the host loop's order)
+    if (n < R.E) {
+        const int m = R.E - n;
+        c->ids.resize(m); c->clip0.assign(m, clip_host[0]); c->start.assign(m, 0); c->len.assign(m, R.clip_len_h[clip_host[0]]);
+        for (int k = 0; k < m; k++) c->ids[k] = n + k;
+        if (uhc_env_reset(e, m, c->ids.data(), c->clip0.data(), c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
+    }
+    c->ids.resize(n); c->start.assign(n, 0); c->len.resize(n);
+    for (int k = 0; k < n; k++) { c->ids[k] = k; c->len[k] = R.clip_len_h[clip_host[k]]; }
+    if (uhc_env_reset(e, n, c->ids.data(), clip_host, c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
+    k_eval_init<<<(R.E + 127) / 128, 128, 0, st>>>(n, c->d_clips, c->d_alive, c->d_reseat, c->d_ones, R.E);
+    CKE(cudaGetLastError());
+
+    EvalKey key; memset(&key, 0, sizeof key);
+    key.n = n; key.nrec_max = nrec_max; key.window = window; key.fail_safe = fail_safe ? 1 : 0; key.states = states; key.zclip = zclip;
+    key.scratch_gen = sgen; key.eval_gen = c->gen; key.view_gen = R.view_gen; key.log_std = log_std; key.zstats = zfilter_stats;
+    if (mcp) { key.nprim = mcp->nprim; for (int k = 0; k < mcp->nprim; k++) key.nets[k] = mcp->prim[k]; key.nets[mcp->nprim] = mcp->composer; }
+    else key.nets[0] = *mlp;
+    // a graph holds the engine view (cfg, clip table), the policy scratch and the window buffers of its capture as kernel parameters:
+    // once any of them has changed it can never be replayed, so it is dropped here rather than kept until eviction
+    for (size_t g = 0; g < c->graphs.size();) {
+        const EvalKey &k = c->graphs[g].first;
+        if (k.view_gen != key.view_gen || k.scratch_gen != key.scratch_gen || k.eval_gen != key.eval_gen) {
+            cudaGraphExecDestroy(c->graphs[g].second); c->graphs.erase(c->graphs.begin() + g);
+        } else g++;
+    }
+    cudaGraphExec_t exec = nullptr;
+    for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
+    if (!exec) {
+        cudaStream_t cs; CKE(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+        cudaGraph_t graph = nullptr;
+        CKE(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+        rc = enqueue_window(c, R, mlp, mcp, log_std, (double *)zfilter_stats, zclip, n, nrec_max, key.fail_safe, window, states, cs);
+        cudaError_t ce = cudaStreamEndCapture(cs, &graph);
+        cudaStreamDestroy(cs);
+        if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+        if (ce != cudaSuccess) { g_ev_err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce); return -1; }
+        ce = cudaGraphInstantiate(&exec, graph, 0);
+        cudaGraphDestroy(graph);
+        CKE(ce);
+        if (c->graphs.size() >= 32) { cudaGraphExecDestroy(c->graphs.front().second); c->graphs.erase(c->graphs.begin()); }
+        c->graphs.emplace_back(key, exec);
+    }
+    for (int s0 = 0; s0 < nrec_max; s0 += window) {
+        CKE(cudaGraphLaunch(exec, st));
+        const int rows = nrec_max - s0 < window ? nrec_max - s0 : window;
+        CKE(cudaMemcpy2DAsync(frames_host + (size_t)s0 * NCOL, (size_t)nrec_max * NCOL * sizeof(double), c->d_win, (size_t)window * NCOL * sizeof(double),
+                              (size_t)rows * NCOL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
+        if (states)
+            CKE(cudaMemcpy2DAsync(states_host + (size_t)s0 * NSTATE, (size_t)nrec_max * NSTATE * sizeof(double), c->d_wstates, (size_t)window * NSTATE * sizeof(double),
+                                  (size_t)rows * NSTATE * sizeof(double), n, cudaMemcpyDeviceToHost, st));
+        CKE(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
+        CKE(cudaEventRecord(c->ev, st));
+        CKE(cudaEventSynchronize(c->ev));
+        if (*c->h_count == 0) break;
+    }
+    CKE(cudaMemcpyAsync(clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
+    CKE(cudaStreamSynchronize(st));
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+const char *uhc_eval_last_error(void) { return g_ev_err.c_str(); }
+
+int uhc_eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
+                 int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
+    if (!mlp) { g_ev_err = "uhc_eval_run: null policy"; return -2; }
+    return eval_run(e, n, clip_host, mlp, nullptr, log_std, zfilter_stats, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+}
+int uhc_eval_run_mcp(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
+                     int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
+    if (!mcp) { g_ev_err = "uhc_eval_run_mcp: null policy"; return -2; }
+    return eval_run(e, n, clip_host, nullptr, mcp, log_std, zfilter_stats, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+}
+
+void uhc_eval_release(UhcEngine *e) {
+    for (size_t i = 0; i < g_ev.size(); i++) if (g_ev[i]->eng == e) {
+        EvalCtx *c = g_ev[i];
+        drop_graphs(c);
+        for (void *p : {(void *)c->d_clips, (void *)c->d_alive, (void *)c->d_reseat, (void *)c->d_count, (void *)c->d_ones, (void *)c->d_ring,
+                        (void *)c->d_win, (void *)c->d_wstates}) if (p) cudaFree(p);
+        if (c->h_count) cudaFreeHost(c->h_count);
+        if (c->ev) cudaEventDestroy(c->ev);
+        delete c; g_ev.erase(g_ev.begin() + i); return;
+    }
+}
+
+}  // extern "C"

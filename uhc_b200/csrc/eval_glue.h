@@ -1,0 +1,32 @@
+// eval_glue.h -- internal interface of the device evaluation (eval.cu) to the engine (step_kernel.cu) and to the policy forward of the
+// rollout (rollout.cu).  Not part of the C ABI.
+#pragma once
+#include <cuda_runtime.h>
+#include <string>
+#include "../../include/uhc_b200.h"
+#include "../../include/uhc_rollout.h"
+
+namespace uhc {
+namespace evalx {
+
+// the engine's device state and its host-API staging buffers (obs / action / step outputs, E rows each)
+struct EngineRefs {
+    int E, precision, obs_dim, act_dim, num_clips;
+    void *state; int *istate; const void *expert; const int *clip_adr;
+    const int *clip_len_h;    // host copy of the clip lengths
+    unsigned long long view_gen;   // changes with every cfg / clip-table / clip-model / CDF / neutral-pose update (graphs hold those by value)
+    float *obs, *act, *rew, *cinfo, *pct; int *fail, *end;
+};
+void engine_refs(UhcEngine *e, EngineRefs *out);                                            // step_kernel.cu
+// fail_safe re-seat of every env i < n with reseat[i] != 0: uhc_env_set_state_batch's reset-with-override onto the expert qpos / qvel
+// of frame min(cur_t, len - 1), rounded to fp32, keeping cur_t and the body quaternions; one launch, no host work
+cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t st);       // step_kernel.cu
+// policy of an evaluation: validates it (-2) and sizes the rollout's scratch outside any capture; *gen changes whenever that scratch
+// is reallocated (graphs holding the old pointers must be dropped)
+int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, unsigned long long *gen, std::string *err);   // rollout.cu
+// obs -> ZFilter (no update) -> policy -> action (the mean where mean_action[e] != 0); enqueues only (capturable)
+int policy_enqueue(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, const float *obs, const float *log_std, double *zstats, float zclip,
+                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err);                 // rollout.cu
+
+}  // namespace evalx
+}  // namespace uhc

@@ -19,6 +19,7 @@
 #include "../../include/uhc_b200.h"
 #include "../../include/uhc_nn.h"
 #include "../../include/uhc_rollout.h"
+#include "eval_glue.h"
 
 static thread_local std::string g_ro_err;
 #define CKR(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_ro_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
@@ -116,6 +117,7 @@ struct RolloutCtx {
     double *d_zws = nullptr; int zws_d = 0;
     unsigned char *d_mean_action = nullptr; float *d_cinfo = nullptr, *d_pct = nullptr; int *d_fail = nullptr, *d_end = nullptr;
     std::vector<std::pair<GraphKey, cudaGraphExec_t>> graphs;
+    unsigned long long scratch_gen = 0;   // bumped whenever the scratch above is reallocated (the evaluation's graphs hold its pointers)
     int launches_per_step = 0;
     std::vector<cudaEvent_t> ev0, ev1;    // optional: events around the env-step kernel of buffer row r (bench roofline: the dominant kernel's live duration)
 };
@@ -139,7 +141,7 @@ int ensure_scratch(RolloutCtx *c, const Policy *pol) {
     const int P = pol->nprim, nnets = P > 0 ? P + 1 : 1;
     if (P < 0 || P > UHC_MCP_MAX_PRIM) { g_ro_err = "UhcMcp: 1..8 primitives"; return -2; }
     const UhcMlp *m0 = &pol->nets[0];
-    auto drop_graphs = [&]() { for (auto &g : c->graphs) cudaGraphExecDestroy(g.second); c->graphs.clear(); };
+    auto drop_graphs = [&]() { for (auto &g : c->graphs) cudaGraphExecDestroy(g.second); c->graphs.clear(); c->scratch_gen++; };
     for (int j = 0; j < nnets; j++) {
         const UhcMlp *m = &pol->nets[j];
         if (m->nlayers < 1 || m->nlayers > 8) { g_ro_err = "UhcMlp: 1..8 layers"; return -2; }
@@ -381,3 +383,33 @@ void uhc_rollout_release(UhcEngine *e) {   // called by the binding before uhc_e
 }
 
 }  // extern "C"
+
+// ---- the policy forward of the device evaluation (eval_glue.h): the kernels of uhc_policy_forward(_mcp), enqueued from eval.cu's graphs
+namespace uhc {
+namespace evalx {
+
+int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, unsigned long long *gen, std::string *err) {
+    Policy pol;
+    if (make_policy(&pol, mlp, mcp, e, mcp ? "uhc_eval_run_mcp" : "uhc_eval_run")) { *err = g_ro_err; return -2; }
+    RolloutCtx *c = ctx_of(e);
+    const int rc = ensure_scratch(c, &pol);
+    if (rc) { *err = g_ro_err; return rc; }
+    *gen = c->scratch_gen;
+    return 0;
+}
+
+int policy_enqueue(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, const float *obs, const float *log_std, double *zstats, float zclip,
+                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err) {
+    Policy pol;
+    if (make_policy(&pol, mlp, mcp, e, "uhc_eval_run")) { *err = g_ro_err; return -2; }
+    RolloutCtx *c = ctx_of(e);
+    if (enqueue_policy(c, obs, &pol, zstats, zclip, 0, nullptr, st) < 0) { *err = g_ro_err; return -1; }
+    const UhcMlp *m = &pol.nets[0];
+    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->d_mean, log_std, mean_action, action, nullptr, c->E, m->dims[m->nlayers], 0, c->d_step);
+    const cudaError_t ce = cudaGetLastError();
+    if (ce != cudaSuccess) { *err = std::string("k_gauss_sample_dev: ") + cudaGetErrorString(ce); return -1; }
+    return 0;
+}
+
+}  // namespace evalx
+}  // namespace uhc

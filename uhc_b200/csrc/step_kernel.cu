@@ -9,6 +9,7 @@
 #include "../../include/uhc_b200.h"
 #include "env_step.h"
 #include "motion_core.h"
+#include "eval_glue.h"
 
 using namespace uhc;
 
@@ -97,6 +98,35 @@ k_env_reset(EngineView<Real> ev, int n, const int *__restrict__ ids, const int *
     env_reset_warp<Real, float>(ev, env, w, clip[i], start[i], len[i], qo, vo, obs ? obs + (size_t)env * ev.cfg.obs_dim : nullptr);
 }
 
+// device evaluation's fail_safe (eval.cu): the re-seat of uhc_env_set_state_batch -- k_save_restore_bquat, k_env_reset with the
+// fp32-rounded expert qpos / qvel of frame min(cur_t, len - 1) as override and no obs, k_save_restore_bquat -- in one launch, for the
+// envs i < n whose flag is set (the flag is written on the device by k_eval_frame, so the graph replays need no host decision)
+template <class Real, int EPB>
+__global__ void __launch_bounds__(32 * EPB)
+k_eval_reseat(EngineView<Real> ev, int n, const int *__restrict__ reseat) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int warp = threadIdx.x >> 5, env = blockIdx.x * EPB + warp, lane = threadIdx.x & 31;
+    const bool mine = env < n && reseat[env] != 0;
+    if (!__syncthreads_or(mine)) return;      // most steps re-seat no env of the block: skip the table staging (uniform per block)
+    stage_tables<Real, EPB>(ev, smem);
+    if (!mine) return;
+    Work<Real> &w = reinterpret_cast<Work<Real> *>(smem)[warp];
+    int *is = ev.istate + (size_t)env * SI_SIZE;
+    const int cur_t = is[SI_CUR_T], clip = is[SI_CLIP], start = is[SI_START], len = is[SI_LEN];
+    Real *bq = ev.state + (size_t)env * ST_SIZE + ST_BQUAT;       // bquat + pbquat: 192 Reals, 6 per lane
+    Real keep[6];
+    for (int k = 0; k < 6; k++) keep[k] = bq[lane + 32 * k];
+    const Real *f = expert_frame(ev, clip, start, len, cur_t);
+    Real *qo = w.as_, *vo = w.Mp;                                  // the override's staging vectors of k_env_reset
+    for (int k = lane; k < NQ; k += 32) qo[k] = (Real)(float)f[EX_QPOS + k];
+    for (int k = lane; k < NV; k += 32) vo[k] = (Real)(float)f[EX_QVEL + k];
+    __syncwarp();
+    env_reset_warp<Real, float>(ev, env, w, clip, start, len, qo, vo, (float *)nullptr);
+    __syncwarp();
+    for (int k = 0; k < 6; k++) bq[lane + 32 * k] = keep[k];
+    if (lane == 0) is[SI_CUR_T] = cur_t;
+}
+
 // parity / evaluation hook: gather q, v, xpos, bquat (+ the integer record) of the listed envs into one staging array
 template <class Real>
 __global__ void k_gather_state(const Real *__restrict__ state, const int *__restrict__ istate, const int *__restrict__ ids, int n, double *__restrict__ out, int *__restrict__ iout) {
@@ -137,6 +167,9 @@ struct UhcEngine {
     int *d_order = nullptr;   // warp slot -> environment (work-sorted each step), null = identity
     std::vector<int> clip_len_h;   // host copy of the clip lengths (argument validation)
     std::vector<int> clip_adr_h;   // host copy of the first frame of every clip
+    // bumped whenever anything a launch captures by value changes: the EngineView (cfg, clip table / model / CDF / neutral pointers).
+    // CUDA graphs of the device evaluation (eval.cu) are keyed on it, so a table load or set_cfg never replays stale parameters
+    unsigned long long view_gen = 0;
     motion::MotionModel mo_model;  // FK tables of the device motion library (uhc_load_motions); mo_model.body = fp64 offsets / ipos on the device
     float mo_ms[2] = {0.f, 0.f};   // kernel / row-copy time of the last uhc_load_motions (CUDA events, ms)
 };
@@ -235,12 +268,14 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
     if (precision == 32) {
         CK(cudaFuncSetAttribute(k_env_step<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         CK(cudaFuncSetAttribute(k_env_reset<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
+        CK(cudaFuncSetAttribute(k_eval_reseat<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         int resident = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, k_env_step<float, EPB_F>, 32 * EPB_F, step_smem<float, EPB_F>()));
         if (resident < 1) { g_err = "uhc_engine_create: k_env_step<float> with " + std::to_string(EPB_F) + " envs per block does not fit one SM"; delete e; return -3; }
     } else {
         CK(cudaFuncSetAttribute(k_env_step<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
         CK(cudaFuncSetAttribute(k_env_reset<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
+        CK(cudaFuncSetAttribute(k_eval_reseat<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
     }
     const size_t E = num_envs;
     CK(cudaMalloc((void **)&e->d_act, E * MAX_ACT_DIM * 4)); CK(cudaMalloc((void **)&e->d_obs, E * (size_t)(precision == 32 ? e->evf.cfg.obs_dim : e->evd.cfg.obs_dim) * 4)); CK(cudaMalloc((void **)&e->d_rew, E * 4));
@@ -289,6 +324,7 @@ static int upload_clip_cdf(UhcEngine *e) {
 
 int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
     if (!e || !cfg) { g_err = "uhc_engine_set_cfg: null"; return -2; }
+    e->view_gen++;
     CK(cudaSetDevice(e->device));
     const int old_tmax = e->precision == 32 ? e->evf.cfg.t_max : e->evd.cfg.t_max;
     const int old_obs_dim = uhc_engine_obs_dim(e);
@@ -301,6 +337,7 @@ int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
 // replaces the clip table (shared by uhc_load_clips and uhc_load_motions): clip addresses, sampling CDF back to the sample_keys rule,
 // clip models back to variant 0, every env record invalidated, shapes uploaded; d_expert is allocated (uninitialised) for the caller
 static int new_clip_table(UhcEngine *e, int nclips, const int *clip_len, const double *shape_host) {
+    e->view_gen++;
     std::vector<int> adr(nclips + 1, 0);
     for (int i = 0; i < nclips; i++) adr[i + 1] = adr[i] + clip_len[i];
     const size_t nf = (size_t)adr[nclips] * EX_SIZE, ns = (size_t)nclips * 17;
@@ -448,6 +485,7 @@ int uhc_load_motions_time(const UhcEngine *e, float *out2) {
 
 int uhc_set_neutral_pose(UhcEngine *e, const double *qpos76, const double *qvel75) {
     if (!e || !qpos76 || !qvel75) { g_err = "uhc_set_neutral_pose: bad argument"; return -2; }
+    e->view_gen++;
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
     std::vector<double> h(NQ + NV);
@@ -459,6 +497,7 @@ int uhc_set_neutral_pose(UhcEngine *e, const double *qpos76, const double *qvel7
 
 int uhc_set_clip_weights(UhcEngine *e, int nclips, const float *weights_host) {
     if (!e || nclips != e->num_clips) { g_err = "uhc_set_clip_weights: call after uhc_load_clips with one weight per clip"; return -2; }
+    e->view_gen++;
     CK(cudaSetDevice(e->device));
     if (!weights_host) e->clip_w.clear();
     else {
@@ -472,6 +511,7 @@ int uhc_set_clip_weights(UhcEngine *e, int nclips, const float *weights_host) {
 
 int uhc_set_clip_models(UhcEngine *e, int nclips, const int *clip_model) {
     if (!e || !clip_model || nclips != e->num_clips) { g_err = "uhc_set_clip_models: call after uhc_load_clips with one entry per clip"; return -2; }
+    e->view_gen++;
     for (int i = 0; i < nclips; i++) if (clip_model[i] < 0 || clip_model[i] >= e->nshape) { g_err = "uhc_set_clip_models: shape index out of range"; return -2; }
     CK(cudaSetDevice(e->device));
     if (e->d_clip_model) cudaFree(e->d_clip_model);
@@ -644,3 +684,25 @@ int uhc_engine_act_dim(const UhcEngine *e) { return e ? (e->precision == 32 ? e-
 int uhc_kernel_launches(const UhcEngine *e) { return e ? e->launches : -1; }
 
 }  // extern "C"
+
+// ---- the device evaluation's view of the engine (eval_glue.h)
+namespace uhc {
+namespace evalx {
+
+void engine_refs(UhcEngine *e, EngineRefs *r) {
+    const bool f32 = e->precision == 32;
+    r->E = e->E; r->precision = e->precision; r->obs_dim = uhc_engine_obs_dim(e); r->act_dim = uhc_engine_act_dim(e); r->num_clips = e->d_expert ? e->num_clips : 0;
+    r->state = f32 ? (void *)e->evf.state : (void *)e->evd.state; r->istate = f32 ? e->evf.istate : e->evd.istate;
+    r->expert = e->d_expert; r->clip_adr = e->d_clip_adr; r->clip_len_h = e->clip_len_h.data(); r->view_gen = e->view_gen;
+    r->obs = e->d_obs; r->act = e->d_act; r->rew = e->d_rew; r->cinfo = e->d_cinfo; r->pct = e->d_pct; r->fail = e->d_fail; r->end = e->d_end;
+}
+
+cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t st) {
+    if (e->precision == 32) k_eval_reseat<float, EPB_F><<<(n + EPB_F - 1) / EPB_F, 32 * EPB_F, step_smem<float, EPB_F>(), st>>>(e->evf, n, reseat);
+    else k_eval_reseat<double, EPB_D><<<(n + EPB_D - 1) / EPB_D, 32 * EPB_D, step_smem<double, EPB_D>(), st>>>(e->evd, n, reseat);
+    e->launches++;
+    return cudaGetLastError();
+}
+
+}  // namespace evalx
+}  // namespace uhc

@@ -24,6 +24,11 @@ class UhcEnvCfg(C.Structure):
                 ("reactive_rate", C.c_double), ("rfc_mode", C.c_int), ("vf_slot", C.c_int * 24), ("obs_v", C.c_int), ("fut_frames", C.c_int), ("fut_skip", C.c_int), ("no_shape", C.c_int), ("term_body", C.c_int), ("head_body", C.c_int), ("reward_mul", C.c_int)]
 
 
+class UhcEvalClip(C.Structure):
+    """include/uhc_eval.h UhcEvalClip"""
+    _fields_ = [("frames", C.c_int), ("last_t", C.c_int), ("fail_any", C.c_int), ("reserved", C.c_int), ("reward_sum", C.c_double)]
+
+
 def make_cfg(precision=32, base_rot=(0.7071, 0.7071, 0.0, 0.0), rfc_scale=100.0, rfc_lim=100.0, rfc_rate=1.0, body_diff_thresh=0.5,
              meta_pd=1, env_episode_len=100000, trail_steps=0, w=(0.3, 0.1, 0.45, 0.1, 0.05), k=(2.0, 0.005, 5.0, 100.0, 1.0),
              newton_max_iter=None, newton_tol=None, auto_reset=0, t_min=5, t_max=300, reset_seed=1, reactive_v=0, reactive_rate=0.3,
@@ -160,6 +165,7 @@ class Engine:
 
     def close(self):
         if getattr(self, "h", None):
+            self.lib.uhc_eval_release(self.h)
             self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
             self.h = None
@@ -292,6 +298,31 @@ class Engine:
         q = np.ascontiguousarray(qpos, np.float64).reshape(len(ids), NQ)
         v = np.ascontiguousarray(qvel, np.float64).reshape(len(ids), NV)
         _chk(self.lib.uhc_env_set_state_batch(self.h, C.c_int(len(ids)), _ip(ids), q.ctypes.data_as(C.POINTER(C.c_double)), v.ctypes.data_as(C.POINTER(C.c_double))))
+
+    def eval_run(self, clips, policy, log_std, zfilter_stats, zclip=5.0, fail_safe=False, window=32, record_states=False):
+        """device evaluation of up to E clips (uhc_eval_run, include/uhc_eval.h): envs 0..n-1 roll out clips[i] from frame 0 with the mean
+        action under the current cfg.  policy: nn.mlp_struct / nn.mcp_struct of the policy; zfilter_stats: the ZFilter's device statistics.
+        Returns dict(frames=[n][max(len)-1][6] per-frame rows (rows past `nframes` unspecified), nframes, last_t, fail_any, reward_sum,
+        states=[n][max(len)-1][148] recorded qpos + xpos when record_states, else None)."""
+        t = self.torch
+        clips = np.ascontiguousarray(clips, dtype=np.int32).reshape(-1)
+        n = len(clips)
+        ok = 0 < n <= self.E and self.clip_len is not None and ((clips >= 0) & (clips < len(self.clip_len))).all()
+        T = int(self.clip_len[clips].max()) - 1 if ok else 1
+        frames = t.empty((max(n, 1), T, 6), dtype=t.float64, pin_memory=True)
+        states = t.empty((max(n, 1), T, 148), dtype=t.float64, pin_memory=True) if record_states else None
+        rec = (UhcEvalClip * max(n, 1))()
+        from .nn import UhcMcp
+        fn = self.lib.uhc_eval_run_mcp if isinstance(policy, UhcMcp) else self.lib.uhc_eval_run
+        rc = fn(self.h, C.c_int(n), _ip(clips), C.byref(policy), C.c_void_p(log_std.data_ptr()), C.c_void_p(zfilter_stats.data_ptr()), C.c_float(zclip),
+                C.c_int(int(bool(fail_safe))), C.c_int(int(window)), C.c_void_p(frames.data_ptr()), rec,
+                C.c_void_p(states.data_ptr() if states is not None else None), self._stream())
+        if rc != 0:
+            self.lib.uhc_eval_last_error.restype = C.c_char_p
+            raise (ValueError if rc == -2 else RuntimeError)("uhc_eval_run: " + self.lib.uhc_eval_last_error().decode())
+        return dict(frames=frames.numpy()[:n], nframes=np.array([r.frames for r in rec][:n]), last_t=np.array([r.last_t for r in rec][:n]),
+                    fail_any=np.array([bool(r.fail_any) for r in rec][:n]), reward_sum=np.array([r.reward_sum for r in rec][:n]),
+                    states=states.numpy()[:n] if states is not None else None)
 
     def set_clip_weights(self, weights=None):
         """sampling weights of the in-kernel re-seeding (None = the reference's sample_keys rule)."""

@@ -64,3 +64,12 @@ def compute_metrics(res):
     out["accel_dist"], out["vel_dist"] = acc * 1000.0, vel * 1000.0
     out["succ"] = np.array([(not res["fail_safe"]) and res["percent"] == 1])
     return out
+
+
+def metrics_from_frames(frames, percent, fail_safe):
+    """compute_metrics' dict from the per-frame rows [T][6] the device evaluation writes (uhc_b200/csrc/eval_core.h; T >= 3):
+    mpjpe_g, mpjpe, pa_mpjpe, vel (valid from frame 1), accel (from frame 2), |I - X_pred X_gt^-1|_F, which root_dist_mm divides by T."""
+    f = np.asarray(frames, dtype=np.float64)
+    T = len(f)
+    return {"root_dist": f[:, 5] / T * 1000.0, "vel_dist": f[1:, 3].copy(), "accel_dist": f[2:, 4].copy(), "mpjpe_g": f[:, 0].copy(),
+            "pa_mpjpe": f[:, 2].copy(), "mpjpe": f[:, 1].copy(), "succ": np.array([(not fail_safe) and percent == 1])}
