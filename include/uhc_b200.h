@@ -121,6 +121,8 @@ int uhc_set_neutral_pose(UhcEngine *e, const double *qpos76, const double *qvel7
  * sampling_freq the clip is drawn from exp(-ewma(success)/temp), else uniformly (dataset_amass_single.py:183-186, math_utils.py:25-29);
  * the caller folds both into one weight per clip: w = sampling_freq * p_fail + (1 - sampling_freq) / C. */
 int uhc_set_clip_weights(UhcEngine *e, int nclips, const float *weights_host);
+/* the sampler's cumulative clip weights as they are now: out_host [C] (synchronises the device) */
+int uhc_get_clip_cdf(UhcEngine *e, float *out_host);
 
 /* env.reset() for n envs (mujoco_env.py:95-104 + humanoid_im.py:1245-1299).  clip/start/len select the expert slice
  * (dataset_amass_single.py:200-253); q/v override (may be NULL) = [n][76]/[n][75] floats on the device.
@@ -150,7 +152,8 @@ int uhc_env_set_state_batch(UhcEngine *e, int n, const int *env_ids_host, const 
  * set), out4[1] = env-steps skipped because the env record was stale (clip table reloaded) or never reset (outputs: fail = end = 1). */
 int uhc_engine_counters(UhcEngine *e, int *out4);
 /* device array [E][2] written by every uhc_env_step: clip index of the episode that ended in that step (-1 = none) and its completed
- * fraction `percent` as float bits -- what the reference appends to its per-clip success history (agent_copycat.py:561). */
+ * fraction `percent` as float bits -- what the reference appends to its per-clip success history (agent_copycat.py:561); followed by [E]
+ * start frames of those episodes, written while the device curriculum is enabled (-1 before it ever was). */
 const int *uhc_episode_log_dev(const UhcEngine *e);
 int uhc_num_envs(const UhcEngine *e);
 int uhc_engine_obs_dim(const UhcEngine *e);      /* env.obs_dim (humanoid_im.py:256-258) */

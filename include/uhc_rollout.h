@@ -45,7 +45,29 @@ typedef struct {
     int *ep_clip;         /* optional [T_cap][E]: clip index of the episode that ended at this step (-1: none) ... */
     float *ep_pct;        /* ... and its completed fraction: the per-clip success history of agent_copycat.py:561 */
     int T_cap, reserved;
+    int *ep_start;        /* optional [T_cap][E] (with ep_clip): the start frame of that episode (fr_start of agent_copycat.py:561), recorded while
+                           * the device curriculum is enabled (its step-kernel variant logs it), -1 before it ever was */
 } UhcRolloutBuf;
+
+/* The failure-weighted curriculum on the device (the training loop's freq_dict, agent_copycat.py:561,590-603 + dataset_amass_single.py:172-232).
+ * uhc_curriculum_enable allocates a ring of the last max_freq (percent, start) outcomes per clip, empty, and from then on owns the
+ * sampler's clip CDF: uhc_set_clip_weights returns -2 while it is enabled.  Called again with the same max_freq it keeps the history and
+ * only changes the parameters; max_freq = 0 disables it (the CDF returns to the sample_keys rule).  temp / freq = sampling_temp /
+ * sampling_freq of the clip mixture; prec_freq = probability of a precision-mode start (0 = off; the reference's precision_mode passes
+ * sampling_freq, or 0.75 with fit_single_key); fit_clip = -1, or the clip every re-seed uses.  A clip-table load with another clip count
+ * disables the curriculum.  Bad arguments return -2 and leave the engine as it was. */
+int uhc_curriculum_enable(UhcEngine *e, int max_freq, double temp, double freq, double prec_freq, int fit_clip);
+/* After a rollout, on `stream`, without a host synchronise: appends the ended episodes of rows 0 .. T-1 of buf (ep_clip, ep_pct, ep_start
+ * all required), step-major then env-minor, keeps each clip's last max_freq, and rewrites the clip CDF in place from the new weights
+ * (the sample_keys rule while every history is empty). */
+int uhc_curriculum_update(UhcEngine *e, const UhcRolloutBuf *buf, int T, void *stream);
+/* host-side history: append n outcomes in order (eval results); read / replace every clip's history, oldest first:
+ * len_host [C], pct_host / start_host [C][max_freq] (entries past len[c] are ignored / zero).  Each updates the CDF. */
+int uhc_curriculum_push(UhcEngine *e, int n, const int *clip_host, const float *pct_host, const int *start_host);
+int uhc_curriculum_get(UhcEngine *e, int *len_host, float *pct_host, int *start_host);
+int uhc_curriculum_set(UhcEngine *e, const int *len_host, const float *pct_host, const int *start_host);
+/* re-seeds every env through the in-kernel sampler (a fit_clip change takes effect at once); obs_dev [E][obs_dim] gets the reset rows */
+int uhc_curriculum_reseed(UhcEngine *e, float *obs_dev, void *stream);
 
 const char *uhc_rollout_last_error(void);
 

@@ -321,6 +321,59 @@ def gen_sampler(cfg):
     np.savez_compressed(os.path.join(OUT, "sampler_hist.npz"), **out)
 
 
+def gen_precision(cfg):
+    """precision_mode draws (dataset_amass_single.py:172-253) on take5_test_small with a synthetic freq_dict of [percent, fr_start]
+    entries: clips without failures, failures near a clip's start or its end, eval-style [False, 0] entries and one empty history.
+    Records the clip histogram and the per-clip start histograms of sample_seq(precision_mode=True, temp 0.2, freq 0.5) and of
+    get_sample_from_key(key, precision_mode=True) (its default sampling_freq 0.75) for two keys."""
+    import random
+    from uhc.data_loaders.dataset_amass_single import DatasetAMASSSingle
+    t_min, t_max = 15, 60
+    cfg.data_specs["t_min"], cfg.data_specs["t_max"] = t_min, t_max
+    dl = DatasetAMASSSingle(cfg.data_specs, data_mode="train")
+    keys = list(dl.data_keys)
+    C = len(keys)
+    lens = np.array([dl.data["pose_aa"][k].shape[0] for k in keys])
+    rs = np.random.RandomState(21)
+    freq = {}
+    for c, k in enumerate(keys):
+        L, kind = int(lens[c]), c % 5
+        n = 1 + rs.randint(0, 50)
+        if kind == 0:                      # no failure
+            freq[k] = [[1.0, int(rs.randint(0, L - t_min))] for _ in range(n)]
+        elif kind == 1:                    # failures near the start
+            freq[k] = [[1.0, int(rs.randint(0, L - t_min))] if rs.uniform() < 0.5 else [float(rs.uniform(0, 0.99)), int(rs.randint(0, 8))] for _ in range(n)]
+        elif kind == 2:                    # failures near the end of the start range
+            freq[k] = [[1.0, 0] if rs.uniform() < 0.3 else [float(rs.uniform(0, 0.99)), int(L - t_min - 1 - rs.randint(0, 6))] for _ in range(n)]
+        elif kind == 3:                    # eval-style outcomes mixed with training ones
+            freq[k] = [[False, 0] if rs.uniform() < 0.5 else [float(rs.uniform(0, 1.0)), int(rs.randint(0, L - t_min))] for _ in range(n)]
+        else:
+            freq[k] = [] if c == C - 1 else [[float(rs.uniform() < 0.7), int(rs.randint(0, L - t_min))] for _ in range(n)]
+    out = dict(lens=lens, t_min=t_min, t_max=t_max, nent=np.array([len(freq[k]) for k in keys]))
+    pct, st = np.zeros((C, 50), np.float32), np.zeros((C, 50), np.int32)
+    for c, k in enumerate(keys):
+        for j, r in enumerate(freq[k]):
+            pct[c, j], st[c, j] = float(r[0]), int(r[1])
+    out["pct"], out["start"] = pct, st
+    n = 40000
+    np.random.seed(5); random.seed(5)
+    clip, start = np.zeros(n, np.int64), np.zeros(n, np.int64)
+    for i in range(n):
+        dl.sample_seq(freq_dict=freq, full_sample=False, sampling_temp=0.2, sampling_freq=0.5, precision_mode=True)
+        clip[i], start[i] = keys.index(dl.curr_key), dl.fr_start
+    out["seq.n"] = n
+    out["seq.clip_hist"] = np.bincount(clip, minlength=C)
+    out["seq.start_hist"] = np.stack([np.bincount(start[clip == c], minlength=int(lens.max())) for c in range(C)])
+    for fk in (1, 2):
+        for i in range(n):
+            dl.get_sample_from_key(keys[fk], freq_dict=freq, precision_mode=True)
+            start[i] = dl.fr_start
+        out[f"key{fk}.start_hist"] = np.bincount(start, minlength=int(lens.max()))
+    out["fit_keys"] = np.array([1, 2])
+    print("precision", out["seq.clip_hist"], out["nent"])
+    np.savez_compressed(os.path.join(OUT, "precision_hist.npz"), **out)
+
+
 def gen_metrics():
     """smpl_eval.compute_metrics / p_mpjpe (uhc/smpllib/smpl_eval.py:24-123) on seeded inputs."""
     from uhc.smpllib.smpl_eval import compute_metrics
@@ -492,6 +545,8 @@ def main():
         gen_metrics()
     if "sampler" in what:
         gen_sampler(H.make_cfg())
+    if "gen_precision" in what or "precision" in what:
+        gen_precision(H.make_cfg())
     if "yaml_keys" in what:
         gen_yaml_keys()
     if "zfilter" in what:

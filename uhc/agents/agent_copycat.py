@@ -118,9 +118,74 @@ class AgentCopycat:
         self.logger = logging.getLogger(f"uhc_b200.{cfg.id}")
         if not self.logger.handlers:
             logging.basicConfig(level=logging.INFO, format="%(message)s")
+        # the failure-weighted curriculum (freq_dict): on the host (default) or, with curriculum_on_device, in device rings updated after
+        # every rollout (Engine.curriculum_*).  precision_mode and fit_single_key need the device curriculum and turn it on
+        self._precision_mode = bool(cfg.get("precision_mode", False))
+        self._fit_single_key = ""
+        self.curriculum_on_device = bool(cfg.get("curriculum_on_device", False)) or self._precision_mode
+        if self.curriculum_on_device:
+            self._enable_device_curriculum()
         if checkpoint_epoch > 0:
             self.load_checkpoint(checkpoint_epoch)
             self.epoch = checkpoint_epoch
+
+    # ---------------------------------------------------------------- device curriculum (agent_copycat.py:503-517, dataset_amass_single.py:172-232)
+    @property
+    def precision_mode(self):
+        return self._precision_mode
+
+    @precision_mode.setter
+    def precision_mode(self, on):      # assignable as scripts/fit_uhc.py does
+        self._precision_mode = bool(on)
+        if self._precision_mode and not self.curriculum_on_device:
+            self.curriculum_on_device = True
+        if self.curriculum_on_device:
+            self._enable_device_curriculum()
+
+    @property
+    def fit_single_key(self):
+        return self._fit_single_key
+
+    @fit_single_key.setter
+    def fit_single_key(self, key):
+        self._fit_single_key = key or ""
+        if self._fit_single_key and not self.curriculum_on_device:
+            self.curriculum_on_device = True
+        if self.curriculum_on_device:
+            self._enable_device_curriculum()
+
+    def _curriculum_params(self):
+        """the sampler's parameters: sample_seq passes sampling_freq to both of its draws; with fit_single_key get_sample_from_key runs
+        with its default sampling_freq 0.75 (agent_copycat.py:504-510)"""
+        cfg, fit = self.cfg, self._fit_single_key
+        freq = float(cfg.get("sampling_freq", 0.5))
+        prec = (0.75 if fit else freq) if self._precision_mode else 0.0
+        return dict(max_freq=self.max_freq, temp=float(cfg.get("sampling_temp", 0.2)), freq=freq, prec_freq=prec,
+                    fit_clip=self.data_loader.data_keys.index(fit) if fit else -1)
+
+    def _enable_device_curriculum(self):
+        fresh = self.agent.engine.cur_cfg is None
+        self.agent.curriculum_enable(**self._curriculum_params())
+        if fresh:
+            self._freq_dict_to_device(self.freq_dict)
+
+    def _freq_dict_to_device(self, fd):
+        keys, M = self.data_loader.data_keys, self.max_freq
+        ln, p, st = np.zeros(len(keys), np.int32), np.zeros((len(keys), M), np.float32), np.zeros((len(keys), M), np.int32)
+        for c, k in enumerate(keys):
+            h = list(fd.get(k, []))[-M:]
+            ln[c] = len(h)
+            for j, r in enumerate(h):
+                p[c, j], st[c, j] = float(r[0]), int(r[1])
+        self.agent.curriculum_set(ln, p, st)
+
+    def _freq_dict_from_device(self):
+        ln, p, st = self.agent.curriculum_get()
+        return {k: [[float(p[c, j]), int(st[c, j])] for j in range(ln[c])] for c, k in enumerate(self.data_loader.data_keys)}
+
+    def get_freq_dict(self):
+        """{key: [[percent, start], ...]} -- the host history, or the device rings read back"""
+        return self._freq_dict_from_device() if self.curriculum_on_device else self.freq_dict
 
     # ---------------------------------------------------------------- schedules (:279-297)
     def per_epoch_update(self, epoch):
@@ -138,7 +203,8 @@ class AgentCopycat:
     def sample(self, min_batch_size=None):
         T = self.horizon if min_batch_size is None else max(2, int(math.ceil(min_batch_size / self.num_envs)))
         buf, log = self.agent.sample(T)
-        self._update_freq_dict(buf)
+        if not self.curriculum_on_device:           # the device curriculum was updated inside agent.sample
+            self._update_freq_dict(buf)
         log = _Log(log)
         log.update(avg_c_reward=log["avg_reward"], avg_episode_c_reward=log["avg_episode_reward"])
         return _Batch(buf), log
@@ -208,10 +274,12 @@ class AgentCopycat:
         res_dicts = []
         eng = self.agent.engine
         E = self.num_envs
+        pending = []        # device curriculum: this loader's eval outcomes (clip, outcome), pushed in one call once the training tables are back
         for loader in self.test_data_loaders:
             n = loader.get_len()
             device_tables = self._device_tables(loader)
             if loader is not self.data_loader:
+                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
                 self._load_tables(loader)      # invalidates every env record: only the envs reset below are stepped
             eng.set_cfg(**self._env_cfg(test=True))
             res = {}
@@ -224,7 +292,7 @@ class AgentCopycat:
                     last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
                     rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
                     self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec,
-                                       lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs))
+                                       lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs), pending)
                     continue
                 if len(ids) < E:                                   # idle envs: park them on clip c0 so every record is valid (their outputs are ignored)
                     eng.reset(np.arange(len(ids), E, dtype=np.int32), np.full(E - len(ids), c0, np.int32), 0, None)
@@ -271,9 +339,14 @@ class AgentCopycat:
                     tt = np.minimum(np.array(traj[i]["t"], dtype=np.int64), ex["len"] - 1)
                     return compute_metrics({"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
                                             "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": pct, "fail_safe": fs})
-                self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics)
+                self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics, pending)
             if loader is not self.data_loader:
                 self._load_tables(self.data_loader)
+                if saved is not None:          # a table of another clip count disabled the device curriculum: restore it
+                    self._restore_device_curriculum(saved)
+            if pending:                        # after the restore, so the outcomes of an overlapping test set stay, as on the host path
+                self.agent.curriculum_push([c for c, _ in pending], [o for _, o in pending], [0] * len(pending))
+                pending = []
             eng.set_cfg(**self._env_cfg(test=False))
             self.agent.obs = None
             names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
@@ -286,24 +359,70 @@ class AgentCopycat:
             if dump:
                 path = osp.join(cfg.output_dir, f"{epoch}_{loader.name}_coverage_full.pkl")
                 joblib.dump(res, path)
-        self._push_clip_weights()
+        if not self.curriculum_on_device:
+            self._push_clip_weights()
         return res_dicts
 
-    def _eval_results(self, res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec, metrics_of):
-        """res[key] of every clip of one evaluation chunk, from either roll-out: the percent / succ rules of eval_seq, the reward
-        average, and the eval outcome fed to the failure-weighted sampler.  metrics_of(i, percent, fail_safe) -> compute_metrics' dict."""
-        cfg = self.cfg
+    def _restore_device_curriculum(self, fd):
+        if self.agent.engine.cur_cfg is None:
+            self.agent.curriculum_enable(**self._curriculum_params())
+        self._freq_dict_to_device(fd)
+
+    def eval_seq(self, take_key, loader):
+        """eval_seq (agent_copycat.py:435-493) for one clip on the device evaluation (BatchedAgent.evaluate with the state record):
+        gt / pred (qpos), gt_jpos / pred_jpos (world joint positions), reward, percent, fail_safe and compute_metrics' keys with succ --
+        the values eval_policy(eval_on_device=True) computes for that clip.  The training tables and cfg are restored afterwards."""
+        from uhc_b200.metrics import metrics_from_frames
+        cfg, eng = self.cfg, self.agent.engine
+        c = loader.data_keys.index(take_key)
+        saved = None
+        if loader is not self.data_loader:
+            saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+            self._load_tables(loader)
+        eng.set_cfg(**self._env_cfg(test=True))
+        d = self.agent.evaluate(np.array([c], np.int32), bool(cfg.fail_safe), window=32, record_states=True)[0]
+        L = int(eng.clip_len[c])
+        gt = eng.clip_frames(c) if self._device_tables(loader) else loader.experts[c]
+        tt = np.minimum(np.arange(1, len(d["frames"]) + 1), L - 1)
+        out = self._clip_result(L, d["last_t"], d["fail_any"], d["reward_sum"], len(d["frames"]), lambda pct, fs: metrics_from_frames(d["frames"], pct, fs))
+        st = d["states"]
+        out.update(gt=np.asarray(gt["qpos"])[tt], pred=st[:, :76].copy(), gt_jpos=np.asarray(gt["wbpos"])[tt].reshape(len(tt), -1),
+                   pred_jpos=st[:, 76:148].copy(), fail_safe=bool(d["fail_any"] and cfg.fail_safe))
+        out["percent"] = float(d["last_t"]) / float(max(L - 1, 1))
+        if loader is not self.data_loader:
+            self._load_tables(self.data_loader)
+            if saved is not None:
+                self._restore_device_curriculum(saved)
+        eng.set_cfg(**self._env_cfg(test=False))
+        self.agent.obs = None
+        return out
+
+    def _clip_result(self, L, last_t, fail_any, rsum, nrec, metrics_of):
+        """res[key] of one evaluated clip of L frames, from either roll-out: the percent / succ rules of eval_seq and the reward average.
+        metrics_of(percent, fail_safe) -> compute_metrics' dict."""
+        percent = float(last_t) / float(max(L - 1, 1))
+        pct = 1.0 if (percent >= 1.0 and not fail_any) else min(percent, 0.999)
+        m = metrics_of(pct, bool(fail_any and self.cfg.fail_safe)) if nrec >= 3 else {"succ": np.array([False])}
+        m["succ"] = np.array([bool(m["succ"][0]) and not fail_any])
+        m["reward"] = rsum / max(L - 1, 1)
+        m["percent"] = percent
+        return m
+
+    def _eval_results(self, res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec, metrics_of, pending):
+        """res[key] of every clip of one evaluation chunk (_clip_result), and the eval outcome fed to the failure-weighted sampler like a
+        training episode ([percent, 0]): appended to freq_dict on the host path, collected in `pending` for one push on the device path.
+        metrics_of(i, percent, fail_safe) -> compute_metrics' dict."""
+        index = {k: c for c, k in enumerate(self.data_loader.data_keys)}
         for i in ids:
             k = loader.data_keys[c0 + i]
-            percent = float(last_t[i]) / float(max(lens[i] - 1, 1))
-            pct = 1.0 if (percent >= 1.0 and not fail_any[i]) else min(percent, 0.999)
-            m = metrics_of(i, pct, bool(fail_any[i] and cfg.fail_safe)) if nrec[i] >= 3 else {"succ": np.array([False])}
-            m["succ"] = np.array([bool(m["succ"][0]) and not fail_any[i]])
-            m["reward"] = rsum[i] / max(lens[i] - 1, 1)
-            m["percent"] = percent
-            res[k] = m
-            if k in self.freq_dict:      # eval outcome feeds the failure-weighted sampler like a training episode ([percent, fr_start])
-                self.freq_dict[k] = (self.freq_dict[k] + [[1.0 if m["succ"][0] else min(percent, 0.999), 0]])[-self.max_freq:]
+            m = res[k] = self._clip_result(lens[i], last_t[i], fail_any[i], rsum[i], nrec[i], lambda pct, fs: metrics_of(i, pct, fs))
+            if k not in index:
+                continue
+            outcome = 1.0 if m["succ"][0] else min(m["percent"], 0.999)
+            if self.curriculum_on_device:
+                pending.append((index[k], outcome))
+            else:
+                self.freq_dict[k] = (self.freq_dict[k] + [[outcome, 0]])[-self.max_freq:]
 
     @staticmethod
     def _device_tables(loader):
@@ -345,8 +464,27 @@ class AgentCopycat:
         if int(os.environ.get("RANK", "0")) == 0:
             with open(path, "wb") as f:
                 pickle.dump(self.agent.state_dicts(), f)
-            joblib.dump(self.freq_dict, osp.join(cfg.result_dir, "freq_dict.pt"))
+            joblib.dump(self.get_freq_dict(), osp.join(cfg.result_dir, "freq_dict.pt"))
         return path
+
+    # ---------------------------------------------------------------- single-clip fitting (scripts/fit_uhc.py; agent_copycat.py:203-236)
+    def _write_cp(self, path):
+        with open(path, "wb") as f:
+            pickle.dump(self.agent.state_dicts(), f)
+
+    def save_singles(self, epoch, key):
+        """{model_dir}_singles/{key}.p: policy_dict / value_dict / running_state"""
+        self._write_cp(f"{self.cfg.model_dir}_singles/{key}.p")
+
+    def save_curr(self):
+        """{model_dir}/iter_best.p"""
+        self._write_cp(f"{self.cfg.model_dir}/iter_best.p")
+
+    def load_curr(self):
+        path = f"{self.cfg.model_dir}/iter_best.p"
+        self.logger.info("loading model from checkpoint: %s" % path)
+        with open(path, "rb") as f:
+            self.agent.load_state_dicts(pickle.load(f))
 
     def load_checkpoint(self, epoch):
         cfg = self.cfg
@@ -357,3 +495,5 @@ class AgentCopycat:
         fd = osp.join(cfg.result_dir, "freq_dict.pt")
         if osp.exists(fd):
             self.freq_dict = joblib.load(fd)
+            if self.curriculum_on_device:
+                self._freq_dict_to_device(self.freq_dict)

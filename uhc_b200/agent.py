@@ -22,7 +22,7 @@ from .motion_lib import MotionSet
 class UhcRolloutBuf(C.Structure):
     """include/uhc_rollout.h UhcRolloutBuf"""
     _fields_ = [(k, C.c_void_p) for k in ("states", "actions", "rewards", "masks", "exps", "logp", "fails", "obs_cur", "ep_clip", "ep_pct")] + \
-               [("T_cap", C.c_int), ("reserved", C.c_int)]
+               [("T_cap", C.c_int), ("reserved", C.c_int), ("ep_start", C.c_void_p)]
 
 
 def ewma(x, alpha=0.05):
@@ -82,10 +82,11 @@ class RolloutBuffer:
         self.fails = torch.zeros(T, E, device=device, dtype=torch.int32)
         self.ep_clip = torch.full((T, E), -1, device=device, dtype=torch.int32)      # clip of the episode that ended at (t, e), -1 = none
         self.ep_pct = torch.zeros(T, E, **f)                                         # its completed fraction (info["percent"])
+        self.ep_start = torch.zeros(T, E, device=device, dtype=torch.int32)          # and its start frame (fr_start)
 
     def c_struct(self, obs_cur):
         b = UhcRolloutBuf()
-        for k in ("states", "actions", "rewards", "masks", "exps", "logp", "fails", "ep_clip", "ep_pct"):
+        for k in ("states", "actions", "rewards", "masks", "exps", "logp", "fails", "ep_clip", "ep_pct", "ep_start"):
             setattr(b, k, getattr(self, k).data_ptr())
         b.obs_cur, b.T_cap = obs_cur.data_ptr(), self.T
         return b
@@ -208,18 +209,25 @@ class BatchedAgent:
         the loop runs behind the C ABI as one CUDA graph; otherwise the Python loop over step_once (identical kernels and results)."""
         t = self.torch
         if self.obs is None:
-            self.reset_envs()
+            if self.engine.cur_cfg is not None:               # the device curriculum's sampler (fit_clip / precision starts) seeds the first episodes too
+                self.obs = self.engine.curriculum_reseed()
+            else:
+                self.reset_envs()
         buf = buf or RolloutBuffer(T, self.E, self.dev, self.act_dim, self.obs_dim)
         t0 = time.time()
         len0, ret0 = self.ep_len.clone(), self.ep_ret.clone()
         if c_loop is None:
             c_loop = self.auto_reset and use_tc
+        if self.engine.cur_cfg is not None and not c_loop:
+            raise RuntimeError("the device curriculum is fed by the C-side rollout's episode log (c_loop): the Python step loop does not record it")
         if c_loop:
             self.rollout(buf, T)
         else:
             for k in range(T):
                 self.step_once(buf, k, use_tc)
         buf.last_obs.copy_(self.obs)
+        if self.engine.cur_cfg is not None and c_loop:
+            self.curriculum_update(buf, T)
         # episode statistics from the buffer (one sync at the end of the rollout): segment the [T][E] masks per env
         m, r = buf.masks[:T], buf.rewards[:T]
         done = m == 0
@@ -347,6 +355,36 @@ class BatchedAgent:
             ms, by, calls = self._ctrainer.comm_stats()
             out.update(allreduce_ms=ms, allreduce_bytes=by, allreduce_calls=calls)
         return out
+
+    # ---- the failure-weighted curriculum on the device (Engine.curriculum_*): updated after every C-side rollout
+    def curriculum_enable(self, max_freq=50, temp=0.2, freq=0.5, prec_freq=0.0, fit_clip=-1):
+        old = self.engine.cur_cfg
+        self.engine.curriculum_enable(max_freq, temp, freq, prec_freq, fit_clip)
+        if max_freq and (old is None or old["fit_clip"] != int(fit_clip)) and self.obs is not None:
+            self.obs = self.engine.curriculum_reseed()      # the new fit_clip applies to every env from the next rollout on
+
+    @property
+    def fit_clip(self):
+        return -1 if self.engine.cur_cfg is None else self.engine.cur_cfg["fit_clip"]
+
+    @fit_clip.setter
+    def fit_clip(self, clip):
+        """the clip every re-seed uses (-1: off); turns the device curriculum on (default parameters) if it is off"""
+        c = dict(self.engine.cur_cfg or dict(max_freq=50, temp=0.2, freq=0.5, prec_freq=0.0))
+        c["fit_clip"] = int(clip)
+        self.curriculum_enable(**c)
+
+    def curriculum_update(self, buf, T):
+        self.engine.curriculum_update(buf, T)
+
+    def curriculum_push(self, clips, pct, starts):
+        self.engine.curriculum_push(clips, pct, starts)
+
+    def curriculum_get(self):
+        return self.engine.curriculum_get()
+
+    def curriculum_set(self, lens, pct, starts):
+        self.engine.curriculum_set(lens, pct, starts)
 
     def evaluate(self, clips, fail_safe, window=32, record_states=False):
         """deterministic roll-out of every listed clip from frame 0 on the device (Engine.eval_run, one call per chunk of E clips) under

@@ -6,10 +6,10 @@ import tempfile
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "libuhc_b200.so")
 SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_wgmma.cu", "rollout.cu", "ppo_update.cu"]
-# compiled on their own without multiply-add contraction: the motion library and the evaluation metrics restate numpy's fp64
+# compiled on their own without multiply-add contraction: the motion library, the evaluation metrics and the curriculum weights restate numpy's fp64
 # arithmetic operation for operation
-NO_FMA_SRCS = ["motion_lib.cu", "eval.cu"]
-DEPS = ["sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h"]
+NO_FMA_SRCS = ["motion_lib.cu", "eval.cu", "curriculum.cu"]
+DEPS = ["sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "curriculum_core.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 

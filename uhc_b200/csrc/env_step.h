@@ -4,8 +4,19 @@
 // uhc/khrylib/rl/envs/common/mujoco_env.py:95-113 (reset / set_state).
 #pragma once
 #include "sim_core.h"
+#include "curriculum_core.h"
 
 namespace uhc {
+
+// the device curriculum as the sampler sees it (uhc_curriculum_enable): the per-clip outcome rings (null = off), fit_clip (-1 = off:
+// every re-seed uses that clip) and prec_freq (0 = off: the probability of a precision-mode start)
+struct CurView {
+    const float *pct;       // [C][max_freq]
+    const int *start;       // [C][max_freq]
+    const int *meta;        // [C][2] head, len (curriculum_core.h)
+    int max_freq, fit_clip;
+    float prec_freq;
+};
 
 // everything a warp needs to find its environment's data
 template <class Real>
@@ -23,7 +34,9 @@ struct EngineView {
     const Real *neutral;    // [76 + 75] standing_neutral qpos / qvel (sample_data/standing_neutral.pkl; humanoid_im.py:66,86), null = reactive starts off
     int *ep_log;            // [E][2] per env: clip index of the episode that ended in the last step (-1: none ended) and its completed fraction (float bits)
                             //   -- the training loop's per-clip success history (agent_copycat.py:561) is built from it
+    int *ep_start_log;      // [E] the start frame of that episode, written by the curriculum variant of the step kernel
     int *counters;          // [4] device counters: 0 = env-steps failed because a body's contacts did not fit MAXCON, 1 = env-steps skipped on an invalid env record
+    CurView cur;
 };
 
 // an env record the step kernel can run: a clip of the CURRENT clip table and at least two frames (uhc_load_clips invalidates every
@@ -63,7 +76,9 @@ UHC_DEV unsigned long long mix64(unsigned long long x) {
     x += 0x9E3779B97F4A7C15ull; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull; x = (x ^ (x >> 27)) * 0x94D049BB133111EBull; return x ^ (x >> 31);
 }
 // DatasetAMASSSingle.sample_seq / get_sample_from_key (dataset_amass_single.py:172-253): clip ~ sample_keys (uniform over
-// len // t_max + 1 copies per clip), start ~ U{0 .. len - t_min - 1}, slice length min(t_max, len - start)
+// len // t_max + 1 copies per clip), start ~ U{0 .. len - t_min - 1}, slice length min(t_max, len - start).  With the device curriculum:
+// fit_clip >= 0 replaces the clip draw (fit_single_key, agent_copycat.py:504-510) and prec_freq > 0 the start draw (precision_mode,
+// curriculum_core.h draw_start); their extra uniforms come from one more mix64 round, so with both off the draw is unchanged
 template <class Real>
 UHC_DEV void sample_clip(const EngineView<Real> &ev, int env, int episode, int *clip, int *start, int *len) {
     const unsigned long long h = mix64(ev.cfg.reset_seed ^ mix64((unsigned long long)env * 0x100000001B3ull + (unsigned long long)episode));
@@ -76,6 +91,36 @@ UHC_DEV void sample_clip(const EngineView<Real> &ev, int env, int episode, int *
     int st = (int)(u2 * (float)span); if (st > span - 1) st = span - 1;
     int ln = L - st; if (ev.cfg.t_max > 0 && ln > ev.cfg.t_max) ln = ev.cfg.t_max;
     *clip = lo; *start = st; *len = ln;
+}
+// the same draw under the device curriculum (the step kernel's curriculum variant): fit_clip >= 0 replaces the clip draw (fit_single_key,
+// agent_copycat.py:504-510), prec_freq > 0 the start draw (precision_mode, curriculum_core.h draw_start).  Same hash and u1 / u2; the extra
+// uniforms come from one more mix64 round, so with both off it is sample_clip's draw
+UHC_DEVNI void sample_clip_cur_draw(const CurView cur, const float *clip_cdf, const int *clip_adr, int num_clips, int t_min, int t_max,
+                                     unsigned long long seed, int env, int episode, int *clip, int *start, int *len) {
+    const unsigned long long h = mix64(seed ^ mix64((unsigned long long)env * 0x100000001B3ull + (unsigned long long)episode));
+    const float u1 = (float)(h >> 40) * (1.0f / 16777216.0f), u2 = (float)(h & 0xFFFFFF) * (1.0f / 16777216.0f);
+    int lo = 0, hi = num_clips - 1;
+    if (cur.fit_clip >= 0) lo = cur.fit_clip;
+    else {
+        const float target = u1 * UHC_LDG(clip_cdf + hi);
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (UHC_LDG(clip_cdf + mid) > target) hi = mid; else lo = mid + 1; }
+    }
+    const int L = UHC_LDG(clip_adr + lo + 1) - UHC_LDG(clip_adr + lo);
+    int st;
+    if (cur.prec_freq > 0.f) {
+        const unsigned long long h2 = mix64(h ^ 0xC3A5C85C97CB3127ull);
+        st = cur::draw_start(cur.pct, cur.start, cur.meta, cur.max_freq, lo, L, t_min, cur.prec_freq,
+                             (float)(h2 >> 40) * (1.0f / 16777216.0f), (float)(h2 & 0xFFFFFF) * (1.0f / 16777216.0f), u2);
+    } else {
+        int span = L - t_min; if (span < 1) span = 1;
+        st = (int)(u2 * (float)span); if (st > span - 1) st = span - 1;
+    }
+    int ln = L - st; if (t_max > 0 && ln > t_max) ln = t_max;
+    *clip = lo; *start = st; *len = ln;
+}
+template <class Real>
+UHC_DEV void sample_clip_cur(const EngineView<Real> &ev, int env, int episode, int *clip, int *start, int *len) {
+    sample_clip_cur_draw(ev.cur, ev.clip_cdf, ev.clip_adr, ev.cfg.num_clips, ev.cfg.t_min, ev.cfg.t_max, ev.cfg.reset_seed, env, episode, clip, start, len);
 }
 
 // model tables of the body shape a clip was recorded with
@@ -209,8 +254,9 @@ UHC_DEV void env_reset_warp(const EngineView<Real> &ev, int env, Work<Real> &w, 
     store_state(ev, env, w);
 }
 
-// one control step.  out_* may be null.  Returns done; fills flags.
-template <class Real, class ObsT>
+// one control step.  out_* may be null.  Returns done; fills flags.  CUR: the device curriculum's variant (start log, curriculum sampler); the
+// default variant is compiled without either, so the step kernel most runs is the same code with the curriculum off
+template <class Real, class ObsT, bool CUR = false>
 UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, const ObsT *action, ObsT *obs, ObsT *reward,
                           ObsT *cinfo_out, int *fail_out, int *end_out, ObsT *percent_out, ObsT *torque_out) {
     int *is = ev.istate + (size_t)env * SI_SIZE;
@@ -300,6 +346,7 @@ UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, co
 #else
             union { float f; int i; } cv; cv.f = pctf; ev.ep_log[2 * env + 1] = cv.i;
 #endif
+            if constexpr (CUR) ev.ep_start_log[env] = start;
         }
     }
     if (cinfo_out && lane < 5) cinfo_out[lane] = (ObsT)ci[lane];
@@ -308,7 +355,8 @@ UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, co
     if (ev.cfg.auto_reset && (fail || end)) {   // re-seed the finished episode in place: the next observation is the reset observation
         int nclip, nstart, nlen;
         const int episode = is[SI_EPISODE] + 1;
-        sample_clip(ev, env, episode, &nclip, &nstart, &nlen);
+        if constexpr (CUR) sample_clip_cur(ev, env, episode, &nclip, &nstart, &nlen);
+        else sample_clip(ev, env, episode, &nclip, &nstart, &nlen);
         env_reset_warp<Real, ObsT>(ev, env, w, nclip, nstart, nlen, (const Real *)nullptr, (const Real *)nullptr, obs);
         LANES_BEGIN
         if (lane == 0) is[SI_EPISODE] = episode;

@@ -21,6 +21,9 @@ void engine_refs(UhcEngine *e, EngineRefs *out);                                
 // fail_safe re-seat of every env i < n with reseat[i] != 0: uhc_env_set_state_batch's reset-with-override onto the expert qpos / qvel
 // of frame min(cur_t, len - 1), rounded to fp32, keeping cur_t and the body quaternions; one launch, no host work
 cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t st);       // step_kernel.cu
+// changes whenever the sampler's curriculum view (rings, fit_clip, prec_freq, CDF pointer under the curriculum) changes; the rollout's
+// graphs are keyed on it                                                                                                   // step_kernel.cu
+unsigned long long curriculum_gen(const UhcEngine *e);
 // policy of an evaluation: validates it (-2) and sizes the rollout's scratch outside any capture; *gen changes whenever that scratch
 // is reallocated (graphs holding the old pointers must be dropped)
 int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, unsigned long long *gen, std::string *err);   // rollout.cu

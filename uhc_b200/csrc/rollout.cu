@@ -89,7 +89,7 @@ __global__ void k_gauss_sample_dev(const float *__restrict__ mean, const float *
 // mask = 0 on fail or clip end (agent_copycat.py:550), fail row, exps = 1 when every action is sampled; advances the step counter
 __global__ void k_rollout_post(const int *__restrict__ fail, const int *__restrict__ end, float *__restrict__ mask_row, int *__restrict__ fail_row,
                                float *__restrict__ exps_row_or_null, int E, unsigned long long *__restrict__ step_ptr, const int *__restrict__ ep_log,
-                               int *__restrict__ ep_clip_row, float *__restrict__ ep_pct_row) {
+                               int *__restrict__ ep_clip_row, float *__restrict__ ep_pct_row, int *__restrict__ ep_start_row) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e < E) {
         const int f = fail[e], d = f | end[e];
@@ -97,6 +97,7 @@ __global__ void k_rollout_post(const int *__restrict__ fail, const int *__restri
         if (fail_row) fail_row[e] = f;
         if (exps_row_or_null) exps_row_or_null[e] = 1.f;
         if (ep_clip_row) { ep_clip_row[e] = ep_log[2 * e]; ep_pct_row[e] = __int_as_float(ep_log[2 * e + 1]); }
+        if (ep_start_row) ep_start_row[e] = ep_log[2 * E + e];
     }
     if (e == 0) *step_ptr += 1ull;   // ordered after every reader of this step's counter by the stream / graph dependencies
 }
@@ -105,6 +106,7 @@ __global__ void k_rollout_post(const int *__restrict__ fail, const int *__restri
 struct Policy { int nprim; int pad; UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; };
 struct GraphKey {
     int T, row0, update_filter; float noise_rate, zclip; unsigned long long seed; Policy pol; UhcRolloutBuf buf; const float *log_std; double *zstats;
+    unsigned long long cur_gen;   // the sampler's curriculum view (uhc_curriculum_enable) is captured by value: a new one needs a new graph
     bool operator==(const GraphKey &o) const { return memcmp(this, &o, sizeof(GraphKey)) == 0; }
 };
 struct RolloutCtx {
@@ -226,7 +228,8 @@ int enqueue_step(RolloutCtx *c, int row, const Policy *pol, const float *log_std
     n++;
     const bool eplog = b->ep_clip && b->ep_pct;
     k_rollout_post<<<(c->E + 255) / 256, 256, 0, st>>>(c->d_fail, c->d_end, mask_row, fail_row, mixed ? nullptr : exps_row, c->E, c->d_step, uhc_episode_log_dev(c->eng),
-                                                       eplog ? b->ep_clip + (size_t)row * E : nullptr, eplog ? b->ep_pct + (size_t)row * E : nullptr);
+                                                       eplog ? b->ep_clip + (size_t)row * E : nullptr, eplog ? b->ep_pct + (size_t)row * E : nullptr,
+                                                       eplog && b->ep_start ? b->ep_start + (size_t)row * E : nullptr);
     CKR(cudaGetLastError()); n++;
     return n;
 }
@@ -291,7 +294,7 @@ static int rollout_impl(UhcEngine *e, int T, int row0, const Policy *pol, const 
     }
     GraphKey key; memset(&key, 0, sizeof key);
     key.T = T; key.row0 = row0; key.update_filter = update_filter; key.noise_rate = noise_rate; key.zclip = zclip; key.seed = seed; key.pol = *pol; key.buf = *buf;
-    key.log_std = log_std; key.zstats = zfilter_stats;
+    key.log_std = log_std; key.zstats = zfilter_stats; key.cur_gen = uhc::evalx::curriculum_gen(e);
     cudaGraphExec_t exec = nullptr;
     for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
     if (!exec) {

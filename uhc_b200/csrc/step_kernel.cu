@@ -7,9 +7,11 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_b200.h"
+#include "../../include/uhc_rollout.h"
 #include "env_step.h"
 #include "motion_core.h"
 #include "eval_glue.h"
+#include "curriculum_core.h"
 
 using namespace uhc;
 
@@ -38,7 +40,7 @@ constexpr int SYNC_GROUP = 8;
 #else
 #define UHC_STEP_BOUNDS(EPB, Real) __launch_bounds__(32 * EPB, 1)
 #endif
-template <class Real, int EPB>
+template <class Real, int EPB, bool CUR = false>
 __global__ void UHC_STEP_BOUNDS(EPB, Real)
 k_env_step(EngineView<Real> ev, const float *__restrict__ act, float *__restrict__ obs, float *__restrict__ rew, float *__restrict__ cinfo,
            int *__restrict__ fail, int *__restrict__ end, float *__restrict__ pct, float *__restrict__ torque, const int *__restrict__ order) {
@@ -62,7 +64,7 @@ k_env_step(EngineView<Real> ev, const float *__restrict__ act, float *__restrict
     Work<Real> &w = reinterpret_cast<Work<Real> *>(smem)[warp];
     if ((threadIdx.x & 31) == 0) { w.sync_threads = 32 * s_nvalid[grp]; w.sync_id = 1 + grp; }
     state_mbar_init(w);            // mbarrier of this warp's bulk-async (TMA) state load
-    env_step_warp<Real, float>(ev, env, w, act + (size_t)env * ev.cfg.act_dim, obs ? obs + (size_t)env * ev.cfg.obs_dim : nullptr, rew ? rew + env : nullptr,
+    env_step_warp<Real, float, CUR>(ev, env, w, act + (size_t)env * ev.cfg.act_dim, obs ? obs + (size_t)env * ev.cfg.obs_dim : nullptr, rew ? rew + env : nullptr,
                                cinfo ? cinfo + (size_t)env * 5 : nullptr, fail ? fail + env : nullptr, end ? end + env : nullptr,
                                pct ? pct + env : nullptr, torque ? torque + (size_t)env * NSUB * NU : nullptr);
 }
@@ -127,6 +129,20 @@ k_eval_reseat(EngineView<Real> ev, int n, const int *__restrict__ reseat) {
     if (lane == 0) is[SI_CUR_T] = cur_t;
 }
 
+// uhc_curriculum_reseed: the re-seed draw of the step kernel for every env (one thread each); the resets follow as k_env_reset
+template <class Real>
+__global__ void k_cur_sample(EngineView<Real> ev, int *__restrict__ out) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= ev.num_envs) return;
+    int *is = ev.istate + (size_t)env * SI_SIZE;
+    const int episode = is[SI_EPISODE] + 1;
+    int c, st, ln;
+    sample_clip_cur(ev, env, episode, &c, &st, &ln);
+    is[SI_EPISODE] = episode;
+    const int E = ev.num_envs;
+    out[env] = env; out[E + env] = c; out[2 * E + env] = st; out[3 * E + env] = ln;
+}
+
 // parity / evaluation hook: gather q, v, xpos, bquat (+ the integer record) of the listed envs into one staging array
 template <class Real>
 __global__ void k_gather_state(const Real *__restrict__ state, const int *__restrict__ istate, const int *__restrict__ ids, int n, double *__restrict__ out, int *__restrict__ iout) {
@@ -172,6 +188,13 @@ struct UhcEngine {
     unsigned long long view_gen = 0;
     motion::MotionModel mo_model;  // FK tables of the device motion library (uhc_load_motions); mo_model.body = fp64 offsets / ipos on the device
     float mo_ms[2] = {0.f, 0.f};   // kernel / row-copy time of the last uhc_load_motions (CUDA events, ms)
+    // device curriculum (uhc_curriculum_*): off while cur.M == 0.  cur_gen changes with everything the sampler reads of it by value
+    cur::Dev cur = {};
+    float prec_freq = 0.f; int fit_clip = -1;
+    unsigned long long cur_gen = 0;
+    size_t cur_cnt_cap = 0, cur_rank_cap = 0;
+    int *d_reseed = nullptr;       // [4][E] ids / clip / start / len of uhc_curriculum_reseed
+    int *d_push = nullptr; int push_cap = 0;   // [3][n] clip / percent bits / start of uhc_curriculum_push
 };
 
 template <class T> static int dev_copy(UhcEngine *e, T **dst, const T *src, size_t n) {
@@ -228,8 +251,9 @@ template <class Real> static int build_view(UhcEngine *e, EngineView<Real> &ev, 
     CK(cudaMemset(is, 0, (size_t)e->E * SI_SIZE * sizeof(int)));
     int *cn; CK(cudaMalloc((void **)&cn, 4 * sizeof(int))); e->allocs.push_back(cn); CK(cudaMemset(cn, 0, 4 * sizeof(int)));
     ev.counters = cn; ev.neutral = nullptr;
-    int *el; CK(cudaMalloc((void **)&el, (size_t)e->E * 2 * sizeof(int))); e->allocs.push_back(el); CK(cudaMemset(el, 0xFF, (size_t)e->E * 2 * sizeof(int)));
-    ev.ep_log = el;
+    int *el; CK(cudaMalloc((void **)&el, (size_t)e->E * 3 * sizeof(int))); e->allocs.push_back(el); CK(cudaMemset(el, 0xFF, (size_t)e->E * 3 * sizeof(int)));
+    ev.ep_log = el; ev.ep_start_log = el + (size_t)2 * e->E;
+    ev.cur.pct = nullptr; ev.cur.start = nullptr; ev.cur.meta = nullptr; ev.cur.max_freq = 0; ev.cur.fit_clip = -1; ev.cur.prec_freq = 0.f;
     ev.state = st; ev.istate = is; ev.expert = nullptr; ev.clip_adr = nullptr; ev.clip_shape = nullptr; ev.clip_model = nullptr; ev.clip_cdf = nullptr;
     return 0;
 }
@@ -267,6 +291,7 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
     }
     if (precision == 32) {
         CK(cudaFuncSetAttribute(k_env_step<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
+        CK(cudaFuncSetAttribute(k_env_step<float, EPB_F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         CK(cudaFuncSetAttribute(k_env_reset<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         CK(cudaFuncSetAttribute(k_eval_reseat<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         int resident = 0;
@@ -274,6 +299,7 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
         if (resident < 1) { g_err = "uhc_engine_create: k_env_step<float> with " + std::to_string(EPB_F) + " envs per block does not fit one SM"; delete e; return -3; }
     } else {
         CK(cudaFuncSetAttribute(k_env_step<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
+        CK(cudaFuncSetAttribute(k_env_step<double, EPB_D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
         CK(cudaFuncSetAttribute(k_env_reset<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
         CK(cudaFuncSetAttribute(k_eval_reseat<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
     }
@@ -302,6 +328,7 @@ void uhc_engine_destroy(UhcEngine *e) {
     if (e->d_keep_t) cudaFree(e->d_keep_t);
     if (e->d_gather) cudaFree(e->d_gather);
     if (e->d_gather_i) cudaFree(e->d_gather_i);
+    for (void *p : {(void *)e->cur.pct, (void *)e->cur.start, (void *)e->cur.meta, (void *)e->cur.p, (void *)e->cur.cnt, (void *)e->cur.rank, (void *)e->cur.ncl, (void *)e->d_reseed, (void *)e->d_push}) if (p) cudaFree(p);
     delete e;
 }
 
@@ -322,6 +349,10 @@ static int upload_clip_cdf(UhcEngine *e) {
     return 0;
 }
 
+static int cur_weights(UhcEngine *e);
+static void cur_free(UhcEngine *e);
+static void cur_view(UhcEngine *e);
+
 int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
     if (!e || !cfg) { g_err = "uhc_engine_set_cfg: null"; return -2; }
     e->view_gen++;
@@ -330,7 +361,7 @@ int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
     const int old_obs_dim = uhc_engine_obs_dim(e);
     if (e->precision == 32) { fill_cfg(e->evf.cfg, cfg); e->evf.cfg.num_clips = e->num_clips; } else { fill_cfg(e->evd.cfg, cfg); e->evd.cfg.num_clips = e->num_clips; }
     if (uhc_engine_obs_dim(e) != old_obs_dim) { g_err = "uhc_engine_set_cfg: the observation width cannot change on a live engine (buffers are sized at creation)"; return -2; }
-    if (cfg->t_max != old_tmax && e->clip_w.empty()) { CK(cudaDeviceSynchronize()); return upload_clip_cdf(e); }   // the sample_keys weights depend on t_max
+    if (cfg->t_max != old_tmax && e->clip_w.empty()) { CK(cudaDeviceSynchronize()); return e->cur.M ? cur_weights(e) : upload_clip_cdf(e); }   // the sample_keys weights depend on t_max
     return 0;
 }
 
@@ -338,6 +369,7 @@ int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
 // clip models back to variant 0, every env record invalidated, shapes uploaded; d_expert is allocated (uninitialised) for the caller
 static int new_clip_table(UhcEngine *e, int nclips, const int *clip_len, const double *shape_host) {
     e->view_gen++;
+    if (e->cur.M && nclips != e->num_clips) cur_free(e);   // the histories belong to the old clips
     std::vector<int> adr(nclips + 1, 0);
     for (int i = 0; i < nclips; i++) adr[i + 1] = adr[i] + clip_len[i];
     const size_t nf = (size_t)adr[nclips] * EX_SIZE, ns = (size_t)nclips * 17;
@@ -347,6 +379,10 @@ static int new_clip_table(UhcEngine *e, int nclips, const int *clip_len, const d
     e->num_clips = nclips; e->clip_len_h.assign(clip_len, clip_len + nclips); e->clip_adr_h = adr; e->clip_w.clear();
     e->evf.cfg.num_clips = nclips; e->evd.cfg.num_clips = nclips;
     if (upload_clip_cdf(e)) return -1;
+    if (e->cur.M) {                                          // same clip count: the curriculum keeps its history and rewrites the new CDF
+        if (cur_weights(e)) return -1;
+        cur_view(e);                                         // the CDF moved: the rollout's graphs must capture the new one
+    }
     if (e->d_clip_model) { cudaFree(e->d_clip_model); e->d_clip_model = nullptr; }
     e->evf.clip_model = nullptr; e->evd.clip_model = nullptr;
     // every env record points into the OLD clip table: invalidate them all (len = 0); the step kernel skips (and flags) an env
@@ -497,6 +533,7 @@ int uhc_set_neutral_pose(UhcEngine *e, const double *qpos76, const double *qvel7
 
 int uhc_set_clip_weights(UhcEngine *e, int nclips, const float *weights_host) {
     if (!e || nclips != e->num_clips) { g_err = "uhc_set_clip_weights: call after uhc_load_clips with one weight per clip"; return -2; }
+    if (e->cur.M) { g_err = "uhc_set_clip_weights: the device curriculum owns the clip weights (uhc_curriculum_enable with max_freq 0 turns it off)"; return -2; }
     e->view_gen++;
     CK(cudaSetDevice(e->device));
     if (!weights_host) e->clip_w.clear();
@@ -564,10 +601,11 @@ int uhc_env_step(UhcEngine *e, const float *actions_dev, float *obs_dev, float *
     CK(cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (e->d_order) { k_order_envs<<<1, 1024, 0, st>>>(e->precision == 32 ? e->evf.istate : e->evd.istate, e->E, e->d_order); e->launches++; }
+    const bool cur = e->cur.M > 0;     // the curriculum variant: start log and curriculum sampler
     if (e->precision == 32)
-        k_env_step<float, EPB_F><<<(e->E + EPB_F - 1) / EPB_F, 32 * EPB_F, step_smem<float, EPB_F>(), st>>>(e->evf, actions_dev, obs_dev, reward_dev, cinfo_dev, fail_dev, end_dev, percent_dev, torque_dev, e->d_order);
+        (cur ? k_env_step<float, EPB_F, true> : k_env_step<float, EPB_F>)<<<(e->E + EPB_F - 1) / EPB_F, 32 * EPB_F, step_smem<float, EPB_F>(), st>>>(e->evf, actions_dev, obs_dev, reward_dev, cinfo_dev, fail_dev, end_dev, percent_dev, torque_dev, e->d_order);
     else
-        k_env_step<double, EPB_D><<<(e->E + EPB_D - 1) / EPB_D, 32 * EPB_D, step_smem<double, EPB_D>(), st>>>(e->evd, actions_dev, obs_dev, reward_dev, cinfo_dev, fail_dev, end_dev, percent_dev, torque_dev, e->d_order);
+        (cur ? k_env_step<double, EPB_D, true> : k_env_step<double, EPB_D>)<<<(e->E + EPB_D - 1) / EPB_D, 32 * EPB_D, step_smem<double, EPB_D>(), st>>>(e->evd, actions_dev, obs_dev, reward_dev, cinfo_dev, fail_dev, end_dev, percent_dev, torque_dev, e->d_order);
     CK(cudaGetLastError());
     e->launches++;
     return 0;
@@ -683,6 +721,191 @@ int uhc_engine_obs_dim(const UhcEngine *e) { return e ? (e->precision == 32 ? e-
 int uhc_engine_act_dim(const UhcEngine *e) { return e ? (e->precision == 32 ? e->evf.cfg.act_dim : e->evd.cfg.act_dim) : -1; }
 int uhc_kernel_launches(const UhcEngine *e) { return e ? e->launches : -1; }
 
+// ---- device curriculum (include/uhc_rollout.h; kernels in curriculum.cu)
+static void cur_view(UhcEngine *e) {   // what the sampler reads: rings, fit_clip, prec_freq
+    CurView v;
+    v.pct = e->cur.pct; v.start = e->cur.start; v.meta = e->cur.meta; v.max_freq = e->cur.M;
+    v.fit_clip = e->cur.M ? e->fit_clip : -1; v.prec_freq = e->cur.M ? e->prec_freq : 0.f;
+    e->evf.cur = v; e->evd.cur = v;
+    e->view_gen++; e->cur_gen++;
+}
+static void cur_free(UhcEngine *e) {
+    cudaDeviceSynchronize();
+    for (void *p : {(void *)e->cur.pct, (void *)e->cur.start, (void *)e->cur.meta, (void *)e->cur.p, (void *)e->cur.cnt, (void *)e->cur.rank, (void *)e->cur.ncl}) if (p) cudaFree(p);
+    if (e->d_push) cudaFree(e->d_push);
+    e->d_push = nullptr; e->push_cap = 0;
+    e->cur = cur::Dev{}; e->cur_cnt_cap = e->cur_rank_cap = 0; e->fit_clip = -1; e->prec_freq = 0.f;
+    // the start log is written by the curriculum's step kernel only: back to "never recorded", as on an engine that never enabled it
+    int *sl = e->precision == 32 ? e->evf.ep_start_log : e->evd.ep_start_log;
+    cudaMemset(sl, 0xFF, (size_t)e->E * sizeof(int));
+    cur_view(e);
+}
+static void cur_bind(UhcEngine *e) {   // the parts of the device state that follow the clip table and the cfg
+    e->cur.C = e->num_clips; e->cur.cdf = e->d_clip_cdf; e->cur.clip_adr = e->d_clip_adr;
+    e->cur.t_max = e->precision == 32 ? e->evf.cfg.t_max : e->evd.cfg.t_max;
+}
+static int cur_weights(UhcEngine *e) {  // CDF from the rings as they are, rewritten in place; synchronous (host-side calls only)
+    cur_bind(e);
+    CK(cur::launch_weights(e->cur, 0));
+    CK(cudaDeviceSynchronize());
+    return 0;
+}
+static int cur_scratch(UhcEngine *e, size_t N) {   // the update's count table and rank array for an N-entry log
+    const size_t ncnt = (N + cur::UPD_CHUNK - 1) / cur::UPD_CHUNK * (size_t)e->num_clips;
+    if (e->cur_cnt_cap < ncnt) { if (e->cur.cnt) cudaFree(e->cur.cnt); e->cur.cnt = nullptr; CK(cudaMalloc((void **)&e->cur.cnt, ncnt * sizeof(int))); e->cur_cnt_cap = ncnt; }
+    if (e->cur_rank_cap < N) { if (e->cur.rank) cudaFree(e->cur.rank); e->cur.rank = nullptr; CK(cudaMalloc((void **)&e->cur.rank, N * sizeof(int))); e->cur_rank_cap = N; }
+    return 0;
+}
+static bool cur_check(UhcEngine *e, const char *who) {
+    if (!e) { g_err = std::string(who) + ": null engine"; return false; }
+    if (!e->cur.M) { g_err = std::string(who) + ": the device curriculum is not enabled"; return false; }
+    return true;
+}
+
+int uhc_curriculum_enable(UhcEngine *e, int max_freq, double temp, double freq, double prec_freq, int fit_clip) {
+    if (!e || max_freq < 0 || max_freq > cur::MAX_FREQ_CAP) { g_err = "uhc_curriculum_enable: max_freq must be 0 .. 4096"; return -2; }
+    CK(cudaSetDevice(e->device));
+    if (max_freq == 0) {
+        if (e->cur.M) { cur_free(e); CK(cudaDeviceSynchronize()); if (upload_clip_cdf(e)) return -1; }
+        return 0;
+    }
+    if (!e->d_expert || e->num_clips <= 0) { g_err = "uhc_curriculum_enable: no clips loaded"; return -2; }
+    if (!(temp > 0.0) || !(temp < 1e300)) { g_err = "uhc_curriculum_enable: temp must be a positive number"; return -2; }
+    if (!(freq >= 0.0 && freq <= 1.0) || !(prec_freq >= 0.0 && prec_freq <= 1.0)) { g_err = "uhc_curriculum_enable: freq and prec_freq must lie in [0, 1]"; return -2; }
+    if (fit_clip < -1 || fit_clip >= e->num_clips) { g_err = "uhc_curriculum_enable: fit_clip must be -1 or a clip index"; return -2; }
+    if (e->cur.M != max_freq) {
+        if (e->cur.M) cur_free(e);
+        const size_t C = e->num_clips, n = C * max_freq;
+        CK(cudaMalloc((void **)&e->cur.pct, n * sizeof(float))); CK(cudaMalloc((void **)&e->cur.start, n * sizeof(int)));
+        CK(cudaMalloc((void **)&e->cur.meta, 2 * C * sizeof(int))); CK(cudaMalloc((void **)&e->cur.p, C * sizeof(double)));
+        CK(cudaMalloc((void **)&e->cur.ncl, C * sizeof(int)));
+        CK(cudaMemset(e->cur.pct, 0, n * sizeof(float))); CK(cudaMemset(e->cur.start, 0, n * sizeof(int))); CK(cudaMemset(e->cur.meta, 0, 2 * C * sizeof(int)));
+        e->cur.M = max_freq;
+    }
+    e->cur.temp = temp; e->cur.freq = freq; e->prec_freq = (float)prec_freq; e->fit_clip = fit_clip;
+    e->clip_w.clear();
+    CK(cudaDeviceSynchronize());
+    if (cur_weights(e)) return -1;
+    cur_view(e);                         // new rings / fit_clip / prec_freq: the rollout's graphs capture them
+    return 0;
+}
+
+int uhc_get_clip_cdf(UhcEngine *e, float *out_host) {
+    if (!e || !out_host || !e->d_clip_cdf) { g_err = "uhc_get_clip_cdf: bad argument or no clips loaded"; return -2; }
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(out_host, e->d_clip_cdf, e->num_clips * sizeof(float), cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int uhc_curriculum_update(UhcEngine *e, const UhcRolloutBuf *buf, int T, void *stream) {
+    if (!cur_check(e, "uhc_curriculum_update")) return -2;
+    if (!buf || !buf->ep_clip || !buf->ep_pct || !buf->ep_start || T <= 0 || T > buf->T_cap) { g_err = "uhc_curriculum_update: needs ep_clip, ep_pct and ep_start rows and 0 < T <= T_cap"; return -2; }
+    CK(cudaSetDevice(e->device));
+    const size_t N = (size_t)T * e->E;
+    if (N > 0x7fffffffu) { g_err = "uhc_curriculum_update: log too long"; return -2; }
+    if (cur_scratch(e, N)) return -1;
+    cur_bind(e);
+    CK(cur::launch_update(e->cur, buf->ep_clip, buf->ep_pct, buf->ep_start, (int)N, (cudaStream_t)stream));
+    e->launches += 4;
+    return 0;
+}
+
+static int cur_to_host(UhcEngine *e, std::vector<int> &meta, std::vector<float> &pct, std::vector<int> &st) {
+    const size_t C = e->num_clips, n = C * e->cur.M;
+    meta.resize(2 * C); pct.resize(n); st.resize(n);
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(meta.data(), e->cur.meta, 2 * C * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(pct.data(), e->cur.pct, n * sizeof(float), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(st.data(), e->cur.start, n * sizeof(int), cudaMemcpyDeviceToHost));
+    return 0;
+}
+static int cur_from_host(UhcEngine *e, const std::vector<int> &meta, const std::vector<float> &pct, const std::vector<int> &st) {
+    CK(cudaMemcpy(e->cur.meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(e->cur.pct, pct.data(), pct.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(e->cur.start, st.data(), st.size() * sizeof(int), cudaMemcpyHostToDevice));
+    return cur_weights(e);
+}
+
+int uhc_curriculum_push(UhcEngine *e, int n, const int *clip, const float *pct, const int *start) {
+    if (!cur_check(e, "uhc_curriculum_push")) return -2;
+    if (n < 0 || (n > 0 && (!clip || !pct || !start))) { g_err = "uhc_curriculum_push: bad argument"; return -2; }
+    for (int i = 0; i < n; i++) if (clip[i] < 0 || clip[i] >= e->num_clips || start[i] < 0 || !(pct[i] == pct[i])) { g_err = "uhc_curriculum_push: clip out of range, negative start or NaN percent"; return -2; }
+    if (n == 0) return 0;
+    CK(cudaSetDevice(e->device));
+    // the n outcomes are a log of their own: the update's kernels append them in order and rewrite the CDF (one copy, one synchronise)
+    if (e->push_cap < n) {
+        if (e->d_push) cudaFree(e->d_push);
+        e->d_push = nullptr; e->push_cap = 0;
+        CK(cudaMalloc((void **)&e->d_push, (size_t)3 * n * sizeof(int))); e->push_cap = n;
+    }
+    std::vector<int> h((size_t)3 * n);
+    memcpy(h.data(), clip, n * sizeof(int)); memcpy(h.data() + n, pct, n * sizeof(float)); memcpy(h.data() + 2 * (size_t)n, start, n * sizeof(int));
+    if (cur_scratch(e, n)) return -1;
+    CK(cudaMemcpy(e->d_push, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice));
+    cur_bind(e);
+    CK(cur::launch_update(e->cur, e->d_push, (const float *)(e->d_push + n), e->d_push + 2 * (size_t)n, n, 0));
+    CK(cudaStreamSynchronize(0));
+    e->launches += 4;
+    return 0;
+}
+
+int uhc_curriculum_get(UhcEngine *e, int *len_host, float *pct_host, int *start_host) {
+    if (!cur_check(e, "uhc_curriculum_get")) return -2;
+    if (!len_host || !pct_host || !start_host) { g_err = "uhc_curriculum_get: bad argument"; return -2; }
+    CK(cudaSetDevice(e->device));
+    std::vector<int> meta, st; std::vector<float> pc;
+    if (cur_to_host(e, meta, pc, st)) return -1;
+    const int M = e->cur.M;
+    for (int c = 0; c < e->num_clips; c++) {
+        len_host[c] = meta[2 * c + 1];
+        for (int k = 0; k < M; k++) {
+            const bool v = k < meta[2 * c + 1];
+            const int s = cur::ring_slot(meta.data(), M, c, k);
+            pct_host[(size_t)c * M + k] = v ? pc[(size_t)c * M + s] : 0.f; start_host[(size_t)c * M + k] = v ? st[(size_t)c * M + s] : 0;
+        }
+    }
+    return 0;
+}
+
+int uhc_curriculum_set(UhcEngine *e, const int *len_host, const float *pct_host, const int *start_host) {
+    if (!cur_check(e, "uhc_curriculum_set")) return -2;
+    if (!len_host || !pct_host || !start_host) { g_err = "uhc_curriculum_set: bad argument"; return -2; }
+    const int M = e->cur.M, C = e->num_clips;
+    std::vector<int> meta(2 * (size_t)C), st((size_t)C * M, 0); std::vector<float> pc((size_t)C * M, 0.f);
+    for (int c = 0; c < C; c++) {
+        if (len_host[c] < 0 || len_host[c] > M) { g_err = "uhc_curriculum_set: history length outside 0 .. max_freq"; return -2; }
+        for (int k = 0; k < len_host[c]; k++) {
+            const float p = pct_host[(size_t)c * M + k]; const int s = start_host[(size_t)c * M + k];
+            if (s < 0 || !(p == p)) { g_err = "uhc_curriculum_set: negative start or NaN percent"; return -2; }
+            pc[(size_t)c * M + k] = p; st[(size_t)c * M + k] = s;
+        }
+        meta[2 * c] = len_host[c] % M; meta[2 * c + 1] = len_host[c];
+    }
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());
+    return cur_from_host(e, meta, pc, st);
+}
+
+int uhc_curriculum_reseed(UhcEngine *e, float *obs_dev, void *stream) {
+    if (!e) { g_err = "uhc_curriculum_reseed: null engine"; return -2; }
+    if (!e->d_expert) { g_err = "uhc_curriculum_reseed: no clips loaded"; return -3; }
+    CK(cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!e->d_reseed) CK(cudaMalloc((void **)&e->d_reseed, (size_t)4 * e->E * sizeof(int)));
+    const int E = e->E, *r = e->d_reseed;
+    if (e->precision == 32) {
+        k_cur_sample<float><<<(E + 127) / 128, 128, 0, st>>>(e->evf, e->d_reseed);
+        k_env_reset<float, EPB_F><<<(E + EPB_F - 1) / EPB_F, 32 * EPB_F, step_smem<float, EPB_F>(), st>>>(e->evf, E, r, r + E, r + 2 * E, r + 3 * E, nullptr, nullptr, obs_dev);
+    } else {
+        k_cur_sample<double><<<(E + 127) / 128, 128, 0, st>>>(e->evd, e->d_reseed);
+        k_env_reset<double, EPB_D><<<(E + EPB_D - 1) / EPB_D, 32 * EPB_D, step_smem<double, EPB_D>(), st>>>(e->evd, E, r, r + E, r + 2 * E, r + 3 * E, nullptr, nullptr, obs_dev);
+    }
+    CK(cudaGetLastError());
+    e->launches += 2;
+    return 0;
+}
+
 }  // extern "C"
 
 // ---- the device evaluation's view of the engine (eval_glue.h)
@@ -696,6 +919,8 @@ void engine_refs(UhcEngine *e, EngineRefs *r) {
     r->expert = e->d_expert; r->clip_adr = e->d_clip_adr; r->clip_len_h = e->clip_len_h.data(); r->view_gen = e->view_gen;
     r->obs = e->d_obs; r->act = e->d_act; r->rew = e->d_rew; r->cinfo = e->d_cinfo; r->pct = e->d_pct; r->fail = e->d_fail; r->end = e->d_end;
 }
+
+unsigned long long curriculum_gen(const UhcEngine *e) { return e->cur_gen; }
 
 cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t st) {
     if (e->precision == 32) k_eval_reseat<float, EPB_F><<<(n + EPB_F - 1) / EPB_F, 32 * EPB_F, step_smem<float, EPB_F>(), st>>>(e->evf, n, reseat);

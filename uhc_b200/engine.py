@@ -121,6 +121,11 @@ def _ip(a):
     return np.ascontiguousarray(a, dtype=np.int32).ctypes.data_as(C.POINTER(C.c_int))
 
 
+def _ip_out(a):
+    assert a.dtype == np.int32 and a.flags.c_contiguous
+    return a.ctypes.data_as(C.POINTER(C.c_int))
+
+
 class Engine:
     """E environments on one GPU.  Mirrors HumanoidEnv.reset/step (+ the agent's custom_reward) for all envs at once."""
 
@@ -151,6 +156,7 @@ class Engine:
         self.fail = torch.zeros(self.E, device=dev, dtype=torch.int32)
         self.end = torch.zeros(self.E, device=dev, dtype=torch.int32)
         self.clip_len = None
+        self.cur_cfg = None            # device curriculum parameters while it is enabled (curriculum_enable)
         if int(cfg.get("reactive_v", 0)) == 1:
             self.set_neutral_pose()
 
@@ -191,7 +197,7 @@ class Engine:
         shp = np.ascontiguousarray(shp)
         _chk(self.lib.uhc_load_clips(self.h, C.c_int(len(experts)), _ip(lens), frames.ctypes.data_as(C.POINTER(C.c_double)),
                                      shp.ctypes.data_as(C.POINTER(C.c_double))))
-        self.clip_len = lens
+        self._table_loaded(lens)
         if clip_models is not None:
             _chk(self.lib.uhc_set_clip_models(self.h, C.c_int(len(experts)), _ip(clip_models)))
 
@@ -209,9 +215,14 @@ class Engine:
         _chk(self.lib.uhc_load_motions(self.h, C.c_int(n), _ip(lens), C.c_int(motions.kind), C.c_int(motions.pose_dim),
                                        rows.ctypes.data_as(C.POINTER(C.c_double)), shp.ctypes.data_as(C.POINTER(C.c_double)),
                                        None if fk is None else _ip(fk), C.c_int(int(chunk_frames))))
-        self.clip_len = lens.copy()
+        self._table_loaded(lens.copy())
         if clip_models is not None:
             _chk(self.lib.uhc_set_clip_models(self.h, C.c_int(n), _ip(clip_models)))
+
+    def _table_loaded(self, lens):
+        if self.cur_cfg is not None and (self.clip_len is None or len(lens) != len(self.clip_len)):
+            self.cur_cfg = None        # the engine disabled the curriculum: its histories belonged to the old clips
+        self.clip_len = lens
 
     @property
     def load_motions_time(self):
@@ -331,6 +342,58 @@ class Engine:
         else:
             w = np.ascontiguousarray(weights, dtype=np.float32)
             _chk(self.lib.uhc_set_clip_weights(self.h, C.c_int(len(w)), w.ctypes.data_as(C.POINTER(C.c_float))))
+
+    # ---- the failure-weighted curriculum on the device (include/uhc_rollout.h uhc_curriculum_*)
+    def _cur_chk(self, rc, who):
+        if rc != 0:
+            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_last_error().decode())
+
+    def curriculum_enable(self, max_freq=50, temp=0.2, freq=0.5, prec_freq=0.0, fit_clip=-1):
+        """per-clip outcome rings of max_freq entries on the device; from here on the curriculum owns the clip CDF.  Called again with the
+        same max_freq it keeps the history; max_freq = 0 turns it off."""
+        self._cur_chk(self.lib.uhc_curriculum_enable(self.h, C.c_int(int(max_freq)), C.c_double(float(temp)), C.c_double(float(freq)),
+                                                     C.c_double(float(prec_freq)), C.c_int(int(fit_clip))), "uhc_curriculum_enable")
+        self.cur_cfg = dict(max_freq=int(max_freq), temp=float(temp), freq=float(freq), prec_freq=float(prec_freq), fit_clip=int(fit_clip)) if max_freq else None
+
+    def curriculum_update(self, buf, T):
+        """append the episodes that ended in rows 0 .. T-1 of a RolloutBuffer and rewrite the clip CDF, stream-ordered, no synchronise"""
+        from .agent import UhcRolloutBuf
+        b = UhcRolloutBuf()
+        b.ep_clip, b.ep_pct, b.ep_start, b.T_cap = buf.ep_clip.data_ptr(), buf.ep_pct.data_ptr(), buf.ep_start.data_ptr(), buf.T
+        self._cur_chk(self.lib.uhc_curriculum_update(self.h, C.byref(b), C.c_int(int(T)), self._stream()), "uhc_curriculum_update")
+
+    def curriculum_push(self, clips, pct, starts):
+        clips = np.ascontiguousarray(clips, np.int32).reshape(-1)
+        p = np.ascontiguousarray(pct, np.float32).reshape(-1)
+        s = np.ascontiguousarray(starts, np.int32).reshape(-1)
+        assert len(clips) == len(p) == len(s)
+        self._cur_chk(self.lib.uhc_curriculum_push(self.h, C.c_int(len(clips)), _ip(clips), p.ctypes.data_as(C.POINTER(C.c_float)), _ip(s)),
+                      "uhc_curriculum_push")
+
+    def curriculum_get(self):
+        """every clip's history, oldest first: (len [C], percent [C][max_freq], start [C][max_freq])"""
+        n, M = len(self.clip_len), self.cur_cfg["max_freq"]
+        ln, p, s = np.zeros(n, np.int32), np.zeros((n, M), np.float32), np.zeros((n, M), np.int32)
+        self._cur_chk(self.lib.uhc_curriculum_get(self.h, _ip_out(ln), p.ctypes.data_as(C.POINTER(C.c_float)), _ip_out(s)), "uhc_curriculum_get")
+        return ln, p, s
+
+    def curriculum_set(self, lens, pct, starts):
+        n, M = len(self.clip_len), self.cur_cfg["max_freq"]
+        ln = np.ascontiguousarray(lens, np.int32).reshape(n)
+        p = np.ascontiguousarray(pct, np.float32).reshape(n, M)
+        s = np.ascontiguousarray(starts, np.int32).reshape(n, M)
+        self._cur_chk(self.lib.uhc_curriculum_set(self.h, _ip(ln), p.ctypes.data_as(C.POINTER(C.c_float)), _ip(s)), "uhc_curriculum_set")
+
+    def clip_cdf(self):
+        """the sampler's cumulative clip weights [C] (fp32)"""
+        out = np.zeros(len(self.clip_len), np.float32)
+        _chk(self.lib.uhc_get_clip_cdf(self.h, out.ctypes.data_as(C.POINTER(C.c_float))))
+        return out
+
+    def curriculum_reseed(self):
+        """re-seed every env through the in-kernel sampler; returns the obs tensor with the reset rows"""
+        self._cur_chk(self.lib.uhc_curriculum_reseed(self.h, C.c_void_p(self.obs.data_ptr()), self._stream()), "uhc_curriculum_reseed")
+        return self.obs
 
     @property
     def counters(self):
