@@ -83,7 +83,8 @@ int uhc_normalize_advantages(float *adv, long n, double *scratch2, void *stream)
 int uhc_adv_moments(const float *adv, long n, double *out2, void *stream);
 int uhc_adv_normalize(float *adv, long n, const double *mom2_dev, const double *ntotal_dev, void *stream);
 
-/* ZFilter (khrylib/utils/zfilter.py:7-73): stats = [n, mean[D], S[D]] doubles; update!=0 merges the batch first. y may be NULL. */
+/* ZFilter (khrylib/utils/zfilter.py:7-73): stats = [n, mean[D], S[D]] doubles; update!=0 merges the batch first (an empty batch, M = 0,
+ * leaves the statistics as they are). y may be NULL. */
 int uhc_zfilter(const float *x, float *y, int M, int D, double *stats, float clip, int update, void *stream);
 /* the same with a caller-owned workspace of uhc_zfilter_workspace_doubles(D) doubles (needed inside a CUDA-graph capture: no allocation) */
 int uhc_zfilter_ws(const float *x, float *y, int M, int D, double *stats, float clip, int update, double *workspace, void *stream);

@@ -124,13 +124,15 @@ __global__ void k_colsum(const float *__restrict__ X, float *__restrict__ out, i
     if (threadIdx.y == 0 && j < N) { float t = 0.f; for (int k = 0; k < 32; k++) t += red[k][threadIdx.x]; out[j] = t; }
 }
 
-// counter-based RNG (philox-style mixing is overkill here: splitmix64 per (seed, stream, index) + Box-Muller)
+// counter-based RNG (philox-style mixing is overkill here: splitmix64 per (seed, stream, index) + Box-Muller).
+// u1 = (k + 1) * fp32(1 / (2^24 + 2)), k < 2^24, lies in (0, 1): the scale is spelled as its exact fp32 value, the one the earlier
+// literal 1.0f / 16777217.0f compiled to, so the stream of normals is unchanged and a host restatement can reproduce it bit for bit.
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
     x += 0x9E3779B97F4A7C15ull; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull; x = (x ^ (x >> 27)) * 0x94D049BB133111EBull; return x ^ (x >> 31);
 }
 __device__ __forceinline__ float gauss_from(uint64_t seed, uint64_t idx) {
     const uint64_t h = splitmix64(seed ^ splitmix64(idx));
-    const float u1 = ((uint32_t)(h >> 40) + 1.0f) * (1.0f / 16777217.0f), u2 = (uint32_t)(h & 0xFFFFFF) * (1.0f / 16777216.0f);
+    const float u1 = ((uint32_t)(h >> 40) + 1.0f) * 0x1.fffffcp-25f, u2 = (uint32_t)(h & 0xFFFFFF) * (1.0f / 16777216.0f);
     return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
 }
 // a = mean + exp(log_std) * eps (or mean when mean_action[i] != 0); logp = sum_d Normal(mean, std).log_prob(a)
@@ -254,32 +256,44 @@ __global__ void k_normalize(float *__restrict__ x, size_t n, const double *__res
 // UPDATED statistics (the reference pushes then normalises each sample; sequential-vs-batched order is the documented deviation).
 // stats layout: [0] = n (as double), then mean[D], S[D] (doubles).  One block per 32 dims (column reduction).
 constexpr int ZF_CHUNKS = 16;   // row chunks of the batch-moment pass (deterministic two-stage reduction: partials, then a fixed-order merge)
-// stage 1: block (column tile, row chunk) -> partial (sum, sum of squares) of its rows for 32 columns, into ws[chunk][D][2]
+// A column that holds one value in every row of the batch (the shape vector while every env holds one subject) is detected exactly: stage 1 also
+// counts the rows that differ from the batch's first row.  Such a column takes that value as its batch mean and 0 as its spread; from raw sums,
+// S2 - n mean^2 leaves a rounding residue of either sign there, and a negative S normalised the column to NaN -> -clip.  Every other column keeps
+// the raw-sum arithmetic, clamped at 0, so the statistics of a batch without such a residue are unchanged to the last bit.
+// stage 1: block (column tile, row chunk) -> partial (sum, sum of squares, rows != first row) of its rows for 32 columns, into ws[chunk][D][3]
 __global__ void k_zfilter_partial(const float *__restrict__ X, int M, int D, double *__restrict__ ws) {
     __shared__ double rs[32][33], rq[32][33];
+    __shared__ int rd[32][33];
     const int j = blockIdx.x * 32 + threadIdx.x, ch = blockIdx.y;
     const int r0 = (int)(((long)M * ch) / ZF_CHUNKS), r1 = (int)(((long)M * (ch + 1)) / ZF_CHUNKS);
     double s = 0.0, q = 0.0;
-    if (j < D) for (int i = r0 + threadIdx.y; i < r1; i += blockDim.y) { const double v = X[(size_t)i * D + j]; s += v; q += v * v; }
-    rs[threadIdx.y][threadIdx.x] = s; rq[threadIdx.y][threadIdx.x] = q;
+    int nd = 0;
+    if (j < D) {
+        const float c = X[j];
+        for (int i = r0 + threadIdx.y; i < r1; i += blockDim.y) { const float x = X[(size_t)i * D + j]; const double v = x; s += v; q += v * v; nd += x != c; }
+    }
+    rs[threadIdx.y][threadIdx.x] = s; rq[threadIdx.y][threadIdx.x] = q; rd[threadIdx.y][threadIdx.x] = nd;
     __syncthreads();
     if (threadIdx.y == 0 && j < D) {
         double S1 = 0.0, S2 = 0.0;
-        for (int k = 0; k < 32; k++) { S1 += rs[k][threadIdx.x]; S2 += rq[k][threadIdx.x]; }
-        ws[((size_t)ch * D + j) * 2] = S1; ws[((size_t)ch * D + j) * 2 + 1] = S2;
+        int N = 0;
+        for (int k = 0; k < 32; k++) { S1 += rs[k][threadIdx.x]; S2 += rq[k][threadIdx.x]; N += rd[k][threadIdx.x]; }
+        double *w = ws + ((size_t)ch * D + j) * 3;
+        w[0] = S1; w[1] = S2; w[2] = (double)N;
     }
 }
-// stage 2: fixed-order sum of the chunk partials, Chan merge into the running (n, mean, S); thread D bumps the count last
-__global__ void k_zfilter_merge(int M, int D, double *__restrict__ stats, const double *__restrict__ ws) {
+// stage 2: fixed-order sum of the chunk partials, Chan merge into the running (n, mean, S); k_zfilter_count bumps the count after it
+__global__ void k_zfilter_merge(const float *__restrict__ X, int M, int D, double *__restrict__ stats, const double *__restrict__ ws) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= D) return;
-    double S1 = 0.0, S2 = 0.0;
-    for (int ch = 0; ch < ZF_CHUNKS; ch++) { S1 += ws[((size_t)ch * D + j) * 2]; S2 += ws[((size_t)ch * D + j) * 2 + 1]; }
-    const double nb = (double)M, mb = S1 / nb, Sb = S2 - nb * mb * mb;
+    double S1 = 0.0, S2 = 0.0, nd = 0.0;
+    for (int ch = 0; ch < ZF_CHUNKS; ch++) { const double *w = ws + ((size_t)ch * D + j) * 3; S1 += w[0]; S2 += w[1]; nd += w[2]; }
+    const bool constant = nd == 0.0;
+    const double nb = (double)M, mb = constant ? (double)X[j] : S1 / nb, Sb = constant ? 0.0 : fmax(0.0, S2 - nb * mb * mb);
     const double na = stats[0], ma = stats[1 + j], Sa = stats[1 + D + j];
     const double n = na + nb, dlt = mb - ma;
-    stats[1 + j] = ma + dlt * nb / n;
-    stats[1 + D + j] = Sa + Sb + dlt * dlt * na * nb / n;
+    stats[1 + j] = ma + dlt * nb / n;              // from empty statistics: c nb is exact (c fp32, nb < 2^29), so a constant column's mean is c
+    stats[1 + D + j] = fmax(0.0, Sa + Sb + dlt * dlt * na * nb / n);
 }
 __global__ void k_zfilter_count(double *stats, int M) { stats[0] += (double)M; }
 __global__ void k_zfilter_apply(const float *__restrict__ X, float *__restrict__ Y, int M, int D, const double *__restrict__ stats, float clip) {
@@ -412,7 +426,7 @@ int uhc_mcp_backward(const float *xall, const float *weight, const float *dmean,
     if (P < 1 || P > MCP_MAX_PRIM) { g_nn_err = "uhc_mcp_backward: 1..16 primitives"; return -2; }
     k_mcp_backward<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(xall, weight, dmean, dxall, dc, M, A, P); CKN(cudaGetLastError()); return 0;
 }
-int uhc_zfilter_workspace_doubles(int D) { return ZF_CHUNKS * D * 2; }
+int uhc_zfilter_workspace_doubles(int D) { return ZF_CHUNKS * D * 3; }
 int uhc_zfilter(const float *x, float *y, int M, int D, double *stats, float clip, int update, void *stream) {
     // without a caller workspace: one per (thread, D), allocated on first use (not legal inside a stream capture -- the rollout passes its own)
     static thread_local double *ws = nullptr; static thread_local int ws_d = 0, ws_dev = -1;
@@ -422,10 +436,11 @@ int uhc_zfilter(const float *x, float *y, int M, int D, double *stats, float cli
 }
 int uhc_zfilter_ws(const float *x, float *y, int M, int D, double *stats, float clip, int update, double *workspace, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (update) {
+    if (M < 0 || D <= 0) { g_nn_err = "uhc_zfilter_ws: M >= 0 and D > 0"; return -2; }
+    if (update && M > 0) {     // an empty batch leaves the statistics as they are
         if (!workspace) { g_nn_err = "uhc_zfilter_ws: workspace is null"; return -2; }
         k_zfilter_partial<<<dim3((D + 31) / 32, ZF_CHUNKS), dim3(32, 32), 0, st>>>(x, M, D, workspace); CKN(cudaGetLastError());
-        k_zfilter_merge<<<(D + 127) / 128, 128, 0, st>>>(M, D, stats, workspace); CKN(cudaGetLastError());
+        k_zfilter_merge<<<(D + 127) / 128, 128, 0, st>>>(x, M, D, stats, workspace); CKN(cudaGetLastError());
         k_zfilter_count<<<1, 1, 0, st>>>(stats, M); CKN(cudaGetLastError());
     }
     if (y) { k_zfilter_apply<<<592, 256, 0, st>>>(x, y, M, D, stats, clip); CKN(cudaGetLastError()); }

@@ -34,7 +34,7 @@ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
 }
 __device__ __forceinline__ float gauss_from(uint64_t seed, uint64_t idx) {   // identical to nn_kernels.cu (same stream of normals as uhc_gaussian_sample)
     const uint64_t h = splitmix64(seed ^ splitmix64(idx));
-    const float u1 = ((uint32_t)(h >> 40) + 1.0f) * (1.0f / 16777217.0f), u2 = (uint32_t)(h & 0xFFFFFF) * (1.0f / 16777216.0f);
+    const float u1 = ((uint32_t)(h >> 40) + 1.0f) * 0x1.fffffcp-25f, u2 = (uint32_t)(h & 0xFFFFFF) * (1.0f / 16777216.0f);
     return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
 }
 // ZFilter apply fused with the bf16 K-padded copy the first GEMM reads: y = clip((x - mean) / (std + 1e-8)) (zfilter.py:59-73);
