@@ -1,0 +1,60 @@
+/* uhc_track.h -- C ABI of the batched physics tracker (part of libuhc_b200.so): the trained controller follows target poses that are
+ * streamed one frame per control step, for all envs at once.
+ *
+ * Reference interface replaced: HumanoidKinEnv.step (uhc/envs/humanoid_kin_v1.py:297-370) -- per step a kinematic model produces the next
+ * target qpos, qpos_fk turns it into the target frame, the cc policy's mean action on the cc obs against that frame drives do_simulation.
+ * Here the caller streams the raw target frames (device memory), the engine turns each into an expert-table record on the device
+ * (the records of uhc_load_motions, bit for bit) and one CUDA-graph replay per call runs observation, policy, physics and fail_safe.
+ *
+ * Tracking mode owns the engine's clip table: env e follows clip e, a window of H rows.  A later uhc_load_clips / uhc_load_motions ends
+ * it (uhc_track_step then returns -2).  Pointers suffixed _dev are CUDA device pointers, _host host pointers.  Returns 0 on success,
+ * -2 on a bad argument (the engine is left as it was), -1 on a CUDA error (uhc_track_last_error()).
+ */
+#ifndef UHC_TRACK_H
+#define UHC_TRACK_H
+#include "uhc_b200.h"
+#include "uhc_rollout.h"
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+/* per env columns of uhc_track_state */
+#define UHC_TRACK_STATE_COLS 4   /* control steps taken since the env's reset, cur_t in the window, rows held, pushes dropped (window full) */
+/* columns of state_out_dev: qpos 76, qvel 75, world body positions xpos 72, in the engine's precision */
+#define UHC_TRACK_OUT 223
+
+const char *uhc_track_last_error(void);
+
+/* Installs a table of E clips x `window` rows (env e owns clip e) through the table set-up of uhc_load_clips: every env record is
+ * invalidated, clip models = fk_model_host (NULL: variant 0; also the FK's shape variant), shape vectors = shape_host [E][17] (NULL: zero).
+ * kind / pose_dim: the raw-row formats of uhc_load_motions (UHC_MOTION_QPOS 76, UHC_MOTION_SMPL 72 | 156; row width pose_dim + 3).
+ * -2 for what a stream cannot serve: obs_v 3 (future frames), term_body root / Head (the whole episode window), auto_reset, reactive_v 1,
+ * window < 3, and a cfg whose `end` could fire inside the window (needs trail_steps >= 1 and env_episode_len >= window). */
+int uhc_track_begin(UhcEngine *e, int window, int kind, int pose_dim, const int *fk_model_host, const double *shape_host);
+/* Frames 0 and 1 of each listed env's stream (frames_dev = [n][2][row width] fp64) become rows 0 and 1, then the env is reset onto row 0
+ * exactly as uhc_env_reset does (qpos_dev / qvel_dev: optional fp32 overrides [n][76] / [n][75]).  Its step count returns to 0. */
+int uhc_track_reset(UhcEngine *e, int n, const int *env_ids_host, const double *frames_dev, const float *qpos_dev, const float *qvel_dev, void *stream);
+/* One control step of every env, in order: push frame t + 1 (next_frames_dev [E][row width] fp64, NULL = no push; mask_dev [E] int32,
+ * NULL = all, 0 = this env gets no frame), the observation of each env's state against row cur_t + 1, ZFilter (no update) + policy mean,
+ * k_env_step, fail_safe re-seat on row cur_t of the envs that failed.  state_out_dev [E][UHC_TRACK_OUT] = the state the step produced
+ * (before a re-seat), reward_dev [E] fp32, fail_dev [E] int32.  An env whose row cur_t + 1 was never pushed is not stepped: fail = 1,
+ * reward 0, counted in uhc_engine_counters' skipped steps.  The first call after a reset passes next_frames_dev = NULL (the reset pushed
+ * frame 1).  Replays one CUDA graph per argument set; no host synchronise. */
+int uhc_track_step(UhcEngine *e, const double *next_frames_dev, const int *mask_dev, const UhcMlp *mlp, const float *log_std,
+                   const double *zfilter_stats, float zclip, int fail_safe, void *state_out_dev, float *reward_dev, int *fail_dev, void *stream);
+int uhc_track_step_mcp(UhcEngine *e, const double *next_frames_dev, const int *mask_dev, const UhcMcp *mcp, const float *log_std,
+                       const double *zfilter_stats, float zclip, int fail_safe, void *state_out_dev, float *reward_dev, int *fail_dev, void *stream);
+/* the push of uhc_track_step on its own (frames known ahead of the steps); a push into a full window whose rows are all still needed is
+ * dropped and counted (uhc_track_state column 3) */
+int uhc_track_push(UhcEngine *e, const double *next_frames_dev, const int *mask_dev, void *stream);
+/* the observation uhc_track_step feeds the policy, without stepping: obs_dev [E][obs dim], zero rows for envs it would not step */
+int uhc_track_obs(UhcEngine *e, float *obs_dev, void *stream);
+/* out_host = [E][UHC_TRACK_STATE_COLS] (synchronises the device) */
+int uhc_track_state(UhcEngine *e, int *out_host);
+/* frees the stream buffers and graphs; the clip table stays loaded (its rows are whatever the windows held) */
+void uhc_track_end(UhcEngine *e);
+
+#ifdef __cplusplus
+}
+#endif
+#endif

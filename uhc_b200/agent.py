@@ -404,6 +404,12 @@ class BatchedAgent:
         self.obs = None       # every env was reset onto an evaluation clip
         return out
 
+    def tracker(self, window=8, kind="qpos", fail_safe=True, **kw):
+        """this agent's policy as a batched physics tracker of streamed target frames (uhc_b200/tracker.py); it takes over the engine's
+        clip table until the next load_clips / load_motions.  The cfg must be a test-mode one: auto_reset off, trail_steps >= 1."""
+        from .tracker import Tracker
+        return Tracker(self, window, kind, fail_safe, **kw)
+
     def optimize_policy(self, T):
         buf, log = self.sample(T)
         log.update(self.update_params(buf))

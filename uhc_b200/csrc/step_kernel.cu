@@ -12,6 +12,8 @@
 #include "motion_core.h"
 #include "eval_glue.h"
 #include "curriculum_core.h"
+#include "track_obs.h"
+#include "track_glue.h"
 
 using namespace uhc;
 
@@ -129,6 +131,20 @@ k_eval_reseat(EngineView<Real> ev, int n, const int *__restrict__ reseat) {
     if (lane == 0) is[SI_CUR_T] = cur_t;
 }
 
+// the tracker's observation pass (track.cu): one warp per env, the observation of its stored state against row cur_t + 1 through the step
+// kernel's write_obs (track_obs.h); an env the step kernel will skip (invalid record, or a missing row: track.cu gates it) gets a zero row
+constexpr int EPB_OBS = 2;
+template <class Real>
+__global__ void __launch_bounds__(32 * EPB_OBS) k_track_obs(EngineView<Real> ev, float *__restrict__ obs) {
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int warp = threadIdx.x >> 5, env = blockIdx.x * EPB_OBS + warp, lane = threadIdx.x & 31;
+    if (env >= ev.num_envs) return;
+    float *o = obs + (size_t)env * ev.cfg.obs_dim;
+    if (!env_record_valid(ev, env)) { for (int i = lane; i < ev.cfg.obs_dim; i += 32) o[i] = 0.f; return; }
+    Work<Real> &w = reinterpret_cast<Work<Real> *>(smem)[warp];
+    track_obs_warp<Real, float>(ev, env, w, o);
+}
+
 // uhc_curriculum_reseed: the re-seed draw of the step kernel for every env (one thread each); the resets follow as k_env_reset
 template <class Real>
 __global__ void k_cur_sample(EngineView<Real> ev, int *__restrict__ out) {
@@ -186,6 +202,7 @@ struct UhcEngine {
     // bumped whenever anything a launch captures by value changes: the EngineView (cfg, clip table / model / CDF / neutral pointers).
     // CUDA graphs of the device evaluation (eval.cu) are keyed on it, so a table load or set_cfg never replays stale parameters
     unsigned long long view_gen = 0;
+    unsigned long long table_gen = 0;   // bumped with every clip-table replacement: a tracker (track.cu) owns the table it installed only
     motion::MotionModel mo_model;  // FK tables of the device motion library (uhc_load_motions); mo_model.body = fp64 offsets / ipos on the device
     float mo_ms[2] = {0.f, 0.f};   // kernel / row-copy time of the last uhc_load_motions (CUDA events, ms)
     // device curriculum (uhc_curriculum_*): off while cur.M == 0.  cur_gen changes with everything the sampler reads of it by value
@@ -368,7 +385,7 @@ int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
 // replaces the clip table (shared by uhc_load_clips and uhc_load_motions): clip addresses, sampling CDF back to the sample_keys rule,
 // clip models back to variant 0, every env record invalidated, shapes uploaded; d_expert is allocated (uninitialised) for the caller
 static int new_clip_table(UhcEngine *e, int nclips, const int *clip_len, const double *shape_host) {
-    e->view_gen++;
+    e->view_gen++; e->table_gen++;
     if (e->cur.M && nclips != e->num_clips) cur_free(e);   // the histories belong to the old clips
     std::vector<int> adr(nclips + 1, 0);
     for (int i = 0; i < nclips; i++) adr[i + 1] = adr[i] + clip_len[i];
@@ -930,4 +947,52 @@ cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t s
 }
 
 }  // namespace evalx
+
+// ---- the tracker's view of the engine (track_glue.h)
+namespace trackx {
+
+const char *cfg_error(const UhcEngine *e, int H) {
+    const bool f32 = e->precision == 32;
+    const int obs_v = f32 ? e->evf.cfg.obs_v : e->evd.cfg.obs_v, term = f32 ? e->evf.cfg.term_body : e->evd.cfg.term_body;
+    const int ar = f32 ? e->evf.cfg.auto_reset : e->evd.cfg.auto_reset, rv = f32 ? e->evf.cfg.reactive_v : e->evd.cfg.reactive_v;
+    const int trail = f32 ? e->evf.cfg.trail_steps : e->evd.cfg.trail_steps, eplen = f32 ? e->evf.cfg.env_episode_len : e->evd.cfg.env_episode_len;
+    if (H < 3) return "the window must hold at least 3 rows";
+    if (obs_v == 3) return "obs_v 3 reads future frames a stream does not have";
+    if (term != 0) return "term_body root / Head read the whole episode window";
+    if (ar) return "auto_reset re-seeds episodes from the clip table";
+    if (rv == 1) return "reactive_v 1 starts episodes from the neutral pose";
+    if (trail < 1 || eplen < H) return "`end` could fire inside the window: needs trail_steps >= 1 and env_episode_len >= window (the caller owns the episode length)";
+    return nullptr;
+}
+
+int install_table(UhcEngine *e, int H, const int *fk_model, const double *shape, std::string *err) {
+    const int E = e->E;
+    if (cudaSetDevice(e->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { *err = "cudaDeviceSynchronize failed"; return -1; }
+    std::vector<int> lens(E, H);
+    std::vector<double> shp;
+    if (!shape) { shp.assign((size_t)E * 17, 0.0); shape = shp.data(); }
+    if (new_clip_table(e, E, lens.data(), shape)) { *err = g_err; return -1; }
+    if (fk_model && uhc_set_clip_models(e, E, fk_model)) { *err = g_err; return -1; }
+    const size_t rs = e->precision == 32 ? 4 : 8;
+    cudaError_t ce = cudaMemset(e->d_expert, 0, (size_t)E * H * EX_SIZE * rs);
+    if (ce == cudaSuccess)
+        ce = e->precision == 32 ? cudaFuncSetAttribute(k_track_obs<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(EPB_OBS * sizeof(Work<float>)))
+                                : cudaFuncSetAttribute(k_track_obs<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(EPB_OBS * sizeof(Work<double>)));
+    if (ce != cudaSuccess) { *err = std::string("install_table: ") + cudaGetErrorString(ce); return -1; }
+    return 0;
+}
+
+unsigned long long table_gen(const UhcEngine *e) { return e->table_gen; }
+int num_shapes(const UhcEngine *e) { return e->nshape; }
+const motion::MotionModel &motion_model(const UhcEngine *e) { return e->mo_model; }
+
+cudaError_t launch_obs(UhcEngine *e, float *obs, cudaStream_t st) {
+    const int E = e->E;
+    if (e->precision == 32) k_track_obs<float><<<(E + EPB_OBS - 1) / EPB_OBS, 32 * EPB_OBS, EPB_OBS * sizeof(Work<float>), st>>>(e->evf, obs);
+    else k_track_obs<double><<<(E + EPB_OBS - 1) / EPB_OBS, 32 * EPB_OBS, EPB_OBS * sizeof(Work<double>), st>>>(e->evd, obs);
+    e->launches++;
+    return cudaGetLastError();
+}
+
+}  // namespace trackx
 }  // namespace uhc

@@ -172,6 +172,7 @@ class Engine:
     def close(self):
         if getattr(self, "h", None):
             self.lib.uhc_eval_release(self.h)
+            self.lib.uhc_track_end(self.h)
             self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
             self.h = None
@@ -334,6 +335,72 @@ class Engine:
         return dict(frames=frames.numpy()[:n], nframes=np.array([r.frames for r in rec][:n]), last_t=np.array([r.last_t for r in rec][:n]),
                     fail_any=np.array([bool(r.fail_any) for r in rec][:n]), reward_sum=np.array([r.reward_sum for r in rec][:n]),
                     states=states.numpy()[:n] if states is not None else None)
+
+    # ---- the batched physics tracker (include/uhc_track.h uhc_track_*)
+    def _trk_chk(self, rc, who):
+        if rc != 0:
+            self.lib.uhc_track_last_error.restype = C.c_char_p
+            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_track_last_error().decode())
+
+    def track_begin(self, window=8, kind="qpos", pose_dim=None, fk_models=None, shapes=None):
+        """tracking mode: env e follows a stream of raw target frames (kind "qpos": qpos rows of 76; "smpl": pose_aa (pose_dim 72 | 156) then
+        trans) held in a window of `window` expert-table rows.  fk_models: shape variant per env (FK and simulated body), shapes: [E][17]."""
+        k = {"qpos": 1, "smpl": 0, 1: 1, 0: 0}[kind]
+        pose_dim = (NQ if k == 1 else 72) if pose_dim is None else int(pose_dim)
+        fk = None if fk_models is None else np.ascontiguousarray(fk_models, np.int32).reshape(self.E)
+        shp = None if shapes is None else np.ascontiguousarray(np.asarray(shapes, np.float64).reshape(self.E, 17))
+        self._trk_chk(self.lib.uhc_track_begin(self.h, C.c_int(int(window)), C.c_int(k), C.c_int(pose_dim), None if fk is None else _ip_out(fk),
+                                               None if shp is None else shp.ctypes.data_as(C.POINTER(C.c_double))), "uhc_track_begin")
+        self.track_row_w = NQ if k == 1 else pose_dim + 3
+        self._table_loaded(np.full(self.E, int(window), np.int32))
+
+    def track_reset(self, env_ids, frames, qpos=None, qvel=None):
+        """frames: float64 cuda tensor [n][2][row width], target frames 0 and 1 of each listed env; qpos / qvel: optional fp32 cuda overrides"""
+        t = self.torch
+        ids = np.ascontiguousarray(env_ids, np.int32).reshape(-1)
+        assert frames.is_cuda and frames.dtype == t.float64 and frames.is_contiguous() and tuple(frames.shape) == (len(ids), 2, self.track_row_w)
+        for x, w in ((qpos, NQ), (qvel, NV)):
+            assert x is None or (x.is_cuda and x.dtype == t.float32 and x.is_contiguous() and tuple(x.shape) == (len(ids), w))
+        self._trk_chk(self.lib.uhc_track_reset(self.h, C.c_int(len(ids)), _ip_out(ids), C.c_void_p(frames.data_ptr()),
+                                               C.c_void_p(qpos.data_ptr() if qpos is not None else None), C.c_void_p(qvel.data_ptr() if qvel is not None else None),
+                                               self._stream()), "uhc_track_reset")
+
+    def track_step(self, next_frames, mask, policy, log_std, zfilter_stats, zclip, fail_safe, state_out, reward_out, fail_out):
+        """one tracker step of every env (uhc_track_step): next_frames float64 [E][row width] or None, mask int32 [E] or None; the outputs
+        are written into state_out [E][223] (engine precision: qpos 76 | qvel 75 | xpos 72), reward_out [E] fp32, fail_out [E] int32"""
+        t = self.torch
+        if next_frames is not None:
+            assert next_frames.is_cuda and next_frames.dtype == t.float64 and next_frames.is_contiguous() and tuple(next_frames.shape) == (self.E, self.track_row_w)
+        if mask is not None:
+            assert mask.is_cuda and mask.dtype == t.int32 and mask.is_contiguous() and tuple(mask.shape) == (self.E,)
+        from .nn import UhcMcp
+        fn = self.lib.uhc_track_step_mcp if isinstance(policy, UhcMcp) else self.lib.uhc_track_step
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        self._trk_chk(fn(self.h, p(next_frames), p(mask), C.byref(policy), p(log_std), p(zfilter_stats), C.c_float(zclip), C.c_int(int(bool(fail_safe))),
+                         p(state_out), p(reward_out), p(fail_out), self._stream()), "uhc_track_step")
+
+    def track_push(self, next_frames, mask=None):
+        """append a frame to every (masked-in) env's stream without stepping (uhc_track_push)"""
+        t = self.torch
+        assert next_frames.is_cuda and next_frames.dtype == t.float64 and next_frames.is_contiguous() and tuple(next_frames.shape) == (self.E, self.track_row_w)
+        assert mask is None or (mask.is_cuda and mask.dtype == t.int32 and mask.is_contiguous() and tuple(mask.shape) == (self.E,))
+        self._trk_chk(self.lib.uhc_track_push(self.h, C.c_void_p(next_frames.data_ptr()), C.c_void_p(mask.data_ptr() if mask is not None else None),
+                                              self._stream()), "uhc_track_push")
+
+    def track_obs(self, out=None):
+        """the observation the next track_step feeds the policy (uhc_track_obs), [E][obs_dim] fp32"""
+        out = self.torch.empty(self.E, self.obs_dim, device=self.obs.device) if out is None else out
+        self._trk_chk(self.lib.uhc_track_obs(self.h, C.c_void_p(out.data_ptr()), self._stream()), "uhc_track_obs")
+        return out
+
+    def track_state(self):
+        """per env: steps since its reset, cur_t in the window, rows held, pushes dropped on a full window (synchronises)"""
+        out = np.zeros((self.E, 4), np.int32)
+        self._trk_chk(self.lib.uhc_track_state(self.h, _ip_out(out)), "uhc_track_state")
+        return dict(steps=out[:, 0], cur_t=out[:, 1], rows=out[:, 2], dropped=out[:, 3])
+
+    def track_end(self):
+        self.lib.uhc_track_end(self.h)
 
     def set_clip_weights(self, weights=None):
         """sampling weights of the in-kernel re-seeding (None = the reference's sample_keys rule)."""

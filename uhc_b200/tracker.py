@@ -1,0 +1,71 @@
+"""The trained controller as a batched physics tracker (include/uhc_track.h): every env follows target poses that exist only once the
+previous step has run, the role the UHC policy plays inside HumanoidKinEnv.step (uhc/envs/humanoid_kin_v1.py:297-370).
+
+    trk = agent.tracker(window=8, kind="qpos")
+    trk.reset(f0, f1)                  # target frames 0 and 1 of every env, float64 cuda [E][76]
+    state, reward, fail = trk.step()   # the first step tracks frame 1, which the reset supplied
+    while ...:
+        state, reward, fail = trk.step(kin(state))   # frame t + 1 from the simulated state
+
+Each step is one CUDA-graph replay on the device: the new frame's expert record, the observation against it, the policy mean, the
+physics step and fail_safe.  The returned tensors are the tracker's own buffers, overwritten by the next step.
+"""
+import numpy as np
+
+from . import nn
+
+
+class Tracker:
+    def __init__(self, agent, window=8, kind="qpos", fail_safe=True, pose_dim=None, fk_models=None, shapes=None):
+        import torch
+        self.torch, self.agent, self.engine = torch, agent, agent.engine
+        self.E, self.fail_safe = agent.E, bool(fail_safe)
+        self.engine.track_begin(window, kind, pose_dim, fk_models, shapes)
+        self.row_w = self.engine.track_row_w
+        dev = agent.dev
+        self.state = torch.zeros(self.E, 223, device=dev, dtype=torch.float32 if self.engine.precision == 32 else torch.float64)
+        self.reward = torch.zeros(self.E, device=dev, dtype=torch.float32)
+        self.fail = torch.zeros(self.E, device=dev, dtype=torch.int32)
+
+    def _policy(self):
+        a = self.agent
+        return nn.mcp_struct(a.policy) if a.actor_type == "mcp" else nn.mlp_struct(a.policy)
+
+    def reset(self, f0, f1, env_ids=None, qpos=None, qvel=None):
+        """frames 0 and 1 ([n][row width] each) of the listed envs (default: all); the envs start on frame 0 (or the fp32 overrides)"""
+        t = self.torch
+        ids = np.arange(self.E, dtype=np.int32) if env_ids is None else np.asarray(env_ids, np.int32).reshape(-1)
+        frames = t.stack([t.as_tensor(f0), t.as_tensor(f1)], 1).to(device=self.state.device, dtype=t.float64).contiguous()
+        cvt = lambda x: None if x is None else t.as_tensor(x).to(device=self.state.device, dtype=t.float32).contiguous()
+        self.engine.track_reset(ids, frames, cvt(qpos), cvt(qvel))
+        self.agent.obs = None          # the envs left whatever episode they were on
+
+    def step(self, next_frames=None, mask=None):
+        """next_frames: target frame t + 1 of every env ([E][row width], None on the first step after a reset); mask: int32 [E], 0 = this
+        env gets no frame.  Returns (state [E][223] = qpos 76 | qvel 75 | xpos 72 as the step left it, reward [E], fail [E])."""
+        t = self.torch
+        nf = None if next_frames is None else t.as_tensor(next_frames).to(device=self.state.device, dtype=t.float64).contiguous()
+        mk = None if mask is None else t.as_tensor(mask).to(device=self.state.device, dtype=t.int32).contiguous()
+        a = self.agent
+        self.engine.track_step(nf, mk, self._policy(), a.log_std, a.running_state.stats, a.running_state.clip, self.fail_safe,
+                               self.state, self.reward, self.fail)
+        return self.state, self.reward, self.fail
+
+    @property
+    def qpos(self):
+        return self.state[:, :76]
+
+    @property
+    def qvel(self):
+        return self.state[:, 76:151]
+
+    @property
+    def xpos(self):
+        return self.state[:, 151:223].reshape(self.E, 24, 3)
+
+    def steps(self):
+        """control steps each env has taken since its reset (synchronises)"""
+        return self.engine.track_state()["steps"]
+
+    def close(self):
+        self.engine.track_end()
