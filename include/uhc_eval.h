@@ -47,7 +47,21 @@ int uhc_eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, c
                  int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
 int uhc_eval_run_mcp(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
                      int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
-void uhc_eval_release(UhcEngine *e);   /* frees the graphs / scratch of this engine; call before uhc_engine_destroy */
+/* Several policies of one architecture in one call (checkpoint sweeps): group g owns envs [off_g, off_g + n_g), off_g = sum_{h<g} n_h,
+ * sum n_g <= E, and runs policy mlps[g] (mcps[g]) with its own ZFilter statistics zfilter_stats_host[g] (a host array of G device pointers)
+ * on clips clip_host[off_g .. off_g + n_g - 1].  Everything else is uhc_eval_run over the sum n of the group sizes: frames_host = [n][max(len) - 1]
+ * [UHC_EVAL_NCOL] with max(len) over every listed clip, clips_host = [n], states_host_or_null = [n][max(len) - 1][UHC_EVAL_STATE]; envs past
+ * the last group are parked on clip_host[0] and step with zero actions.  Each group's rows are bit-identical to a uhc_eval_run of its own
+ * policy on its own clips (with any finite log_std: the mean action needs none).  The policy GEMMs of all groups run as one grouped
+ * tensor-core launch per layer.  Bad arguments (-2, the engine stays usable): G < 1 or G > UHC_EVAL_MAX_GROUPS, an n_g < 1, sum n > E, a clip
+ * out of range, no clip table, window < 1, a null policy or statistics pointer, policies whose layer widths, K padding, activation or
+ * primitive count differ between groups, widths that are not the engine's obs / action dims. */
+#define UHC_EVAL_MAX_GROUPS 64
+int uhc_eval_run_groups(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
+                        float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
+int uhc_eval_run_groups_mcp(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
+                            float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
+void uhc_eval_release(UhcEngine *e);   /* frees the graphs / scratch of this engine (the grouped path's too); call before uhc_engine_destroy */
 
 #ifdef __cplusplus
 }

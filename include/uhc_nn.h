@@ -24,6 +24,14 @@ int uhc_act_backward(const float *dh, const float *z, float *dz, long n, int act
  * x_bf16 [M][Kp], W_bf16 [N][Kp] with Kp a multiple of 64 (zero padded); y_bf16 [M][Np] (next layer's input) and/or y_f32 [M][N]. */
 int uhc_linear_forward_tc(const void *x_bf16, const void *W_bf16, const float *b, void *y_bf16_or_null, float *y_f32_or_null,
                           int M, int N, int Kp, int ldy_bf16, int act, void *stream);
+/* the same for G <= UHC_TC_MAX_GROUPS weight sets in one launch: rows [row0_host[g], row0_host[g] + rows_host[g]) of x and y use W_bf16_host[g]
+ * and b_host[g] (host arrays of device pointers; b_host may be NULL, as may an entry).  The ranges must be non-empty, ascending, disjoint
+ * and inside [0, M); rows outside every range are not written.  Each row's output is bit-identical to uhc_linear_forward_tc with its
+ * group's weights (the row tiles of a launch never straddle two groups: uhc_b200/csrc/group_core.h). */
+#define UHC_TC_MAX_GROUPS 64
+int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_host, const void *x_bf16, const void *const *W_bf16_host,
+                                  const float *const *b_host_or_null, void *y_bf16_or_null, float *y_f32_or_null, int M, int N, int Kp, int ldy_bf16,
+                                  int act, void *stream);
 int uhc_f32_to_bf16_padded(const float *x, void *y_bf16, int M, int K, int Kp, void *stream);
 /* training variants on the tensor cores (bf16 operands, fp32 accumulate; autograd of nn.Linear + activation):
  *   forward that also stores the pre-activation z (fp32) ; dX = dZ W and dW = dZ^T X are plain calls of uhc_linear_forward_tc on

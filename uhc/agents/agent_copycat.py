@@ -5,6 +5,7 @@
   .sample(min_batch_size)   -> (batch, log)      batch: states / actions / masks / rewards / exps (device resident, numpy on demand)
   .update_params(batch)     GAE + PPO epochs (khrylib agent_pg.py:39-56, agent_ppo.py:16-51)
   .eval_policy(epoch, dump) deterministic roll-out of every clip, coverage / error statistics                               (:354-494)
+  .eval_checkpoints(epochs, dump)   eval_policy of several saved checkpoints at once (device evaluation, checkpoints side by side)
   .save_checkpoint / .load_checkpoint   pickle {"policy_dict", "value_dict", "running_state"} at models/iter_%04d.p        (:190-260)
 
 Differences that are inherent to the batched design are listed in DESIGN.md (lock-step horizon with value bootstrap, batched
@@ -349,19 +350,66 @@ class AgentCopycat:
                 pending = []
             eng.set_cfg(**self._env_cfg(test=False))
             self.agent.obs = None
-            names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
-            metrics = {m: float(np.mean([np.mean(r[m]) for r in res.values() if m in r])) if any(m in r for r in res.values()) else float("nan") for m in names}
-            coverage = int(round(metrics["succ"] * n))
-            self.logger.info(f"Coverage {loader.name} of {coverage} out of {n} | " + " \t".join(f"{k}: {v:.3f}" for k, v in metrics.items()))
-            metrics.update(mean_coverage=coverage / n, num_coverage=coverage, all_coverage=n)
-            del metrics["succ"]
-            res_dicts.append({f"coverage_{loader.name}": metrics})
-            if dump:
-                path = osp.join(cfg.output_dir, f"{epoch}_{loader.name}_coverage_full.pkl")
-                joblib.dump(res, path)
+            res_dicts.append(self._coverage(loader, res, epoch, dump))
         if not self.curriculum_on_device:
             self._push_clip_weights()
         return res_dicts
+
+    def _coverage(self, loader, res, epoch, dump):
+        """the coverage line and metric dict of one loader's results (and with dump its {epoch}_{loader}_coverage_full.pkl)"""
+        n = loader.get_len()
+        names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
+        metrics = {m: float(np.mean([np.mean(r[m]) for r in res.values() if m in r])) if any(m in r for r in res.values()) else float("nan") for m in names}
+        coverage = int(round(metrics["succ"] * n))
+        self.logger.info(f"Coverage {loader.name} of {coverage} out of {n} | " + " \t".join(f"{k}: {v:.3f}" for k, v in metrics.items()))
+        metrics.update(mean_coverage=coverage / n, num_coverage=coverage, all_coverage=n)
+        del metrics["succ"]
+        if dump:
+            joblib.dump(res, osp.join(self.cfg.output_dir, f"{epoch}_{loader.name}_coverage_full.pkl"))
+        return {f"coverage_{loader.name}": metrics}
+
+    def eval_checkpoints(self, epochs, dump=False):
+        """eval_policy(eval_on_device: true) of several saved checkpoints (models/iter_%04d.p) at once: every test loader is evaluated for all
+        of them in shared device calls (BatchedAgent.evaluate_policies).  Returns {epoch: res_dicts}, each what load_checkpoint(epoch) +
+        eval_policy(epoch, dump) gives, and logs the same coverage lines.  Comparing checkpoints is not training: no outcome reaches freq_dict
+        or the device curriculum, and the agent's weights, log_std and running_state stay as they are."""
+        from uhc_b200.metrics import metrics_from_frames
+        cfg, eng = self.cfg, self.agent.engine
+        epochs = list(epochs)
+        cps = []
+        for epoch in epochs:
+            path = "%s/iter_%04d.p" % (cfg.model_dir, epoch)
+            self.logger.info("loading model from checkpoint: %s" % path)
+            with open(path, "rb") as f:
+                cps.append(pickle.load(f))
+        out = {epoch: [] for epoch in epochs}
+        for loader in self.test_data_loaders:
+            n = loader.get_len()
+            saved = None
+            if loader is not self.data_loader:
+                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+                self._load_tables(loader)
+            eng.set_cfg(**self._env_cfg(test=True))
+            clips = np.arange(n, dtype=np.int32)
+            lens = eng.clip_len[clips]
+            per_cp = self.agent.evaluate_policies(cps, clips, bool(cfg.fail_safe), window=32)
+            if loader is not self.data_loader:
+                self._load_tables(self.data_loader)
+                if saved is not None:
+                    self._restore_device_curriculum(saved)
+            eng.set_cfg(**self._env_cfg(test=False))
+            self.agent.obs = None
+            for epoch, dev in zip(epochs, per_cp):
+                last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
+                rsum = np.array([d["reward_sum"] for d in dev])
+                res = {}
+                for i in range(n):
+                    res[loader.data_keys[i]] = self._clip_result(lens[i], last_t[i], fail_any[i], rsum[i], len(dev[i]["frames"]),
+                                                                 lambda pct, fs, d=dev[i]: metrics_from_frames(d["frames"], pct, fs))
+                out[epoch].append(self._coverage(loader, res, epoch, dump))
+        if not self.curriculum_on_device:
+            self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
+        return out
 
     def _restore_device_curriculum(self, fd):
         if self.agent.engine.cur_cfg is None:

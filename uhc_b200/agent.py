@@ -44,6 +44,28 @@ def failure_weights(success_hist, sampling_temp=0.2, sampling_freq=0.5):
     return (sampling_freq * p + (1.0 - sampling_freq) / len(p)).astype(np.float32)
 
 
+MAX_EVAL_GROUPS = 64       # include/uhc_eval.h UHC_EVAL_MAX_GROUPS
+
+
+def pack_groups(K, n, E, max_groups=MAX_EVAL_GROUPS):
+    """calls of a K-checkpoint x n-clip sweep on E envs: the K * n (checkpoint, clip) pairs, checkpoint-major, cut into calls of at most E envs
+    and max_groups groups, a group being one checkpoint's run of consecutive clips inside a call.  Returns [[(k, c0, c1), ...] per call]."""
+    assert K >= 1 and n >= 1 and E >= 1 and max_groups >= 1
+    calls, cur, used = [], [], 0
+    for k in range(K):
+        c0 = 0
+        while c0 < n:
+            if used == E or len(cur) == max_groups:
+                calls.append(cur)
+                cur, used = [], 0
+            c1 = min(n, c0 + E - used)
+            cur.append((k, c0, c1))
+            used += c1 - c0
+            c0 = c1
+    calls.append(cur)
+    return calls
+
+
 class ClipSampler:
     """DatasetAMASSSingle.sample_seq / get_sample_from_key (dataset_amass_single.py:172-253): uniform clip choice (or
     failure-weighted when freq stats are given), start ~ U[0, len - t_min), slice length min(t_max, len - start)."""
@@ -401,6 +423,53 @@ class BatchedAgent:
                 if record_states:
                     d["states"] = r["states"][i, :nf].copy()
                 out.append(d)
+        self.obs = None       # every env was reset onto an evaluation clip
+        return out
+
+    def _checkpoint_policy(self, k, cp):
+        """(policy net, ZFilter) slot k of the evaluation pool, beside the agent's own (which stay untouched), loaded from a checkpoint in the
+        reference's wire format.  The pool is kept: its tensors keep their addresses, so a repeated sweep replays its captured graphs."""
+        pool = self.__dict__.setdefault("_eval_pool", [])
+        pol = self.policy
+        while len(pool) <= k:
+            if self.actor_type == "mcp":
+                net = nn.MCPNet(self.obs_dim, pol.dims[1:-1], self.act_dim, pol.htype, num_primitive=pol.num_primitive,
+                                composer_dim=tuple(pol.composer.dims[1:-1]), device=self.dev, seed=0)
+            else:
+                net = nn.MLPNet(self.obs_dim, pol.dims[1:-1], self.act_dim, pol.htype, device=self.dev, head_name="action_mean", seed=0)
+            pool.append((net, nn.ZFilter(self.obs_dim, clip=self.running_state.clip, device=self.dev)))
+        net, zf = pool[k]
+        net.load_state_dict(cp["policy_dict"])
+        rs = cp.get("running_state")
+        if isinstance(rs, dict):
+            zf.load(rs["n"], rs["mean"], rs["std"])
+        elif rs is not None:
+            zf.load_sums(rs.rs._n, rs.rs._M, rs.rs._S)
+        else:                 # as load_state_dicts: a checkpoint without statistics is normalised by the agent's
+            zf.stats.copy_(self.running_state.stats)
+        return net, zf
+
+    def evaluate_policies(self, checkpoints, clips, fail_safe, window=32, record_states=False):
+        """evaluate() of every listed clip for each checkpoint ({"policy_dict", "running_state"}, what state_dicts writes), with the checkpoints
+        side by side in each device call (Engine.eval_run_groups, packed by pack_groups).  Returns one list per checkpoint, each equal to
+        what load_state_dicts(cp) + evaluate(clips, ...) returns.  The agent's own weights, log_std and running_state are not touched."""
+        clips = np.asarray(clips, dtype=np.int32).reshape(-1)
+        K, n = len(checkpoints), len(clips)
+        out = [[] for _ in range(K)]
+        if K == 0 or n == 0:
+            return out
+        mcp = self.actor_type == "mcp"
+        pols = [self._checkpoint_policy(k, cp) for k, cp in enumerate(checkpoints)]
+        structs = [(nn.mcp_struct(net) if mcp else nn.mlp_struct(net), zf) for net, zf in pols]
+        for call in pack_groups(K, n, self.E):
+            groups = [(clips[c0:c1], structs[k][0], structs[k][1].stats) for k, c0, c1 in call]
+            res = self.engine.eval_run_groups(groups, self.running_state.clip, fail_safe, window, record_states)
+            for (k, _, _), r in zip(call, res):
+                for i, nf in enumerate(r["nframes"]):
+                    d = dict(frames=r["frames"][i, :nf].copy(), last_t=int(r["last_t"][i]), fail_any=bool(r["fail_any"][i]), reward_sum=float(r["reward_sum"][i]))
+                    if record_states:
+                        d["states"] = r["states"][i, :nf].copy()
+                    out[k].append(d)
         self.obs = None       # every env was reset onto an evaluation clip
         return out
 

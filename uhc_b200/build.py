@@ -9,7 +9,7 @@ SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_wgmma.cu", "rollout.cu", "ppo_up
 # compiled on their own without multiply-add contraction: the motion library, the evaluation metrics, the curriculum weights and the tracker's
 # streamed rows restate numpy's fp64 arithmetic operation for operation
 NO_FMA_SRCS = ["motion_lib.cu", "eval.cu", "curriculum.cu", "track.cu"]
-DEPS = ["sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "curriculum_core.h", "track_core.h", "track_obs.h", "track_glue.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h", "../../include/uhc_track.h"]
+DEPS = ["sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "group_core.h", "curriculum_core.h", "track_core.h", "track_obs.h", "track_glue.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h", "../../include/uhc_track.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 

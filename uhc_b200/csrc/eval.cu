@@ -90,6 +90,21 @@ struct EvalKey {
     UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; const float *log_std; const double *zstats;
     bool operator==(const EvalKey &o) const { return memcmp(this, &o, sizeof(EvalKey)) == 0; }
 };
+// the grouped evaluation's graphs: G, the group sizes, every group's policy by value and its ZFilter statistics pointer, and the generations
+// of the grouped policy scratch, the window buffers and the engine view
+struct GroupKeyHead {
+    int G, ntot, nrec_max, window, fail_safe, states, nprim; float zclip; unsigned long long group_gen, eval_gen, view_gen;
+};
+struct GroupKey {
+    GroupKeyHead h; std::vector<int> n; std::vector<UhcMlp> nets; std::vector<const double *> zs;
+    bool operator==(const GroupKey &o) const {
+        return memcmp(&h, &o.h, sizeof h) == 0 && n == o.n && zs == o.zs && nets.size() == o.nets.size() &&
+               memcmp(nets.data(), o.nets.data(), nets.size() * sizeof(UhcMlp)) == 0;
+    }
+};
+// the policies of one grouped call: group g on env rows [row0[g], row0[g + 1])
+struct GroupSet { int G; const int *row0; const UhcMlp *mlps; const UhcMcp *mcps; const double *const *zstats; };
+
 struct EvalCtx {
     UhcEngine *eng = nullptr;
     int E = 0, n_cap = 0, win_cap = 0, states_cap = 0;
@@ -100,6 +115,7 @@ struct EvalCtx {
     cudaEvent_t ev = nullptr;
     std::vector<int> ids, clip0, start, len;      // reset arguments (kept: no allocation in the steady state)
     std::vector<std::pair<EvalKey, cudaGraphExec_t>> graphs;
+    std::vector<std::pair<GroupKey, cudaGraphExec_t>> ggraphs;   // uhc_eval_run_groups
 };
 std::vector<EvalCtx *> g_ev;
 
@@ -109,7 +125,12 @@ EvalCtx *ev_ctx(UhcEngine *e) {
     g_ev.push_back(c);
     return c;
 }
-void drop_graphs(EvalCtx *c) { for (auto &g : c->graphs) cudaGraphExecDestroy(g.second); c->graphs.clear(); }
+void drop_graphs(EvalCtx *c) {
+    for (auto &g : c->graphs) cudaGraphExecDestroy(g.second);
+    c->graphs.clear();
+    for (auto &g : c->ggraphs) cudaGraphExecDestroy(g.second);
+    c->ggraphs.clear();
+}
 
 // per-env arrays sized by E once; the window buffers grow with n * window (and the state record with it when requested)
 int ensure(EvalCtx *c, int n, int window, bool states) {
@@ -133,10 +154,11 @@ int ensure(EvalCtx *c, int n, int window, bool states) {
 }
 
 int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
-                   int n, int nrec_max, int fail_safe, int window, bool states, cudaStream_t st) {
+                   int n, int nrec_max, int fail_safe, int window, bool states, cudaStream_t st, const GroupSet *grp = nullptr) {
     std::string err;
     for (int s = 0; s < window; s++) {
-        int rc = evalx::policy_enqueue(c->eng, mlp, mcp, R.obs, log_std, zstats, zclip, c->d_ones, R.act, st, &err);
+        int rc = grp ? evalx::groups_enqueue(c->eng, grp->G, grp->row0, grp->mlps, grp->mcps, grp->zstats, zclip, R.obs, c->d_ones, R.act, st, &err)
+                     : evalx::policy_enqueue(c->eng, mlp, mcp, R.obs, log_std, zstats, zclip, c->d_ones, R.act, st, &err);
         if (rc) { g_ev_err = err; return rc; }
         if (uhc_env_step(c->eng, R.act, R.obs, R.rew, R.cinfo, R.fail, R.end, R.pct, nullptr, st)) { g_ev_err = std::string("env step: ") + uhc_last_error(); return -1; }
         const bool last = s == window - 1;
@@ -152,6 +174,59 @@ int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, co
         CKE(cudaGetLastError());
         if (fail_safe) CKE(evalx::launch_reseat(c->eng, n, c->d_reseat, st));
     }
+    return 0;
+}
+
+// reset: idle envs parked on the chunk's first clip, then envs 0..n-1 on their clips from frame 0 (the host loop's order)
+int reset_envs(EvalCtx *c, UhcEngine *e, const evalx::EngineRefs &R, int n, const int *clip_host, cudaStream_t st) {
+    if (n < R.E) {
+        const int m = R.E - n;
+        c->ids.resize(m); c->clip0.assign(m, clip_host[0]); c->start.assign(m, 0); c->len.assign(m, R.clip_len_h[clip_host[0]]);
+        for (int k = 0; k < m; k++) c->ids[k] = n + k;
+        if (uhc_env_reset(e, m, c->ids.data(), c->clip0.data(), c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
+    }
+    c->ids.resize(n); c->start.assign(n, 0); c->len.resize(n);
+    for (int k = 0; k < n; k++) { c->ids[k] = k; c->len[k] = R.clip_len_h[clip_host[k]]; }
+    if (uhc_env_reset(e, n, c->ids.data(), clip_host, c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
+    k_eval_init<<<(R.E + 127) / 128, 128, 0, st>>>(n, c->d_clips, c->d_alive, c->d_reseat, c->d_ones, R.E);
+    CKE(cudaGetLastError());
+    return 0;
+}
+
+// `window` steps captured on a private stream into an instantiated graph
+int capture_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
+                   int n, int nrec_max, int fail_safe, int window, bool states, const GroupSet *grp, cudaGraphExec_t *exec) {
+    cudaStream_t cs; CKE(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+    cudaGraph_t graph = nullptr;
+    CKE(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+    const int rc = enqueue_window(c, R, mlp, mcp, log_std, zstats, zclip, n, nrec_max, fail_safe, window, states, cs, grp);
+    cudaError_t ce = cudaStreamEndCapture(cs, &graph);
+    cudaStreamDestroy(cs);
+    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+    if (ce != cudaSuccess) { g_ev_err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce); return -1; }
+    ce = cudaGraphInstantiate(exec, graph, 0);
+    cudaGraphDestroy(graph);
+    CKE(ce);
+    return 0;
+}
+
+// replays until every env has stopped or nrec_max steps have run; after each, the window's rows of envs 0..n-1 go to the caller's arrays
+int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host, cudaStream_t st) {
+    for (int s0 = 0; s0 < nrec_max; s0 += window) {
+        CKE(cudaGraphLaunch(exec, st));
+        const int rows = nrec_max - s0 < window ? nrec_max - s0 : window;
+        CKE(cudaMemcpy2DAsync(frames_host + (size_t)s0 * NCOL, (size_t)nrec_max * NCOL * sizeof(double), c->d_win, (size_t)window * NCOL * sizeof(double),
+                              (size_t)rows * NCOL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
+        if (states_host)
+            CKE(cudaMemcpy2DAsync(states_host + (size_t)s0 * NSTATE, (size_t)nrec_max * NSTATE * sizeof(double), c->d_wstates, (size_t)window * NSTATE * sizeof(double),
+                                  (size_t)rows * NSTATE * sizeof(double), n, cudaMemcpyDeviceToHost, st));
+        CKE(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
+        CKE(cudaEventRecord(c->ev, st));
+        CKE(cudaEventSynchronize(c->ev));
+        if (*c->h_count == 0) break;
+    }
+    CKE(cudaMemcpyAsync(clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
+    CKE(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -176,18 +251,7 @@ int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const
     if (ensure(c, n, window, states)) return -1;
     cudaStream_t st = (cudaStream_t)stream;
     const int nrec_max = max_len - 1;
-    // reset: idle envs parked on the chunk's first clip, then envs 0..n-1 on their clips from frame 0 (the host loop's order)
-    if (n < R.E) {
-        const int m = R.E - n;
-        c->ids.resize(m); c->clip0.assign(m, clip_host[0]); c->start.assign(m, 0); c->len.assign(m, R.clip_len_h[clip_host[0]]);
-        for (int k = 0; k < m; k++) c->ids[k] = n + k;
-        if (uhc_env_reset(e, m, c->ids.data(), c->clip0.data(), c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
-    }
-    c->ids.resize(n); c->start.assign(n, 0); c->len.resize(n);
-    for (int k = 0; k < n; k++) { c->ids[k] = k; c->len[k] = R.clip_len_h[clip_host[k]]; }
-    if (uhc_env_reset(e, n, c->ids.data(), clip_host, c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
-    k_eval_init<<<(R.E + 127) / 128, 128, 0, st>>>(n, c->d_clips, c->d_alive, c->d_reseat, c->d_ones, R.E);
-    CKE(cudaGetLastError());
+    if (reset_envs(c, e, R, n, clip_host, st)) return -1;
 
     EvalKey key; memset(&key, 0, sizeof key);
     key.n = n; key.nrec_max = nrec_max; key.window = window; key.fail_safe = fail_safe ? 1 : 0; key.states = states; key.zclip = zclip;
@@ -205,36 +269,72 @@ int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const
     cudaGraphExec_t exec = nullptr;
     for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
     if (!exec) {
-        cudaStream_t cs; CKE(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaGraph_t graph = nullptr;
-        CKE(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-        rc = enqueue_window(c, R, mlp, mcp, log_std, (double *)zfilter_stats, zclip, n, nrec_max, key.fail_safe, window, states, cs);
-        cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-        cudaStreamDestroy(cs);
-        if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-        if (ce != cudaSuccess) { g_ev_err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce); return -1; }
-        ce = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        CKE(ce);
+        rc = capture_window(c, R, mlp, mcp, log_std, (double *)zfilter_stats, zclip, n, nrec_max, key.fail_safe, window, states, nullptr, &exec);
+        if (rc) return rc;
         if (c->graphs.size() >= 32) { cudaGraphExecDestroy(c->graphs.front().second); c->graphs.erase(c->graphs.begin()); }
         c->graphs.emplace_back(key, exec);
     }
-    for (int s0 = 0; s0 < nrec_max; s0 += window) {
-        CKE(cudaGraphLaunch(exec, st));
-        const int rows = nrec_max - s0 < window ? nrec_max - s0 : window;
-        CKE(cudaMemcpy2DAsync(frames_host + (size_t)s0 * NCOL, (size_t)nrec_max * NCOL * sizeof(double), c->d_win, (size_t)window * NCOL * sizeof(double),
-                              (size_t)rows * NCOL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
-        if (states)
-            CKE(cudaMemcpy2DAsync(states_host + (size_t)s0 * NSTATE, (size_t)nrec_max * NSTATE * sizeof(double), c->d_wstates, (size_t)window * NSTATE * sizeof(double),
-                                  (size_t)rows * NSTATE * sizeof(double), n, cudaMemcpyDeviceToHost, st));
-        CKE(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
-        CKE(cudaEventRecord(c->ev, st));
-        CKE(cudaEventSynchronize(c->ev));
-        if (*c->h_count == 0) break;
+    return replay(c, exec, n, nrec_max, window, frames_host, clips_host, states_host, st);
+}
+
+// G policies side by side: group g on envs [off_g, off_g + n_g), the rest as eval_run over the sum of the n_g envs
+int eval_run_groups(UhcEngine *e, int G, const int *group_n, const int *clip_host, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats,
+                    float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host, void *stream) {
+    const char *who = mcps ? "uhc_eval_run_groups_mcp" : "uhc_eval_run_groups";
+    if (!e || !group_n || !clip_host || (!mlps && !mcps) || !zstats || !frames_host || !clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
+    if (G < 1 || G > UHC_EVAL_MAX_GROUPS) { g_ev_err = std::string(who) + ": G must be 1 .. UHC_EVAL_MAX_GROUPS"; return -2; }
+    evalx::EngineRefs R; evalx::engine_refs(e, &R);
+    std::vector<int> row0(G + 1, 0);
+    for (int g = 0; g < G; g++) {
+        if (group_n[g] < 1) { g_ev_err = std::string(who) + ": every group needs at least one env"; return -2; }
+        if (!zstats[g]) { g_ev_err = std::string(who) + ": null ZFilter statistics"; return -2; }
+        row0[g + 1] = row0[g] + group_n[g];
+        if (row0[g + 1] > R.E) { g_ev_err = std::string(who) + ": the groups hold more than E envs"; return -2; }
     }
-    CKE(cudaMemcpyAsync(clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
-    CKE(cudaStreamSynchronize(st));
-    return 0;
+    const int n = row0[G];
+    if (window < 1) { g_ev_err = std::string(who) + ": window < 1"; return -2; }
+    if (R.num_clips <= 0) { g_ev_err = std::string(who) + ": no clips loaded"; return -2; }
+    int max_len = 0;
+    for (int i = 0; i < n; i++) {
+        if (clip_host[i] < 0 || clip_host[i] >= R.num_clips) { g_ev_err = std::string(who) + ": clip index out of range"; return -2; }
+        max_len = R.clip_len_h[clip_host[i]] > max_len ? R.clip_len_h[clip_host[i]] : max_len;
+    }
+    unsigned long long ggen = 0; std::string err;
+    int rc = evalx::groups_prepare(e, G, mlps, mcps, &ggen, &err);
+    if (rc) { g_ev_err = err; return rc; }
+    EvalCtx *c = ev_ctx(e);
+    const bool states = states_host != nullptr;
+    if (ensure(c, n, window, states)) return -1;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int nrec_max = max_len - 1;
+    if (reset_envs(c, e, R, n, clip_host, st)) return -1;
+    // no policy covers the parked envs: they step with zero actions (the graph writes action rows 0 .. n-1 only)
+    if (n < R.E) CKE(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
+
+    GroupKey key; memset(&key.h, 0, sizeof key.h);
+    key.h.G = G; key.h.ntot = n; key.h.nrec_max = nrec_max; key.h.window = window; key.h.fail_safe = fail_safe ? 1 : 0; key.h.states = states;
+    key.h.zclip = zclip; key.h.group_gen = ggen; key.h.eval_gen = c->gen; key.h.view_gen = R.view_gen;
+    key.n.assign(group_n, group_n + G); key.zs.assign(zstats, zstats + G);
+    for (int g = 0; g < G; g++) {
+        if (mcps) { key.h.nprim = mcps[g].nprim; for (int k = 0; k < mcps[g].nprim; k++) key.nets.push_back(mcps[g].prim[k]); key.nets.push_back(mcps[g].composer); }
+        else key.nets.push_back(mlps[g]);
+    }
+    for (size_t g = 0; g < c->ggraphs.size();) {      // graphs holding a changed engine view or reallocated scratch can never be replayed
+        const GroupKeyHead &k = c->ggraphs[g].first.h;
+        if (k.view_gen != key.h.view_gen || k.group_gen != key.h.group_gen || k.eval_gen != key.h.eval_gen) {
+            cudaGraphExecDestroy(c->ggraphs[g].second); c->ggraphs.erase(c->ggraphs.begin() + g);
+        } else g++;
+    }
+    cudaGraphExec_t exec = nullptr;
+    for (auto &g : c->ggraphs) if (g.first == key) { exec = g.second; break; }
+    if (!exec) {
+        const GroupSet gs{G, row0.data(), mlps, mcps, zstats};
+        rc = capture_window(c, R, nullptr, nullptr, nullptr, nullptr, zclip, n, nrec_max, key.h.fail_safe, window, states, &gs, &exec);
+        if (rc) return rc;
+        if (c->ggraphs.size() >= 16) { cudaGraphExecDestroy(c->ggraphs.front().second); c->ggraphs.erase(c->ggraphs.begin()); }
+        c->ggraphs.emplace_back(std::move(key), exec);
+    }
+    return replay(c, exec, n, nrec_max, window, frames_host, clips_host, states_host, st);
 }
 
 }  // namespace
@@ -254,7 +354,19 @@ int uhc_eval_run_mcp(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mc
     return eval_run(e, n, clip_host, nullptr, mcp, log_std, zfilter_stats, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
 }
 
+int uhc_eval_run_groups(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
+                        float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
+    if (!mlps) { g_ev_err = "uhc_eval_run_groups: null policy"; return -2; }
+    return eval_run_groups(e, G, group_n_host, clip_host, mlps, nullptr, zfilter_stats_host, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+}
+int uhc_eval_run_groups_mcp(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
+                            float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
+    if (!mcps) { g_ev_err = "uhc_eval_run_groups_mcp: null policy"; return -2; }
+    return eval_run_groups(e, G, group_n_host, clip_host, nullptr, mcps, zfilter_stats_host, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+}
+
 void uhc_eval_release(UhcEngine *e) {
+    evalx::groups_release(e);
     for (size_t i = 0; i < g_ev.size(); i++) if (g_ev[i]->eng == e) {
         EvalCtx *c = g_ev[i];
         drop_graphs(c);

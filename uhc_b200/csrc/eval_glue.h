@@ -30,6 +30,14 @@ int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, unsigned 
 // obs -> ZFilter (no update) -> policy -> action (the mean where mean_action[e] != 0); enqueues only (capturable)
 int policy_enqueue(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, const float *obs, const float *log_std, double *zstats, float zclip,
                    const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err);                 // rollout.cu
+// the grouped evaluation (uhc_eval_run_groups): G policies (mlps[G] or mcps[G]) of one architecture, group g on rows [row0[g], row0[g + 1]).
+// groups_prepare validates them (-2) and sizes the grouped scratch, which is its own (never the rollout's); *gen changes whenever that
+// scratch is reallocated.  groups_enqueue: obs -> ZFilter of each group (zstats[g], no update) -> grouped GEMMs (+ mixture head) -> the
+// mean action (with mean_action all ones) of rows 0 .. row0[G] - 1; enqueues only (capturable).  groups_release frees the scratch.
+int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, unsigned long long *gen, std::string *err);              // rollout.cu
+int groups_enqueue(UhcEngine *e, int G, const int *row0, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats, float zclip, const float *obs,
+                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err);                 // rollout.cu
+void groups_release(UhcEngine *e);                                                                                         // rollout.cu
 
 }  // namespace evalx
 }  // namespace uhc

@@ -12,8 +12,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 #include <string>
 #include "../../include/uhc_nn.h"
+#include "group_core.h"
 
 namespace {
 constexpr int BM = 128, BN = 128, BK = 64, UK = 16, STAGES = 5;   // 5 stages x 32 KB in flight: one CTA per SM (up to 227 KB of shared memory per block)
@@ -375,6 +377,124 @@ k_linear_tc(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     }
 }
 
+// Grouped forward: G weight sets in one launch (the policy forward of several checkpoints side by side, eval.cu).  Row tile blockIdx.y
+// belongs to one group (group_core.h): it loads 128 rows of x from the group's first row on, multiplies them by that group's weights
+// (its tensor map in ga.mapB) and stores only the group's rows.  Main loop and epilogue arithmetic are k_linear_tc's without split-K, so
+// a row's output is bit-identical to uhc_linear_forward_tc on that row; the outputs leave through per-thread stores bounded by the group.
+struct GroupedArgs {
+    CUtensorMap mapB[uhc::grp::MAX_GROUPS];
+    const float *bias[uhc::grp::MAX_GROUPS];
+    uhc::grp::TilePlan plan;
+};
+static_assert(sizeof(GroupedArgs) + sizeof(CUtensorMap) + 64 <= 32764, "the grouped kernel's parameters must fit the 32 KB parameter space");
+
+__global__ void __launch_bounds__(NTHREADS, 1)
+k_linear_tc_grouped(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ GroupedArgs ga, __nv_bfloat16 *__restrict__ ybf, float *__restrict__ yf,
+                    int N, int Kp, int ldy, int act) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t *smem = (uint8_t *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint64_t *bars = (uint64_t *)(smem + STAGES * STAGE_BYTES);   // full[STAGES], empty[STAGES]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int m0, row_end;
+    const int grp = uhc::grp::tile_rows(ga.plan, blockIdx.y, &m0, &row_end);
+    const int n0 = blockIdx.x * BN, nkb = Kp / BK;
+    const CUtensorMap *mapB = &ga.mapB[grp];
+    const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + STAGES);
+
+    if (warp == 8 && lane == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA));
+        asm volatile("prefetch.tensormap [%0];" ::"l"(mapB));
+        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 8); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        if (lane == 0) {
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int s = kb % STAGES; const uint32_t ph = (kb / STAGES) & 1;
+                mbar_wait(empty0 + 8 * s, ph ^ 1);
+                mbar_expect_tx(full0 + 8 * s, STAGE_BYTES);
+                const uint32_t a = smem_u32(smem + s * STAGE_BYTES), b = a + BM * BK * 2;
+                tma_load_2d(a, &mapA, full0 + 8 * s, kb * BK, m0);       // rows past M read as zeros; rows of a later group are loaded, never stored
+                tma_load_2d(b, mapB, full0 + 8 * s, kb * BK, n0);
+            }
+        }
+        return;
+    }
+    const int g = warp >> 2, wl = warp & 3;
+    {
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < nkb; ++kb) {
+            const int s = kb % STAGES; const uint32_t ph = (kb / STAGES) & 1;
+            mbar_wait(full0 + 8 * s, ph);
+            const uint32_t a = smem_u32(smem + s * STAGE_BYTES) + g * 64 * BK * 2, b = smem_u32(smem + s * STAGE_BYTES) + BM * BK * 2;
+            const uint64_t ad = make_desc(a), bd = make_desc(b);
+            fence_acc(acc);
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+            for (int k = 0; k < BK / UK; ++k) wgmma_m64n128k16(acc, ad + (uint64_t)(k * UK * 2 >> 4), bd + (uint64_t)(k * UK * 2 >> 4), (kb | k) != 0);
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+            fence_acc(acc);
+            if (kb > 0 && lane == 0) mbar_arrive(empty0 + 8 * ((kb - 1) % STAGES));
+        }
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        fence_acc(acc);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        float *acc_s = reinterpret_cast<float *>(smem + ACC_OFF) + g * 64 * ACC_LD;
+        const int fr = 16 * wl + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            *reinterpret_cast<float2 *>(acc_s + fr * ACC_LD + 8 * j + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2 *>(acc_s + (fr + 8) * ACC_LD + 8 * j + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
+    }
+    const int q = 2 * g + (wl & 1), half = wl >> 1, lr = 32 * (wl & 1) + lane;
+    const float *acc_s = reinterpret_cast<const float *>(smem + ACC_OFF) + g * 64 * ACC_LD;
+    const int row = m0 + 32 * q + lane;
+    const float *bias = ga.bias[grp];
+    uint8_t *blk = smem + warp * EPI_BLOCK;
+    float *stg = reinterpret_cast<float *>(blk);
+    float *sbias = reinterpret_cast<float *>(blk + EPI_BIAS);
+#pragma unroll 1
+    for (int c = half * (BN / 64); c < (half + 1) * (BN / 64); ++c) {
+        float v[32];
+        load_acc_row(acc_s, lr, c * 32, v);
+        const int nb = n0 + c * 32;
+        __syncwarp();
+        sbias[lane] = (bias && nb + lane < N) ? __ldg(bias + nb + lane) : 0.f;
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = (row < row_end && nb + j < N) ? v[j] + sbias[j] : 0.f;
+        if (act == UHC_ACT_GELU) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = gelu_fast(v[j]);
+        } else if (act != UHC_ACT_NONE) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = (row < row_end && nb + j < N) ? act_f(v[j], act) : 0.f;
+        }
+        if (yf) stage_store(stg, yf, v, m0 + 32 * q, nb, row_end, N, lane, false);
+        if (ybf && nb < ldy && row < row_end) {       // ldy is a multiple of 8 and nb of 32: a chunk below ldy is whole or ends at ldy
+            if (nb + 32 <= ldy) {
+                uint4 *dst = (uint4 *)(ybf + (size_t)row * ldy + nb);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    __nv_bfloat162 p0 = __floats2bfloat162_rn(v[8 * j], v[8 * j + 1]), p1 = __floats2bfloat162_rn(v[8 * j + 2], v[8 * j + 3]);
+                    __nv_bfloat162 p2 = __floats2bfloat162_rn(v[8 * j + 4], v[8 * j + 5]), p3 = __floats2bfloat162_rn(v[8 * j + 6], v[8 * j + 7]);
+                    uint4 u; u.x = *(uint32_t *)&p0; u.y = *(uint32_t *)&p1; u.z = *(uint32_t *)&p2; u.w = *(uint32_t *)&p3;
+                    dst[j] = u;
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) if (nb + j < ldy) ybf[(size_t)row * ldy + nb + j] = __float2bfloat16_rn(v[j]);
+            }
+        }
+    }
+}
 
 __global__ void k_f32_to_bf16_padded(const float *__restrict__ x, __nv_bfloat16 *__restrict__ y, int M, int K, int Kp) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)M * Kp; i += (size_t)gridDim.x * blockDim.x) {
@@ -635,6 +755,38 @@ int uhc_linear_forward_tc_f32_pitched(const void *x_bf16, const void *W_bf16, fl
     return linear_tc_impl(x_bf16, W_bf16, nullptr, nullptr, y_f32, nullptr, M, N, Kp, 0, UHC_ACT_NONE, stream, nullptr, 0, ld_y);
 }
 int uhc_tc_tma_store_enabled(void) { return tma_store_enabled() ? 1 : 0; }
+/* G weight sets in one launch: rows [row0[g], row0[g] + rows[g]) of x are multiplied by W[g] (+ b[g]) and written to the same rows of y;
+ * every other row of y is left as it was.  One launch per layer for several policies side by side (uhc_eval_run_groups). */
+int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_host, const void *x_bf16, const void *const *W_bf16_host,
+                                  const float *const *b_host_or_null, void *y_bf16_or_null, float *y_f32_or_null, int M, int N, int Kp, int ldy_bf16,
+                                  int act, void *stream) {
+    if (!x_bf16 || !W_bf16_host || (!y_bf16_or_null && !y_f32_or_null)) { g_tc_err = "uhc_linear_forward_tc_grouped: null argument"; return -2; }
+    if (Kp % BK != 0 || Kp <= 0 || M <= 0 || N <= 0) { g_tc_err = "uhc_linear_forward_tc_grouped: M, N > 0 and Kp a positive multiple of 64"; return -2; }
+    if (y_bf16_or_null && (ldy_bf16 % 8 != 0 || ldy_bf16 < N)) { g_tc_err = "uhc_linear_forward_tc_grouped: ldy must be a multiple of 8 and >= N"; return -2; }
+    GroupedArgs ga;
+    memset(&ga, 0, sizeof ga);
+    if (uhc::grp::plan_tiles(G, row0_host, rows_host, M, &ga.plan)) {
+        g_tc_err = "uhc_linear_forward_tc_grouped: groups must be 1..64 ascending, disjoint, non-empty row ranges inside [0, M)"; return -2;
+    }
+    for (int g = 0; g < G; g++) if (!W_bf16_host[g]) { g_tc_err = "uhc_linear_forward_tc_grouped: null weights"; return -2; }
+    int dev = 0; cudaGetDevice(&dev);
+    static bool attr_set[64] = {false};
+    if (!(dev >= 0 && dev < 64 && attr_set[dev])) {
+        if (cudaFuncSetAttribute(k_linear_tc_grouped, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { g_tc_err = "cudaFuncSetAttribute failed"; return -1; }
+        if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    }
+    CUtensorMap ma;
+    if (make_map(&ma, x_bf16, M, Kp, BM)) return -1;
+    for (int g = 0; g < G; g++) {
+        if (make_map(&ga.mapB[g], W_bf16_host[g], N, Kp, BN)) return -1;
+        ga.bias[g] = b_host_or_null ? b_host_or_null[g] : nullptr;
+    }
+    dim3 grid((N + BN - 1) / BN, ga.plan.tile0[G], 1);
+    k_linear_tc_grouped<<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(ma, ga, (__nv_bfloat16 *)y_bf16_or_null, y_f32_or_null, N, Kp, ldy_bf16, act);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { g_tc_err = cudaGetErrorString(e); return -1; }
+    return 0;
+}
 /* backward through one Linear + the previous layer's activation in ONE kernel:  dz_prev = (dz W) * act'(z_prev)  as bf16 [M][ld_dz] and transposed [K][ld_dzT],
  * db_prev[k] += sum_m dz_prev[m][k].  dz [M][Np] and WT [K][Np] are the K-major bf16 operands (Np = N rounded up to 64).  Needs the TMA-store path, K % 4 == 0
  * and 16-byte aligned buffers (returns -2 otherwise: run uhc_linear_forward_tc + uhc_dact_bf16 instead). */

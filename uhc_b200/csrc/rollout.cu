@@ -20,6 +20,7 @@
 #include "../../include/uhc_nn.h"
 #include "../../include/uhc_rollout.h"
 #include "eval_glue.h"
+#include "group_core.h"
 
 static thread_local std::string g_ro_err;
 #define CKR(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_ro_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
@@ -52,6 +53,29 @@ __global__ void k_zfilter_apply_bf16(const float *__restrict__ X, float *__restr
             if (Y) Y[r * D + j] = y;
         }
         // round-to-nearest-even bf16 (what __float2bfloat16_rn does)
+        unsigned u = __float_as_uint(y);
+        unsigned short b = (y != y) ? 0x7FFF : (unsigned short)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+        Yb[i] = b;
+    }
+}
+// the same with one ZFilter per group of rows (the grouped evaluation: several checkpoints side by side): rows [row0[g], row0[g + 1])
+// are normalised by stats[g], with k_zfilter_apply_bf16's arithmetic
+struct ZGroups { const double *stats[uhc::grp::MAX_GROUPS]; int row0[uhc::grp::MAX_GROUPS + 1]; int G; };
+__global__ void k_zfilter_apply_bf16_grouped(const float *__restrict__ X, float *__restrict__ Y, unsigned short *__restrict__ Yb, int M, int D, int Kp,
+                                             const __grid_constant__ ZGroups zg, float clip) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)M * Kp; i += (size_t)gridDim.x * blockDim.x) {
+        const int j = (int)(i % Kp); const size_t r = i / Kp;
+        int lo = 0, hi = zg.G - 1;                 // the last group starting at or before row r
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if ((size_t)zg.row0[mid] <= r) lo = mid; else hi = mid - 1; }
+        const double *stats = zg.stats[lo];
+        const double n = stats[0];
+        float y = 0.f;
+        if (j < D) {
+            const double mean = stats[1 + j], var = n > 1.0 ? stats[1 + D + j] / (n - 1.0) : mean * mean;
+            y = (float)(((double)X[r * D + j] - mean) / (sqrt(var) + 1e-8));
+            if (clip > 0.f) y = fminf(fmaxf(y, -clip), clip);
+            if (Y) Y[r * D + j] = y;
+        }
         unsigned u = __float_as_uint(y);
         unsigned short b = (y != y) ? 0x7FFF : (unsigned short)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
         Yb[i] = b;
@@ -412,6 +436,161 @@ int policy_enqueue(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, const flo
     const cudaError_t ce = cudaGetLastError();
     if (ce != cudaSuccess) { *err = std::string("k_gauss_sample_dev: ") + cudaGetErrorString(ce); return -1; }
     return 0;
+}
+
+// ---- the grouped policy forward of uhc_eval_run_groups: G policies of one architecture over consecutive row ranges, with scratch of its
+// own (the rollout's ns[] / d_mean pointers are baked into its graphs and the single-policy evaluation's)
+namespace {
+struct GroupCtx {
+    UhcEngine *eng = nullptr; int E = 0;
+    RolloutCtx::NetScratch ns[UHC_MCP_MAX_PRIM + 1];
+    float *d_mean = nullptr; int mean_cap = 0;
+    float *d_xall = nullptr, *d_comp = nullptr; size_t xall_cap = 0;
+    float *d_log_std0 = nullptr; int ls_cap = 0;   // zeros: with the all-ones mask k_gauss_sample_dev then writes mean + 1 * 0, what any finite log_std gives
+    unsigned long long *d_step = nullptr;          // read (not used) by the deterministic sampler
+    unsigned long long gen = 0;                    // bumped whenever the scratch above is reallocated
+};
+std::vector<GroupCtx *> g_gctx;
+
+GroupCtx *gctx_of(UhcEngine *e) {
+    for (GroupCtx *c : g_gctx) if (c->eng == e) return c;
+    GroupCtx *c = new GroupCtx(); c->eng = e; c->E = uhc_num_envs(e);
+    g_gctx.push_back(c);
+    return c;
+}
+
+// the checks ensure_scratch makes, without allocating
+int check_policy(const Policy *pol) {
+    const int P = pol->nprim, nnets = P > 0 ? P + 1 : 1;
+    const UhcMlp *m0 = &pol->nets[0];
+    for (int j = 0; j < nnets; j++) {
+        const UhcMlp *m = &pol->nets[j];
+        if (m->nlayers < 1 || m->nlayers > 8) { g_ro_err = "UhcMlp: 1..8 layers"; return -2; }
+        if (m->dims[0] != m0->dims[0]) { g_ro_err = "UhcMcp: every net reads the same observation"; return -2; }
+        if (j < P && m->dims[m->nlayers] != m0->dims[m0->nlayers]) { g_ro_err = "UhcMcp: the primitives must share the action width"; return -2; }
+        if (P > 0 && j == P && m->dims[m->nlayers] != P) { g_ro_err = "UhcMcp: the composer's output width must be the number of primitives"; return -2; }
+        for (int i = 0; i < m->nlayers; i++) {
+            if (m->kp[i] != pad64(m->dims[i])) { g_ro_err = "UhcMlp: kp[i] must be dims[i] rounded up to 64"; return -2; }
+            if (!m->W_bf16[i]) { g_ro_err = "UhcMlp: null weights"; return -2; }
+        }
+    }
+    return 0;
+}
+// every group's policy must have group 0's architecture: primitive count, and per net the layer count, activation, widths and K padding
+bool same_arch(const Policy *a, const Policy *b) {
+    if (a->nprim != b->nprim) return false;
+    for (int j = 0; j < (a->nprim > 0 ? a->nprim + 1 : 1); j++) {
+        const UhcMlp &x = a->nets[j], &y = b->nets[j];
+        if (x.nlayers != y.nlayers || x.act != y.act) return false;
+        for (int i = 0; i <= x.nlayers; i++) if (x.dims[i] != y.dims[i]) return false;
+        for (int i = 0; i < x.nlayers; i++) if (x.kp[i] != y.kp[i]) return false;
+    }
+    return true;
+}
+int make_group_policies(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, std::vector<Policy> *pols) {
+    const char *who = mcps ? "uhc_eval_run_groups_mcp" : "uhc_eval_run_groups";
+    pols->resize(G);
+    for (int g = 0; g < G; g++) {
+        if (make_policy(&(*pols)[g], mlps ? mlps + g : nullptr, mcps ? mcps + g : nullptr, e, who)) return -2;
+        if (check_policy(&(*pols)[g])) { g_ro_err = std::string(who) + ": " + g_ro_err; return -2; }
+        if (g > 0 && !same_arch(&(*pols)[0], &(*pols)[g])) { g_ro_err = std::string(who) + ": every group's policy must have the same layer widths, K padding, activation and primitive count"; return -2; }
+    }
+    return 0;
+}
+int ensure_group_scratch(GroupCtx *c, const Policy *pol) {
+    const size_t E = c->E;
+    const int P = pol->nprim;
+    const UhcMlp *m0 = &pol->nets[0];
+    const int A = m0->dims[m0->nlayers];
+    if (!c->d_step) { CKR(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); CKR(cudaMemset(c->d_step, 0, sizeof(unsigned long long))); }
+    for (int j = 0; j < (P > 0 ? P + 1 : 1); j++) {
+        const UhcMlp *m = &pol->nets[j];
+        for (int i = 0; i < m->nlayers; i++) {
+            if (i == 0 && j > 0) continue;       // the normalised observation feeds every net
+            const int ld = m->kp[i];
+            if (c->ns[j].ld[i] != ld) {
+                if (c->ns[j].acts[i]) cudaFree(c->ns[j].acts[i]);
+                CKR(cudaMalloc(&c->ns[j].acts[i], E * ld * 2)); CKR(cudaMemset(c->ns[j].acts[i], 0, E * ld * 2));
+                c->ns[j].ld[i] = ld; c->gen++;
+            }
+        }
+    }
+    if (c->mean_cap < A) {
+        if (c->d_mean) cudaFree(c->d_mean);
+        if (c->d_log_std0) cudaFree(c->d_log_std0);
+        CKR(cudaMalloc((void **)&c->d_mean, E * A * 4)); CKR(cudaMemset(c->d_mean, 0, E * A * 4));
+        CKR(cudaMalloc((void **)&c->d_log_std0, A * 4)); CKR(cudaMemset(c->d_log_std0, 0, A * 4));
+        c->mean_cap = A; c->gen++;
+    }
+    if (P > 0 && c->xall_cap < (size_t)P * E * A) {
+        if (c->d_xall) cudaFree(c->d_xall);
+        if (c->d_comp) cudaFree(c->d_comp);
+        CKR(cudaMalloc((void **)&c->d_xall, (size_t)P * E * A * 4)); CKR(cudaMemset(c->d_xall, 0, (size_t)P * E * A * 4));
+        CKR(cudaMalloc((void **)&c->d_comp, E * UHC_MCP_MAX_PRIM * 4)); CKR(cudaMemset(c->d_comp, 0, E * UHC_MCP_MAX_PRIM * 4));
+        c->xall_cap = (size_t)P * E * A; c->gen++;
+    }
+    return 0;
+}
+}  // namespace
+
+int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, unsigned long long *gen, std::string *err) {
+    std::vector<Policy> pols;
+    if (make_group_policies(e, G, mlps, mcps, &pols)) { *err = g_ro_err; return -2; }
+    GroupCtx *c = gctx_of(e);
+    const int rc = ensure_group_scratch(c, &pols[0]);
+    if (rc) { *err = g_ro_err; return rc; }
+    *gen = c->gen;
+    return 0;
+}
+
+int groups_enqueue(UhcEngine *e, int G, const int *row0, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats, float zclip, const float *obs,
+                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err) {
+    std::vector<Policy> pols;
+    if (make_group_policies(e, G, mlps, mcps, &pols)) { *err = g_ro_err; return -2; }
+    GroupCtx *c = gctx_of(e);
+    const Policy &p0 = pols[0];
+    const UhcMlp *m0 = &p0.nets[0];
+    const int E = c->E, D = m0->dims[0], P = p0.nprim, A = m0->dims[m0->nlayers], ntot = row0[G];
+    ZGroups zg;
+    memset(&zg, 0, sizeof zg);
+    zg.G = G;
+    std::vector<int> rows(G);
+    for (int g = 0; g <= G; g++) zg.row0[g] = row0[g];
+    for (int g = 0; g < G; g++) { zg.stats[g] = zstats[g]; rows[g] = row0[g + 1] - row0[g]; }
+    k_zfilter_apply_bf16_grouped<<<1056, 256, 0, st>>>(obs, nullptr, (unsigned short *)c->ns[0].acts[0], ntot, D, m0->kp[0], zg, zclip);
+    cudaError_t ce = cudaGetLastError();
+    if (ce != cudaSuccess) { *err = std::string("k_zfilter_apply_bf16_grouped: ") + cudaGetErrorString(ce); return -1; }
+    std::vector<const void *> W(G);
+    std::vector<const float *> b(G);
+    for (int j = 0; j < (P > 0 ? P + 1 : 1); j++) {
+        const UhcMlp *m = &p0.nets[j];
+        const bool composer = P > 0 && j == P;
+        float *out = P == 0 ? c->d_mean : (composer ? c->d_comp : c->d_xall + (size_t)j * E * A);
+        for (int i = 0; i < m->nlayers; i++) {
+            const bool last = i == m->nlayers - 1;
+            const void *in = i == 0 ? c->ns[0].acts[0] : c->ns[j].acts[i];
+            for (int g = 0; g < G; g++) { W[g] = pols[g].nets[j].W_bf16[i]; b[g] = pols[g].nets[j].bias[i]; }
+            if (uhc_linear_forward_tc_grouped(G, row0, rows.data(), in, W.data(), b.data(), last ? nullptr : c->ns[j].acts[i + 1], last ? out : nullptr, E,
+                                              m->dims[i + 1], m->kp[i], last ? 0 : c->ns[j].ld[i + 1], (last && !composer) ? UHC_ACT_NONE : m->act, st)) {
+                *err = std::string("grouped policy GEMM: ") + uhc_tc_last_error(); return -1;
+            }
+        }
+    }
+    // the mixture head is row-wise: run over every row (rows past the groups hold zeros or earlier values and are never read)
+    if (P > 0 && uhc_mcp_combine(c->d_xall, c->d_comp, nullptr, c->d_mean, E, A, P, st)) { *err = std::string("mixture head: ") + uhc_nn_last_error(); return -1; }
+    k_gauss_sample_dev<<<(ntot + 7) / 8, 256, 0, st>>>(c->d_mean, c->d_log_std0, mean_action, action, nullptr, ntot, A, 0, c->d_step);
+    ce = cudaGetLastError();
+    if (ce != cudaSuccess) { *err = std::string("k_gauss_sample_dev: ") + cudaGetErrorString(ce); return -1; }
+    return 0;
+}
+
+void groups_release(UhcEngine *e) {
+    for (size_t i = 0; i < g_gctx.size(); i++) if (g_gctx[i]->eng == e) {
+        GroupCtx *c = g_gctx[i];
+        for (auto &nsj : c->ns) for (void *p : nsj.acts) if (p) cudaFree(p);
+        for (void *p : {(void *)c->d_mean, (void *)c->d_xall, (void *)c->d_comp, (void *)c->d_log_std0, (void *)c->d_step}) if (p) cudaFree(p);
+        delete c; g_gctx.erase(g_gctx.begin() + i); return;
+    }
 }
 
 }  // namespace evalx

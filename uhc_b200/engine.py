@@ -336,6 +336,41 @@ class Engine:
                     fail_any=np.array([bool(r.fail_any) for r in rec][:n]), reward_sum=np.array([r.reward_sum for r in rec][:n]),
                     states=states.numpy()[:n] if states is not None else None)
 
+    def eval_run_groups(self, groups, zclip=5.0, fail_safe=False, window=32, record_states=False):
+        """several policies of one architecture in one device evaluation (uhc_eval_run_groups): groups = [(clips, policy, zfilter_stats)], group g
+        on the envs after those of groups 0 .. g-1.  Returns one eval_run dict per group, bit-identical to eval_run(clips, policy, ...) of that
+        group alone (any finite log_std)."""
+        t = self.torch
+        from .nn import UhcMcp, UhcMlp
+        G = len(groups)
+        clips = [np.ascontiguousarray(c, dtype=np.int32).reshape(-1) for c, _, _ in groups]
+        sizes = np.array([len(c) for c in clips], np.int32)
+        allc = np.concatenate(clips) if G else np.zeros(0, np.int32)
+        n = int(sizes.sum())
+        ok = 0 < n <= self.E and self.clip_len is not None and ((allc >= 0) & (allc < len(self.clip_len))).all()
+        T = int(self.clip_len[allc].max()) - 1 if ok else 1
+        frames = t.empty((max(n, 1), T, 6), dtype=t.float64, pin_memory=True)
+        states = t.empty((max(n, 1), T, 148), dtype=t.float64, pin_memory=True) if record_states else None
+        rec = (UhcEvalClip * max(n, 1))()
+        mcp = G > 0 and isinstance(groups[0][1], UhcMcp)
+        pols = ((UhcMcp if mcp else UhcMlp) * max(G, 1))(*[p for _, p, _ in groups])
+        zs = (C.c_void_p * max(G, 1))(*[z.data_ptr() for _, _, z in groups])
+        fn = self.lib.uhc_eval_run_groups_mcp if mcp else self.lib.uhc_eval_run_groups
+        rc = fn(self.h, C.c_int(G), _ip(sizes), _ip(allc), pols, zs, C.c_float(zclip), C.c_int(int(bool(fail_safe))), C.c_int(int(window)),
+                C.c_void_p(frames.data_ptr()), rec, C.c_void_p(states.data_ptr() if states is not None else None), self._stream())
+        if rc != 0:
+            self.lib.uhc_eval_last_error.restype = C.c_char_p
+            raise (ValueError if rc == -2 else RuntimeError)("uhc_eval_run_groups: " + self.lib.uhc_eval_last_error().decode())
+        fr, st = frames.numpy(), states.numpy() if states is not None else None
+        out, o = [], 0
+        for k in sizes:
+            r = rec[o:o + k]
+            out.append(dict(frames=fr[o:o + k], nframes=np.array([x.frames for x in r]), last_t=np.array([x.last_t for x in r]),
+                            fail_any=np.array([bool(x.fail_any) for x in r]), reward_sum=np.array([x.reward_sum for x in r]),
+                            states=st[o:o + k] if st is not None else None))
+            o += k
+        return out
+
     # ---- the batched physics tracker (include/uhc_track.h uhc_track_*)
     def _trk_chk(self, rc, who):
         if rc != 0:
