@@ -32,6 +32,17 @@ typedef struct {
 #define UHC_EVAL_NCOL 6
 /* states_host columns: the recorded qpos (76) and world body positions xpos (72) of every frame, as doubles */
 #define UHC_EVAL_STATE 148
+/* smpl_host columns: the recorded qpos as SMPL (include/uhc_export.h uhc_qpos_to_smpl), pose 72 (axis-angle, SMPL_BONE_ORDER_NAMES order)
+ * then trans 3, as doubles */
+#define UHC_EVAL_SMPL 75
+
+/* the outputs of one evaluation call (the _ex entry points) */
+typedef struct {
+    double *frames_host;           /* [n][max(len) - 1][UHC_EVAL_NCOL] */
+    UhcEvalClip *clips_host;       /* [n] */
+    double *states_host_or_null;   /* [n][max(len) - 1][UHC_EVAL_STATE] */
+    double *smpl_host_or_null;     /* [n][max(len) - 1][UHC_EVAL_SMPL] */
+} UhcEvalOut;
 
 const char *uhc_eval_last_error(void);
 
@@ -42,7 +53,7 @@ const char *uhc_eval_last_error(void);
  * uhc_env_set_state_batch does.  The steps run as a CUDA graph of `window` steps captured once per argument set and replayed.
  * frames_host = [n][max(len) - 1][UHC_EVAL_NCOL]: rows past an env's `frames` are unspecified.  clips_host = [n].
  * states_host_or_null = [n][max(len) - 1][UHC_EVAL_STATE] (parity tests; NULL costs nothing).  Bad arguments (-2): n < 1 or n > E,
- * a clip index out of range, no clip table loaded, window < 1, a policy whose widths are not the engine's obs / action dims. */
+ * a clip index out of range, no clip table loaded, window < 1 or n * window > INT_MAX, a policy whose widths are not the engine's obs / action dims. */
 int uhc_eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
                  int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
 int uhc_eval_run_mcp(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
@@ -61,6 +72,19 @@ int uhc_eval_run_groups(UhcEngine *e, int G, const int *group_n_host, const int 
                         float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
 int uhc_eval_run_groups_mcp(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
                             float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream);
+/* The four calls above with their outputs in one UhcEvalOut, which adds the SMPL export: with out->smpl_host_or_null set, each recorded frame's
+ * qpos -- the stepped state before any fail_safe re-seat, the state record's qpos -- is converted on the device by uhc_qpos_to_smpl's code with
+ * the shape variant of the env's clip, and row [i][f] of smpl_host equals uhc_qpos_to_smpl of row [i][f] of states_host bit for bit.  Rows past
+ * an env's `frames` are unspecified.  With smpl_host_or_null = NULL each is the call above (the same graph and outputs); the graphs with and
+ * without the export are cached side by side. */
+int uhc_eval_run_ex(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
+                    int fail_safe, int window, const UhcEvalOut *out, void *stream);
+int uhc_eval_run_mcp_ex(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
+                        int fail_safe, int window, const UhcEvalOut *out, void *stream);
+int uhc_eval_run_groups_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
+                           float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream);
+int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
+                               float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream);
 void uhc_eval_release(UhcEngine *e);   /* frees the graphs / scratch of this engine (the grouped path's too); call before uhc_engine_destroy */
 
 #ifdef __cplusplus

@@ -9,6 +9,7 @@ Runs only in the build container (needs /root/reference); the vectors it writes 
   ppo_small.npz         PolicyGaussian / Value / estimate_advantages / AgentPPO.update_policy / ZFilter traces
                         (uhc/khrylib/rl/core/*, uhc/khrylib/rl/agents/agent_ppo.py, khrylib/utils/zfilter.py)
   math_doctest.npz      the known-answer constants in uhc/utils/transformation.py doctests
+  qpos_to_smpl.npz      qpos_to_smpl (uhc/smpllib/smpl_mujoco.py:738-752) on expert, random and singular qpos rows
 """
 import os
 import sys
@@ -442,6 +443,47 @@ def gen_math():
     print("math goldens ok", out["mul_doctest"])
 
 
+def qpos_to_smpl_inputs():
+    """qpos rows for the qpos_to_smpl golden: the golden clips' expert qpos, seeded random poses, hinge pitches at and within 1e-9 of +-pi/2,
+    root quaternions with w < 0, w ~ 0 (angle ~ pi) and rotation angles below 1e-3 (as_rotvec's series)"""
+    g = os.path.join(H.ROOT, "tests", "golden")
+    rows = [np.load(os.path.join(g, f"expert_{t}.npz"))["qpos"] for t in ("sway", "kick")]
+    rng = np.random.RandomState(21)
+    q = np.zeros((64, 76))
+    q[:, :3] = rng.normal(0, 0.5, (64, 3)) + [0, 0, 0.9]
+    q[:, 3:7] = rng.normal(size=(64, 4))
+    q[:, 3:7] /= np.linalg.norm(q[:, 3:7], axis=1, keepdims=True)
+    q[:, 7:] = rng.uniform(-np.pi, np.pi, (64, 69))
+    rows.append(q)
+    s = q[:40].copy()
+    pitch = np.array([np.pi / 2, -np.pi / 2, np.pi / 2 - 1e-9, np.pi / 2 + 1e-9, -np.pi / 2 + 1e-9, -np.pi / 2 - 1e-9, np.pi / 2 - 4e-10, -np.pi / 2 + 7e-10])
+    for i in range(40):
+        s[i, 8::3] = np.roll(pitch, i)[np.arange(23) % 8]                         # every hinge's middle (y) angle
+    s[:8, 3:7] = -np.abs(s[:8, 3:7])                                               # w < 0 (and every component negative)
+    s[8:16, 3] = rng.choice([0.0, 1e-12, -1e-12, 3e-9], 8)                         # w ~ 0: angle ~ pi
+    ax = rng.normal(size=(16, 3))
+    ax /= np.linalg.norm(ax, axis=1, keepdims=True)
+    ang = np.concatenate([[0.0, 1e-12, 1e-8, 1e-5], np.linspace(2e-4, 9.99e-4, 8), [1e-3, 1.0001e-3, 1.2e-3, 5e-3]])
+    sgn = np.where(np.arange(16) % 2, 1.0, -1.0)[:, None]                          # half of them with w < 0
+    s[16:32, 3:7] = sgn * np.concatenate([np.cos(ang / 2)[:, None], np.sin(ang / 2)[:, None] * ax], 1)
+    s[32:40, 3:7] *= rng.uniform(0.5, 2.0, (8, 1))                                 # not normalised: from_quat divides by the norm
+    s[16:32, 7:] *= 1e-4                                                           # small hinge rotations too
+    rows.append(s)
+    return np.concatenate(rows)
+
+
+def gen_qpos_to_smpl():
+    """qpos_to_smpl.npz: the reference's qpos_to_smpl (uhc/smpllib/smpl_mujoco.py:738-752, scipy Rotation) on qpos_to_smpl_inputs(), with the
+    fake mujoco_py model of tools/ref_harness.py (body_pos[1] = the root offset)"""
+    from uhc.smpllib.smpl_mujoco import qpos_to_smpl
+    qpos = qpos_to_smpl_inputs()
+    model = H.FakeModel(H.O.Model())
+    pose, trans = qpos_to_smpl(qpos, model)
+    np.savez_compressed(os.path.join(OUT, "qpos_to_smpl.npz"), qpos=qpos, pose=pose.reshape(len(qpos), 72), trans=trans,
+                        root_offset=np.asarray(model.body_pos[1]))
+    print("qpos_to_smpl golden:", qpos.shape, np.abs(pose).max())
+
+
 YAML_KEYS = ("agent_name", "obs_v", "actor_type", "reward_id", "fix_std", "residual_force", "obs_vel", "obs_coord", "obs_phase", "has_shape", "env_term_body",
              "residual_force_mode", "residual_force_bodies", "residual_force_torque", "residual_force_bodies_num", "residual_contact_only",
              "residual_contact_projection", "env_init_noise")
@@ -551,6 +593,8 @@ def main():
         gen_yaml_keys()
     if "zfilter" in what:
         gen_zfilter_pickle()
+    if "gen_qpos_to_smpl" in what or "qpos_to_smpl" in what:
+        gen_qpos_to_smpl()
 
 
 if __name__ == "__main__":

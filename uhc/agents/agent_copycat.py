@@ -272,6 +272,7 @@ class AgentCopycat:
         from uhc_b200.metrics import compute_metrics, metrics_from_frames
         cfg = self.cfg
         on_device = bool(cfg.get("eval_on_device", False))     # opt-in: BatchedAgent.evaluate (uhc_eval_run) instead of the host loop below
+        motion = dump and bool(cfg.get("eval_dump_motion", False))   # opt-in: the dump also holds eval_seq's trajectories + SMPL per clip
         res_dicts = []
         eng = self.agent.engine
         E = self.num_envs
@@ -289,11 +290,16 @@ class AgentCopycat:
                 clips = (c0 + ids).astype(np.int32)
                 lens = eng.clip_len[clips]
                 if on_device:                                      # the same roll-out as the loop below, as CUDA-graph replays with the metrics on the device
-                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32)
+                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, **(dict(record_states=True, export_smpl=True) if motion else {}))
                     last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
                     rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
                     self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec,
                                        lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs), pending)
+                    if motion:
+                        for i in ids:
+                            d = dev[i]
+                            self._add_motion(res[loader.data_keys[c0 + i]], loader, int(clips[i]), d["states"][:, :76], d["states"][:, 76:148],
+                                             d["pose_aa"], d["trans"], np.arange(1, len(d["frames"]) + 1), bool(d["fail_any"]))
                     continue
                 if len(ids) < E:                                   # idle envs: park them on clip c0 so every record is valid (their outputs are ignored)
                     eng.reset(np.arange(len(ids), E, dtype=np.int32), np.full(E - len(ids), c0, np.int32), 0, None)
@@ -341,6 +347,12 @@ class AgentCopycat:
                     return compute_metrics({"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
                                             "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": pct, "fail_safe": fs})
                 self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics, pending)
+                if motion:                          # the host loop's recorded qpos as SMPL through the device conversion
+                    for i in ids:
+                        pred = np.array(traj[i]["pred"]).reshape(-1, 76)
+                        pose, trans = eng.qpos_to_smpl(pred)
+                        self._add_motion(res[loader.data_keys[c0 + i]], loader, int(clips[i]), pred, np.array(traj[i]["pred_jpos"]).reshape(-1, 72),
+                                         pose.cpu().numpy(), trans.cpu().numpy(), np.array(traj[i]["t"], np.int64), bool(fail_any[i]), expert(i))
             if loader is not self.data_loader:
                 self._load_tables(self.data_loader)
                 if saved is not None:          # a table of another clip count disabled the device curriculum: restore it
@@ -407,6 +419,51 @@ class AgentCopycat:
                     res[loader.data_keys[i]] = self._clip_result(lens[i], last_t[i], fail_any[i], rsum[i], len(dev[i]["frames"]),
                                                                  lambda pct, fs, d=dev[i]: metrics_from_frames(d["frames"], pct, fs))
                 out[epoch].append(self._coverage(loader, res, epoch, dump))
+        if not self.curriculum_on_device:
+            self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
+        return out
+
+    def _add_motion(self, r, loader, clip, pred, pred_jpos, pose_aa, trans, t, fail_any, gt=None):
+        """eval_seq's trajectory keys (gt / pred qpos, gt_jpos / pred_jpos world joint positions, fail_safe) and the SMPL pose / trans of one
+        clip's recorded frames into its result dict r; t = cur_t after each recorded step (the expert frame min(t, len - 1) it is compared with)"""
+        if gt is None:
+            gt = self.agent.engine.clip_frames(clip) if self._device_tables(loader) else loader.experts[clip]
+        tt = np.minimum(np.asarray(t, np.int64), int(self.agent.engine.clip_len[clip]) - 1)
+        r.update(gt=np.asarray(gt["qpos"])[tt], pred=np.array(pred), gt_jpos=np.asarray(gt["wbpos"])[tt].reshape(len(tt), -1), pred_jpos=np.array(pred_jpos),
+                 pose_aa=np.array(pose_aa), trans=np.array(trans), fail_safe=bool(fail_any and self.cfg.fail_safe))
+
+    def export_motion(self, epoch=0, loaders=None, dump=True):
+        """the simulated motion of every clip of the test loaders (or `loaders`), from the device evaluation (BatchedAgent.export_motion):
+        {loader name: {key: eval_seq's dict (gt, pred, gt_jpos, pred_jpos, percent, fail_safe, reward and compute_metrics' keys with succ) plus
+        pose_aa [frames][72] and trans [frames][3]}}; with dump each loader's dict goes to {epoch}_{loader}_motion.pkl.  Like eval_checkpoints
+        it is not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored."""
+        from uhc_b200.metrics import metrics_from_frames
+        cfg, eng = self.cfg, self.agent.engine
+        out = {}
+        for loader in (self.test_data_loaders if loaders is None else loaders):
+            n = loader.get_len()
+            saved = None
+            if loader is not self.data_loader:
+                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+                self._load_tables(loader)
+            eng.set_cfg(**self._env_cfg(test=True))
+            clips = np.arange(n, dtype=np.int32)
+            lens = eng.clip_len[clips].copy()
+            mot = self.agent.export_motion(clips, bool(cfg.fail_safe), window=32)
+            res = {}
+            for i, d in enumerate(mot):
+                r = res[loader.data_keys[i]] = self._clip_result(lens[i], d["last_t"], d["fail_any"], d["reward_sum"], len(d["frames"]),
+                                                                 lambda pct, fs, d=d: metrics_from_frames(d["frames"], pct, fs))
+                self._add_motion(r, loader, i, d["pred"], d["pred_jpos"], d["pose_aa"], d["trans"], np.arange(1, len(d["frames"]) + 1), d["fail_any"])
+            if loader is not self.data_loader:
+                self._load_tables(self.data_loader)
+                if saved is not None:
+                    self._restore_device_curriculum(saved)
+            eng.set_cfg(**self._env_cfg(test=False))
+            self.agent.obs = None
+            if dump:
+                joblib.dump(res, osp.join(cfg.output_dir, f"{epoch}_{loader.name}_motion.pkl"))
+            out[loader.name] = res
         if not self.curriculum_on_device:
             self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
         return out

@@ -15,7 +15,7 @@ import time
 import numpy as np
 
 from . import nn
-from .engine import Engine
+from .engine import EVAL_SMPL, Engine
 from .motion_lib import MotionSet
 
 
@@ -408,22 +408,57 @@ class BatchedAgent:
     def curriculum_set(self, lens, pct, starts):
         self.engine.curriculum_set(lens, pct, starts)
 
-    def evaluate(self, clips, fail_safe, window=32, record_states=False):
+    def evaluate(self, clips, fail_safe, window=32, record_states=False, export_smpl=False):
         """deterministic roll-out of every listed clip from frame 0 on the device (Engine.eval_run, one call per chunk of E clips) under
         the engine's current cfg.  Returns one dict per clip: frames = [nframes][6] per-frame rows (uhc_b200/metrics.py
-        metrics_from_frames), last_t, fail_any, reward_sum (and states = [nframes][148] when record_states)."""
-        mcp = self.actor_type == "mcp"
-        pol = nn.mcp_struct(self.policy) if mcp else nn.mlp_struct(self.policy)
+        metrics_from_frames), last_t, fail_any, reward_sum (and states = [nframes][148] when record_states; pose_aa = [nframes][72] and
+        trans = [nframes][3], the simulated motion as SMPL, when export_smpl)."""
         clips = np.asarray(clips, dtype=np.int32).reshape(-1)
         out = []
         for c0 in range(0, len(clips), self.E):
-            r = self.engine.eval_run(clips[c0:c0 + self.E], pol, self.log_std, self.running_state.stats, self.running_state.clip, fail_safe, window, record_states)
-            for i, nf in enumerate(r["nframes"]):
-                d = dict(frames=r["frames"][i, :nf].copy(), last_t=int(r["last_t"][i]), fail_any=bool(r["fail_any"][i]), reward_sum=float(r["reward_sum"][i]))
-                if record_states:
-                    d["states"] = r["states"][i, :nf].copy()
-                out.append(d)
+            out += self._evaluate_call(clips[c0:c0 + self.E], fail_safe, window, record_states, export_smpl)
         self.obs = None       # every env was reset onto an evaluation clip
+        return out
+
+    def _evaluate_call(self, clips, fail_safe, window, record_states, export_smpl):
+        pol = nn.mcp_struct(self.policy) if self.actor_type == "mcp" else nn.mlp_struct(self.policy)
+        r = self.engine.eval_run(clips, pol, self.log_std, self.running_state.stats, self.running_state.clip, fail_safe, window, record_states, export_smpl)
+        out = []
+        for i, nf in enumerate(r["nframes"]):
+            d = dict(frames=r["frames"][i, :nf].copy(), last_t=int(r["last_t"][i]), fail_any=bool(r["fail_any"][i]), reward_sum=float(r["reward_sum"][i]))
+            if record_states:
+                d["states"] = r["states"][i, :nf].copy()
+            if export_smpl:
+                d["pose_aa"], d["trans"] = r["pose_aa"][i, :nf].copy(), r["trans"][i, :nf].copy()
+            out.append(d)
+        return out
+
+    def export_motion(self, clips, fail_safe, window=32, max_bytes=1 << 30):
+        """the simulated motion of every listed clip, as evaluate() rolls it out: per clip pred = [nframes][76] qpos, pred_jpos = [nframes][72]
+        world body positions, pose_aa = [nframes][72] and trans = [nframes][3] (the qpos as SMPL, uhc_qpos_to_smpl on the device) and evaluate()'s
+        summary (frames, last_t, fail_any, reward_sum), in the caller's order.  Clips of similar length share a device call; a call takes at most
+        E clips and as many as keep its pinned state and SMPL arrays, n * (max(len) - 1) * (148 + 75) * 8 bytes, within max_bytes (a clip that
+        alone needs more runs on its own).  Every env is independent of the others, so a clip's result does not depend on the chunking.  Needs
+        the engine's test-mode cfg (auto_reset off, as eval_policy sets it): with auto_reset an ended env would re-seed itself from the sampler,
+        whose draws depend on the env it runs on."""
+        if self.engine._cfg.auto_reset:
+            raise ValueError("export_motion needs the test-mode cfg: engine.set_cfg(auto_reset=0) first")
+        clips = np.asarray(clips, dtype=np.int32).reshape(-1)
+        per_frame = (148 + EVAL_SMPL) * 8
+        order = np.argsort(self.engine.clip_len[clips], kind="stable")
+        out = [None] * len(clips)
+        k = 0
+        while k < len(clips):
+            m = 1
+            while k + m < len(clips) and m < self.E and (m + 1) * (int(self.engine.clip_len[clips[order[k + m]]]) - 1) * per_frame <= max_bytes:
+                m += 1
+            idx = order[k:k + m]
+            for i, d in zip(idx, self._evaluate_call(clips[idx], fail_safe, window, True, True)):
+                st = d.pop("states")
+                d["pred"], d["pred_jpos"] = st[:, :76], st[:, 76:]
+                out[i] = d
+            k += m
+        self.obs = None
         return out
 
     def _checkpoint_policy(self, k, cp):

@@ -7,6 +7,7 @@
 //   k_env_step                                                                   uhc_env_step under the engine's current (test-mode) cfg
 //   k_eval_frame                                                                 per env still alive: the frame's metrics into a window buffer,
 //                                                                                the reward sum, fail / end, the fail_safe flag
+//   k_eval_export (SMPL export only)                                               per env that recorded a frame: its qpos as SMPL (export.cu)
 //   k_eval_reseat (fail_safe only)                                               uhc_env_set_state_batch's re-seat of the flagged envs
 // `window` steps are captured once per argument set into a CUDA graph; after each replay one 2-D copy moves the window's frame rows
 // into the caller's (pinned) array and one 4-byte copy returns the number of envs still alive, the host loop's early exit.
@@ -14,6 +15,7 @@
 // Compiled on its own with -fmad=false (uhc_b200/build.py) like motion_lib.cu: k_eval_frame restates numpy's fp64 arithmetic
 // (eval_core.h) without contracted multiply-adds.  The policy and physics kernels it replays are compiled with the rest of the library.
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <string.h>
 #include <string>
 #include <vector>
@@ -21,6 +23,8 @@
 #include "eval_core.h"
 #include "eval_glue.h"
 #include "sim_core.h"
+#include "smpl_export_core.h"
+#include "track_glue.h"
 
 using namespace uhc;
 
@@ -86,14 +90,14 @@ __global__ void k_eval_init(int n, UhcEvalClip *__restrict__ clips, int *__restr
 }
 
 struct EvalKey {
-    int n, nrec_max, window, fail_safe, states, nprim; float zclip; unsigned long long scratch_gen, eval_gen, view_gen;
+    int n, nrec_max, window, fail_safe, states, smpl, nprim; float zclip; unsigned long long scratch_gen, eval_gen, view_gen;
     UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; const float *log_std; const double *zstats;
     bool operator==(const EvalKey &o) const { return memcmp(this, &o, sizeof(EvalKey)) == 0; }
 };
 // the grouped evaluation's graphs: G, the group sizes, every group's policy by value and its ZFilter statistics pointer, and the generations
 // of the grouped policy scratch, the window buffers and the engine view
 struct GroupKeyHead {
-    int G, ntot, nrec_max, window, fail_safe, states, nprim; float zclip; unsigned long long group_gen, eval_gen, view_gen;
+    int G, ntot, nrec_max, window, fail_safe, states, smpl, nprim; float zclip; unsigned long long group_gen, eval_gen, view_gen;
 };
 struct GroupKey {
     GroupKeyHead h; std::vector<int> n; std::vector<UhcMlp> nets; std::vector<const double *> zs;
@@ -108,9 +112,11 @@ struct GroupSet { int G; const int *row0; const UhcMlp *mlps; const UhcMcp *mcps
 struct EvalCtx {
     UhcEngine *eng = nullptr;
     int E = 0, n_cap = 0, win_cap = 0, states_cap = 0;
+    size_t smpl_cap = 0;                          // rows (env x slot) of d_wsmpl
     unsigned long long gen = 0;                   // bumped when the scratch below is reallocated
     UhcEvalClip *d_clips = nullptr; int *d_alive = nullptr, *d_reseat = nullptr, *d_count = nullptr; unsigned char *d_ones = nullptr;
     double *d_ring = nullptr, *d_win = nullptr, *d_wstates = nullptr;
+    double *d_wsmpl = nullptr; int *d_xdone = nullptr;   // SMPL export: window rows [n][window][UHC_EVAL_SMPL], frames exported per env
     int *h_count = nullptr;                       // pinned
     cudaEvent_t ev = nullptr;
     std::vector<int> ids, clip0, start, len;      // reset arguments (kept: no allocation in the steady state)
@@ -132,8 +138,9 @@ void drop_graphs(EvalCtx *c) {
     c->ggraphs.clear();
 }
 
-// per-env arrays sized by E once; the window buffers grow with n * window (and the state record with it when requested)
-int ensure(EvalCtx *c, int n, int window, bool states) {
+// per-env arrays sized by E once; the window buffers grow with n * window (and the state record and the SMPL export with it when requested).
+// Called before any capture: a graph holds these pointers, so they never change while one of them can be replayed (gen)
+int ensure(EvalCtx *c, int n, int window, bool states, bool smpl) {
     const size_t E = c->E;
     if (!c->d_clips) {
         CKE(cudaMalloc((void **)&c->d_clips, E * sizeof(UhcEvalClip))); CKE(cudaMalloc((void **)&c->d_alive, E * 4)); CKE(cudaMalloc((void **)&c->d_reseat, E * 4));
@@ -150,11 +157,17 @@ int ensure(EvalCtx *c, int n, int window, bool states) {
         if (c->d_wstates) cudaFree(c->d_wstates);
         CKE(cudaMalloc((void **)&c->d_wstates, (size_t)need * NSTATE * sizeof(double))); c->states_cap = need; c->gen++;
     }
+    if (smpl && (size_t)need > c->smpl_cap) {
+        if (c->d_wsmpl) cudaFree(c->d_wsmpl);
+        c->d_wsmpl = nullptr; c->smpl_cap = 0; c->gen++;
+        CKE(cudaMalloc((void **)&c->d_wsmpl, (size_t)need * UHC_EVAL_SMPL * sizeof(double))); c->smpl_cap = (size_t)need;
+    }
+    if (smpl && !c->d_xdone) { CKE(cudaMalloc((void **)&c->d_xdone, E * sizeof(int))); c->gen++; }
     return 0;
 }
 
 int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
-                   int n, int nrec_max, int fail_safe, int window, bool states, cudaStream_t st, const GroupSet *grp = nullptr) {
+                   int n, int nrec_max, int fail_safe, int window, bool states, bool smpl, cudaStream_t st, const GroupSet *grp = nullptr) {
     std::string err;
     for (int s = 0; s < window; s++) {
         int rc = grp ? evalx::groups_enqueue(c->eng, grp->G, grp->row0, grp->mlps, grp->mcps, grp->zstats, zclip, R.obs, c->d_ones, R.act, st, &err)
@@ -172,6 +185,8 @@ int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, co
                                                                  fail_safe, window, s, c->d_clips, c->d_alive, c->d_reseat, c->d_ring, c->d_win,
                                                                  states ? c->d_wstates : nullptr, last ? c->d_count : nullptr);
         CKE(cudaGetLastError());
+        if (smpl) CKE(smplx::launch_eval_export(R.precision, R.state, R.istate, trackx::clip_models(c->eng), trackx::motion_model(c->eng).body, c->d_clips,
+                                                c->d_xdone, n, window, s, c->d_wsmpl, st));
         if (fail_safe) CKE(evalx::launch_reseat(c->eng, n, c->d_reseat, st));
     }
     return 0;
@@ -195,11 +210,11 @@ int reset_envs(EvalCtx *c, UhcEngine *e, const evalx::EngineRefs &R, int n, cons
 
 // `window` steps captured on a private stream into an instantiated graph
 int capture_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
-                   int n, int nrec_max, int fail_safe, int window, bool states, const GroupSet *grp, cudaGraphExec_t *exec) {
+                   int n, int nrec_max, int fail_safe, int window, bool states, bool smpl, const GroupSet *grp, cudaGraphExec_t *exec) {
     cudaStream_t cs; CKE(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
     cudaGraph_t graph = nullptr;
     CKE(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-    const int rc = enqueue_window(c, R, mlp, mcp, log_std, zstats, zclip, n, nrec_max, fail_safe, window, states, cs, grp);
+    const int rc = enqueue_window(c, R, mlp, mcp, log_std, zstats, zclip, n, nrec_max, fail_safe, window, states, smpl, cs, grp);
     cudaError_t ce = cudaStreamEndCapture(cs, &graph);
     cudaStreamDestroy(cs);
     if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
@@ -211,7 +226,9 @@ int capture_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, co
 }
 
 // replays until every env has stopped or nrec_max steps have run; after each, the window's rows of envs 0..n-1 go to the caller's arrays
-int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host, cudaStream_t st) {
+int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, const UhcEvalOut &o, cudaStream_t st) {
+    double *frames_host = o.frames_host, *states_host = o.states_host_or_null, *smpl_host = o.smpl_host_or_null;
+    if (smpl_host && (!c->d_wsmpl || c->smpl_cap < (size_t)n * (size_t)window)) { g_ev_err = "SMPL export: the window buffer is smaller than n * window rows"; return -1; }
     for (int s0 = 0; s0 < nrec_max; s0 += window) {
         CKE(cudaGraphLaunch(exec, st));
         const int rows = nrec_max - s0 < window ? nrec_max - s0 : window;
@@ -220,23 +237,27 @@ int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, do
         if (states_host)
             CKE(cudaMemcpy2DAsync(states_host + (size_t)s0 * NSTATE, (size_t)nrec_max * NSTATE * sizeof(double), c->d_wstates, (size_t)window * NSTATE * sizeof(double),
                                   (size_t)rows * NSTATE * sizeof(double), n, cudaMemcpyDeviceToHost, st));
+        if (smpl_host)
+            CKE(cudaMemcpy2DAsync(smpl_host + (size_t)s0 * UHC_EVAL_SMPL, (size_t)nrec_max * UHC_EVAL_SMPL * sizeof(double), c->d_wsmpl,
+                                  (size_t)window * UHC_EVAL_SMPL * sizeof(double), (size_t)rows * UHC_EVAL_SMPL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
         CKE(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
         CKE(cudaEventRecord(c->ev, st));
         CKE(cudaEventSynchronize(c->ev));
         if (*c->h_count == 0) break;
     }
-    CKE(cudaMemcpyAsync(clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
+    CKE(cudaMemcpyAsync(o.clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
     CKE(cudaStreamSynchronize(st));
     return 0;
 }
 
 int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats,
-             float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host, void *stream) {
+             float zclip, int fail_safe, int window, const UhcEvalOut &o, void *stream) {
     const char *who = mcp ? "uhc_eval_run_mcp" : "uhc_eval_run";
-    if (!e || !clip_host || (!mlp && !mcp) || !log_std || !zfilter_stats || !frames_host || !clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
+    if (!e || !clip_host || (!mlp && !mcp) || !log_std || !zfilter_stats || !o.frames_host || !o.clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     if (n < 1 || n > R.E) { g_ev_err = std::string(who) + ": n must be 1 .. E"; return -2; }
     if (window < 1) { g_ev_err = std::string(who) + ": window < 1"; return -2; }
+    if ((long long)n * window > INT_MAX) { g_ev_err = std::string(who) + ": n * window exceeds INT_MAX window rows"; return -2; }
     if (R.num_clips <= 0) { g_ev_err = std::string(who) + ": no clips loaded"; return -2; }
     int max_len = 0;
     for (int i = 0; i < n; i++) {
@@ -247,14 +268,15 @@ int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const
     int rc = evalx::policy_prepare(e, mlp, mcp, &sgen, &err);
     if (rc) { g_ev_err = err; return rc; }
     EvalCtx *c = ev_ctx(e);
-    const bool states = states_host != nullptr;
-    if (ensure(c, n, window, states)) return -1;
+    const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr;
+    if (ensure(c, n, window, states, smpl)) return -1;
     cudaStream_t st = (cudaStream_t)stream;
     const int nrec_max = max_len - 1;
     if (reset_envs(c, e, R, n, clip_host, st)) return -1;
+    if (smpl) CKE(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
 
     EvalKey key; memset(&key, 0, sizeof key);
-    key.n = n; key.nrec_max = nrec_max; key.window = window; key.fail_safe = fail_safe ? 1 : 0; key.states = states; key.zclip = zclip;
+    key.n = n; key.nrec_max = nrec_max; key.window = window; key.fail_safe = fail_safe ? 1 : 0; key.states = states; key.smpl = smpl; key.zclip = zclip;
     key.scratch_gen = sgen; key.eval_gen = c->gen; key.view_gen = R.view_gen; key.log_std = log_std; key.zstats = zfilter_stats;
     if (mcp) { key.nprim = mcp->nprim; for (int k = 0; k < mcp->nprim; k++) key.nets[k] = mcp->prim[k]; key.nets[mcp->nprim] = mcp->composer; }
     else key.nets[0] = *mlp;
@@ -269,19 +291,19 @@ int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const
     cudaGraphExec_t exec = nullptr;
     for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
     if (!exec) {
-        rc = capture_window(c, R, mlp, mcp, log_std, (double *)zfilter_stats, zclip, n, nrec_max, key.fail_safe, window, states, nullptr, &exec);
+        rc = capture_window(c, R, mlp, mcp, log_std, (double *)zfilter_stats, zclip, n, nrec_max, key.fail_safe, window, states, smpl, nullptr, &exec);
         if (rc) return rc;
         if (c->graphs.size() >= 32) { cudaGraphExecDestroy(c->graphs.front().second); c->graphs.erase(c->graphs.begin()); }
         c->graphs.emplace_back(key, exec);
     }
-    return replay(c, exec, n, nrec_max, window, frames_host, clips_host, states_host, st);
+    return replay(c, exec, n, nrec_max, window, o, st);
 }
 
 // G policies side by side: group g on envs [off_g, off_g + n_g), the rest as eval_run over the sum of the n_g envs
 int eval_run_groups(UhcEngine *e, int G, const int *group_n, const int *clip_host, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats,
-                    float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host, void *stream) {
+                    float zclip, int fail_safe, int window, const UhcEvalOut &o, void *stream) {
     const char *who = mcps ? "uhc_eval_run_groups_mcp" : "uhc_eval_run_groups";
-    if (!e || !group_n || !clip_host || (!mlps && !mcps) || !zstats || !frames_host || !clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
+    if (!e || !group_n || !clip_host || (!mlps && !mcps) || !zstats || !o.frames_host || !o.clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
     if (G < 1 || G > UHC_EVAL_MAX_GROUPS) { g_ev_err = std::string(who) + ": G must be 1 .. UHC_EVAL_MAX_GROUPS"; return -2; }
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     std::vector<int> row0(G + 1, 0);
@@ -293,6 +315,7 @@ int eval_run_groups(UhcEngine *e, int G, const int *group_n, const int *clip_hos
     }
     const int n = row0[G];
     if (window < 1) { g_ev_err = std::string(who) + ": window < 1"; return -2; }
+    if ((long long)n * window > INT_MAX) { g_ev_err = std::string(who) + ": n * window exceeds INT_MAX window rows"; return -2; }
     if (R.num_clips <= 0) { g_ev_err = std::string(who) + ": no clips loaded"; return -2; }
     int max_len = 0;
     for (int i = 0; i < n; i++) {
@@ -303,16 +326,17 @@ int eval_run_groups(UhcEngine *e, int G, const int *group_n, const int *clip_hos
     int rc = evalx::groups_prepare(e, G, mlps, mcps, &ggen, &err);
     if (rc) { g_ev_err = err; return rc; }
     EvalCtx *c = ev_ctx(e);
-    const bool states = states_host != nullptr;
-    if (ensure(c, n, window, states)) return -1;
+    const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr;
+    if (ensure(c, n, window, states, smpl)) return -1;
     cudaStream_t st = (cudaStream_t)stream;
     const int nrec_max = max_len - 1;
     if (reset_envs(c, e, R, n, clip_host, st)) return -1;
+    if (smpl) CKE(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
     // no policy covers the parked envs: they step with zero actions (the graph writes action rows 0 .. n-1 only)
     if (n < R.E) CKE(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
 
     GroupKey key; memset(&key.h, 0, sizeof key.h);
-    key.h.G = G; key.h.ntot = n; key.h.nrec_max = nrec_max; key.h.window = window; key.h.fail_safe = fail_safe ? 1 : 0; key.h.states = states;
+    key.h.G = G; key.h.ntot = n; key.h.nrec_max = nrec_max; key.h.window = window; key.h.fail_safe = fail_safe ? 1 : 0; key.h.states = states; key.h.smpl = smpl;
     key.h.zclip = zclip; key.h.group_gen = ggen; key.h.eval_gen = c->gen; key.h.view_gen = R.view_gen;
     key.n.assign(group_n, group_n + G); key.zs.assign(zstats, zstats + G);
     for (int g = 0; g < G; g++) {
@@ -329,12 +353,12 @@ int eval_run_groups(UhcEngine *e, int G, const int *group_n, const int *clip_hos
     for (auto &g : c->ggraphs) if (g.first == key) { exec = g.second; break; }
     if (!exec) {
         const GroupSet gs{G, row0.data(), mlps, mcps, zstats};
-        rc = capture_window(c, R, nullptr, nullptr, nullptr, nullptr, zclip, n, nrec_max, key.h.fail_safe, window, states, &gs, &exec);
+        rc = capture_window(c, R, nullptr, nullptr, nullptr, nullptr, zclip, n, nrec_max, key.h.fail_safe, window, states, smpl, &gs, &exec);
         if (rc) return rc;
         if (c->ggraphs.size() >= 16) { cudaGraphExecDestroy(c->ggraphs.front().second); c->ggraphs.erase(c->ggraphs.begin()); }
         c->ggraphs.emplace_back(std::move(key), exec);
     }
-    return replay(c, exec, n, nrec_max, window, frames_host, clips_host, states_host, st);
+    return replay(c, exec, n, nrec_max, window, o, st);
 }
 
 }  // namespace
@@ -343,26 +367,56 @@ extern "C" {
 
 const char *uhc_eval_last_error(void) { return g_ev_err.c_str(); }
 
+static UhcEvalOut eval_out(double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null) {
+    UhcEvalOut o; o.frames_host = frames_host; o.clips_host = clips_host; o.states_host_or_null = states_host_or_null; o.smpl_host_or_null = nullptr;
+    return o;
+}
+
 int uhc_eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
                  int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
-    if (!mlp) { g_ev_err = "uhc_eval_run: null policy"; return -2; }
-    return eval_run(e, n, clip_host, mlp, nullptr, log_std, zfilter_stats, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+    const UhcEvalOut o = eval_out(frames_host, clips_host, states_host_or_null);
+    return uhc_eval_run_ex(e, n, clip_host, mlp, log_std, zfilter_stats, zclip, fail_safe, window, &o, stream);
 }
 int uhc_eval_run_mcp(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
                      int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
-    if (!mcp) { g_ev_err = "uhc_eval_run_mcp: null policy"; return -2; }
-    return eval_run(e, n, clip_host, nullptr, mcp, log_std, zfilter_stats, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+    const UhcEvalOut o = eval_out(frames_host, clips_host, states_host_or_null);
+    return uhc_eval_run_mcp_ex(e, n, clip_host, mcp, log_std, zfilter_stats, zclip, fail_safe, window, &o, stream);
 }
 
 int uhc_eval_run_groups(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
                         float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
-    if (!mlps) { g_ev_err = "uhc_eval_run_groups: null policy"; return -2; }
-    return eval_run_groups(e, G, group_n_host, clip_host, mlps, nullptr, zfilter_stats_host, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+    const UhcEvalOut o = eval_out(frames_host, clips_host, states_host_or_null);
+    return uhc_eval_run_groups_ex(e, G, group_n_host, clip_host, mlps, zfilter_stats_host, zclip, fail_safe, window, &o, stream);
 }
 int uhc_eval_run_groups_mcp(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
                             float zclip, int fail_safe, int window, double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null, void *stream) {
+    const UhcEvalOut o = eval_out(frames_host, clips_host, states_host_or_null);
+    return uhc_eval_run_groups_mcp_ex(e, G, group_n_host, clip_host, mcps, zfilter_stats_host, zclip, fail_safe, window, &o, stream);
+}
+
+int uhc_eval_run_ex(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
+                    int fail_safe, int window, const UhcEvalOut *out, void *stream) {
+    if (!mlp) { g_ev_err = "uhc_eval_run: null policy"; return -2; }
+    if (!out) { g_ev_err = "uhc_eval_run: null output struct"; return -2; }
+    return eval_run(e, n, clip_host, mlp, nullptr, log_std, zfilter_stats, zclip, fail_safe, window, *out, stream);
+}
+int uhc_eval_run_mcp_ex(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
+                        int fail_safe, int window, const UhcEvalOut *out, void *stream) {
+    if (!mcp) { g_ev_err = "uhc_eval_run_mcp: null policy"; return -2; }
+    if (!out) { g_ev_err = "uhc_eval_run_mcp: null output struct"; return -2; }
+    return eval_run(e, n, clip_host, nullptr, mcp, log_std, zfilter_stats, zclip, fail_safe, window, *out, stream);
+}
+int uhc_eval_run_groups_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
+                           float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream) {
+    if (!mlps) { g_ev_err = "uhc_eval_run_groups: null policy"; return -2; }
+    if (!out) { g_ev_err = "uhc_eval_run_groups: null output struct"; return -2; }
+    return eval_run_groups(e, G, group_n_host, clip_host, mlps, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
+}
+int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
+                               float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream) {
     if (!mcps) { g_ev_err = "uhc_eval_run_groups_mcp: null policy"; return -2; }
-    return eval_run_groups(e, G, group_n_host, clip_host, nullptr, mcps, zfilter_stats_host, zclip, fail_safe, window, frames_host, clips_host, states_host_or_null, stream);
+    if (!out) { g_ev_err = "uhc_eval_run_groups_mcp: null output struct"; return -2; }
+    return eval_run_groups(e, G, group_n_host, clip_host, nullptr, mcps, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
 }
 
 void uhc_eval_release(UhcEngine *e) {
@@ -371,7 +425,7 @@ void uhc_eval_release(UhcEngine *e) {
         EvalCtx *c = g_ev[i];
         drop_graphs(c);
         for (void *p : {(void *)c->d_clips, (void *)c->d_alive, (void *)c->d_reseat, (void *)c->d_count, (void *)c->d_ones, (void *)c->d_ring,
-                        (void *)c->d_win, (void *)c->d_wstates}) if (p) cudaFree(p);
+                        (void *)c->d_win, (void *)c->d_wstates, (void *)c->d_wsmpl, (void *)c->d_xdone}) if (p) cudaFree(p);
         if (c->h_count) cudaFreeHost(c->h_count);
         if (c->ev) cudaEventDestroy(c->ev);
         delete c; g_ev.erase(g_ev.begin() + i); return;

@@ -985,6 +985,7 @@ int install_table(UhcEngine *e, int H, const int *fk_model, const double *shape,
 unsigned long long table_gen(const UhcEngine *e) { return e->table_gen; }
 int num_shapes(const UhcEngine *e) { return e->nshape; }
 const motion::MotionModel &motion_model(const UhcEngine *e) { return e->mo_model; }
+const int *clip_models(const UhcEngine *e) { return e->d_clip_model; }
 
 cudaError_t launch_obs(UhcEngine *e, float *obs, cudaStream_t st) {
     const int E = e->E;

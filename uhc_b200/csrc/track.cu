@@ -337,3 +337,8 @@ void uhc_track_end(UhcEngine *e) {
 }
 
 }  // extern "C"
+
+bool uhc::trackx::tracking(UhcEngine *e) {
+    const TrackCtx *c = e ? find_ctx(e) : nullptr;
+    return c && trackx::table_gen(e) == c->table_gen;
+}

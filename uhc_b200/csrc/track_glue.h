@@ -17,6 +17,10 @@ int install_table(UhcEngine *e, int H, const int *fk_model, const double *shape,
 unsigned long long table_gen(const UhcEngine *e);
 int num_shapes(const UhcEngine *e);
 const motion::MotionModel &motion_model(const UhcEngine *e);
+// the shape variant of every loaded clip on the device (uhc_set_clip_models, range-checked there); null while every clip uses variant 0
+const int *clip_models(const UhcEngine *e);
+// track.cu: a tracker (uhc_track_begin) owns the engine's current clip table, so env e follows clip e
+bool tracking(UhcEngine *e);
 // k_track_obs over every env into obs [E][obs_dim]; capturable
 cudaError_t launch_obs(UhcEngine *e, float *obs, cudaStream_t st);
 

@@ -29,6 +29,14 @@ class UhcEvalClip(C.Structure):
     _fields_ = [("frames", C.c_int), ("last_t", C.c_int), ("fail_any", C.c_int), ("reserved", C.c_int), ("reward_sum", C.c_double)]
 
 
+class UhcEvalOut(C.Structure):
+    """include/uhc_eval.h UhcEvalOut"""
+    _fields_ = [("frames_host", C.c_void_p), ("clips_host", C.c_void_p), ("states_host_or_null", C.c_void_p), ("smpl_host_or_null", C.c_void_p)]
+
+
+EVAL_SMPL = 75      # include/uhc_eval.h UHC_EVAL_SMPL: pose 72, trans 3
+
+
 def make_cfg(precision=32, base_rot=(0.7071, 0.7071, 0.0, 0.0), rfc_scale=100.0, rfc_lim=100.0, rfc_rate=1.0, body_diff_thresh=0.5,
              meta_pd=1, env_episode_len=100000, trail_steps=0, w=(0.3, 0.1, 0.45, 0.1, 0.05), k=(2.0, 0.005, 5.0, 100.0, 1.0),
              newton_max_iter=None, newton_tol=None, auto_reset=0, t_min=5, t_max=300, reset_seed=1, reactive_v=0, reactive_rate=0.3,
@@ -311,11 +319,12 @@ class Engine:
         v = np.ascontiguousarray(qvel, np.float64).reshape(len(ids), NV)
         _chk(self.lib.uhc_env_set_state_batch(self.h, C.c_int(len(ids)), _ip(ids), q.ctypes.data_as(C.POINTER(C.c_double)), v.ctypes.data_as(C.POINTER(C.c_double))))
 
-    def eval_run(self, clips, policy, log_std, zfilter_stats, zclip=5.0, fail_safe=False, window=32, record_states=False):
+    def eval_run(self, clips, policy, log_std, zfilter_stats, zclip=5.0, fail_safe=False, window=32, record_states=False, export_smpl=False):
         """device evaluation of up to E clips (uhc_eval_run, include/uhc_eval.h): envs 0..n-1 roll out clips[i] from frame 0 with the mean
         action under the current cfg.  policy: nn.mlp_struct / nn.mcp_struct of the policy; zfilter_stats: the ZFilter's device statistics.
         Returns dict(frames=[n][max(len)-1][6] per-frame rows (rows past `nframes` unspecified), nframes, last_t, fail_any, reward_sum,
-        states=[n][max(len)-1][148] recorded qpos + xpos when record_states, else None)."""
+        states=[n][max(len)-1][148] recorded qpos + xpos when record_states, else None, and with export_smpl pose_aa=[n][max(len)-1][72] and
+        trans=[n][max(len)-1][3], every recorded qpos as SMPL (uhc_eval_run_ex), else None)."""
         t = self.torch
         clips = np.ascontiguousarray(clips, dtype=np.int32).reshape(-1)
         n = len(clips)
@@ -323,23 +332,38 @@ class Engine:
         T = int(self.clip_len[clips].max()) - 1 if ok else 1
         frames = t.empty((max(n, 1), T, 6), dtype=t.float64, pin_memory=True)
         states = t.empty((max(n, 1), T, 148), dtype=t.float64, pin_memory=True) if record_states else None
+        smpl = t.empty((max(n, 1), T, EVAL_SMPL), dtype=t.float64, pin_memory=True) if export_smpl else None
         rec = (UhcEvalClip * max(n, 1))()
+        out = self._eval_out(frames, rec, states, smpl)
         from .nn import UhcMcp
-        fn = self.lib.uhc_eval_run_mcp if isinstance(policy, UhcMcp) else self.lib.uhc_eval_run
+        fn = self.lib.uhc_eval_run_mcp_ex if isinstance(policy, UhcMcp) else self.lib.uhc_eval_run_ex
         rc = fn(self.h, C.c_int(n), _ip(clips), C.byref(policy), C.c_void_p(log_std.data_ptr()), C.c_void_p(zfilter_stats.data_ptr()), C.c_float(zclip),
-                C.c_int(int(bool(fail_safe))), C.c_int(int(window)), C.c_void_p(frames.data_ptr()), rec,
-                C.c_void_p(states.data_ptr() if states is not None else None), self._stream())
+                C.c_int(int(bool(fail_safe))), C.c_int(int(window)), C.byref(out), self._stream())
         if rc != 0:
             self.lib.uhc_eval_last_error.restype = C.c_char_p
             raise (ValueError if rc == -2 else RuntimeError)("uhc_eval_run: " + self.lib.uhc_eval_last_error().decode())
-        return dict(frames=frames.numpy()[:n], nframes=np.array([r.frames for r in rec][:n]), last_t=np.array([r.last_t for r in rec][:n]),
-                    fail_any=np.array([bool(r.fail_any) for r in rec][:n]), reward_sum=np.array([r.reward_sum for r in rec][:n]),
-                    states=states.numpy()[:n] if states is not None else None)
+        return self._eval_result(rec, 0, n, frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None)
 
-    def eval_run_groups(self, groups, zclip=5.0, fail_safe=False, window=32, record_states=False):
+    @staticmethod
+    def _eval_out(frames, rec, states, smpl):
+        o = UhcEvalOut()
+        o.frames_host, o.clips_host = frames.data_ptr(), C.addressof(rec)
+        o.states_host_or_null = states.data_ptr() if states is not None else None
+        o.smpl_host_or_null = smpl.data_ptr() if smpl is not None else None
+        return o
+
+    @staticmethod
+    def _eval_result(rec, o, k, fr, st, sm):
+        r = rec[o:o + k]
+        return dict(frames=fr[o:o + k], nframes=np.array([x.frames for x in r]), last_t=np.array([x.last_t for x in r]),
+                    fail_any=np.array([bool(x.fail_any) for x in r]), reward_sum=np.array([x.reward_sum for x in r]),
+                    states=st[o:o + k] if st is not None else None,
+                    pose_aa=sm[o:o + k, :, :72] if sm is not None else None, trans=sm[o:o + k, :, 72:] if sm is not None else None)
+
+    def eval_run_groups(self, groups, zclip=5.0, fail_safe=False, window=32, record_states=False, export_smpl=False):
         """several policies of one architecture in one device evaluation (uhc_eval_run_groups): groups = [(clips, policy, zfilter_stats)], group g
         on the envs after those of groups 0 .. g-1.  Returns one eval_run dict per group, bit-identical to eval_run(clips, policy, ...) of that
-        group alone (any finite log_std)."""
+        group alone (any finite log_std).  export_smpl: as eval_run's."""
         t = self.torch
         from .nn import UhcMcp, UhcMlp
         G = len(groups)
@@ -351,25 +375,60 @@ class Engine:
         T = int(self.clip_len[allc].max()) - 1 if ok else 1
         frames = t.empty((max(n, 1), T, 6), dtype=t.float64, pin_memory=True)
         states = t.empty((max(n, 1), T, 148), dtype=t.float64, pin_memory=True) if record_states else None
+        smpl = t.empty((max(n, 1), T, EVAL_SMPL), dtype=t.float64, pin_memory=True) if export_smpl else None
         rec = (UhcEvalClip * max(n, 1))()
+        out = self._eval_out(frames, rec, states, smpl)
         mcp = G > 0 and isinstance(groups[0][1], UhcMcp)
         pols = ((UhcMcp if mcp else UhcMlp) * max(G, 1))(*[p for _, p, _ in groups])
         zs = (C.c_void_p * max(G, 1))(*[z.data_ptr() for _, _, z in groups])
-        fn = self.lib.uhc_eval_run_groups_mcp if mcp else self.lib.uhc_eval_run_groups
+        fn = self.lib.uhc_eval_run_groups_mcp_ex if mcp else self.lib.uhc_eval_run_groups_ex
         rc = fn(self.h, C.c_int(G), _ip(sizes), _ip(allc), pols, zs, C.c_float(zclip), C.c_int(int(bool(fail_safe))), C.c_int(int(window)),
-                C.c_void_p(frames.data_ptr()), rec, C.c_void_p(states.data_ptr() if states is not None else None), self._stream())
+                C.byref(out), self._stream())
         if rc != 0:
             self.lib.uhc_eval_last_error.restype = C.c_char_p
             raise (ValueError if rc == -2 else RuntimeError)("uhc_eval_run_groups: " + self.lib.uhc_eval_last_error().decode())
-        fr, st = frames.numpy(), states.numpy() if states is not None else None
-        out, o = [], 0
+        fr, st, sm = frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None
+        res, o = [], 0
         for k in sizes:
-            r = rec[o:o + k]
-            out.append(dict(frames=fr[o:o + k], nframes=np.array([x.frames for x in r]), last_t=np.array([x.last_t for x in r]),
-                            fail_any=np.array([bool(x.fail_any) for x in r]), reward_sum=np.array([x.reward_sum for x in r]),
-                            states=st[o:o + k] if st is not None else None))
-            o += k
-        return out
+            res.append(self._eval_result(rec, o, int(k), fr, st, sm))
+            o += int(k)
+        return res
+
+    # ---- the SMPL export (include/uhc_export.h)
+    def _exp_chk(self, rc, who):
+        if rc != 0:
+            self.lib.uhc_export_last_error.restype = C.c_char_p
+            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_export_last_error().decode())
+
+    def qpos_to_smpl(self, qpos, variants=None):
+        """qpos_to_smpl (uhc/smpllib/smpl_mujoco.py:738-752) on the device (uhc_qpos_to_smpl): qpos = a cuda tensor [n][>= 76] of float32 | float64
+        whose rows are contiguous (its first 76 columns are read, in place) or anything numpy takes (copied to the device as float64); variants =
+        shape variant per row (None: 0), the root offset trans is taken against.  Returns (pose_aa [n][72], trans [n][3]), float64 cuda tensors."""
+        t = self.torch
+        dev = self.obs.device
+        q = qpos if t.is_tensor(qpos) and qpos.is_cuda else t.as_tensor(np.ascontiguousarray(qpos, np.float64), device=dev)
+        if q.dim() != 2 or q.dtype not in (t.float32, t.float64) or q.shape[1] < 76 or q.stride(1) != 1:
+            raise ValueError("qpos_to_smpl: qpos must be [n][>= 76] contiguous rows of float32 | float64")
+        n = q.shape[0]
+        v = None if variants is None else t.as_tensor(np.array(np.broadcast_to(np.asarray(variants, np.int32), (n,))), device=dev)
+        pose, trans = t.empty(n, 72, dtype=t.float64, device=dev), t.empty(n, 3, dtype=t.float64, device=dev)
+        self._exp_chk(self.lib.uhc_qpos_to_smpl(self.h, C.c_void_p(q.data_ptr()), C.c_int(32 if q.dtype == t.float32 else 64), C.c_long(n),
+                                                C.c_long(q.stride(0) if n > 1 else q.shape[1]), C.c_void_p(v.data_ptr() if v is not None else None),
+                                                C.c_void_p(pose.data_ptr()), C.c_void_p(trans.data_ptr()), self._stream()), "uhc_qpos_to_smpl")
+        return pose, trans
+
+    def track_smpl(self, state_out, pose=None, trans=None):
+        """the tracker's state_out [E][223] as SMPL (uhc_track_smpl), env e with the shape variant of uhc_track_begin's fk_models; stream-ordered,
+        no synchronise.  Returns (pose_aa [E][72], trans [E][3]) float64 cuda tensors (written into pose / trans when given)."""
+        t = self.torch
+        dev = self.obs.device
+        pose = t.empty(self.E, 72, dtype=t.float64, device=dev) if pose is None else pose
+        trans = t.empty(self.E, 3, dtype=t.float64, device=dev) if trans is None else trans
+        assert state_out.is_cuda and state_out.is_contiguous() and tuple(state_out.shape) == (self.E, 223)
+        assert state_out.dtype == (t.float32 if self.precision == 32 else t.float64)
+        self._exp_chk(self.lib.uhc_track_smpl(self.h, C.c_void_p(state_out.data_ptr()), C.c_void_p(pose.data_ptr()), C.c_void_p(trans.data_ptr()),
+                                              self._stream()), "uhc_track_smpl")
+        return pose, trans
 
     # ---- the batched physics tracker (include/uhc_track.h uhc_track_*)
     def _trk_chk(self, rc, who):

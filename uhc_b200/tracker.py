@@ -63,6 +63,14 @@ class Tracker:
     def xpos(self):
         return self.state[:, 151:223].reshape(self.E, 24, 3)
 
+    def smpl(self):
+        """the state of the last step as SMPL (qpos_to_smpl on the device, each env with its fk_models shape variant), enqueued on the tracker's
+        stream with no host synchronise.  Returns (pose_aa [E][72], trans [E][3]), float64 tensors overwritten by the next call."""
+        if getattr(self, "_smpl", None) is None:
+            t = self.torch
+            self._smpl = (t.empty(self.E, 72, device=self.state.device, dtype=t.float64), t.empty(self.E, 3, device=self.state.device, dtype=t.float64))
+        return self.engine.track_smpl(self.state, *self._smpl)
+
     def steps(self):
         """control steps each env has taken since its reset (synchronises)"""
         return self.engine.track_state()["steps"]
