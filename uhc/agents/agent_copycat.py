@@ -468,6 +468,43 @@ class AgentCopycat:
             self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
         return out
 
+    def render_motion(self, epoch=0, loaders=None, out_dir=None, size=(1920, 1080)):
+        """CopycatVisualizer's render_video without MuJoCo: every clip of the test loaders (or `loaders`) evaluated on the device and drawn
+        there (BatchedAgent.render_motion), the simulated `pred` beside the expert `gt` as eval_seq pairs them, one mp4 per clip written by
+        write_frames_to_video to {out_dir or cfg.output}/{take_key}_{cfg.id}_{epoch}_0.mp4 (the visualizer's video_path).  The view follows cfg's
+        hide_im / hide_expert / shift_expert / focus as update_pose does.  Returns {loader name: {take_key: path}}; clips of two loaders with
+        the same key share a file name, as in the visualizer, so such loaders want one call each with their own out_dir.  Like export_motion it is
+        not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored."""
+        from uhc.utils.image_utils import write_frames_to_video
+        cfg, eng = self.cfg, self.agent.engine
+        out_dir = out_dir or getattr(cfg, "output", None) or cfg.output_dir
+        os.makedirs(out_dir, exist_ok=True)
+        cam = {k: bool(getattr(cfg, k, False)) for k in ("hide_im", "hide_expert", "focus")}
+        cam["shift_expert"] = 1.0 if getattr(cfg, "shift_expert", False) else 0.0
+        out = {}
+        for loader in (self.test_data_loaders if loaders is None else loaders):
+            saved = None
+            if loader is not self.data_loader:
+                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+                self._load_tables(loader)
+            eng.set_cfg(**self._env_cfg(test=True))
+            paths = {k: osp.join(out_dir, f"{k}_{cfg.id}_{epoch}_0.mp4") for k in loader.data_keys}
+
+            def writer(i, chunks, keys=loader.data_keys, paths=paths):
+                write_frames_to_video((f for ch in chunks for f in ch), paths[keys[i]])
+
+            self.agent.render_motion(np.arange(loader.get_len(), dtype=np.int32), bool(cfg.fail_safe), size, cam, writer=writer)
+            if loader is not self.data_loader:
+                self._load_tables(self.data_loader)
+                if saved is not None:
+                    self._restore_device_curriculum(saved)
+            eng.set_cfg(**self._env_cfg(test=False))
+            self.agent.obs = None
+            out[loader.name] = paths
+        if not self.curriculum_on_device:
+            self._push_clip_weights()
+        return out
+
     def _restore_device_curriculum(self, fd):
         if self.agent.engine.cur_cfg is None:
             self.agent.curriculum_enable(**self._curriculum_params())

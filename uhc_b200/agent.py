@@ -461,6 +461,44 @@ class BatchedAgent:
         self.obs = None
         return out
 
+    def render_motion(self, clips, fail_safe, size=(640, 360), camera=None, ghost=True, max_bytes=1 << 30, writer=None, window=32):
+        """export_motion's evaluation of every listed clip, drawn on the device (Engine.render): frame k of clip i shows the simulated qpos
+        pred[k] (grey) and, with ghost, the expert frame eval_seq pairs it with, gt[k] = qpos[min(k + 1, len - 1)] (red), with the clip's
+        shape variant.  Frames come to the host in chunks of at most max_bytes of rgb (at least one frame).  writer(i, chunks) is called once
+        per clip, in the caller's order, with an iterator over its uint8 chunks [k][H][W][3], rendered as it is consumed; without a writer
+        the frames are returned.  Returns per clip export_motion's dict plus gt (and frames without a writer).  self.render_times holds the
+        seconds spent in evaluation, rendering, device-to-host copies and the writer."""
+        W, H = (int(x) for x in size)
+        step = max(1, int(max_bytes) // (W * H * 3))
+        t0 = time.perf_counter()
+        mot = self.export_motion(clips, fail_safe, window, max_bytes)
+        times = self.render_times = dict(evaluation=time.perf_counter() - t0, rendering=0.0, copy=0.0, writer=0.0)
+        eng, clips = self.engine, np.asarray(clips, dtype=np.int32).reshape(-1)
+
+        def chunks(d, var):
+            for k0 in range(0, len(d["pred"]), step):
+                t1 = time.perf_counter()
+                rgb = eng.render(d["pred"][k0:k0 + step], d["gt"][k0:k0 + step] if ghost else None, var, camera, (W, H))[0]
+                self.torch.cuda.synchronize(self.dev)
+                t2 = time.perf_counter()
+                host = rgb.cpu().numpy()
+                t3 = time.perf_counter()
+                times["rendering"] += t2 - t1
+                times["copy"] += t3 - t2
+                yield host
+
+        for i, (c, d) in enumerate(zip(clips, mot)):
+            nf, L = len(d["pred"]), int(eng.clip_len[c])
+            d["gt"] = eng.clip_frames(int(c))["qpos"][np.minimum(np.arange(1, nf + 1), L - 1)]
+            var = None if eng.clip_models is None else int(eng.clip_models[c])
+            if writer is None:
+                d["frames"] = np.concatenate(list(chunks(d, var))) if nf else np.zeros((0, H, W, 3), np.uint8)
+            else:
+                t1, inner = time.perf_counter(), times["rendering"] + times["copy"]
+                writer(i, chunks(d, var))
+                times["writer"] += time.perf_counter() - t1 - (times["rendering"] + times["copy"] - inner)
+        return mot
+
     def _checkpoint_policy(self, k, cp):
         """(policy net, ZFilter) slot k of the evaluation pool, beside the agent's own (which stay untouched), loaded from a checkpoint in the
         reference's wire format.  The pool is kept: its tensors keep their addresses, so a repeated sweep replays its captured graphs."""

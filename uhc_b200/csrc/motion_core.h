@@ -140,6 +140,16 @@ UHC_MDEV void m_local_quats(const double *qpos, double *bq) {
     for (int k = 0; k < 4; k++) bq[k] = qpos[3 + k];
     for (int b = 1; b < MB; b++) m_euler_zyx_quat(qpos + 7 + 3 * (b - 1), bq + 4 * b);
 }
+// one step of the FK down the tree: body b's world position / quaternion from its parent's (the root's from qpos); body = the variant's
+// [MB][BODY6] table, bq = m_local_quats of q.  Called for b = 0, 1, .. in order (motion_frame, and the renderer's pose pass).
+UHC_MDEV void m_fk_body(const MotionModel &m, int b, const double *q, const double *bq, const double *body, double *wpos, double *wq) {
+    if (b == 0) { for (int k = 0; k < 3; k++) wpos[k] = q[k]; for (int k = 0; k < 4; k++) wq[k] = q[3 + k]; }
+    else {
+        const int p = m.parent[b];
+        m_qrot_add(wq + 4 * p, body + b * BODY6, wpos + 3 * p, wpos + 3 * b);
+        m_qmul(wq + 4 * p, bq + 4 * b, wq + 4 * b);
+    }
+}
 
 // The record of frame t of a clip whose rows start at `rows` (row width row_w); variant = the clip's body-shape variant.
 template <class Out>
@@ -187,12 +197,7 @@ UHC_MDEV void motion_frame(const MotionModel &m, int kind, int pose_dim, const d
     // FK down the tree: world positions / quaternions, body centres of mass
     double wpos[3 * MB], wq[4 * MB];
     for (int b = 0; b < MB; b++) {
-        if (b == 0) { for (int k = 0; k < 3; k++) wpos[k] = q[k]; for (int k = 0; k < 4; k++) wq[k] = q[3 + k]; }
-        else {
-            const int p = m.parent[b];
-            m_qrot_add(wq + 4 * p, body + b * BODY6, wpos + 3 * p, wpos + 3 * b);
-            m_qmul(wq + 4 * p, bq + 4 * b, wq + 4 * b);
-        }
+        m_fk_body(m, b, q, bq, body, wpos, wq);
         double com[3];
         m_qrot_add(wq + 4 * b, body + b * BODY6 + 3, wpos + 3 * b, com);
         for (int k = 0; k < 3; k++) { rec[R_WBPOS + 3 * b + k] = (Out)wpos[3 * b + k]; rec[R_BCOM + 3 * b + k] = (Out)com[k]; }

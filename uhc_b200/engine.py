@@ -37,6 +37,31 @@ class UhcEvalOut(C.Structure):
 EVAL_SMPL = 75      # include/uhc_eval.h UHC_EVAL_SMPL: pose 72, trans 3
 
 
+class UhcRenderCamera(C.Structure):
+    """include/uhc_render.h UhcRenderCamera"""
+    _fields_ = [("lookat", C.c_double * 3), ("azimuth", C.c_double), ("elevation", C.c_double), ("distance", C.c_double), ("fovy", C.c_double),
+                ("focus", C.c_int), ("hide_im", C.c_int), ("hide_expert", C.c_int), ("shift_expert", C.c_double)]
+
+
+def make_camera(camera=None):
+    """UhcRenderCamera from a dict (or None): CopycatVisualizer.setup_viewing_angle's view by default -- lookat (0, 0, 1), azimuth 45,
+    elevation -8, distance 5, fovy 45 (MuJoCo's default) -- with focus / hide_im / hide_expert (bools) and shift_expert (x offset of the
+    ghost in m; True means update_pose's 1 m)."""
+    c = dict(lookat=(0.0, 0.0, 1.0), azimuth=45.0, elevation=-8.0, distance=5.0, fovy=45.0, focus=False, hide_im=False, hide_expert=False,
+             shift_expert=0.0)
+    unknown = set(camera or {}) - set(c)
+    if unknown:
+        raise ValueError(f"camera: unknown keys {sorted(unknown)}")
+    c.update(camera or {})
+    s = c["shift_expert"]
+    cam = UhcRenderCamera()
+    cam.lookat = (C.c_double * 3)(*[float(x) for x in c["lookat"]])
+    cam.azimuth, cam.elevation, cam.distance, cam.fovy = (float(c[k]) for k in ("azimuth", "elevation", "distance", "fovy"))
+    cam.focus, cam.hide_im, cam.hide_expert = (int(bool(c[k])) for k in ("focus", "hide_im", "hide_expert"))
+    cam.shift_expert = 1.0 if s is True else float(s)
+    return cam
+
+
 def make_cfg(precision=32, base_rot=(0.7071, 0.7071, 0.0, 0.0), rfc_scale=100.0, rfc_lim=100.0, rfc_rate=1.0, body_diff_thresh=0.5,
              meta_pd=1, env_episode_len=100000, trail_steps=0, w=(0.3, 0.1, 0.45, 0.1, 0.05), k=(2.0, 0.005, 5.0, 100.0, 1.0),
              newton_max_iter=None, newton_tol=None, auto_reset=0, t_min=5, t_max=300, reset_seed=1, reactive_v=0, reactive_rate=0.3,
@@ -163,7 +188,8 @@ class Engine:
         self.percent = torch.zeros(self.E, **f)
         self.fail = torch.zeros(self.E, device=dev, dtype=torch.int32)
         self.end = torch.zeros(self.E, device=dev, dtype=torch.int32)
-        self.clip_len = None
+        self.clip_len = self.clip_models = None
+        self._render_ready = False
         self.cur_cfg = None            # device curriculum parameters while it is enabled (curriculum_enable)
         if int(cfg.get("reactive_v", 0)) == 1:
             self.set_neutral_pose()
@@ -181,6 +207,7 @@ class Engine:
         if getattr(self, "h", None):
             self.lib.uhc_eval_release(self.h)
             self.lib.uhc_track_end(self.h)
+            self.lib.uhc_render_release(self.h)
             self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
             self.h = None
@@ -206,7 +233,7 @@ class Engine:
         shp = np.ascontiguousarray(shp)
         _chk(self.lib.uhc_load_clips(self.h, C.c_int(len(experts)), _ip(lens), frames.ctypes.data_as(C.POINTER(C.c_double)),
                                      shp.ctypes.data_as(C.POINTER(C.c_double))))
-        self._table_loaded(lens)
+        self._table_loaded(lens, clip_models)
         if clip_models is not None:
             _chk(self.lib.uhc_set_clip_models(self.h, C.c_int(len(experts)), _ip(clip_models)))
 
@@ -224,11 +251,12 @@ class Engine:
         _chk(self.lib.uhc_load_motions(self.h, C.c_int(n), _ip(lens), C.c_int(motions.kind), C.c_int(motions.pose_dim),
                                        rows.ctypes.data_as(C.POINTER(C.c_double)), shp.ctypes.data_as(C.POINTER(C.c_double)),
                                        None if fk is None else _ip(fk), C.c_int(int(chunk_frames))))
-        self._table_loaded(lens.copy())
+        self._table_loaded(lens.copy(), clip_models)
         if clip_models is not None:
             _chk(self.lib.uhc_set_clip_models(self.h, C.c_int(n), _ip(clip_models)))
 
-    def _table_loaded(self, lens):
+    def _table_loaded(self, lens, clip_models=None):
+        self.clip_models = None if clip_models is None else np.array(clip_models, np.int32).reshape(len(lens))
         if self.cur_cfg is not None and (self.clip_len is None or len(lens) != len(self.clip_len)):
             self.cur_cfg = None        # the engine disabled the curriculum: its histories belonged to the old clips
         self.clip_len = lens
@@ -430,6 +458,89 @@ class Engine:
                                               self._stream()), "uhc_track_smpl")
         return pose, trans
 
+    # ---- the renderer (include/uhc_render.h)
+    def _rnd_chk(self, rc, who):
+        if rc != 0:
+            self.lib.uhc_render_last_error.restype = C.c_char_p
+            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_render_last_error().decode())
+
+    def _render_init(self):
+        if not self._render_ready:
+            self._rhulls = self.model.render_struct(self.variants)
+            self._rnd_chk(self.lib.uhc_render_init(self.h, C.byref(self._rhulls)), "uhc_render_init")
+            self._render_ready = True
+
+    def _rows(self, q, n=None):
+        """a cuda tensor [n][>= 76] of float32 | float64 with contiguous rows (read in place), or anything numpy takes (copied as float64)"""
+        t = self.torch
+        q = q if t.is_tensor(q) and q.is_cuda else t.as_tensor(np.ascontiguousarray(q, np.float64), device=self.obs.device)
+        if q.dim() != 2 or q.dtype not in (t.float32, t.float64) or q.shape[1] < NQ or q.stride(1) != 1 or (n is not None and q.shape[0] != n):
+            raise ValueError("render: qpos rows must be [n][>= 76] contiguous rows of float32 | float64 (the ghost as many as qpos)")
+        return q
+
+    def _variant_arg(self, variants, n):
+        if variants is None:
+            return None
+        return self.torch.as_tensor(np.array(np.broadcast_to(np.asarray(variants, np.int32), (n,))), device=self.obs.device)
+
+    def render_pose(self, qpos, ghost=None, variants=None):
+        """the renderer's pose table (uhc_render_pose) [n][2][24][12] float32: per body the world rotation (row-major) and position of qpos row
+        i (humanoid 0) and ghost row i (humanoid 1, zero without a ghost), from the fp64 FK with shape variant variants[i] (None: 0)"""
+        t = self.torch
+        q = self._rows(qpos)
+        n = q.shape[0]
+        g = None if ghost is None else self._rows(ghost, n)
+        v = self._variant_arg(variants, n)
+        pose = t.zeros(n, 2, 24, 12, dtype=t.float32, device=self.obs.device)
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        pitch = lambda x: C.c_long(x.stride(0) if x is not None and x.shape[0] > 1 else (x.shape[1] if x is not None else NQ))
+        self._rnd_chk(self.lib.uhc_render_pose(self.h, C.c_long(n), p(q), C.c_int(32 if q.dtype == t.float32 else 64), pitch(q), p(g), pitch(g), p(v),
+                                               p(pose), self._stream()), "uhc_render_pose")
+        return pose
+
+    def _render_out(self, n, size, depth, label):
+        t = self.torch
+        W, H = (int(x) for x in size)
+        dev = self.obs.device
+        rgb = t.empty(n, H, W, 3, dtype=t.uint8, device=dev)
+        dep = t.empty(n, H, W, dtype=t.float32, device=dev) if depth else None
+        lab = t.empty(n, H, W, dtype=t.uint8, device=dev) if label else None
+        return W, H, rgb, dep, lab
+
+    def render(self, qpos, ghost=None, variants=None, camera=None, size=(640, 360), depth=False, label=False):
+        """n frames of W x H pixels (uhc_render_qpos): frame i shows the humanoid at qpos row i (grey) and, with a ghost, the ghost at ghost row i
+        (red).  qpos / ghost: cuda tensors [n][>= 76] of float32 | float64 read in place (a state record of 148 or the tracker's state_out of 223
+        as they are), or arrays numpy takes.  variants: shape variant per frame (None: 0).  camera: a dict for make_camera (MuJoCo's free camera
+        with focus / hide_im / hide_expert / shift_expert).  Returns (rgb [n][H][W][3] uint8, depth [n][H][W] float32 (m along the ray, inf on
+        sky) or None, label [n][H][W] uint8 (0 sky, 1 floor, 2 + b body b, 26 + b the ghost's body b) or None), cuda tensors."""
+        t = self.torch
+        self._render_init()
+        q = self._rows(qpos)
+        n = q.shape[0]
+        g = None if ghost is None else self._rows(ghost, n)
+        v = self._variant_arg(variants, n)
+        W, H, rgb, dep, lab = self._render_out(n, size, depth, label)
+        cam = make_camera(camera)
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        pitch = lambda x: C.c_long(x.stride(0) if x is not None and x.shape[0] > 1 else (x.shape[1] if x is not None else NQ))
+        self._rnd_chk(self.lib.uhc_render_qpos(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(q), C.c_int(32 if q.dtype == t.float32 else 64),
+                                               pitch(q), p(g), pitch(g), p(v), p(rgb), p(dep), p(lab), self._stream()), "uhc_render_qpos")
+        return rgb, dep, lab
+
+    def render_bodies(self, pose, humanoids=2, variants=None, camera=None, size=(640, 360), depth=False, label=False):
+        """render() from a pose table [n][2][24][12] float32 cuda tensor (render_pose's layout) instead of qpos (uhc_render_bodies)"""
+        t = self.torch
+        self._render_init()
+        assert pose.is_cuda and pose.dtype == t.float32 and pose.is_contiguous() and pose.dim() == 4 and tuple(pose.shape[1:]) == (2, 24, 12)
+        n = pose.shape[0]
+        v = self._variant_arg(variants, n)
+        W, H, rgb, dep, lab = self._render_out(n, size, depth, label)
+        cam = make_camera(camera)
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        self._rnd_chk(self.lib.uhc_render_bodies(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(pose), C.c_int(int(humanoids)), p(v),
+                                                 p(rgb), p(dep), p(lab), self._stream()), "uhc_render_bodies")
+        return rgb, dep, lab
+
     # ---- the batched physics tracker (include/uhc_track.h uhc_track_*)
     def _trk_chk(self, rc, who):
         if rc != 0:
@@ -446,7 +557,7 @@ class Engine:
         self._trk_chk(self.lib.uhc_track_begin(self.h, C.c_int(int(window)), C.c_int(k), C.c_int(pose_dim), None if fk is None else _ip_out(fk),
                                                None if shp is None else shp.ctypes.data_as(C.POINTER(C.c_double))), "uhc_track_begin")
         self.track_row_w = NQ if k == 1 else pose_dim + 3
-        self._table_loaded(np.full(self.E, int(window), np.int32))
+        self._table_loaded(np.full(self.E, int(window), np.int32), fk)
 
     def track_reset(self, env_ids, frames, qpos=None, qvel=None):
         """frames: float64 cuda tensor [n][2][row width], target frames 0 and 1 of each listed env; qpos / qvel: optional fp32 cuda overrides"""

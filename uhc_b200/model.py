@@ -29,6 +29,12 @@ class UhcModelHost(C.Structure):
                 ("solimp", C.c_double * 5), ("gravz", C.c_double), ("nshape", C.c_int), ("dof_lim", C.POINTER(C.c_double))]
 
 
+class UhcRenderHulls(C.Structure):
+    """C mirror: include/uhc_render.h `UhcRenderHulls`."""
+    _fields_ = [("nshape", C.c_int), ("nplane", C.c_int), ("plane", C.POINTER(C.c_double)), ("plane_adr", C.POINTER(C.c_int)),
+                ("plane_num", C.POINTER(C.c_int)), ("sphere", C.POINTER(C.c_double))]
+
+
 class HumanoidModel:
     def __init__(self, npz=ASSET, scale=None, jnt_range=None):
         """jnt_range: optional [69][2] hinge limits in radians overriding the model's (xml: +-180 deg on every hinge; smpl_robot.py:1087-1110 tightens
@@ -182,6 +188,43 @@ class HumanoidModel:
     def vf_slot(self):
         """residual-force slot of every model body (bodies are numbered depth-first, the slots follow the SMPL joint order)"""
         return [self.SMPL_BONE_ORDER.index(n) for n in self.body_names]
+
+    def hull_planes(self):
+        """face planes of every body hull in body frame, [nplane][4] (unit outward normal n, offset d; n . x + d <= 0 inside), from
+        scipy's ConvexHull(...).equations with faces coplanar to 1e-9 merged, and per body plane_adr / plane_num [24]"""
+        from scipy.spatial import ConvexHull
+        planes, num = [], []
+        for b in range(NB):
+            eq = ConvexHull(self.hull[self.hull_adr[b]:self.hull_adr[b] + self.hull_num[b]]).equations
+            keep = []
+            for e in eq:
+                if not any(np.abs(e - k).max() <= 1e-9 for k in keep):
+                    keep.append(e)
+            planes.append(np.array(keep))
+            num.append(len(keep))
+        return np.concatenate(planes), np.concatenate([[0], np.cumsum(num)[:-1]]).astype(np.int32), np.array(num, np.int32)
+
+    def render_struct(self, variants=None):
+        """ctypes UhcRenderHulls of the shape variants host_struct(variants) builds, in the same order (arrays kept alive on self).  Variants
+        share plane_adr / plane_num: a body whose hull has fewer merged faces in one variant repeats its last plane, which clips nothing more."""
+        models = variants or [self]
+        assert models[0] is self
+        per = [m.hull_planes() for m in models]
+        num = np.max([p[2] for p in per], axis=0).astype(np.int32)
+        adr = np.concatenate([[0], np.cumsum(num)[:-1]]).astype(np.int32)
+        plane = np.zeros((len(models), int(num.sum()), 4))
+        for s, (pl, a, k) in enumerate(per):
+            for b in range(NB):
+                rows = pl[a[b]:a[b] + k[b]]
+                plane[s, adr[b]:adr[b] + num[b]] = np.concatenate([rows, np.repeat(rows[-1:], num[b] - k[b], 0)])
+        sphere = np.ascontiguousarray(np.stack([m.body_f[:, 14:18] for m in models]))
+        keep = self._rkeep = dict(plane=np.ascontiguousarray(plane), adr=adr, num=num, sphere=sphere)
+        h = UhcRenderHulls()
+        h.nshape, h.nplane = len(models), plane.shape[1]
+        h.plane = keep["plane"].ctypes.data_as(C.POINTER(C.c_double))
+        h.plane_adr, h.plane_num = adr.ctypes.data_as(C.POINTER(C.c_int)), num.ctypes.data_as(C.POINTER(C.c_int))
+        h.sphere = sphere.ctypes.data_as(C.POINTER(C.c_double))
+        return h
 
     def host_struct(self, variants=None):
         """ctypes struct of host pointers for uhc_engine_create / the emulation (arrays kept alive on self).
