@@ -9,7 +9,7 @@
 //                                                                                the reward sum, fail / end, the fail_safe flag
 //   k_eval_export (SMPL export only)                                               per env that recorded a frame: its qpos as SMPL (export.cu)
 //   k_eval_reseat (fail_safe only)                                               uhc_env_set_state_batch's re-seat of the flagged envs
-// `window` steps are captured once per argument set into a CUDA graph; after each replay one 2-D copy moves the window's frame rows
+// `window` steps are captured once per argument set into a CUDA graph (graph_cache.h); after each replay one 2-D copy moves the window's frame rows
 // into the caller's (pinned) array and one 4-byte copy returns the number of envs still alive, the host loop's early exit.
 //
 // Compiled on its own with -fmad=false (uhc_b200/build.py) like motion_lib.cu: k_eval_frame restates numpy's fp64 arithmetic
@@ -22,6 +22,7 @@
 #include "../../include/uhc_eval.h"
 #include "eval_core.h"
 #include "eval_glue.h"
+#include "graph_cache.h"
 #include "sim_core.h"
 #include "smpl_export_core.h"
 #include "track_glue.h"
@@ -89,25 +90,9 @@ __global__ void k_eval_init(int n, UhcEvalClip *__restrict__ clips, int *__restr
     if (i < E) ones[i] = 1;
 }
 
-struct EvalKey {
-    int n, nrec_max, window, fail_safe, states, smpl, nprim; float zclip; unsigned long long scratch_gen, eval_gen, view_gen;
-    UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; const float *log_std; const double *zstats;
-    bool operator==(const EvalKey &o) const { return memcmp(this, &o, sizeof(EvalKey)) == 0; }
-};
-// the grouped evaluation's graphs: G, the group sizes, every group's policy by value and its ZFilter statistics pointer, and the generations
-// of the grouped policy scratch, the window buffers and the engine view
-struct GroupKeyHead {
-    int G, ntot, nrec_max, window, fail_safe, states, smpl, nprim; float zclip; unsigned long long group_gen, eval_gen, view_gen;
-};
-struct GroupKey {
-    GroupKeyHead h; std::vector<int> n; std::vector<UhcMlp> nets; std::vector<const double *> zs;
-    bool operator==(const GroupKey &o) const {
-        return memcmp(&h, &o.h, sizeof h) == 0 && n == o.n && zs == o.zs && nets.size() == o.nets.size() &&
-               memcmp(nets.data(), o.nets.data(), nets.size() * sizeof(UhcMlp)) == 0;
-    }
-};
-// the policies of one grouped call: group g on env rows [row0[g], row0[g + 1])
-struct GroupSet { int G; const int *row0; const UhcMlp *mlps; const UhcMcp *mcps; const double *const *zstats; };
+// the policies of one call: group g on env rows [row0[g], row0[g + 1]).  A single-policy call is one group over rows 0 .. n-1 that takes
+// the ungrouped kernels and the caller's log_std
+struct EvalPolicies { bool grouped; std::vector<evalx::Policy> pols; std::vector<int> row0; const float *log_std; const double *const *zstats; };
 
 struct EvalCtx {
     UhcEngine *eng = nullptr;
@@ -120,8 +105,7 @@ struct EvalCtx {
     int *h_count = nullptr;                       // pinned
     cudaEvent_t ev = nullptr;
     std::vector<int> ids, clip0, start, len;      // reset arguments (kept: no allocation in the steady state)
-    std::vector<std::pair<EvalKey, cudaGraphExec_t>> graphs;
-    std::vector<std::pair<GroupKey, cudaGraphExec_t>> ggraphs;   // uhc_eval_run_groups
+    GraphCache graphs{32}, ggraphs{16};           // of uhc_eval_run and of uhc_eval_run_groups (graph_cache.h)
 };
 std::vector<EvalCtx *> g_ev;
 
@@ -131,13 +115,6 @@ EvalCtx *ev_ctx(UhcEngine *e) {
     g_ev.push_back(c);
     return c;
 }
-void drop_graphs(EvalCtx *c) {
-    for (auto &g : c->graphs) cudaGraphExecDestroy(g.second);
-    c->graphs.clear();
-    for (auto &g : c->ggraphs) cudaGraphExecDestroy(g.second);
-    c->ggraphs.clear();
-}
-
 // per-env arrays sized by E once; the window buffers grow with n * window (and the state record and the SMPL export with it when requested).
 // Called before any capture: a graph holds these pointers, so they never change while one of them can be replayed (gen)
 int ensure(EvalCtx *c, int n, int window, bool states, bool smpl) {
@@ -166,13 +143,12 @@ int ensure(EvalCtx *c, int n, int window, bool states, bool smpl) {
     return 0;
 }
 
-int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
-                   int n, int nrec_max, int fail_safe, int window, bool states, bool smpl, cudaStream_t st, const GroupSet *grp = nullptr) {
-    std::string err;
+int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const EvalPolicies &P, float zclip, int n, int nrec_max, int fail_safe, int window, bool states,
+                   bool smpl, cudaStream_t st) {
     for (int s = 0; s < window; s++) {
-        int rc = grp ? evalx::groups_enqueue(c->eng, grp->G, grp->row0, grp->mlps, grp->mcps, grp->zstats, zclip, R.obs, c->d_ones, R.act, st, &err)
-                     : evalx::policy_enqueue(c->eng, mlp, mcp, R.obs, log_std, zstats, zclip, c->d_ones, R.act, st, &err);
-        if (rc) { g_ev_err = err; return rc; }
+        const int rc = P.grouped ? evalx::groups_enqueue(c->eng, P.pols, P.row0.data(), P.zstats, zclip, R.obs, c->d_ones, R.act, st)
+                                 : evalx::policy_enqueue(c->eng, P.pols[0], R.obs, P.log_std, (double *)P.zstats[0], zclip, c->d_ones, R.act, st);
+        if (rc) { g_ev_err = uhc_rollout_last_error(); return rc; }
         if (uhc_env_step(c->eng, R.act, R.obs, R.rew, R.cinfo, R.fail, R.end, R.pct, nullptr, st)) { g_ev_err = std::string("env step: ") + uhc_last_error(); return -1; }
         const bool last = s == window - 1;
         if (last) CKE(cudaMemsetAsync(c->d_count, 0, 4, st));
@@ -208,23 +184,6 @@ int reset_envs(EvalCtx *c, UhcEngine *e, const evalx::EngineRefs &R, int n, cons
     return 0;
 }
 
-// `window` steps captured on a private stream into an instantiated graph
-int capture_window(EvalCtx *c, const evalx::EngineRefs &R, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, double *zstats, float zclip,
-                   int n, int nrec_max, int fail_safe, int window, bool states, bool smpl, const GroupSet *grp, cudaGraphExec_t *exec) {
-    cudaStream_t cs; CKE(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-    cudaGraph_t graph = nullptr;
-    CKE(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-    const int rc = enqueue_window(c, R, mlp, mcp, log_std, zstats, zclip, n, nrec_max, fail_safe, window, states, smpl, cs, grp);
-    cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-    cudaStreamDestroy(cs);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) { g_ev_err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce); return -1; }
-    ce = cudaGraphInstantiate(exec, graph, 0);
-    cudaGraphDestroy(graph);
-    CKE(ce);
-    return 0;
-}
-
 // replays until every env has stopped or nrec_max steps have run; after each, the window's rows of envs 0..n-1 go to the caller's arrays
 int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, const UhcEvalOut &o, cudaStream_t st) {
     double *frames_host = o.frames_host, *states_host = o.states_host_or_null, *smpl_host = o.smpl_host_or_null;
@@ -250,23 +209,34 @@ int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, co
     return 0;
 }
 
-int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats,
-             float zclip, int fail_safe, int window, const UhcEvalOut &o, void *stream) {
-    const char *who = mcp ? "uhc_eval_run_mcp" : "uhc_eval_run";
-    if (!e || !clip_host || (!mlp && !mcp) || !log_std || !zfilter_stats || !o.frames_host || !o.clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
+// One chunk: G policies side by side, group g on envs [row0[g], row0[g] + group_n[g]); uhc_eval_run is the ungrouped call of one group
+int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *clip_host, const UhcMlp *mlps, const UhcMcp *mcps, const float *log_std,
+             const double *const *zstats, float zclip, int fail_safe, int window, const UhcEvalOut &o, void *stream) {
+    const std::string who = std::string(grouped ? "uhc_eval_run_groups" : "uhc_eval_run") + (mcps ? "_mcp" : "");
+    auto refuse = [&](const char *why) { g_ev_err = who + ": " + why; return -2; };
+    if (!e || !group_n || !clip_host || (!mlps && !mcps) || !zstats || (!grouped && (!log_std || !zstats[0])) || !o.frames_host || !o.clips_host) return refuse("null argument");
+    if (G < 1 || G > UHC_EVAL_MAX_GROUPS) return refuse("G must be 1 .. UHC_EVAL_MAX_GROUPS");
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
-    if (n < 1 || n > R.E) { g_ev_err = std::string(who) + ": n must be 1 .. E"; return -2; }
-    if (window < 1) { g_ev_err = std::string(who) + ": window < 1"; return -2; }
-    if ((long long)n * window > INT_MAX) { g_ev_err = std::string(who) + ": n * window exceeds INT_MAX window rows"; return -2; }
-    if (R.num_clips <= 0) { g_ev_err = std::string(who) + ": no clips loaded"; return -2; }
+    if (!grouped && (group_n[0] < 1 || group_n[0] > R.E)) return refuse("n must be 1 .. E");
+    EvalPolicies P{grouped, std::vector<evalx::Policy>(G), std::vector<int>(G + 1, 0), log_std, zstats};
+    for (int g = 0; g < G; g++) {
+        if (group_n[g] < 1) return refuse("every group needs at least one env");
+        if (!zstats[g]) return refuse("null ZFilter statistics");
+        P.row0[g + 1] = P.row0[g] + group_n[g];
+        if (P.row0[g + 1] > R.E) return refuse("the groups hold more than E envs");
+    }
+    const int n = P.row0[G];
+    if (window < 1) return refuse("window < 1");
+    if ((long long)n * window > INT_MAX) return refuse("n * window exceeds INT_MAX window rows");
+    if (R.num_clips <= 0) return refuse("no clips loaded");
     int max_len = 0;
     for (int i = 0; i < n; i++) {
-        if (clip_host[i] < 0 || clip_host[i] >= R.num_clips) { g_ev_err = std::string(who) + ": clip index out of range"; return -2; }
+        if (clip_host[i] < 0 || clip_host[i] >= R.num_clips) return refuse("clip index out of range");
         max_len = R.clip_len_h[clip_host[i]] > max_len ? R.clip_len_h[clip_host[i]] : max_len;
     }
-    unsigned long long sgen = 0; std::string err;
-    int rc = evalx::policy_prepare(e, mlp, mcp, &sgen, &err);
-    if (rc) { g_ev_err = err; return rc; }
+    unsigned long long pgen = 0;
+    int rc = grouped ? evalx::groups_prepare(e, G, mlps, mcps, &P.pols, &pgen) : evalx::policy_prepare(e, mlps, mcps, &P.pols[0], &pgen);
+    if (rc) { g_ev_err = uhc_rollout_last_error(); return rc; }
     EvalCtx *c = ev_ctx(e);
     const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr;
     if (ensure(c, n, window, states, smpl)) return -1;
@@ -274,89 +244,25 @@ int eval_run(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const
     const int nrec_max = max_len - 1;
     if (reset_envs(c, e, R, n, clip_host, st)) return -1;
     if (smpl) CKE(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
+    // no grouped policy covers the parked envs: they step with zero actions (the graph writes action rows 0 .. n-1 only)
+    if (grouped && n < R.E) CKE(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
 
-    EvalKey key; memset(&key, 0, sizeof key);
-    key.n = n; key.nrec_max = nrec_max; key.window = window; key.fail_safe = fail_safe ? 1 : 0; key.states = states; key.smpl = smpl; key.zclip = zclip;
-    key.scratch_gen = sgen; key.eval_gen = c->gen; key.view_gen = R.view_gen; key.log_std = log_std; key.zstats = zfilter_stats;
-    if (mcp) { key.nprim = mcp->nprim; for (int k = 0; k < mcp->nprim; k++) key.nets[k] = mcp->prim[k]; key.nets[mcp->nprim] = mcp->composer; }
-    else key.nets[0] = *mlp;
-    // a graph holds the engine view (cfg, clip table), the policy scratch and the window buffers of its capture as kernel parameters:
-    // once any of them has changed it can never be replayed, so it is dropped here rather than kept until eviction
-    for (size_t g = 0; g < c->graphs.size();) {
-        const EvalKey &k = c->graphs[g].first;
-        if (k.view_gen != key.view_gen || k.scratch_gen != key.scratch_gen || k.eval_gen != key.eval_gen) {
-            cudaGraphExecDestroy(c->graphs[g].second); c->graphs.erase(c->graphs.begin() + g);
-        } else g++;
-    }
-    cudaGraphExec_t exec = nullptr;
-    for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
+    // the key: every argument the graph's kernels got.  The generations: the graph also holds the policy scratch, the window buffers and
+    // the engine view (cfg, clip table) of its capture, and is dropped once any of them has changed
+    struct { int n, nrec_max, window, fail_safe, states, smpl; float zclip; const float *log_std; } head;
+    memset(&head, 0, sizeof head);
+    head.n = n; head.nrec_max = nrec_max; head.window = window; head.fail_safe = fail_safe ? 1 : 0; head.states = states; head.smpl = smpl; head.zclip = zclip;
+    head.log_std = log_std;
+    std::string key;
+    GraphCache::append(&key, &head); GraphCache::append(&key, group_n, G); GraphCache::append(&key, zstats, G); GraphCache::append(&key, P.pols.data(), G);
+    const GraphCache::Gens gens{pgen, c->gen, R.view_gen};
+    GraphCache &cache = grouped ? c->ggraphs : c->graphs;
+    cache.drop_stale(gens);
+    cudaGraphExec_t exec = cache.find(key);
     if (!exec) {
-        rc = capture_window(c, R, mlp, mcp, log_std, (double *)zfilter_stats, zclip, n, nrec_max, key.fail_safe, window, states, smpl, nullptr, &exec);
+        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_window(c, R, P, zclip, n, nrec_max, head.fail_safe, window, states, smpl, cs); }, &exec, &g_ev_err);
         if (rc) return rc;
-        if (c->graphs.size() >= 32) { cudaGraphExecDestroy(c->graphs.front().second); c->graphs.erase(c->graphs.begin()); }
-        c->graphs.emplace_back(key, exec);
-    }
-    return replay(c, exec, n, nrec_max, window, o, st);
-}
-
-// G policies side by side: group g on envs [off_g, off_g + n_g), the rest as eval_run over the sum of the n_g envs
-int eval_run_groups(UhcEngine *e, int G, const int *group_n, const int *clip_host, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats,
-                    float zclip, int fail_safe, int window, const UhcEvalOut &o, void *stream) {
-    const char *who = mcps ? "uhc_eval_run_groups_mcp" : "uhc_eval_run_groups";
-    if (!e || !group_n || !clip_host || (!mlps && !mcps) || !zstats || !o.frames_host || !o.clips_host) { g_ev_err = std::string(who) + ": null argument"; return -2; }
-    if (G < 1 || G > UHC_EVAL_MAX_GROUPS) { g_ev_err = std::string(who) + ": G must be 1 .. UHC_EVAL_MAX_GROUPS"; return -2; }
-    evalx::EngineRefs R; evalx::engine_refs(e, &R);
-    std::vector<int> row0(G + 1, 0);
-    for (int g = 0; g < G; g++) {
-        if (group_n[g] < 1) { g_ev_err = std::string(who) + ": every group needs at least one env"; return -2; }
-        if (!zstats[g]) { g_ev_err = std::string(who) + ": null ZFilter statistics"; return -2; }
-        row0[g + 1] = row0[g] + group_n[g];
-        if (row0[g + 1] > R.E) { g_ev_err = std::string(who) + ": the groups hold more than E envs"; return -2; }
-    }
-    const int n = row0[G];
-    if (window < 1) { g_ev_err = std::string(who) + ": window < 1"; return -2; }
-    if ((long long)n * window > INT_MAX) { g_ev_err = std::string(who) + ": n * window exceeds INT_MAX window rows"; return -2; }
-    if (R.num_clips <= 0) { g_ev_err = std::string(who) + ": no clips loaded"; return -2; }
-    int max_len = 0;
-    for (int i = 0; i < n; i++) {
-        if (clip_host[i] < 0 || clip_host[i] >= R.num_clips) { g_ev_err = std::string(who) + ": clip index out of range"; return -2; }
-        max_len = R.clip_len_h[clip_host[i]] > max_len ? R.clip_len_h[clip_host[i]] : max_len;
-    }
-    unsigned long long ggen = 0; std::string err;
-    int rc = evalx::groups_prepare(e, G, mlps, mcps, &ggen, &err);
-    if (rc) { g_ev_err = err; return rc; }
-    EvalCtx *c = ev_ctx(e);
-    const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr;
-    if (ensure(c, n, window, states, smpl)) return -1;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int nrec_max = max_len - 1;
-    if (reset_envs(c, e, R, n, clip_host, st)) return -1;
-    if (smpl) CKE(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
-    // no policy covers the parked envs: they step with zero actions (the graph writes action rows 0 .. n-1 only)
-    if (n < R.E) CKE(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
-
-    GroupKey key; memset(&key.h, 0, sizeof key.h);
-    key.h.G = G; key.h.ntot = n; key.h.nrec_max = nrec_max; key.h.window = window; key.h.fail_safe = fail_safe ? 1 : 0; key.h.states = states; key.h.smpl = smpl;
-    key.h.zclip = zclip; key.h.group_gen = ggen; key.h.eval_gen = c->gen; key.h.view_gen = R.view_gen;
-    key.n.assign(group_n, group_n + G); key.zs.assign(zstats, zstats + G);
-    for (int g = 0; g < G; g++) {
-        if (mcps) { key.h.nprim = mcps[g].nprim; for (int k = 0; k < mcps[g].nprim; k++) key.nets.push_back(mcps[g].prim[k]); key.nets.push_back(mcps[g].composer); }
-        else key.nets.push_back(mlps[g]);
-    }
-    for (size_t g = 0; g < c->ggraphs.size();) {      // graphs holding a changed engine view or reallocated scratch can never be replayed
-        const GroupKeyHead &k = c->ggraphs[g].first.h;
-        if (k.view_gen != key.h.view_gen || k.group_gen != key.h.group_gen || k.eval_gen != key.h.eval_gen) {
-            cudaGraphExecDestroy(c->ggraphs[g].second); c->ggraphs.erase(c->ggraphs.begin() + g);
-        } else g++;
-    }
-    cudaGraphExec_t exec = nullptr;
-    for (auto &g : c->ggraphs) if (g.first == key) { exec = g.second; break; }
-    if (!exec) {
-        const GroupSet gs{G, row0.data(), mlps, mcps, zstats};
-        rc = capture_window(c, R, nullptr, nullptr, nullptr, nullptr, zclip, n, nrec_max, key.h.fail_safe, window, states, smpl, &gs, &exec);
-        if (rc) return rc;
-        if (c->ggraphs.size() >= 16) { cudaGraphExecDestroy(c->ggraphs.front().second); c->ggraphs.erase(c->ggraphs.begin()); }
-        c->ggraphs.emplace_back(std::move(key), exec);
+        cache.insert(std::move(key), gens, exec);
     }
     return replay(c, exec, n, nrec_max, window, o, st);
 }
@@ -398,32 +304,31 @@ int uhc_eval_run_ex(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp
                     int fail_safe, int window, const UhcEvalOut *out, void *stream) {
     if (!mlp) { g_ev_err = "uhc_eval_run: null policy"; return -2; }
     if (!out) { g_ev_err = "uhc_eval_run: null output struct"; return -2; }
-    return eval_run(e, n, clip_host, mlp, nullptr, log_std, zfilter_stats, zclip, fail_safe, window, *out, stream);
+    return eval_run(e, false, 1, &n, clip_host, mlp, nullptr, log_std, &zfilter_stats, zclip, fail_safe, window, *out, stream);
 }
 int uhc_eval_run_mcp_ex(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
                         int fail_safe, int window, const UhcEvalOut *out, void *stream) {
     if (!mcp) { g_ev_err = "uhc_eval_run_mcp: null policy"; return -2; }
     if (!out) { g_ev_err = "uhc_eval_run_mcp: null output struct"; return -2; }
-    return eval_run(e, n, clip_host, nullptr, mcp, log_std, zfilter_stats, zclip, fail_safe, window, *out, stream);
+    return eval_run(e, false, 1, &n, clip_host, nullptr, mcp, log_std, &zfilter_stats, zclip, fail_safe, window, *out, stream);
 }
 int uhc_eval_run_groups_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
                            float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream) {
     if (!mlps) { g_ev_err = "uhc_eval_run_groups: null policy"; return -2; }
     if (!out) { g_ev_err = "uhc_eval_run_groups: null output struct"; return -2; }
-    return eval_run_groups(e, G, group_n_host, clip_host, mlps, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
+    return eval_run(e, true, G, group_n_host, clip_host, mlps, nullptr, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
 }
 int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
                                float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream) {
     if (!mcps) { g_ev_err = "uhc_eval_run_groups_mcp: null policy"; return -2; }
     if (!out) { g_ev_err = "uhc_eval_run_groups_mcp: null output struct"; return -2; }
-    return eval_run_groups(e, G, group_n_host, clip_host, nullptr, mcps, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
+    return eval_run(e, true, G, group_n_host, clip_host, nullptr, mcps, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
 }
 
 void uhc_eval_release(UhcEngine *e) {
-    evalx::groups_release(e);
     for (size_t i = 0; i < g_ev.size(); i++) if (g_ev[i]->eng == e) {
         EvalCtx *c = g_ev[i];
-        drop_graphs(c);
+        c->graphs.clear(); c->ggraphs.clear();
         for (void *p : {(void *)c->d_clips, (void *)c->d_alive, (void *)c->d_reseat, (void *)c->d_count, (void *)c->d_ones, (void *)c->d_ring,
                         (void *)c->d_win, (void *)c->d_wstates, (void *)c->d_wsmpl, (void *)c->d_xdone}) if (p) cudaFree(p);
         if (c->h_count) cudaFreeHost(c->h_count);

@@ -1,8 +1,9 @@
-// eval_glue.h -- internal interface of the device evaluation (eval.cu) to the engine (step_kernel.cu) and to the policy forward of the
-// rollout (rollout.cu).  Not part of the C ABI.
+// eval_glue.h -- internal interface of the device evaluation (eval.cu) and the tracker (track.cu) to the engine (step_kernel.cu) and to
+// the policy forward of the rollout (rollout.cu).  Not part of the C ABI.  Host-only declarations and plain structs.
 #pragma once
 #include <cuda_runtime.h>
 #include <string>
+#include <vector>
 #include "../../include/uhc_b200.h"
 #include "../../include/uhc_rollout.h"
 
@@ -24,20 +25,23 @@ cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t s
 // changes whenever the sampler's curriculum view (rings, fit_clip, prec_freq, CDF pointer under the curriculum) changes; the rollout's
 // graphs are keyed on it                                                                                                   // step_kernel.cu
 unsigned long long curriculum_gen(const UhcEngine *e);
-// policy of an evaluation: validates it (-2) and sizes the rollout's scratch outside any capture; *gen changes whenever that scratch
-// is reallocated (graphs holding the old pointers must be dropped)
-int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, unsigned long long *gen, std::string *err);   // rollout.cu
+// the policy of a rollout as a flat net list: one MLP (PolicyGaussian, nprim = 0: nets[0]) or a PolicyMCP mixture (nets[0 .. nprim-1] =
+// primitives, nets[nprim] = composer).  Zeroed before it is filled, so its bytes can go into a graph key
+struct Policy { int nprim; int pad; UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; };
+// The four calls below return 0 or an error code with its text in uhc_rollout_last_error().
+// policy of an evaluation or a tracker step: converts and validates it (-2) and sizes the rollout's policy scratch outside any capture;
+// *gen changes whenever that scratch is reallocated (graphs holding the old pointers must be dropped)
+int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, Policy *pol, unsigned long long *gen);   // rollout.cu
 // obs -> ZFilter (no update) -> policy -> action (the mean where mean_action[e] != 0); enqueues only (capturable)
-int policy_enqueue(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, const float *obs, const float *log_std, double *zstats, float zclip,
-                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err);                 // rollout.cu
+int policy_enqueue(UhcEngine *e, const Policy &pol, const float *obs, const float *log_std, double *zstats, float zclip,
+                   const unsigned char *mean_action, float *action, cudaStream_t st);                 // rollout.cu
 // the grouped evaluation (uhc_eval_run_groups): G policies (mlps[G] or mcps[G]) of one architecture, group g on rows [row0[g], row0[g + 1]).
-// groups_prepare validates them (-2) and sizes the grouped scratch, which is its own (never the rollout's); *gen changes whenever that
-// scratch is reallocated.  groups_enqueue: obs -> ZFilter of each group (zstats[g], no update) -> grouped GEMMs (+ mixture head) -> the
-// mean action (with mean_action all ones) of rows 0 .. row0[G] - 1; enqueues only (capturable).  groups_release frees the scratch.
-int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, unsigned long long *gen, std::string *err);              // rollout.cu
-int groups_enqueue(UhcEngine *e, int G, const int *row0, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats, float zclip, const float *obs,
-                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err);                 // rollout.cu
-void groups_release(UhcEngine *e);                                                                                         // rollout.cu
+// groups_prepare converts and validates them (-2) and sizes the grouped policy scratch, a second instance (never the rollout's own); *gen
+// changes whenever that scratch is reallocated.  groups_enqueue: obs -> ZFilter of each group (zstats[g], no update) -> grouped GEMMs
+// (+ mixture head) -> the mean action (with mean_action all ones) of rows 0 .. row0[G] - 1; enqueues only (capturable).
+int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, std::vector<Policy> *pols, unsigned long long *gen);   // rollout.cu
+int groups_enqueue(UhcEngine *e, const std::vector<Policy> &pols, const int *row0, const double *const *zstats, float zclip, const float *obs,
+                   const unsigned char *mean_action, float *action, cudaStream_t st);                 // rollout.cu
 
 }  // namespace evalx
 }  // namespace uhc

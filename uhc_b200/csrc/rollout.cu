@@ -8,9 +8,12 @@
 //   k_gauss_sample_dev                                        action + log-prob into the buffer row                                  (a13)
 //   k_env_step                                                15 physics substeps + obs + reward + termination + in-kernel re-seeding (a1-a10)
 //   k_rollout_post                                            mask / fail / exp rows, device step counter += 1                        (a11)
-// and the whole T-step sequence is captured ONCE per (T, buffers, weights) into a CUDA graph and replayed: no host code and no torch
-// glue between the kernels.  Everything that varies between replays lives in device memory (the RNG step counter, the ZFilter
+// and the whole T-step sequence is captured ONCE per (T, buffers, weights) into a CUDA graph (graph_cache.h) and replayed: no host code
+// and no torch glue between the kernels.  Everything that varies between replays lives in device memory (the RNG step counter, the ZFilter
 // statistics, the env state), so a replay needs no new kernel parameters.
+//
+// The policy forward (scratch, validation, the walk over nets and layers) is written once here and also serves the evaluation and the
+// tracker (eval_glue.h), for one policy over all rows or for several side by side.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -20,6 +23,7 @@
 #include "../../include/uhc_nn.h"
 #include "../../include/uhc_rollout.h"
 #include "eval_glue.h"
+#include "graph_cache.h"
 #include "group_core.h"
 
 static thread_local std::string g_ro_err;
@@ -39,27 +43,30 @@ __device__ __forceinline__ float gauss_from(uint64_t seed, uint64_t idx) {   // 
     return sqrtf(-2.0f * logf(u1)) * cospif(2.0f * u2);
 }
 // ZFilter apply fused with the bf16 K-padded copy the first GEMM reads: y = clip((x - mean) / (std + 1e-8)) (zfilter.py:59-73);
-// arithmetic identical to k_zfilter_apply + k_f32_to_bf16_padded
+// arithmetic identical to k_zfilter_apply + k_f32_to_bf16_padded.  Element i = (row r, column j) of the [M][Kp] copy, under the statistics
+// `stats` of count n
+__device__ __forceinline__ void zfilter_apply_bf16_elem(const float *__restrict__ X, float *__restrict__ Y, unsigned short *__restrict__ Yb, size_t i, size_t r, int j,
+                                                        int D, const double *__restrict__ stats, double n, float clip) {
+    float y = 0.f;
+    if (j < D) {
+        const double mean = stats[1 + j], var = n > 1.0 ? stats[1 + D + j] / (n - 1.0) : mean * mean;
+        y = (float)(((double)X[r * D + j] - mean) / (sqrt(var) + 1e-8));
+        if (clip > 0.f) y = fminf(fmaxf(y, -clip), clip);
+        if (Y) Y[r * D + j] = y;
+    }
+    // round-to-nearest-even bf16 (what __float2bfloat16_rn does)
+    unsigned u = __float_as_uint(y);
+    unsigned short b = (y != y) ? 0x7FFF : (unsigned short)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+    Yb[i] = b;
+}
 __global__ void k_zfilter_apply_bf16(const float *__restrict__ X, float *__restrict__ Y, unsigned short *__restrict__ Yb, int M, int D, int Kp,
                                      const double *__restrict__ stats, float clip) {
     const double n = stats[0];
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)M * Kp; i += (size_t)gridDim.x * blockDim.x) {
-        const int j = (int)(i % Kp); const size_t r = i / Kp;
-        float y = 0.f;
-        if (j < D) {
-            const double mean = stats[1 + j], var = n > 1.0 ? stats[1 + D + j] / (n - 1.0) : mean * mean;
-            y = (float)(((double)X[r * D + j] - mean) / (sqrt(var) + 1e-8));
-            if (clip > 0.f) y = fminf(fmaxf(y, -clip), clip);
-            if (Y) Y[r * D + j] = y;
-        }
-        // round-to-nearest-even bf16 (what __float2bfloat16_rn does)
-        unsigned u = __float_as_uint(y);
-        unsigned short b = (y != y) ? 0x7FFF : (unsigned short)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
-        Yb[i] = b;
-    }
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)M * Kp; i += (size_t)gridDim.x * blockDim.x)
+        zfilter_apply_bf16_elem(X, Y, Yb, i, i / Kp, (int)(i % Kp), D, stats, n, clip);
 }
 // the same with one ZFilter per group of rows (the grouped evaluation: several checkpoints side by side): rows [row0[g], row0[g + 1])
-// are normalised by stats[g], with k_zfilter_apply_bf16's arithmetic
+// are normalised by stats[g]
 struct ZGroups { const double *stats[uhc::grp::MAX_GROUPS]; int row0[uhc::grp::MAX_GROUPS + 1]; int G; };
 __global__ void k_zfilter_apply_bf16_grouped(const float *__restrict__ X, float *__restrict__ Y, unsigned short *__restrict__ Yb, int M, int D, int Kp,
                                              const __grid_constant__ ZGroups zg, float clip) {
@@ -68,17 +75,7 @@ __global__ void k_zfilter_apply_bf16_grouped(const float *__restrict__ X, float 
         int lo = 0, hi = zg.G - 1;                 // the last group starting at or before row r
         while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if ((size_t)zg.row0[mid] <= r) lo = mid; else hi = mid - 1; }
         const double *stats = zg.stats[lo];
-        const double n = stats[0];
-        float y = 0.f;
-        if (j < D) {
-            const double mean = stats[1 + j], var = n > 1.0 ? stats[1 + D + j] / (n - 1.0) : mean * mean;
-            y = (float)(((double)X[r * D + j] - mean) / (sqrt(var) + 1e-8));
-            if (clip > 0.f) y = fminf(fmaxf(y, -clip), clip);
-            if (Y) Y[r * D + j] = y;
-        }
-        unsigned u = __float_as_uint(y);
-        unsigned short b = (y != y) ? 0x7FFF : (unsigned short)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
-        Yb[i] = b;
+        zfilter_apply_bf16_elem(X, Y, Yb, i, r, j, D, stats, stats[0], clip);
     }
 }
 // Bernoulli(1 - noise_rate) per env and step: mean_action flag and the `exp` row (agent_copycat.py:530,551)
@@ -126,24 +123,37 @@ __global__ void k_rollout_post(const int *__restrict__ fail, const int *__restri
     if (e == 0) *step_ptr += 1ull;   // ordered after every reader of this step's counter by the stream / graph dependencies
 }
 
-// the policy of a rollout: one MLP (PolicyGaussian, nprim = 0: nets[0]) or a PolicyMCP mixture (nets[0 .. nprim-1] = primitives, nets[nprim] = composer)
-struct Policy { int nprim; int pad; UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; };
+using uhc::GraphCache;
+using uhc::evalx::Policy;
+
+int num_nets(const Policy *pol) { return pol->nprim > 0 ? pol->nprim + 1 : 1; }
+int pad64(int n) { return (n + 63) / 64 * 64; }
+
+// every argument of uhc_rollout that reaches a kernel; zeroed, then filled: its bytes are the graph's key
 struct GraphKey {
     int T, row0, update_filter; float noise_rate, zclip; unsigned long long seed; Policy pol; UhcRolloutBuf buf; const float *log_std; double *zstats;
     unsigned long long cur_gen;   // the sampler's curriculum view (uhc_curriculum_enable) is captured by value: a new one needs a new graph
-    bool operator==(const GraphKey &o) const { return memcmp(this, &o, sizeof(GraphKey)) == 0; }
+};
+// the buffers of one policy forward over E rows.  Graphs hold these pointers as kernel parameters, so gen moves whenever one of them is
+// reallocated.  Zero filled once: the GEMMs write the first N columns of a K-padded activation only, and the grouped forward leaves the
+// rows past its groups alone
+struct PolicyScratch {
+    struct Net { void *acts[9] = {nullptr}; int ld[9] = {0}; };
+    Net ns[UHC_MCP_MAX_PRIM + 1];            // bf16 activations per net of the policy; ns[0].acts[0] (the normalised observation) feeds every net
+    float *d_mean = nullptr, *d_log_std0 = nullptr; int mean_cap = 0;   // d_log_std0: zeros, the grouped forward's log_std (its mask is all ones, so
+                                                                         // k_gauss_sample_dev writes mean + 1 * 0, what any finite log_std gives)
+    float *d_xall = nullptr, *d_comp = nullptr; size_t xall_cap = 0;    // PolicyMCP: primitive outputs [P][E][A], composer outputs [E][P]
+    unsigned long long gen = 0;
 };
 struct RolloutCtx {
     UhcEngine *eng = nullptr; int E = 0, device = 0;
     unsigned long long *d_step = nullptr;
-    struct NetScratch { void *acts[9] = {nullptr}; int ld[9] = {0}; };
-    NetScratch ns[UHC_MCP_MAX_PRIM + 1];     // bf16 activations per net of the policy; ns[0].acts[0] (the normalised observation) feeds every net
-    float *d_mean = nullptr; int mean_cap = 0;
-    float *d_xall = nullptr, *d_comp = nullptr; size_t xall_cap = 0;   // PolicyMCP: primitive outputs [P][E][A], composer outputs [E][P]
+    // two instances that never share an allocation: the rollout's, the single-policy evaluation's and the tracker's graphs hold `own`, the
+    // grouped evaluation's graphs hold `grouped`, and either may be resized while graphs over the other stay cached
+    PolicyScratch own, grouped;
     double *d_zws = nullptr; int zws_d = 0;
     unsigned char *d_mean_action = nullptr; float *d_cinfo = nullptr, *d_pct = nullptr; int *d_fail = nullptr, *d_end = nullptr;
-    std::vector<std::pair<GraphKey, cudaGraphExec_t>> graphs;
-    unsigned long long scratch_gen = 0;   // bumped whenever the scratch above is reallocated (the evaluation's graphs hold its pointers)
+    GraphCache graphs{64};
     int launches_per_step = 0;
     std::vector<cudaEvent_t> ev0, ev1;    // optional: events around the env-step kernel of buffer row r (bench roofline: the dominant kernel's live duration)
 };
@@ -155,77 +165,128 @@ RolloutCtx *ctx_of(UhcEngine *e) {
     g_ctx.push_back(c);
     return c;
 }
-int pad64(int n) { return (n + 63) / 64 * 64; }
 
-int ensure_scratch(RolloutCtx *c, const Policy *pol) {
+int check_policy(const Policy *pol) {
+    const int P = pol->nprim;
+    if (P < 0 || P > UHC_MCP_MAX_PRIM) { g_ro_err = "UhcMcp: 1..8 primitives"; return -2; }
+    const UhcMlp *m0 = &pol->nets[0];
+    for (int j = 0; j < num_nets(pol); j++) {
+        const UhcMlp *m = &pol->nets[j];
+        if (m->nlayers < 1 || m->nlayers > 8) { g_ro_err = "UhcMlp: 1..8 layers"; return -2; }
+        if (m->dims[0] != m0->dims[0]) { g_ro_err = "UhcMcp: every net reads the same observation"; return -2; }
+        if (j < P && m->dims[m->nlayers] != m0->dims[m0->nlayers]) { g_ro_err = "UhcMcp: the primitives must share the action width"; return -2; }
+        if (P > 0 && j == P && m->dims[m->nlayers] != P) { g_ro_err = "UhcMcp: the composer's output width must be the number of primitives"; return -2; }
+        for (int i = 0; i < m->nlayers; i++) {
+            if (m->kp[i] != pad64(m->dims[i])) { g_ro_err = "UhcMlp: kp[i] must be dims[i] rounded up to 64"; return -2; }
+            if (!m->W_bf16[i]) { g_ro_err = "UhcMlp: null weights"; return -2; }
+        }
+    }
+    return 0;
+}
+
+int realloc_zero(void **p, size_t bytes) {
+    if (*p) { cudaFree(*p); *p = nullptr; }
+    CKR(cudaMalloc(p, bytes)); CKR(cudaMemset(*p, 0, bytes));
+    return 0;
+}
+// validates pol (-2, nothing touched) and sizes s for it over E rows
+int ensure(PolicyScratch *s, size_t E, const Policy *pol) {
+    if (const int rc = check_policy(pol)) return rc;
+    const UhcMlp *m0 = &pol->nets[0];
+    const size_t P = pol->nprim, A = m0->dims[m0->nlayers];
+    for (int j = 0; j < num_nets(pol); j++) {
+        const UhcMlp *m = &pol->nets[j];
+        for (int i = 0; i < m->nlayers; i++) {
+            if ((i == 0 && j > 0) || s->ns[j].ld[i] == m->kp[i]) continue;       // the input is shared
+            s->gen++; s->ns[j].ld[i] = 0;
+            if (realloc_zero(&s->ns[j].acts[i], E * m->kp[i] * 2)) return -1;
+            s->ns[j].ld[i] = m->kp[i];
+        }
+    }
+    if ((size_t)s->mean_cap < A) {
+        s->gen++; s->mean_cap = 0;
+        if (realloc_zero((void **)&s->d_mean, E * A * 4) || realloc_zero((void **)&s->d_log_std0, A * 4)) return -1;
+        s->mean_cap = (int)A;
+    }
+    if (P > 0 && s->xall_cap < P * E * A) {
+        s->gen++; s->xall_cap = 0;
+        if (realloc_zero((void **)&s->d_xall, P * E * A * 4) || realloc_zero((void **)&s->d_comp, E * UHC_MCP_MAX_PRIM * 4)) return -1;
+        s->xall_cap = P * E * A;
+    }
+    return 0;
+}
+void release(PolicyScratch *s) {
+    for (auto &nsj : s->ns) for (void *p : nsj.acts) if (p) cudaFree(p);
+    for (void *p : {(void *)s->d_mean, (void *)s->d_log_std0, (void *)s->d_xall, (void *)s->d_comp}) if (p) cudaFree(p);
+}
+// the step counter and the per-env arrays of the context: allocated once, never moved
+int ensure_ctx(RolloutCtx *c) {
     const size_t E = c->E;
     if (!c->d_step) { CKR(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); CKR(cudaMemset(c->d_step, 0, sizeof(unsigned long long))); }
     if (!c->d_mean_action) {
         CKR(cudaMalloc((void **)&c->d_mean_action, E)); CKR(cudaMalloc((void **)&c->d_cinfo, E * 5 * 4)); CKR(cudaMalloc((void **)&c->d_pct, E * 4));
         CKR(cudaMalloc((void **)&c->d_fail, E * 4)); CKR(cudaMalloc((void **)&c->d_end, E * 4));
     }
-    const int P = pol->nprim, nnets = P > 0 ? P + 1 : 1;
-    if (P < 0 || P > UHC_MCP_MAX_PRIM) { g_ro_err = "UhcMcp: 1..8 primitives"; return -2; }
-    const UhcMlp *m0 = &pol->nets[0];
-    auto drop_graphs = [&]() { for (auto &g : c->graphs) cudaGraphExecDestroy(g.second); c->graphs.clear(); c->scratch_gen++; };
-    for (int j = 0; j < nnets; j++) {
-        const UhcMlp *m = &pol->nets[j];
-        if (m->nlayers < 1 || m->nlayers > 8) { g_ro_err = "UhcMlp: 1..8 layers"; return -2; }
-        if (m->dims[0] != m0->dims[0]) { g_ro_err = "UhcMcp: every net reads the same observation"; return -2; }
-        if (j < P && m->dims[m->nlayers] != m0->dims[m0->nlayers]) { g_ro_err = "UhcMcp: the primitives must share the action width"; return -2; }
-        if (P > 0 && j == P && m->dims[m->nlayers] != P) { g_ro_err = "UhcMcp: the composer's output width must be the number of primitives"; return -2; }
-        for (int i = 0; i < m->nlayers; i++) {   // bf16 activations, K padded to 64 and zero filled once (the GEMMs write the first N columns only)
-            const int ld = pad64(m->dims[i]);
-            if (m->kp[i] != ld) { g_ro_err = "UhcMlp: kp[i] must be dims[i] rounded up to 64"; return -2; }
-            if (i == 0 && j > 0) continue;       // the input is shared
-            if (c->ns[j].ld[i] != ld) {
-                if (c->ns[j].acts[i]) cudaFree(c->ns[j].acts[i]);
-                CKR(cudaMalloc(&c->ns[j].acts[i], E * ld * 2)); CKR(cudaMemset(c->ns[j].acts[i], 0, E * ld * 2));
-                c->ns[j].ld[i] = ld;
-                drop_graphs();
-            }
-        }
-    }
-    if (c->zws_d < m0->dims[0]) {
-        if (c->d_zws) cudaFree(c->d_zws);
-        CKR(cudaMalloc((void **)&c->d_zws, (size_t)uhc_zfilter_workspace_doubles(m0->dims[0]) * sizeof(double))); c->zws_d = m0->dims[0];
-        drop_graphs();
-    }
-    const int A = m0->dims[m0->nlayers];
-    if (c->mean_cap < A) { if (c->d_mean) cudaFree(c->d_mean); CKR(cudaMalloc((void **)&c->d_mean, E * A * 4)); c->mean_cap = A; drop_graphs(); }
-    if (P > 0 && c->xall_cap < (size_t)P * E * A) {
-        if (c->d_xall) cudaFree(c->d_xall);
-        if (c->d_comp) cudaFree(c->d_comp);
-        CKR(cudaMalloc((void **)&c->d_xall, (size_t)P * E * A * 4)); CKR(cudaMalloc((void **)&c->d_comp, E * UHC_MCP_MAX_PRIM * 4)); c->xall_cap = (size_t)P * E * A;
-        drop_graphs();
-    }
     return 0;
 }
+// the context's own scratch for pol.  Its graphs hold those pointers, so a reallocation drops them all; own.gen (the evaluation's and the
+// tracker's graphs hold the same pointers) has moved then
+int ensure_own(RolloutCtx *c, const Policy *pol) {
+    const unsigned long long gen0 = c->own.gen;
+    int rc = ensure_ctx(c);
+    if (!rc) rc = ensure(&c->own, c->E, pol);
+    const int D = pol->nets[0].dims[0];
+    if (!rc && c->zws_d < D) {
+        c->own.gen++; c->zws_d = 0;
+        rc = realloc_zero((void **)&c->d_zws, (size_t)uhc_zfilter_workspace_doubles(D) * sizeof(double));
+        if (!rc) c->zws_d = D;
+    }
+    if (c->own.gen != gen0) c->graphs.clear();
+    return rc;
+}
 
-// obs -> (state row, bf16 copy) -> MLP (or the PolicyMCP mixture: primitives, composer + softmax, weighted sum) -> mean (ctx scratch).
-// Returns the number of kernels enqueued (or < 0).
-int enqueue_policy(RolloutCtx *c, const float *obs, const Policy *pol, double *zstats, float zclip, int update_filter, float *state_out, cudaStream_t st) {
+// One layer of the walk below: the GEMM in [E][Kp] bf16 -> N columns, into the next bf16 activation (leading dimension ld) or, for a
+// net's last layer, into its fp32 output
+struct Layer { int net, i; const void *in; void *out_bf16; float *out_f32; int N, Kp, ld, act; };
+// the policy's nets layer by layer over the scratch s, then the mixture head: MLP -> d_mean; PolicyMCP: primitives -> d_xall, composer
+// (+ softmax) -> d_comp, weighted sum -> d_mean.  gemm(Layer) enqueues one layer.  Returns the number of kernels enqueued (or < 0).
+template <class Gemm>
+int enqueue_layers(const PolicyScratch &s, const Policy *pol, int E, cudaStream_t st, Gemm &&gemm) {
     const UhcMlp *m0 = &pol->nets[0];
-    const int E = c->E, D = m0->dims[0], P = pol->nprim, A = m0->dims[m0->nlayers];
+    const int P = pol->nprim, A = m0->dims[m0->nlayers];
     int n = 0;
-    if (update_filter) { CKC(uhc_zfilter_ws(obs, nullptr, E, D, zstats, zclip, 1, c->d_zws, st), "zfilter update"); n += 3; }
-    k_zfilter_apply_bf16<<<1056, 256, 0, st>>>(obs, state_out, (unsigned short *)c->ns[0].acts[0], E, D, m0->kp[0], zstats, zclip);
-    CKR(cudaGetLastError()); n++;
-    for (int j = 0; j < (P > 0 ? P + 1 : 1); j++) {
+    for (int j = 0; j < num_nets(pol); j++) {
         const UhcMlp *m = &pol->nets[j];
         const bool composer = P > 0 && j == P;
-        float *out = P == 0 ? c->d_mean : (composer ? c->d_comp : c->d_xall + (size_t)j * E * A);
+        float *out = P == 0 ? s.d_mean : (composer ? s.d_comp : s.d_xall + (size_t)j * E * A);
         for (int i = 0; i < m->nlayers; i++) {
             const bool last = i == m->nlayers - 1;
-            const void *in = i == 0 ? c->ns[0].acts[0] : c->ns[j].acts[i];
             // the composer is a plain MLP (mlp.py:24-27): its last affine layer is followed by the activation too, then the softmax (policy_mcp.py:26)
-            CKC(uhc_linear_forward_tc(in, m->W_bf16[i], m->bias[i], last ? nullptr : c->ns[j].acts[i + 1], last ? out : nullptr, E, m->dims[i + 1], m->kp[i],
-                                      last ? 0 : c->ns[j].ld[i + 1], (last && !composer) ? UHC_ACT_NONE : m->act, st), "policy GEMM");
+            const Layer l{j, i, i == 0 ? s.ns[0].acts[0] : s.ns[j].acts[i], last ? nullptr : s.ns[j].acts[i + 1], last ? out : nullptr, m->dims[i + 1], m->kp[i],
+                          last ? 0 : s.ns[j].ld[i + 1], (last && !composer) ? UHC_ACT_NONE : m->act};
+            if (gemm(l)) return -1;
             n++;
         }
     }
-    if (P > 0) { CKC(uhc_mcp_combine(c->d_xall, c->d_comp, nullptr, c->d_mean, E, A, P, st), "mixture head"); n++; }
+    // the mixture head is row-wise: run over every row (a row no policy covers holds zeros or earlier values and is never read)
+    if (P > 0) { CKC(uhc_mcp_combine(s.d_xall, s.d_comp, nullptr, s.d_mean, E, A, P, st), "mixture head"); n++; }
     return n;
+}
+
+// obs -> (state row, bf16 copy) -> policy -> mean (the context's own scratch).  Returns the number of kernels enqueued (or < 0).
+int enqueue_policy(RolloutCtx *c, const float *obs, const Policy *pol, double *zstats, float zclip, int update_filter, float *state_out, cudaStream_t st) {
+    const UhcMlp *m0 = &pol->nets[0];
+    const int E = c->E, D = m0->dims[0];
+    int n = 0;
+    if (update_filter) { CKC(uhc_zfilter_ws(obs, nullptr, E, D, zstats, zclip, 1, c->d_zws, st), "zfilter update"); n += 3; }
+    k_zfilter_apply_bf16<<<1056, 256, 0, st>>>(obs, state_out, (unsigned short *)c->own.ns[0].acts[0], E, D, m0->kp[0], zstats, zclip);
+    CKR(cudaGetLastError()); n++;
+    const int nl = enqueue_layers(c->own, pol, E, st, [&](const Layer &l) {
+        const UhcMlp *m = &pol->nets[l.net];
+        CKC(uhc_linear_forward_tc(l.in, m->W_bf16[l.i], m->bias[l.i], l.out_bf16, l.out_f32, E, l.N, l.Kp, l.ld, l.act, st), "policy GEMM");
+        return 0;
+    });
+    return nl < 0 ? nl : n + nl;
 }
 
 int enqueue_step(RolloutCtx *c, int row, const Policy *pol, const float *log_std, double *zstats, float zclip, int update_filter, unsigned long long seed,
@@ -239,7 +300,7 @@ int enqueue_step(RolloutCtx *c, int row, const Policy *pol, const float *log_std
     if (n < 0) return n;
     const bool mixed = noise_rate < 1.0f;
     if (mixed) { k_mean_action<<<(c->E + 255) / 256, 256, 0, st>>>(c->d_mean_action, exps_row, c->E, 1.0f - noise_rate, seed, c->d_step); CKR(cudaGetLastError()); n++; }
-    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->d_mean, log_std, mixed ? c->d_mean_action : nullptr, act_row, logp_row, c->E, A, seed, c->d_step);
+    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->own.d_mean, log_std, mixed ? c->d_mean_action : nullptr, act_row, logp_row, c->E, A, seed, c->d_step);
     CKR(cudaGetLastError()); n++;
     const bool timed = row < (int)c->ev0.size();
     // inside stream capture the record must be an EXTERNAL event-record node, or the event is owned by the graph and cannot be read from the host
@@ -297,46 +358,39 @@ static int policy_forward_impl(UhcEngine *e, const float *obs_dev, const Policy 
                                unsigned long long seed, const unsigned char *mean_action_or_null, float *state_out_or_null, float *action_out, float *logp_out_or_null,
                                void *stream) {
     RolloutCtx *c = ctx_of(e);
-    int rc = ensure_scratch(c, pol);
+    int rc = ensure_own(c, pol);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (enqueue_policy(c, obs_dev, pol, zfilter_stats, zclip, update_filter, state_out_or_null, st) < 0) return -1;
     const UhcMlp *m = &pol->nets[0];
-    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->d_mean, log_std, mean_action_or_null, action_out, logp_out_or_null, c->E, m->dims[m->nlayers], seed, c->d_step);
+    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->own.d_mean, log_std, mean_action_or_null, action_out, logp_out_or_null, c->E, m->dims[m->nlayers], seed, c->d_step);
     CKR(cudaGetLastError());
     return 0;
 }
 static int rollout_impl(UhcEngine *e, int T, int row0, const Policy *pol, const float *log_std, double *zfilter_stats, float zclip, int update_filter,
                         unsigned long long seed, float noise_rate, const UhcRolloutBuf *buf, int use_graph, void *stream) {
     RolloutCtx *c = ctx_of(e);
-    int rc = ensure_scratch(c, pol);
+    int rc = ensure_own(c, pol);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (!use_graph) {
         for (int k = 0; k < T; k++) { const int n = enqueue_step(c, row0 + k, pol, log_std, zfilter_stats, zclip, update_filter, seed, noise_rate, buf, st); if (n < 0) return -1; c->launches_per_step = n; }
         return 0;
     }
-    GraphKey key; memset(&key, 0, sizeof key);
-    key.T = T; key.row0 = row0; key.update_filter = update_filter; key.noise_rate = noise_rate; key.zclip = zclip; key.seed = seed; key.pol = *pol; key.buf = *buf;
-    key.log_std = log_std; key.zstats = zfilter_stats; key.cur_gen = uhc::evalx::curriculum_gen(e);
-    cudaGraphExec_t exec = nullptr;
-    for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
+    GraphKey k; memset(&k, 0, sizeof k);
+    k.T = T; k.row0 = row0; k.update_filter = update_filter; k.noise_rate = noise_rate; k.zclip = zclip; k.seed = seed; k.pol = *pol; k.buf = *buf;
+    k.log_std = log_std; k.zstats = zfilter_stats; k.cur_gen = uhc::evalx::curriculum_gen(e);
+    std::string key; GraphCache::append(&key, &k);
+    cudaGraphExec_t exec = c->graphs.find(key);
     if (!exec) {
-        // capture on a private stream (legacy-stream capture is not allowed), ordered after the caller's stream by an event
-        cudaStream_t cs; CKR(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaGraph_t graph = nullptr;
-        CKR(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
         int n = 0;
-        for (int k = 0; k < T && n >= 0; k++) n = enqueue_step(c, row0 + k, pol, log_std, zfilter_stats, zclip, update_filter, seed, noise_rate, buf, cs);
-        cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-        cudaStreamDestroy(cs);
-        if (n < 0) { if (graph) cudaGraphDestroy(graph); return -1; }
-        if (ce != cudaSuccess) { g_ro_err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce); return -1; }
+        rc = GraphCache::capture([&](cudaStream_t cs) {
+            for (int i = 0; i < T && n >= 0; i++) n = enqueue_step(c, row0 + i, pol, log_std, zfilter_stats, zclip, update_filter, seed, noise_rate, buf, cs);
+            return n < 0 ? -1 : 0;
+        }, &exec, &g_ro_err);
+        if (rc) return rc;
         c->launches_per_step = n;
-        CKR(cudaGraphInstantiate(&exec, graph, 0));
-        cudaGraphDestroy(graph);
-        if (c->graphs.size() >= 64) { cudaGraphExecDestroy(c->graphs.front().second); c->graphs.erase(c->graphs.begin()); }
-        c->graphs.emplace_back(key, exec);
+        c->graphs.insert(std::move(key), GraphCache::Gens{}, exec);   // nothing goes stale: the scratch drops them all, the rest is in the key
     }
     CKR(cudaGraphLaunch(exec, st));
     return 0;
@@ -378,7 +432,6 @@ int uhc_rollout_time_env_step(UhcEngine *e, int nrows) {
     if (!e || nrows < 0) { g_ro_err = "uhc_rollout_time_env_step: bad argument"; return -2; }
     RolloutCtx *c = ctx_of(e);
     CKR(cudaDeviceSynchronize());
-    for (auto &g : c->graphs) cudaGraphExecDestroy(g.second);
     c->graphs.clear();
     for (cudaEvent_t ev : c->ev0) cudaEventDestroy(ev);
     for (cudaEvent_t ev : c->ev1) cudaEventDestroy(ev);
@@ -400,86 +453,47 @@ int uhc_rollout_launches_per_step(UhcEngine *e) { return e ? ctx_of(e)->launches
 void uhc_rollout_release(UhcEngine *e) {   // called by the binding before uhc_engine_destroy
     for (size_t i = 0; i < g_ctx.size(); i++) if (g_ctx[i]->eng == e) {
         RolloutCtx *c = g_ctx[i];
-        for (auto &g : c->graphs) cudaGraphExecDestroy(g.second);
+        c->graphs.clear();
         for (cudaEvent_t ev : c->ev0) cudaEventDestroy(ev);
         for (cudaEvent_t ev : c->ev1) cudaEventDestroy(ev);
-        for (auto &nsj : c->ns) for (void *p : nsj.acts) if (p) cudaFree(p);
-        for (void *p : {(void *)c->d_xall, (void *)c->d_comp, (void *)c->d_zws, (void *)c->d_step, (void *)c->d_mean, (void *)c->d_mean_action, (void *)c->d_cinfo, (void *)c->d_pct, (void *)c->d_fail, (void *)c->d_end}) if (p) cudaFree(p);
+        release(&c->own); release(&c->grouped);
+        for (void *p : {(void *)c->d_zws, (void *)c->d_step, (void *)c->d_mean_action, (void *)c->d_cinfo, (void *)c->d_pct, (void *)c->d_fail, (void *)c->d_end}) if (p) cudaFree(p);
         delete c; g_ctx.erase(g_ctx.begin() + i); return;
     }
 }
 
 }  // extern "C"
 
-// ---- the policy forward of the device evaluation (eval_glue.h): the kernels of uhc_policy_forward(_mcp), enqueued from eval.cu's graphs
+// ---- the policy forward of the device evaluation and the tracker (eval_glue.h): the kernels of uhc_policy_forward(_mcp), enqueued from
+// eval.cu's and track.cu's graphs.  On failure the text is uhc_rollout_last_error()'s
 namespace uhc {
 namespace evalx {
 
-int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, unsigned long long *gen, std::string *err) {
-    Policy pol;
-    if (make_policy(&pol, mlp, mcp, e, mcp ? "uhc_eval_run_mcp" : "uhc_eval_run")) { *err = g_ro_err; return -2; }
+int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, Policy *pol, unsigned long long *gen) {
+    if (make_policy(pol, mlp, mcp, e, mcp ? "uhc_eval_run_mcp" : "uhc_eval_run")) return -2;
     RolloutCtx *c = ctx_of(e);
-    const int rc = ensure_scratch(c, &pol);
-    if (rc) { *err = g_ro_err; return rc; }
-    *gen = c->scratch_gen;
-    return 0;
+    const int rc = ensure_own(c, pol);
+    *gen = c->own.gen;
+    return rc;
 }
 
-int policy_enqueue(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, const float *obs, const float *log_std, double *zstats, float zclip,
-                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err) {
-    Policy pol;
-    if (make_policy(&pol, mlp, mcp, e, "uhc_eval_run")) { *err = g_ro_err; return -2; }
+int policy_enqueue(UhcEngine *e, const Policy &pol, const float *obs, const float *log_std, double *zstats, float zclip, const unsigned char *mean_action,
+                   float *action, cudaStream_t st) {
     RolloutCtx *c = ctx_of(e);
-    if (enqueue_policy(c, obs, &pol, zstats, zclip, 0, nullptr, st) < 0) { *err = g_ro_err; return -1; }
+    if (enqueue_policy(c, obs, &pol, zstats, zclip, 0, nullptr, st) < 0) return -1;
     const UhcMlp *m = &pol.nets[0];
-    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->d_mean, log_std, mean_action, action, nullptr, c->E, m->dims[m->nlayers], 0, c->d_step);
-    const cudaError_t ce = cudaGetLastError();
-    if (ce != cudaSuccess) { *err = std::string("k_gauss_sample_dev: ") + cudaGetErrorString(ce); return -1; }
+    k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->own.d_mean, log_std, mean_action, action, nullptr, c->E, m->dims[m->nlayers], 0, c->d_step);
+    CKR(cudaGetLastError());
     return 0;
 }
 
-// ---- the grouped policy forward of uhc_eval_run_groups: G policies of one architecture over consecutive row ranges, with scratch of its
-// own (the rollout's ns[] / d_mean pointers are baked into its graphs and the single-policy evaluation's)
+// ---- the grouped policy forward of uhc_eval_run_groups: G policies of one architecture over consecutive row ranges of the context's
+// second scratch
 namespace {
-struct GroupCtx {
-    UhcEngine *eng = nullptr; int E = 0;
-    RolloutCtx::NetScratch ns[UHC_MCP_MAX_PRIM + 1];
-    float *d_mean = nullptr; int mean_cap = 0;
-    float *d_xall = nullptr, *d_comp = nullptr; size_t xall_cap = 0;
-    float *d_log_std0 = nullptr; int ls_cap = 0;   // zeros: with the all-ones mask k_gauss_sample_dev then writes mean + 1 * 0, what any finite log_std gives
-    unsigned long long *d_step = nullptr;          // read (not used) by the deterministic sampler
-    unsigned long long gen = 0;                    // bumped whenever the scratch above is reallocated
-};
-std::vector<GroupCtx *> g_gctx;
-
-GroupCtx *gctx_of(UhcEngine *e) {
-    for (GroupCtx *c : g_gctx) if (c->eng == e) return c;
-    GroupCtx *c = new GroupCtx(); c->eng = e; c->E = uhc_num_envs(e);
-    g_gctx.push_back(c);
-    return c;
-}
-
-// the checks ensure_scratch makes, without allocating
-int check_policy(const Policy *pol) {
-    const int P = pol->nprim, nnets = P > 0 ? P + 1 : 1;
-    const UhcMlp *m0 = &pol->nets[0];
-    for (int j = 0; j < nnets; j++) {
-        const UhcMlp *m = &pol->nets[j];
-        if (m->nlayers < 1 || m->nlayers > 8) { g_ro_err = "UhcMlp: 1..8 layers"; return -2; }
-        if (m->dims[0] != m0->dims[0]) { g_ro_err = "UhcMcp: every net reads the same observation"; return -2; }
-        if (j < P && m->dims[m->nlayers] != m0->dims[m0->nlayers]) { g_ro_err = "UhcMcp: the primitives must share the action width"; return -2; }
-        if (P > 0 && j == P && m->dims[m->nlayers] != P) { g_ro_err = "UhcMcp: the composer's output width must be the number of primitives"; return -2; }
-        for (int i = 0; i < m->nlayers; i++) {
-            if (m->kp[i] != pad64(m->dims[i])) { g_ro_err = "UhcMlp: kp[i] must be dims[i] rounded up to 64"; return -2; }
-            if (!m->W_bf16[i]) { g_ro_err = "UhcMlp: null weights"; return -2; }
-        }
-    }
-    return 0;
-}
 // every group's policy must have group 0's architecture: primitive count, and per net the layer count, activation, widths and K padding
 bool same_arch(const Policy *a, const Policy *b) {
     if (a->nprim != b->nprim) return false;
-    for (int j = 0; j < (a->nprim > 0 ? a->nprim + 1 : 1); j++) {
+    for (int j = 0; j < num_nets(a); j++) {
         const UhcMlp &x = a->nets[j], &y = b->nets[j];
         if (x.nlayers != y.nlayers || x.act != y.act) return false;
         for (int i = 0; i <= x.nlayers; i++) if (x.dims[i] != y.dims[i]) return false;
@@ -487,110 +501,48 @@ bool same_arch(const Policy *a, const Policy *b) {
     }
     return true;
 }
-int make_group_policies(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, std::vector<Policy> *pols) {
+}  // namespace
+
+int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, std::vector<Policy> *pols, unsigned long long *gen) {
     const char *who = mcps ? "uhc_eval_run_groups_mcp" : "uhc_eval_run_groups";
     pols->resize(G);
     for (int g = 0; g < G; g++) {
-        if (make_policy(&(*pols)[g], mlps ? mlps + g : nullptr, mcps ? mcps + g : nullptr, e, who)) return -2;
-        if (check_policy(&(*pols)[g])) { g_ro_err = std::string(who) + ": " + g_ro_err; return -2; }
-        if (g > 0 && !same_arch(&(*pols)[0], &(*pols)[g])) { g_ro_err = std::string(who) + ": every group's policy must have the same layer widths, K padding, activation and primitive count"; return -2; }
+        Policy *p = &(*pols)[g];
+        if (make_policy(p, mlps ? mlps + g : nullptr, mcps ? mcps + g : nullptr, e, who)) return -2;
+        if (check_policy(p)) { g_ro_err = std::string(who) + ": " + g_ro_err; return -2; }
+        if (g > 0 && !same_arch(&(*pols)[0], p)) { g_ro_err = std::string(who) + ": every group's policy must have the same layer widths, K padding, activation and primitive count"; return -2; }
     }
-    return 0;
-}
-int ensure_group_scratch(GroupCtx *c, const Policy *pol) {
-    const size_t E = c->E;
-    const int P = pol->nprim;
-    const UhcMlp *m0 = &pol->nets[0];
-    const int A = m0->dims[m0->nlayers];
-    if (!c->d_step) { CKR(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); CKR(cudaMemset(c->d_step, 0, sizeof(unsigned long long))); }
-    for (int j = 0; j < (P > 0 ? P + 1 : 1); j++) {
-        const UhcMlp *m = &pol->nets[j];
-        for (int i = 0; i < m->nlayers; i++) {
-            if (i == 0 && j > 0) continue;       // the normalised observation feeds every net
-            const int ld = m->kp[i];
-            if (c->ns[j].ld[i] != ld) {
-                if (c->ns[j].acts[i]) cudaFree(c->ns[j].acts[i]);
-                CKR(cudaMalloc(&c->ns[j].acts[i], E * ld * 2)); CKR(cudaMemset(c->ns[j].acts[i], 0, E * ld * 2));
-                c->ns[j].ld[i] = ld; c->gen++;
-            }
-        }
-    }
-    if (c->mean_cap < A) {
-        if (c->d_mean) cudaFree(c->d_mean);
-        if (c->d_log_std0) cudaFree(c->d_log_std0);
-        CKR(cudaMalloc((void **)&c->d_mean, E * A * 4)); CKR(cudaMemset(c->d_mean, 0, E * A * 4));
-        CKR(cudaMalloc((void **)&c->d_log_std0, A * 4)); CKR(cudaMemset(c->d_log_std0, 0, A * 4));
-        c->mean_cap = A; c->gen++;
-    }
-    if (P > 0 && c->xall_cap < (size_t)P * E * A) {
-        if (c->d_xall) cudaFree(c->d_xall);
-        if (c->d_comp) cudaFree(c->d_comp);
-        CKR(cudaMalloc((void **)&c->d_xall, (size_t)P * E * A * 4)); CKR(cudaMemset(c->d_xall, 0, (size_t)P * E * A * 4));
-        CKR(cudaMalloc((void **)&c->d_comp, E * UHC_MCP_MAX_PRIM * 4)); CKR(cudaMemset(c->d_comp, 0, E * UHC_MCP_MAX_PRIM * 4));
-        c->xall_cap = (size_t)P * E * A; c->gen++;
-    }
-    return 0;
-}
-}  // namespace
-
-int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, unsigned long long *gen, std::string *err) {
-    std::vector<Policy> pols;
-    if (make_group_policies(e, G, mlps, mcps, &pols)) { *err = g_ro_err; return -2; }
-    GroupCtx *c = gctx_of(e);
-    const int rc = ensure_group_scratch(c, &pols[0]);
-    if (rc) { *err = g_ro_err; return rc; }
-    *gen = c->gen;
-    return 0;
+    RolloutCtx *c = ctx_of(e);
+    int rc = ensure_ctx(c);
+    if (!rc) rc = ensure(&c->grouped, c->E, &(*pols)[0]);
+    *gen = c->grouped.gen;
+    return rc;
 }
 
-int groups_enqueue(UhcEngine *e, int G, const int *row0, const UhcMlp *mlps, const UhcMcp *mcps, const double *const *zstats, float zclip, const float *obs,
-                   const unsigned char *mean_action, float *action, cudaStream_t st, std::string *err) {
-    std::vector<Policy> pols;
-    if (make_group_policies(e, G, mlps, mcps, &pols)) { *err = g_ro_err; return -2; }
-    GroupCtx *c = gctx_of(e);
-    const Policy &p0 = pols[0];
-    const UhcMlp *m0 = &p0.nets[0];
-    const int E = c->E, D = m0->dims[0], P = p0.nprim, A = m0->dims[m0->nlayers], ntot = row0[G];
+int groups_enqueue(UhcEngine *e, const std::vector<Policy> &pols, const int *row0, const double *const *zstats, float zclip, const float *obs,
+                   const unsigned char *mean_action, float *action, cudaStream_t st) {
+    RolloutCtx *c = ctx_of(e);
+    const PolicyScratch &s = c->grouped;
+    const UhcMlp *m0 = &pols[0].nets[0];
+    const int G = (int)pols.size(), ntot = row0[G];
     ZGroups zg;
     memset(&zg, 0, sizeof zg);
     zg.G = G;
-    std::vector<int> rows(G);
+    int rows[uhc::grp::MAX_GROUPS];
     for (int g = 0; g <= G; g++) zg.row0[g] = row0[g];
     for (int g = 0; g < G; g++) { zg.stats[g] = zstats[g]; rows[g] = row0[g + 1] - row0[g]; }
-    k_zfilter_apply_bf16_grouped<<<1056, 256, 0, st>>>(obs, nullptr, (unsigned short *)c->ns[0].acts[0], ntot, D, m0->kp[0], zg, zclip);
-    cudaError_t ce = cudaGetLastError();
-    if (ce != cudaSuccess) { *err = std::string("k_zfilter_apply_bf16_grouped: ") + cudaGetErrorString(ce); return -1; }
-    std::vector<const void *> W(G);
-    std::vector<const float *> b(G);
-    for (int j = 0; j < (P > 0 ? P + 1 : 1); j++) {
-        const UhcMlp *m = &p0.nets[j];
-        const bool composer = P > 0 && j == P;
-        float *out = P == 0 ? c->d_mean : (composer ? c->d_comp : c->d_xall + (size_t)j * E * A);
-        for (int i = 0; i < m->nlayers; i++) {
-            const bool last = i == m->nlayers - 1;
-            const void *in = i == 0 ? c->ns[0].acts[0] : c->ns[j].acts[i];
-            for (int g = 0; g < G; g++) { W[g] = pols[g].nets[j].W_bf16[i]; b[g] = pols[g].nets[j].bias[i]; }
-            if (uhc_linear_forward_tc_grouped(G, row0, rows.data(), in, W.data(), b.data(), last ? nullptr : c->ns[j].acts[i + 1], last ? out : nullptr, E,
-                                              m->dims[i + 1], m->kp[i], last ? 0 : c->ns[j].ld[i + 1], (last && !composer) ? UHC_ACT_NONE : m->act, st)) {
-                *err = std::string("grouped policy GEMM: ") + uhc_tc_last_error(); return -1;
-            }
-        }
-    }
-    // the mixture head is row-wise: run over every row (rows past the groups hold zeros or earlier values and are never read)
-    if (P > 0 && uhc_mcp_combine(c->d_xall, c->d_comp, nullptr, c->d_mean, E, A, P, st)) { *err = std::string("mixture head: ") + uhc_nn_last_error(); return -1; }
-    k_gauss_sample_dev<<<(ntot + 7) / 8, 256, 0, st>>>(c->d_mean, c->d_log_std0, mean_action, action, nullptr, ntot, A, 0, c->d_step);
-    ce = cudaGetLastError();
-    if (ce != cudaSuccess) { *err = std::string("k_gauss_sample_dev: ") + cudaGetErrorString(ce); return -1; }
+    k_zfilter_apply_bf16_grouped<<<1056, 256, 0, st>>>(obs, nullptr, (unsigned short *)s.ns[0].acts[0], ntot, m0->dims[0], m0->kp[0], zg, zclip);
+    CKR(cudaGetLastError());
+    const int nl = enqueue_layers(s, &pols[0], c->E, st, [&](const Layer &l) {
+        const void *W[uhc::grp::MAX_GROUPS]; const float *b[uhc::grp::MAX_GROUPS];
+        for (int g = 0; g < G; g++) { W[g] = pols[g].nets[l.net].W_bf16[l.i]; b[g] = pols[g].nets[l.net].bias[l.i]; }
+        CKC(uhc_linear_forward_tc_grouped(G, row0, rows, l.in, W, b, l.out_bf16, l.out_f32, c->E, l.N, l.Kp, l.ld, l.act, st), "grouped policy GEMM");
+        return 0;
+    });
+    if (nl < 0) return -1;
+    k_gauss_sample_dev<<<(ntot + 7) / 8, 256, 0, st>>>(s.d_mean, s.d_log_std0, mean_action, action, nullptr, ntot, m0->dims[m0->nlayers], 0, c->d_step);
+    CKR(cudaGetLastError());
     return 0;
-}
-
-void groups_release(UhcEngine *e) {
-    for (size_t i = 0; i < g_gctx.size(); i++) if (g_gctx[i]->eng == e) {
-        GroupCtx *c = g_gctx[i];
-        for (auto &nsj : c->ns) for (void *p : nsj.acts) if (p) cudaFree(p);
-        for (void *p : {(void *)c->d_mean, (void *)c->d_xall, (void *)c->d_comp, (void *)c->d_log_std0, (void *)c->d_step}) if (p) cudaFree(p);
-        delete c; g_gctx.erase(g_gctx.begin() + i); return;
-    }
 }
 
 }  // namespace evalx

@@ -1,5 +1,5 @@
 // track.cu -- the batched physics tracker behind the C ABI (include/uhc_track.h): target frames streamed one per control step into a
-// per-env window of expert-table rows, and one CUDA-graph replay per step of
+// per-env window of expert-table rows, and one CUDA-graph replay (graph_cache.h) per step of
 //   k_track_push  (when frames are passed)   per env: rebase a full window, the record of the new frame (track_core.h)
 //   k_track_gate                             per env: an env whose row cur_t + 1 was never pushed gets an invalid record for this step
 //   k_track_obs   (step_kernel.cu)           the observation of the stored state against row cur_t + 1 (track_obs.h)
@@ -16,6 +16,7 @@
 #include <vector>
 #include "../../include/uhc_track.h"
 #include "eval_glue.h"
+#include "graph_cache.h"
 #include "track_glue.h"
 #include "track_core.h"
 #include "sim_core.h"
@@ -99,10 +100,9 @@ __global__ void __launch_bounds__(128) k_track_post(const Real *__restrict__ sta
 
 __global__ void k_fill_ones(unsigned char *p, int n) { const int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = 1; }
 
+// every argument of a step that reaches a kernel; zeroed, then filled: its bytes are the graph's key
 struct TrackKey {
-    int has_next, has_mask, fail_safe, nprim; float zclip; unsigned long long scratch_gen, track_gen, view_gen;
-    UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; const float *log_std; const double *zstats; void *out; float *rew; int *fail;
-    bool operator==(const TrackKey &o) const { return memcmp(this, &o, sizeof(TrackKey)) == 0; }
+    int has_next, has_mask, fail_safe; float zclip; evalx::Policy pol; const float *log_std; const double *zstats; void *out; float *rew; int *fail;
 };
 struct TrackCtx {
     UhcEngine *eng = nullptr;
@@ -114,7 +114,7 @@ struct TrackCtx {
     int *h_ids = nullptr;                          // pinned staging of the reset's env ids
     cudaEvent_t ids_done = nullptr;                // the last k_track_rows that read d_ids has been enqueued before it
     std::vector<int> zeros, lens;                  // reset arguments of uhc_env_reset (start 0, length H)
-    std::vector<std::pair<TrackKey, cudaGraphExec_t>> graphs;
+    GraphCache graphs{32};                         // one step each (graph_cache.h)
 };
 std::vector<TrackCtx *> g_tr;
 unsigned long long g_tr_gen = 0;                   // distinct per begin: graphs never outlive the buffers they hold
@@ -122,7 +122,7 @@ unsigned long long g_tr_gen = 0;                   // distinct per begin: graphs
 TrackCtx *find_ctx(UhcEngine *e) { for (TrackCtx *c : g_tr) if (c->eng == e) return c; return nullptr; }
 void free_ctx(TrackCtx *c) {
     cudaDeviceSynchronize();
-    for (auto &g : c->graphs) cudaGraphExecDestroy(g.second);
+    c->graphs.clear();
     for (void *p : {(void *)c->d_raw, (void *)c->d_next, (void *)c->d_have, (void *)c->d_steps, (void *)c->d_dropped, (void *)c->d_status, (void *)c->d_reseat,
                     (void *)c->d_mask, (void *)c->d_fk, (void *)c->d_ids, (void *)c->d_ones}) if (p) cudaFree(p);
     if (c->h_ids) cudaFreeHost(c->h_ids);
@@ -153,16 +153,15 @@ int enqueue_push(TrackCtx *c, const evalx::EngineRefs &R, const double *next, co
     return 0;
 }
 
-int enqueue_step(TrackCtx *c, const evalx::EngineRefs &R, const TrackKey &k, const UhcMlp *mlp, const UhcMcp *mcp, cudaStream_t st) {
+int enqueue_step(TrackCtx *c, const evalx::EngineRefs &R, const TrackKey &k, cudaStream_t st) {
     UhcEngine *e = c->eng;
     const int E = c->E, nb = (E + 127) / 128;
     if (k.has_next && enqueue_push(c, R, c->d_next, k.has_mask ? c->d_mask : nullptr, st)) return -1;
     k_track_gate<<<nb, 128, 0, st>>>(R.istate, c->d_have, c->H, E, R.num_clips, c->d_status);
     CKT(cudaGetLastError());
     CKT(trackx::launch_obs(e, R.obs, st));
-    std::string err;
-    int rc = evalx::policy_enqueue(e, mlp, mcp, R.obs, k.log_std, (double *)k.zstats, k.zclip, c->d_ones, R.act, st, &err);
-    if (rc) { g_tr_err = err; return rc; }
+    const int rc = evalx::policy_enqueue(e, k.pol, R.obs, k.log_std, (double *)k.zstats, k.zclip, c->d_ones, R.act, st);
+    if (rc) { g_tr_err = uhc_rollout_last_error(); return rc; }
     if (uhc_env_step(e, R.act, nullptr, k.rew, R.cinfo, k.fail, R.end, R.pct, nullptr, st)) { g_tr_err = std::string("env step: ") + uhc_last_error(); return -1; }
     if (R.precision == 32)
         k_track_post<float><<<(E + 3) / 4, 128, 0, st>>>((const float *)R.state, R.istate, c->d_status, k.fail, k.fail_safe, E, c->d_steps, c->d_reseat, (float *)k.out);
@@ -179,43 +178,26 @@ int track_step(UhcEngine *e, const double *next, const int *mask, const UhcMlp *
     if (!e || (!mlp && !mcp) || !log_std || !zstats || !out || !rew || !fail) { g_tr_err = std::string(who) + ": null argument"; return -2; }
     TrackCtx *c = live_ctx(e, who);
     if (!c) return -2;
-    unsigned long long sgen = 0; std::string err;
-    int rc = evalx::policy_prepare(e, mlp, mcp, &sgen, &err);
-    if (rc) { g_tr_err = err; return rc; }
+    TrackKey k; memset(&k, 0, sizeof k);
+    unsigned long long sgen = 0;
+    int rc = evalx::policy_prepare(e, mlp, mcp, &k.pol, &sgen);
+    if (rc) { g_tr_err = uhc_rollout_last_error(); return rc; }
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     cudaStream_t st = (cudaStream_t)stream;
-    TrackKey key; memset(&key, 0, sizeof key);
-    key.has_next = next != nullptr; key.has_mask = next && mask; key.fail_safe = fail_safe ? 1 : 0; key.zclip = zclip;
-    key.scratch_gen = sgen; key.track_gen = c->gen; key.view_gen = R.view_gen; key.log_std = log_std; key.zstats = zstats;
-    key.out = out; key.rew = rew; key.fail = fail;
-    if (mcp) { key.nprim = mcp->nprim; for (int k = 0; k < mcp->nprim; k++) key.nets[k] = mcp->prim[k]; key.nets[mcp->nprim] = mcp->composer; }
-    else key.nets[0] = *mlp;
-    // the graphs hold the engine view, the policy scratch and the stream buffers as kernel parameters: a changed generation drops them
-    for (size_t g = 0; g < c->graphs.size();) {
-        const TrackKey &k = c->graphs[g].first;
-        if (k.view_gen != key.view_gen || k.scratch_gen != key.scratch_gen || k.track_gen != key.track_gen) {
-            cudaGraphExecDestroy(c->graphs[g].second); c->graphs.erase(c->graphs.begin() + g);
-        } else g++;
-    }
+    k.has_next = next != nullptr; k.has_mask = next && mask; k.fail_safe = fail_safe ? 1 : 0; k.zclip = zclip;
+    k.log_std = log_std; k.zstats = zstats; k.out = out; k.rew = rew; k.fail = fail;
+    std::string key; GraphCache::append(&key, &k);
+    // the graphs also hold the policy scratch, the stream buffers and the engine view as kernel parameters: a changed generation drops them
+    const GraphCache::Gens gens{sgen, c->gen, R.view_gen};
+    c->graphs.drop_stale(gens);
     // the caller's frames and mask are copied into the tracker's own buffers, so a new tensor per step replays the same graph
     if (next) CKT(cudaMemcpyAsync(c->d_next, next, (size_t)c->E * c->row_w * sizeof(double), cudaMemcpyDeviceToDevice, st));
     if (next && mask) CKT(cudaMemcpyAsync(c->d_mask, mask, (size_t)c->E * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    cudaGraphExec_t exec = nullptr;
-    for (auto &g : c->graphs) if (g.first == key) { exec = g.second; break; }
+    cudaGraphExec_t exec = c->graphs.find(key);
     if (!exec) {
-        cudaStream_t cs; CKT(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-        cudaGraph_t graph = nullptr;
-        CKT(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-        rc = enqueue_step(c, R, key, mlp, mcp, cs);
-        cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-        cudaStreamDestroy(cs);
-        if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-        if (ce != cudaSuccess) { g_tr_err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce); return -1; }
-        ce = cudaGraphInstantiate(&exec, graph, 0);
-        cudaGraphDestroy(graph);
-        CKT(ce);
-        if (c->graphs.size() >= 32) { cudaGraphExecDestroy(c->graphs.front().second); c->graphs.erase(c->graphs.begin()); }
-        c->graphs.emplace_back(key, exec);
+        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_step(c, R, k, cs); }, &exec, &g_tr_err);
+        if (rc) return rc;
+        c->graphs.insert(std::move(key), gens, exec);
     }
     CKT(cudaGraphLaunch(exec, st));
     return 0;
