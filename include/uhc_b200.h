@@ -78,6 +78,8 @@ typedef struct {
     int reward_mul;             /* != 0: reward_id world_rfc_implicit_v1_mul (reward_function.py:174-250): pose * vel * ee * com * (vf if w[4] != 0), same five c_info terms */
 } UhcEnvCfg;
 
+/* the calling thread's one error text, written by whichever call of the library (any header) last failed; the uhc_*_last_error
+ * of the other headers are aliases of it */
 const char *uhc_last_error(void);
 
 /* precision: 32 (product) or 64 (fp64 debug build of the same kernels). */

@@ -8,7 +8,7 @@
  * one "any env alive" count per `window` steps.
  * Pointers suffixed _host are host memory (frames_host / states_host should be pinned: their copies are asynchronous); the others are
  * CUDA device pointers (PyTorch tensors).  Returns 0 on success, -2 on a bad argument (the engine stays usable), -1 on a CUDA error
- * (uhc_eval_last_error()).  The call returns after its last copy has landed.
+ * (uhc_last_error()).  The call returns after its last copy has landed.
  */
 #ifndef UHC_EVAL_H
 #define UHC_EVAL_H
@@ -44,7 +44,7 @@ typedef struct {
     double *smpl_host_or_null;     /* [n][max(len) - 1][UHC_EVAL_SMPL] */
 } UhcEvalOut;
 
-const char *uhc_eval_last_error(void);
+const char *uhc_eval_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
 
 /* Envs 0..n-1 are reset onto clips clip_host[0..n-1] from frame 0 (envs n..E-1 are parked on clip_host[0]), then stepped with the
  * deterministic policy (the mean action; zfilter_stats are read, not updated) for up to max(len) - 1 control steps under the engine's

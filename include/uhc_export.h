@@ -4,7 +4,7 @@
  * pose [T][24][3] (SMPL_BONE_ORDER_NAMES order) and a translation [T][3] through scipy's Rotation.  Here one thread per frame restates it in
  * fp64 (uhc_b200/csrc/smpl_export_core.h), the inverse of the SMPL -> qpos conversion of uhc_load_motions.
  * Pointers suffixed _dev are CUDA device pointers.  Returns 0 on success, -2 on a bad argument (nothing is launched and the engine stays
- * usable), -1 on a CUDA error (uhc_export_last_error()).
+ * usable), -1 on a CUDA error (uhc_last_error()).
  */
 #ifndef UHC_EXPORT_H
 #define UHC_EXPORT_H
@@ -14,7 +14,7 @@
 extern "C" {
 #endif
 
-const char *uhc_export_last_error(void);
+const char *uhc_export_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
 
 /* n frames, frame i's qpos (76 values) at qpos_dev + i * qpos_pitch elements, fp32 (precision 32) or fp64 (64): a pitch of 223 reads the
  * tracker's state_out rows, 148 the evaluation's state record, 76 a plain qpos array.  variant_dev_or_null = [n] shape variant per frame

@@ -1,7 +1,7 @@
 /* uhc_nn.h -- C ABI of the policy/value network, Gaussian head, observation normaliser, GAE and PPO-update kernels
  * (part of libuhc_b200.so).  All pointers are CUDA device pointers owned by the caller (PyTorch tensors hold the weights --
  * the checkpoint format of the reference is a torch state_dict, uhc/agents/agent_copycat.py:190-201); `stream` is a cudaStream_t.
- * Return 0 on success, <0 on error (uhc_nn_last_error()).  Each entry cites the reference Python it replaces.
+ * Return 0 on success, <0 on error (uhc_last_error()).  Each entry cites the reference Python it replaces.
  */
 #ifndef UHC_NN_H
 #define UHC_NN_H
@@ -11,8 +11,9 @@ extern "C" {
 
 enum { UHC_ACT_NONE = 0, UHC_ACT_GELU = 1, UHC_ACT_TANH = 2, UHC_ACT_RELU = 3, UHC_ACT_SIGMOID = 4 };  /* mlp.py:9-16 */
 
+/* aliases of uhc_last_error (uhc_b200.h): the library keeps one error text, the tensor-core entry points included */
 const char *uhc_nn_last_error(void);
-const char *uhc_tc_last_error(void);   /* last error of the tensor-core entry points (uhc_linear_forward_tc*, uhc_transpose_bf16, uhc_dact_bf16) */
+const char *uhc_tc_last_error(void);
 
 /* nn.Linear + activation (khrylib/models/mlp.py:24-27):  y[M][N] = act(x[M][K] W[N][K]^T + b[N]); z (optional) = pre-activation. */
 int uhc_linear_forward(const float *x, const float *W, const float *b, float *y, float *z_or_null, int M, int N, int K, int act, void *stream);

@@ -11,7 +11,7 @@
  * global-batch statistics (advantage moments and count, selected-row count, the ranks' ZFilter increments) ride in the tail of the first one.
  *
  * Every GEMM runs on the wgmma kernel (bf16 operands, fp32 accumulate; mlp_wgmma.cu); parameters, gradients and Adam moments are fp32.
- * All pointers are device pointers unless marked host.  Functions return 0 on success; uhc_ppo_last_error() describes the last failure.
+ * All pointers are device pointers unless marked host.  Functions return 0 on success; uhc_last_error() describes the last failure.
  */
 #ifndef UHC_PPO_H
 #define UHC_PPO_H
@@ -44,7 +44,7 @@ typedef struct UhcPpoCfg {
 
 typedef struct UhcPpoTrainer UhcPpoTrainer;
 
-const char *uhc_ppo_last_error(void);
+const char *uhc_ppo_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
 
 /* workspace for updates of up to max_rows transitions from up to max_envs environments (both nets, shared backward scratch) */
 int uhc_ppo_trainer_create(const UhcNetDesc *policy, const UhcNetDesc *value, long max_rows, int max_envs, int device, UhcPpoTrainer **out);

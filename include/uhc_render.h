@@ -5,7 +5,7 @@
  * `gt` in one MuJoCo scene and reads 1920x1080 frames back from the GL viewer.  The camera is MuJoCo's free camera as the visualizer sets it
  * (setup_viewing_angle: lookat z 1, azimuth 45, elevation -8, distance 5; update_pose's focus / hide_im / hide_expert / shift_expert).
  * Pointers suffixed _dev are CUDA device pointers.  Every call returns 0 on success, -2 on a bad argument (nothing is launched and the engine
- * stays usable), -1 on a CUDA error (uhc_render_last_error()).  Pixel indices are size_t: n * H * W * 3 may exceed 2^31.
+ * stays usable), -1 on a CUDA error (uhc_last_error()).  Pixel indices are size_t: n * H * W * 3 may exceed 2^31.
  */
 #ifndef UHC_RENDER_H
 #define UHC_RENDER_H
@@ -37,7 +37,7 @@ typedef struct {
     double shift_expert;
 } UhcRenderCamera;
 
-const char *uhc_render_last_error(void);
+const char *uhc_render_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
 
 /* Uploads the plane tables (as fp32) once per engine; a second call replaces them.  -2 unless nshape equals the engine's shape variants,
  * every body has 4 .. UHC_RENDER_MAX_PLANES planes inside 0 .. nplane - 1, and every value is finite.  Synchronises the device. */

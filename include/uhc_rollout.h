@@ -7,7 +7,7 @@
  *                        normalise -> policy -> sample -> env.step -> custom_reward -> push(state, action, mask, reward, exp); finished
  *                        episodes are re-seeded inside the step kernel (UhcEnvCfg.auto_reset, :503-517 + dataset_amass_single.py:172-253).
  * All pointers are CUDA device pointers owned by the caller (PyTorch tensors: weights, ZFilter statistics, rollout buffer) unless
- * suffixed _host.  Calls are stream-ordered on `stream`; return 0 on success, <0 on error (uhc_rollout_last_error()).
+ * suffixed _host.  Calls are stream-ordered on `stream`; return 0 on success, <0 on error (uhc_last_error()).
  */
 #ifndef UHC_ROLLOUT_H
 #define UHC_ROLLOUT_H
@@ -69,7 +69,7 @@ int uhc_curriculum_set(UhcEngine *e, const int *len_host, const float *pct_host,
 /* re-seeds every env through the in-kernel sampler (a fit_clip change takes effect at once); obs_dev [E][obs_dim] gets the reset rows */
 int uhc_curriculum_reseed(UhcEngine *e, float *obs_dev, void *stream);
 
-const char *uhc_rollout_last_error(void);
+const char *uhc_rollout_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
 
 /* RNG stream position of the action noise: element (step, env, dim) of the stream `seed`; advanced by one per rollout step. */
 int uhc_rollout_set_step(UhcEngine *e, unsigned long long step);

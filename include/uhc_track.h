@@ -8,7 +8,7 @@
  *
  * Tracking mode owns the engine's clip table: env e follows clip e, a window of H rows.  A later uhc_load_clips / uhc_load_motions ends
  * it (uhc_track_step then returns -2).  Pointers suffixed _dev are CUDA device pointers, _host host pointers.  Returns 0 on success,
- * -2 on a bad argument (the engine is left as it was), -1 on a CUDA error (uhc_track_last_error()).
+ * -2 on a bad argument (the engine is left as it was), -1 on a CUDA error (uhc_last_error()).
  */
 #ifndef UHC_TRACK_H
 #define UHC_TRACK_H
@@ -23,7 +23,7 @@ extern "C" {
 /* columns of state_out_dev: qpos 76, qvel 75, world body positions xpos 72, in the engine's precision */
 #define UHC_TRACK_OUT 223
 
-const char *uhc_track_last_error(void);
+const char *uhc_track_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
 
 /* Installs a table of E clips x `window` rows (env e owns clip e) through the table set-up of uhc_load_clips: every env record is
  * invalidated, clip models = fk_model_host (NULL: variant 0; also the FK's shape variant), shape vectors = shape_host [E][17] (NULL: zero).

@@ -15,7 +15,7 @@ import time
 import numpy as np
 
 from . import nn
-from .engine import EVAL_SMPL, Engine
+from .engine import EVAL_SMPL, Engine, _chk
 from .motion_lib import MotionSet
 
 
@@ -207,9 +207,6 @@ class BatchedAgent:
         replayed as one CUDA graph.  Needs auto_reset (finished episodes are re-seeded inside the step kernel)."""
         assert self.auto_reset, "uhc_rollout re-seeds finished episodes in the step kernel: build the agent with auto_reset=True"
         L = self.engine.lib
-        if not getattr(self, "_ro_ready", False):
-            L.uhc_rollout_last_error.restype = C.c_char_p
-            self._ro_ready = True
         mcp = self.actor_type == "mcp"
         if self.policy._bf16 is None or getattr(self, "_mlp_c", None) is None:
             self._mlp_c = nn.mcp_struct(self.policy) if mcp else nn.mlp_struct(self.policy)
@@ -220,8 +217,7 @@ class BatchedAgent:
         rc = (L.uhc_rollout_mcp if mcp else L.uhc_rollout)(self.engine.h, C.c_int(T), C.c_int(row0), C.byref(self._mlp_c), C.c_void_p(self.log_std.data_ptr()),
                            C.c_void_p(self.running_state.stats.data_ptr()), C.c_float(self.running_state.clip), C.c_int(1),
                            C.c_ulonglong(self.seed * 1000003 + self.rank), C.c_float(self.noise_rate), C.byref(bs), C.c_int(int(use_graph)), st)
-        if rc != 0:
-            raise RuntimeError("uhc_rollout: " + L.uhc_rollout_last_error().decode())
+        _chk(rc, "uhc_rollout")
         self.global_step += T
         self._ro_step = self.global_step
         self.nn_launches += T * (L.uhc_rollout_launches_per_step(self.engine.h) - 1)      # the env-step launch is counted by the engine

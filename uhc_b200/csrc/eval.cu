@@ -20,6 +20,7 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_eval.h"
+#include "errors.h"
 #include "eval_core.h"
 #include "eval_glue.h"
 #include "graph_cache.h"
@@ -28,9 +29,6 @@
 #include "track_glue.h"
 
 using namespace uhc;
-
-static thread_local std::string g_ev_err;
-#define CKE(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_ev_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
 
 namespace {
 
@@ -120,26 +118,26 @@ EvalCtx *ev_ctx(UhcEngine *e) {
 int ensure(EvalCtx *c, int n, int window, bool states, bool smpl) {
     const size_t E = c->E;
     if (!c->d_clips) {
-        CKE(cudaMalloc((void **)&c->d_clips, E * sizeof(UhcEvalClip))); CKE(cudaMalloc((void **)&c->d_alive, E * 4)); CKE(cudaMalloc((void **)&c->d_reseat, E * 4));
-        CKE(cudaMalloc((void **)&c->d_count, 4)); CKE(cudaMalloc((void **)&c->d_ones, E)); CKE(cudaMalloc((void **)&c->d_ring, E * RING * sizeof(double)));
-        CKE(cudaHostAlloc((void **)&c->h_count, 4, cudaHostAllocDefault)); CKE(cudaEventCreateWithFlags(&c->ev, cudaEventDisableTiming));
+        CK(cudaMalloc((void **)&c->d_clips, E * sizeof(UhcEvalClip))); CK(cudaMalloc((void **)&c->d_alive, E * 4)); CK(cudaMalloc((void **)&c->d_reseat, E * 4));
+        CK(cudaMalloc((void **)&c->d_count, 4)); CK(cudaMalloc((void **)&c->d_ones, E)); CK(cudaMalloc((void **)&c->d_ring, E * RING * sizeof(double)));
+        CK(cudaHostAlloc((void **)&c->h_count, 4, cudaHostAllocDefault)); CK(cudaEventCreateWithFlags(&c->ev, cudaEventDisableTiming));
         c->gen++;
     }
     const int need = n * window;
     if (need > c->win_cap) {
         if (c->d_win) cudaFree(c->d_win);
-        CKE(cudaMalloc((void **)&c->d_win, (size_t)need * NCOL * sizeof(double))); c->win_cap = need; c->gen++;
+        CK(cudaMalloc((void **)&c->d_win, (size_t)need * NCOL * sizeof(double))); c->win_cap = need; c->gen++;
     }
     if (states && need > c->states_cap) {
         if (c->d_wstates) cudaFree(c->d_wstates);
-        CKE(cudaMalloc((void **)&c->d_wstates, (size_t)need * NSTATE * sizeof(double))); c->states_cap = need; c->gen++;
+        CK(cudaMalloc((void **)&c->d_wstates, (size_t)need * NSTATE * sizeof(double))); c->states_cap = need; c->gen++;
     }
     if (smpl && (size_t)need > c->smpl_cap) {
         if (c->d_wsmpl) cudaFree(c->d_wsmpl);
         c->d_wsmpl = nullptr; c->smpl_cap = 0; c->gen++;
-        CKE(cudaMalloc((void **)&c->d_wsmpl, (size_t)need * UHC_EVAL_SMPL * sizeof(double))); c->smpl_cap = (size_t)need;
+        CK(cudaMalloc((void **)&c->d_wsmpl, (size_t)need * UHC_EVAL_SMPL * sizeof(double))); c->smpl_cap = (size_t)need;
     }
-    if (smpl && !c->d_xdone) { CKE(cudaMalloc((void **)&c->d_xdone, E * sizeof(int))); c->gen++; }
+    if (smpl && !c->d_xdone) { CK(cudaMalloc((void **)&c->d_xdone, E * sizeof(int))); c->gen++; }
     return 0;
 }
 
@@ -148,10 +146,10 @@ int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const EvalPolicies &P
     for (int s = 0; s < window; s++) {
         const int rc = P.grouped ? evalx::groups_enqueue(c->eng, P.pols, P.row0.data(), P.zstats, zclip, R.obs, c->d_ones, R.act, st)
                                  : evalx::policy_enqueue(c->eng, P.pols[0], R.obs, P.log_std, (double *)P.zstats[0], zclip, c->d_ones, R.act, st);
-        if (rc) { g_ev_err = uhc_rollout_last_error(); return rc; }
-        if (uhc_env_step(c->eng, R.act, R.obs, R.rew, R.cinfo, R.fail, R.end, R.pct, nullptr, st)) { g_ev_err = std::string("env step: ") + uhc_last_error(); return -1; }
+        if (rc) return rc;
+        if (uhc_env_step(c->eng, R.act, R.obs, R.rew, R.cinfo, R.fail, R.end, R.pct, nullptr, st)) return uhc_err_prefix("env step");
         const bool last = s == window - 1;
-        if (last) CKE(cudaMemsetAsync(c->d_count, 0, 4, st));
+        if (last) CK(cudaMemsetAsync(c->d_count, 0, 4, st));
         if (R.precision == 32)
             k_eval_frame<float><<<(n + 127) / 128, 128, 0, st>>>((const float *)R.state, R.istate, (const float *)R.expert, R.clip_adr, R.rew, R.fail, R.end, n, nrec_max,
                                                                 fail_safe, window, s, c->d_clips, c->d_alive, c->d_reseat, c->d_ring, c->d_win,
@@ -160,10 +158,10 @@ int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const EvalPolicies &P
             k_eval_frame<double><<<(n + 127) / 128, 128, 0, st>>>((const double *)R.state, R.istate, (const double *)R.expert, R.clip_adr, R.rew, R.fail, R.end, n, nrec_max,
                                                                  fail_safe, window, s, c->d_clips, c->d_alive, c->d_reseat, c->d_ring, c->d_win,
                                                                  states ? c->d_wstates : nullptr, last ? c->d_count : nullptr);
-        CKE(cudaGetLastError());
-        if (smpl) CKE(smplx::launch_eval_export(R.precision, R.state, R.istate, trackx::clip_models(c->eng), trackx::motion_model(c->eng).body, c->d_clips,
+        CK(cudaGetLastError());
+        if (smpl) CK(smplx::launch_eval_export(R.precision, R.state, R.istate, trackx::clip_models(c->eng), trackx::motion_model(c->eng).body, c->d_clips,
                                                 c->d_xdone, n, window, s, c->d_wsmpl, st));
-        if (fail_safe) CKE(evalx::launch_reseat(c->eng, n, c->d_reseat, st));
+        if (fail_safe) CK(evalx::launch_reseat(c->eng, n, c->d_reseat, st));
     }
     return 0;
 }
@@ -174,38 +172,38 @@ int reset_envs(EvalCtx *c, UhcEngine *e, const evalx::EngineRefs &R, int n, cons
         const int m = R.E - n;
         c->ids.resize(m); c->clip0.assign(m, clip_host[0]); c->start.assign(m, 0); c->len.assign(m, R.clip_len_h[clip_host[0]]);
         for (int k = 0; k < m; k++) c->ids[k] = n + k;
-        if (uhc_env_reset(e, m, c->ids.data(), c->clip0.data(), c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
+        if (uhc_env_reset(e, m, c->ids.data(), c->clip0.data(), c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) return uhc_err_prefix("reset");
     }
     c->ids.resize(n); c->start.assign(n, 0); c->len.resize(n);
     for (int k = 0; k < n; k++) { c->ids[k] = k; c->len[k] = R.clip_len_h[clip_host[k]]; }
-    if (uhc_env_reset(e, n, c->ids.data(), clip_host, c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) { g_ev_err = std::string("reset: ") + uhc_last_error(); return -1; }
+    if (uhc_env_reset(e, n, c->ids.data(), clip_host, c->start.data(), c->len.data(), nullptr, nullptr, R.obs, st)) return uhc_err_prefix("reset");
     k_eval_init<<<(R.E + 127) / 128, 128, 0, st>>>(n, c->d_clips, c->d_alive, c->d_reseat, c->d_ones, R.E);
-    CKE(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
 // replays until every env has stopped or nrec_max steps have run; after each, the window's rows of envs 0..n-1 go to the caller's arrays
 int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, const UhcEvalOut &o, cudaStream_t st) {
     double *frames_host = o.frames_host, *states_host = o.states_host_or_null, *smpl_host = o.smpl_host_or_null;
-    if (smpl_host && (!c->d_wsmpl || c->smpl_cap < (size_t)n * (size_t)window)) { g_ev_err = "SMPL export: the window buffer is smaller than n * window rows"; return -1; }
+    if (smpl_host && (!c->d_wsmpl || c->smpl_cap < (size_t)n * (size_t)window)) { uhc_err() = "SMPL export: the window buffer is smaller than n * window rows"; return -1; }
     for (int s0 = 0; s0 < nrec_max; s0 += window) {
-        CKE(cudaGraphLaunch(exec, st));
+        CK(cudaGraphLaunch(exec, st));
         const int rows = nrec_max - s0 < window ? nrec_max - s0 : window;
-        CKE(cudaMemcpy2DAsync(frames_host + (size_t)s0 * NCOL, (size_t)nrec_max * NCOL * sizeof(double), c->d_win, (size_t)window * NCOL * sizeof(double),
+        CK(cudaMemcpy2DAsync(frames_host + (size_t)s0 * NCOL, (size_t)nrec_max * NCOL * sizeof(double), c->d_win, (size_t)window * NCOL * sizeof(double),
                               (size_t)rows * NCOL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
         if (states_host)
-            CKE(cudaMemcpy2DAsync(states_host + (size_t)s0 * NSTATE, (size_t)nrec_max * NSTATE * sizeof(double), c->d_wstates, (size_t)window * NSTATE * sizeof(double),
+            CK(cudaMemcpy2DAsync(states_host + (size_t)s0 * NSTATE, (size_t)nrec_max * NSTATE * sizeof(double), c->d_wstates, (size_t)window * NSTATE * sizeof(double),
                                   (size_t)rows * NSTATE * sizeof(double), n, cudaMemcpyDeviceToHost, st));
         if (smpl_host)
-            CKE(cudaMemcpy2DAsync(smpl_host + (size_t)s0 * UHC_EVAL_SMPL, (size_t)nrec_max * UHC_EVAL_SMPL * sizeof(double), c->d_wsmpl,
+            CK(cudaMemcpy2DAsync(smpl_host + (size_t)s0 * UHC_EVAL_SMPL, (size_t)nrec_max * UHC_EVAL_SMPL * sizeof(double), c->d_wsmpl,
                                   (size_t)window * UHC_EVAL_SMPL * sizeof(double), (size_t)rows * UHC_EVAL_SMPL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
-        CKE(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
-        CKE(cudaEventRecord(c->ev, st));
-        CKE(cudaEventSynchronize(c->ev));
+        CK(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaEventRecord(c->ev, st));
+        CK(cudaEventSynchronize(c->ev));
         if (*c->h_count == 0) break;
     }
-    CKE(cudaMemcpyAsync(o.clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
-    CKE(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(o.clips_host, c->d_clips, (size_t)n * sizeof(UhcEvalClip), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     return 0;
 }
 
@@ -213,7 +211,7 @@ int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, co
 int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *clip_host, const UhcMlp *mlps, const UhcMcp *mcps, const float *log_std,
              const double *const *zstats, float zclip, int fail_safe, int window, const UhcEvalOut &o, void *stream) {
     const std::string who = std::string(grouped ? "uhc_eval_run_groups" : "uhc_eval_run") + (mcps ? "_mcp" : "");
-    auto refuse = [&](const char *why) { g_ev_err = who + ": " + why; return -2; };
+    auto refuse = [&](const char *why) { uhc_err() = who + ": " + why; return -2; };
     if (!e || !group_n || !clip_host || (!mlps && !mcps) || !zstats || (!grouped && (!log_std || !zstats[0])) || !o.frames_host || !o.clips_host) return refuse("null argument");
     if (G < 1 || G > UHC_EVAL_MAX_GROUPS) return refuse("G must be 1 .. UHC_EVAL_MAX_GROUPS");
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
@@ -236,16 +234,16 @@ int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *c
     }
     unsigned long long pgen = 0;
     int rc = grouped ? evalx::groups_prepare(e, G, mlps, mcps, &P.pols, &pgen) : evalx::policy_prepare(e, mlps, mcps, &P.pols[0], &pgen);
-    if (rc) { g_ev_err = uhc_rollout_last_error(); return rc; }
+    if (rc) return rc;
     EvalCtx *c = ev_ctx(e);
     const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr;
     if (ensure(c, n, window, states, smpl)) return -1;
     cudaStream_t st = (cudaStream_t)stream;
     const int nrec_max = max_len - 1;
     if (reset_envs(c, e, R, n, clip_host, st)) return -1;
-    if (smpl) CKE(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
+    if (smpl) CK(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
     // no grouped policy covers the parked envs: they step with zero actions (the graph writes action rows 0 .. n-1 only)
-    if (grouped && n < R.E) CKE(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
+    if (grouped && n < R.E) CK(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
 
     // the key: every argument the graph's kernels got.  The generations: the graph also holds the policy scratch, the window buffers and
     // the engine view (cfg, clip table) of its capture, and is dropped once any of them has changed
@@ -260,7 +258,7 @@ int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *c
     cache.drop_stale(gens);
     cudaGraphExec_t exec = cache.find(key);
     if (!exec) {
-        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_window(c, R, P, zclip, n, nrec_max, head.fail_safe, window, states, smpl, cs); }, &exec, &g_ev_err);
+        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_window(c, R, P, zclip, n, nrec_max, head.fail_safe, window, states, smpl, cs); }, &exec);
         if (rc) return rc;
         cache.insert(std::move(key), gens, exec);
     }
@@ -270,8 +268,6 @@ int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *c
 }  // namespace
 
 extern "C" {
-
-const char *uhc_eval_last_error(void) { return g_ev_err.c_str(); }
 
 static UhcEvalOut eval_out(double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null) {
     UhcEvalOut o; o.frames_host = frames_host; o.clips_host = clips_host; o.states_host_or_null = states_host_or_null; o.smpl_host_or_null = nullptr;
@@ -302,26 +298,26 @@ int uhc_eval_run_groups_mcp(UhcEngine *e, int G, const int *group_n_host, const 
 
 int uhc_eval_run_ex(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
                     int fail_safe, int window, const UhcEvalOut *out, void *stream) {
-    if (!mlp) { g_ev_err = "uhc_eval_run: null policy"; return -2; }
-    if (!out) { g_ev_err = "uhc_eval_run: null output struct"; return -2; }
+    if (!mlp) { uhc_err() = "uhc_eval_run: null policy"; return -2; }
+    if (!out) { uhc_err() = "uhc_eval_run: null output struct"; return -2; }
     return eval_run(e, false, 1, &n, clip_host, mlp, nullptr, log_std, &zfilter_stats, zclip, fail_safe, window, *out, stream);
 }
 int uhc_eval_run_mcp_ex(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
                         int fail_safe, int window, const UhcEvalOut *out, void *stream) {
-    if (!mcp) { g_ev_err = "uhc_eval_run_mcp: null policy"; return -2; }
-    if (!out) { g_ev_err = "uhc_eval_run_mcp: null output struct"; return -2; }
+    if (!mcp) { uhc_err() = "uhc_eval_run_mcp: null policy"; return -2; }
+    if (!out) { uhc_err() = "uhc_eval_run_mcp: null output struct"; return -2; }
     return eval_run(e, false, 1, &n, clip_host, nullptr, mcp, log_std, &zfilter_stats, zclip, fail_safe, window, *out, stream);
 }
 int uhc_eval_run_groups_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMlp *mlps, const double *const *zfilter_stats_host,
                            float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream) {
-    if (!mlps) { g_ev_err = "uhc_eval_run_groups: null policy"; return -2; }
-    if (!out) { g_ev_err = "uhc_eval_run_groups: null output struct"; return -2; }
+    if (!mlps) { uhc_err() = "uhc_eval_run_groups: null policy"; return -2; }
+    if (!out) { uhc_err() = "uhc_eval_run_groups: null output struct"; return -2; }
     return eval_run(e, true, G, group_n_host, clip_host, mlps, nullptr, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
 }
 int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
                                float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream) {
-    if (!mcps) { g_ev_err = "uhc_eval_run_groups_mcp: null policy"; return -2; }
-    if (!out) { g_ev_err = "uhc_eval_run_groups_mcp: null output struct"; return -2; }
+    if (!mcps) { uhc_err() = "uhc_eval_run_groups_mcp: null policy"; return -2; }
+    if (!out) { uhc_err() = "uhc_eval_run_groups_mcp: null output struct"; return -2; }
     return eval_run(e, true, G, group_n_host, clip_host, nullptr, mcps, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
 }
 

@@ -28,7 +28,7 @@ unsigned long long curriculum_gen(const UhcEngine *e);
 // the policy of a rollout as a flat net list: one MLP (PolicyGaussian, nprim = 0: nets[0]) or a PolicyMCP mixture (nets[0 .. nprim-1] =
 // primitives, nets[nprim] = composer).  Zeroed before it is filled, so its bytes can go into a graph key
 struct Policy { int nprim; int pad; UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; };
-// The four calls below return 0 or an error code with its text in uhc_rollout_last_error().
+// The four calls below return 0 or an error code with its text in uhc_err() (errors.h).
 // policy of an evaluation or a tracker step: converts and validates it (-2) and sizes the rollout's policy scratch outside any capture;
 // *gen changes whenever that scratch is reallocated (graphs holding the old pointers must be dropped)
 int policy_prepare(UhcEngine *e, const UhcMlp *mlp, const UhcMcp *mcp, Policy *pol, unsigned long long *gen);   // rollout.cu

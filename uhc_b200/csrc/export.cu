@@ -8,14 +8,13 @@
 #include "../../include/uhc_eval.h"
 #include "../../include/uhc_export.h"
 #include "../../include/uhc_track.h"
+#include "errors.h"
 #include "eval_glue.h"
 #include "sim_core.h"
 #include "smpl_export_core.h"
 #include "track_glue.h"
 
 using namespace uhc;
-
-static thread_local std::string g_ex_err;
 
 namespace uhc {
 namespace smplx {
@@ -72,39 +71,37 @@ cudaError_t launch_eval_export(int precision, const void *state, const int *ista
 
 extern "C" {
 
-const char *uhc_export_last_error(void) { return g_ex_err.c_str(); }
-
 int uhc_qpos_to_smpl(UhcEngine *e, const void *qpos_dev, int precision, long n, long qpos_pitch, const int *variant_dev_or_null,
                      double *pose_dev, double *trans_dev, void *stream) {
-    if (!e) { g_ex_err = "uhc_qpos_to_smpl: null engine"; return -2; }
-    if (n < 0) { g_ex_err = "uhc_qpos_to_smpl: n < 0"; return -2; }
-    if (precision != 32 && precision != 64) { g_ex_err = "uhc_qpos_to_smpl: precision must be 32 or 64"; return -2; }
-    if (qpos_pitch < 76) { g_ex_err = "uhc_qpos_to_smpl: qpos_pitch < 76"; return -2; }
-    if (n > 0 && (!qpos_dev || !pose_dev || !trans_dev)) { g_ex_err = "uhc_qpos_to_smpl: null pointer"; return -2; }
+    if (!e) { uhc_err() = "uhc_qpos_to_smpl: null engine"; return -2; }
+    if (n < 0) { uhc_err() = "uhc_qpos_to_smpl: n < 0"; return -2; }
+    if (precision != 32 && precision != 64) { uhc_err() = "uhc_qpos_to_smpl: precision must be 32 or 64"; return -2; }
+    if (qpos_pitch < 76) { uhc_err() = "uhc_qpos_to_smpl: qpos_pitch < 76"; return -2; }
+    if (n > 0 && (!qpos_dev || !pose_dev || !trans_dev)) { uhc_err() = "uhc_qpos_to_smpl: null pointer"; return -2; }
     if (n == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     if (variant_dev_or_null) {
         std::vector<int> v((size_t)n);
         cudaError_t ce = cudaMemcpyAsync(v.data(), variant_dev_or_null, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st);
         if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-        if (ce != cudaSuccess) { g_ex_err = std::string("uhc_qpos_to_smpl: reading the variants: ") + cudaGetErrorString(ce); return -1; }
+        if (ce != cudaSuccess) { uhc_err() = std::string("uhc_qpos_to_smpl: reading the variants: ") + cudaGetErrorString(ce); return -1; }
         const int ns = trackx::num_shapes(e);
         for (long i = 0; i < n; i++)
-            if (v[(size_t)i] < 0 || v[(size_t)i] >= ns) { g_ex_err = "uhc_qpos_to_smpl: variant out of range"; return -2; }
+            if (v[(size_t)i] < 0 || v[(size_t)i] >= ns) { uhc_err() = "uhc_qpos_to_smpl: variant out of range"; return -2; }
     }
     const cudaError_t ce = smplx::launch_qpos_to_smpl(qpos_dev, precision, n, qpos_pitch, variant_dev_or_null, trackx::motion_model(e).body,
                                                       pose_dev, trans_dev, st);
-    if (ce != cudaSuccess) { g_ex_err = std::string("uhc_qpos_to_smpl: ") + cudaGetErrorString(ce); return -1; }
+    if (ce != cudaSuccess) { uhc_err() = std::string("uhc_qpos_to_smpl: ") + cudaGetErrorString(ce); return -1; }
     return 0;
 }
 
 int uhc_track_smpl(UhcEngine *e, const void *state_out_dev, double *pose_dev, double *trans_dev, void *stream) {
-    if (!e || !state_out_dev || !pose_dev || !trans_dev) { g_ex_err = "uhc_track_smpl: null argument"; return -2; }
+    if (!e || !state_out_dev || !pose_dev || !trans_dev) { uhc_err() = "uhc_track_smpl: null argument"; return -2; }
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
-    if (!trackx::tracking(e) || R.num_clips != R.E) { g_ex_err = "uhc_track_smpl: not tracking (uhc_track_begin), or the tracker's table was replaced"; return -2; }
+    if (!trackx::tracking(e) || R.num_clips != R.E) { uhc_err() = "uhc_track_smpl: not tracking (uhc_track_begin), or the tracker's table was replaced"; return -2; }
     const cudaError_t ce = smplx::launch_qpos_to_smpl(state_out_dev, R.precision, R.E, UHC_TRACK_OUT, trackx::clip_models(e),
                                                       trackx::motion_model(e).body, pose_dev, trans_dev, (cudaStream_t)stream);
-    if (ce != cudaSuccess) { g_ex_err = std::string("uhc_track_smpl: ") + cudaGetErrorString(ce); return -1; }
+    if (ce != cudaSuccess) { uhc_err() = std::string("uhc_track_smpl: ") + cudaGetErrorString(ce); return -1; }
     return 0;
 }
 

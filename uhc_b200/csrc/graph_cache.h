@@ -11,6 +11,7 @@
 #include <string>
 #include <utility>
 #include <vector>
+#include "errors.h"
 
 namespace uhc {
 
@@ -31,12 +32,12 @@ public:
         return nullptr;
     }
     // enqueue(stream) -> 0 or its error code, run under capture on a private stream (a legacy-stream capture is not allowed; the replay
-    // is ordered by the stream it is launched on).  Returns enqueue's code unchanged, with the error text it left, or -1 and the CUDA
-    // error in *err.
-    template <class Enqueue> static int capture(Enqueue &&enqueue, cudaGraphExec_t *exec, std::string *err) {
+    // is ordered by the stream it is launched on).  Returns enqueue's code unchanged, with the error text it left, or -1 with the CUDA
+    // error in uhc_err().
+    template <class Enqueue> static int capture(Enqueue &&enqueue, cudaGraphExec_t *exec) {
         cudaStream_t cs; cudaGraph_t graph = nullptr;
         cudaError_t ce = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
-        if (ce != cudaSuccess) { *err = std::string("cudaStreamCreateWithFlags: ") + cudaGetErrorString(ce); return -1; }
+        if (ce != cudaSuccess) { uhc_err() = std::string("cudaStreamCreateWithFlags: ") + cudaGetErrorString(ce); return -1; }
         int rc = 0; const char *what = "begin of the stream capture";
         ce = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
         if (ce == cudaSuccess) {
@@ -47,7 +48,7 @@ public:
         if (rc == 0 && ce == cudaSuccess) { what = "cudaGraphInstantiate"; ce = cudaGraphInstantiate(exec, graph, 0); }
         if (graph) cudaGraphDestroy(graph);
         if (rc) return rc;
-        if (ce != cudaSuccess) { *err = std::string(what) + ": " + cudaGetErrorString(ce); return -1; }
+        if (ce != cudaSuccess) { uhc_err() = std::string(what) + ": " + cudaGetErrorString(ce); return -1; }
         return 0;
     }
     void insert(std::string key, const Gens &gens, cudaGraphExec_t exec) {

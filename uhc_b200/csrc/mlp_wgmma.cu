@@ -15,6 +15,7 @@
 #include <string.h>
 #include <string>
 #include "../../include/uhc_nn.h"
+#include "errors.h"
 #include "group_core.h"
 
 namespace {
@@ -31,7 +32,6 @@ static_assert(ACC_OFF + BM * ACC_LD * 4 <= STAGES * STAGE_BYTES, "epilogue stagi
 #ifndef UHC_TC_TMA_STORE
 #define UHC_TC_TMA_STORE 1       /* outputs leave through the TMA engine (cp.async.bulk.tensor shared -> global) where their row pitch allows it */
 #endif
-thread_local std::string g_tc_err;
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t cnt) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(cnt)); }
@@ -638,23 +638,23 @@ EncodeFn get_encode() {
 }
 int make_map(CUtensorMap *m, const void *base, int rows, int Kp, int box_rows = BM) {  // row-major [rows][Kp] bf16, box 64 x 128, 128B swizzle
     EncodeFn enc = get_encode();
-    if (!enc) { g_tc_err = "cuTensorMapEncodeTiled unavailable"; return -1; }
+    if (!enc) { uhc_err() = "cuTensorMapEncodeTiled unavailable"; return -1; }
     cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)Kp * 2};
     cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows}, estr[2] = {1, 1};
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void *)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled failed: " + std::to_string((int)r); return -1; }
+    if (r != CUDA_SUCCESS) { uhc_err() = "cuTensorMapEncodeTiled failed: " + std::to_string((int)r); return -1; }
     return 0;
 }
 // output tensor map: row-major [rows][cols] with a row pitch of `pitch` bytes, 32 x 32 boxes; the staging tiles use the 128-byte (fp32) / 64-byte (bf16) swizzle
 int make_map_out(CUtensorMap *m, const void *base, int rows, int cols, size_t pitch, bool bf16) {
     EncodeFn enc = get_encode();
-    if (!enc) { g_tc_err = "cuTensorMapEncodeTiled unavailable"; return -1; }
+    if (!enc) { uhc_err() = "cuTensorMapEncodeTiled unavailable"; return -1; }
     cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)pitch};
     cuuint32_t box[2] = {32, 32}, estr[2] = {1, 1};
     CUresult r = enc(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void *)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      bf16 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { g_tc_err = "cuTensorMapEncodeTiled (output) failed: " + std::to_string((int)r); return -1; }
+    if (r != CUDA_SUCCESS) { uhc_err() = "cuTensorMapEncodeTiled (output) failed: " + std::to_string((int)r); return -1; }
     return 0;
 }
 bool tma_store_enabled() {
@@ -668,25 +668,23 @@ int set_smem_attr(int dev) {
     static bool attr_set[64] = {false};
     if (dev >= 0 && dev < 64 && attr_set[dev]) return 0;
     if (cudaFuncSetAttribute(k_linear_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
-        cudaFuncSetAttribute(k_linear_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { g_tc_err = "cudaFuncSetAttribute failed"; return -1; }
+        cudaFuncSetAttribute(k_linear_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { uhc_err() = "cudaFuncSetAttribute failed"; return -1; }
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
     return 0;
 }
 }  // namespace
 
 extern "C" {
-const char *uhc_tc_last_error(void) { return g_tc_err.c_str(); }
-
 int uhc_f32_to_bf16_padded(const float *x, void *y_bf16, int M, int K, int Kp, void *stream) {
     k_f32_to_bf16_padded<<<1056, 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)y_bf16, M, K, Kp);
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+    CK(cudaGetLastError()); return 0;
 }
 
 static int linear_tc_impl(const void *x_bf16, const void *W_bf16, const float *b, void *y_bf16_or_null, float *y_f32_or_null, float *z_f32_or_null,
                           int M, int N, int Kp, int ldy_bf16, int act, void *stream, void *yT_bf16_or_null = nullptr, int ld_yT = 0, int ld_yf = 0) {
     if (ld_yf <= 0) ld_yf = N;      // row pitch of the fp32 y in floats (only a plain fp32 product through the TMA engine takes a pitch other than N)
-    if (Kp % BK != 0 || M <= 0 || N <= 0) { g_tc_err = "uhc_linear_forward_tc: Kp must be a positive multiple of 64"; return -2; }
-    if (y_bf16_or_null && (ldy_bf16 % 8 != 0)) { g_tc_err = "uhc_linear_forward_tc: ldy must be a multiple of 8"; return -2; }
+    if (Kp % BK != 0 || M <= 0 || N <= 0) { uhc_err() = "uhc_linear_forward_tc: Kp must be a positive multiple of 64"; return -2; }
+    if (y_bf16_or_null && (ldy_bf16 % 8 != 0)) { uhc_err() = "uhc_linear_forward_tc: ldy must be a multiple of 8"; return -2; }
     int dev = 0; cudaGetDevice(&dev);
     if (set_smem_attr(dev)) return -1;
     CUtensorMap ma, mb;
@@ -718,18 +716,18 @@ static int linear_tc_impl(const void *x_bf16, const void *W_bf16, const float *b
         }
         if (y_bf16_or_null && ok(y_bf16_or_null, pb)) { if (make_map_out(&myb, y_bf16_or_null, M, ldy_bf16, pb, true)) return -1; tma_mask |= 4; }
     }
-    if (ld_yf != N && !(tma_mask & 2)) { g_tc_err = "uhc_linear_forward_tc_f32_pitched: a padded pitch needs the TMA store path and a 16-byte aligned output"; return -2; }
-    if ((ksplit > 1 || ld_yf != N) && cudaMemsetAsync(y_f32_or_null, 0, (size_t)M * ld_yf * sizeof(float), (cudaStream_t)stream) != cudaSuccess) { g_tc_err = "memset failed"; return -1; }   // (a padded pitch: the padding columns read as zeros)
+    if (ld_yf != N && !(tma_mask & 2)) { uhc_err() = "uhc_linear_forward_tc_f32_pitched: a padded pitch needs the TMA store path and a 16-byte aligned output"; return -2; }
+    if ((ksplit > 1 || ld_yf != N) && cudaMemsetAsync(y_f32_or_null, 0, (size_t)M * ld_yf * sizeof(float), (cudaStream_t)stream) != cudaSuccess) { uhc_err() = "memset failed"; return -1; }   // (a padded pitch: the padding columns read as zeros)
     CUtensorMap myt = ma;
     if (yT_bf16_or_null) {      // transposed activation [N][ld_yT] (ld_yT >= M rounded up to 64, the padding columns receive the tile's zero rows)
-        if (!tma_store_enabled() || y_f32_or_null || ((uintptr_t)yT_bf16_or_null & 15) || ld_yT % 8 != 0 || ld_yT < M) { g_tc_err = "uhc_linear_forward_tc_train_t: the transposed output needs the TMA store path, no fp32 y, and a pitch >= M that is a multiple of 8"; return -2; }
+        if (!tma_store_enabled() || y_f32_or_null || ((uintptr_t)yT_bf16_or_null & 15) || ld_yT % 8 != 0 || ld_yT < M) { uhc_err() = "uhc_linear_forward_tc_train_t: the transposed output needs the TMA store path, no fp32 y, and a pitch >= M that is a multiple of 8"; return -2; }
         if (make_map_out(&myt, yT_bf16_or_null, N, ld_yT, (size_t)ld_yT * 2, true)) return -1;
         tma_mask |= 8;
     }
     k_linear_tc<false><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(ma, mb, b, (__nv_bfloat16 *)y_bf16_or_null, y_f32_or_null, z_f32_or_null, M, N, Kp, ldy_bf16, act, ksplit,
                                                                             mz, myf, myb, tma_mask, myt, nullptr);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { g_tc_err = cudaGetErrorString(e); return -1; }
+    if (e != cudaSuccess) { uhc_err() = cudaGetErrorString(e); return -1; }
     return 0;
 }
 
@@ -745,13 +743,13 @@ int uhc_linear_forward_tc_train(const void *x_bf16, const void *W_bf16, const fl
  * written by the same epilogue through the TMA engine instead of by a separate transpose kernel */
 int uhc_linear_forward_tc_train_t(const void *x_bf16, const void *W_bf16, const float *b, void *y_bf16, void *yT_bf16, int ld_yT, float *z_f32_or_null,
                                   int M, int N, int Kp, int ldy_bf16, int act, void *stream) {
-    if (!y_bf16 || !yT_bf16) { g_tc_err = "uhc_linear_forward_tc_train_t: y and yT are required"; return -2; }
+    if (!y_bf16 || !yT_bf16) { uhc_err() = "uhc_linear_forward_tc_train_t: y and yT are required"; return -2; }
     return linear_tc_impl(x_bf16, W_bf16, b, y_bf16, nullptr, z_f32_or_null, M, N, Kp, ldy_bf16, act, stream, yT_bf16, ld_yT);
 }
 /* plain fp32 product y[M][ld_y] = x W^T with a row pitch ld_y >= N (floats, multiple of 4): lets an output whose own pitch no tensor map accepts (N % 4 != 0) be
  * computed through the TMA engine (split-K included) into a padded scratch.  Returns -2 when the arguments do not qualify (then use uhc_linear_forward_tc). */
 int uhc_linear_forward_tc_f32_pitched(const void *x_bf16, const void *W_bf16, float *y_f32, int ld_y, int M, int N, int Kp, void *stream) {
-    if (!y_f32 || ld_y < N || ld_y % 4 != 0 || ((uintptr_t)y_f32 & 15) || !tma_store_enabled()) { g_tc_err = "uhc_linear_forward_tc_f32_pitched: arguments not eligible"; return -2; }
+    if (!y_f32 || ld_y < N || ld_y % 4 != 0 || ((uintptr_t)y_f32 & 15) || !tma_store_enabled()) { uhc_err() = "uhc_linear_forward_tc_f32_pitched: arguments not eligible"; return -2; }
     return linear_tc_impl(x_bf16, W_bf16, nullptr, nullptr, y_f32, nullptr, M, N, Kp, 0, UHC_ACT_NONE, stream, nullptr, 0, ld_y);
 }
 int uhc_tc_tma_store_enabled(void) { return tma_store_enabled() ? 1 : 0; }
@@ -760,19 +758,19 @@ int uhc_tc_tma_store_enabled(void) { return tma_store_enabled() ? 1 : 0; }
 int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_host, const void *x_bf16, const void *const *W_bf16_host,
                                   const float *const *b_host_or_null, void *y_bf16_or_null, float *y_f32_or_null, int M, int N, int Kp, int ldy_bf16,
                                   int act, void *stream) {
-    if (!x_bf16 || !W_bf16_host || (!y_bf16_or_null && !y_f32_or_null)) { g_tc_err = "uhc_linear_forward_tc_grouped: null argument"; return -2; }
-    if (Kp % BK != 0 || Kp <= 0 || M <= 0 || N <= 0) { g_tc_err = "uhc_linear_forward_tc_grouped: M, N > 0 and Kp a positive multiple of 64"; return -2; }
-    if (y_bf16_or_null && (ldy_bf16 % 8 != 0 || ldy_bf16 < N)) { g_tc_err = "uhc_linear_forward_tc_grouped: ldy must be a multiple of 8 and >= N"; return -2; }
+    if (!x_bf16 || !W_bf16_host || (!y_bf16_or_null && !y_f32_or_null)) { uhc_err() = "uhc_linear_forward_tc_grouped: null argument"; return -2; }
+    if (Kp % BK != 0 || Kp <= 0 || M <= 0 || N <= 0) { uhc_err() = "uhc_linear_forward_tc_grouped: M, N > 0 and Kp a positive multiple of 64"; return -2; }
+    if (y_bf16_or_null && (ldy_bf16 % 8 != 0 || ldy_bf16 < N)) { uhc_err() = "uhc_linear_forward_tc_grouped: ldy must be a multiple of 8 and >= N"; return -2; }
     GroupedArgs ga;
     memset(&ga, 0, sizeof ga);
     if (uhc::grp::plan_tiles(G, row0_host, rows_host, M, &ga.plan)) {
-        g_tc_err = "uhc_linear_forward_tc_grouped: groups must be 1..64 ascending, disjoint, non-empty row ranges inside [0, M)"; return -2;
+        uhc_err() = "uhc_linear_forward_tc_grouped: groups must be 1..64 ascending, disjoint, non-empty row ranges inside [0, M)"; return -2;
     }
-    for (int g = 0; g < G; g++) if (!W_bf16_host[g]) { g_tc_err = "uhc_linear_forward_tc_grouped: null weights"; return -2; }
+    for (int g = 0; g < G; g++) if (!W_bf16_host[g]) { uhc_err() = "uhc_linear_forward_tc_grouped: null weights"; return -2; }
     int dev = 0; cudaGetDevice(&dev);
     static bool attr_set[64] = {false};
     if (!(dev >= 0 && dev < 64 && attr_set[dev])) {
-        if (cudaFuncSetAttribute(k_linear_tc_grouped, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { g_tc_err = "cudaFuncSetAttribute failed"; return -1; }
+        if (cudaFuncSetAttribute(k_linear_tc_grouped, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { uhc_err() = "cudaFuncSetAttribute failed"; return -1; }
         if (dev >= 0 && dev < 64) attr_set[dev] = true;
     }
     CUtensorMap ma;
@@ -784,7 +782,7 @@ int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_h
     dim3 grid((N + BN - 1) / BN, ga.plan.tile0[G], 1);
     k_linear_tc_grouped<<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(ma, ga, (__nv_bfloat16 *)y_bf16_or_null, y_f32_or_null, N, Kp, ldy_bf16, act);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { g_tc_err = cudaGetErrorString(e); return -1; }
+    if (e != cudaSuccess) { uhc_err() = cudaGetErrorString(e); return -1; }
     return 0;
 }
 /* backward through one Linear + the previous layer's activation in ONE kernel:  dz_prev = (dz W) * act'(z_prev)  as bf16 [M][ld_dz] and transposed [K][ld_dzT],
@@ -792,10 +790,10 @@ int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_h
  * and 16-byte aligned buffers (returns -2 otherwise: run uhc_linear_forward_tc + uhc_dact_bf16 instead). */
 int uhc_linear_dx_dact_tc(const void *dz_bf16, const void *WT_bf16, const float *z_prev, void *dzp_bf16, void *dzpT_bf16, float *db_prev_or_null,
                           int M, int K, int Np, int ld_dz, int ld_dzT, int act, void *stream) {
-    if (Np % BK != 0 || M <= 0 || K <= 0) { g_tc_err = "uhc_linear_dx_dact_tc: Np must be a positive multiple of 64"; return -2; }
+    if (Np % BK != 0 || M <= 0 || K <= 0) { uhc_err() = "uhc_linear_dx_dact_tc: Np must be a positive multiple of 64"; return -2; }
     auto al = [](const void *p) { return p && ((uintptr_t)p & 15) == 0; };
     if (!tma_store_enabled() || K % 4 != 0 || ld_dz % 8 != 0 || ld_dzT % 8 != 0 || ld_dz < K || ld_dzT < M || !al(z_prev) || !al(dzp_bf16) || !al(dzpT_bf16)) {
-        g_tc_err = "uhc_linear_dx_dact_tc: needs the TMA store path, K % 4 == 0, pitches that are multiples of 8 elements and 16-byte aligned buffers"; return -2;
+        uhc_err() = "uhc_linear_dx_dact_tc: needs the TMA store path, K % 4 == 0, pitches that are multiples of 8 elements and 16-byte aligned buffers"; return -2;
     }
     int dev = 0; cudaGetDevice(&dev);
     if (set_smem_attr(dev)) return -1;
@@ -803,11 +801,11 @@ int uhc_linear_dx_dact_tc(const void *dz_bf16, const void *WT_bf16, const float 
     if (make_map(&ma, dz_bf16, M, Np, BM) || make_map(&mb, WT_bf16, K, Np, BN)) return -1;
     if (make_map_out(&mz, z_prev, M, K, (size_t)K * 4, false) || make_map_out(&mdz, dzp_bf16, M, ld_dz, (size_t)ld_dz * 2, true) ||
         make_map_out(&mdzT, dzpT_bf16, K, ld_dzT, (size_t)ld_dzT * 2, true)) return -1;
-    if (db_prev_or_null && cudaMemsetAsync(db_prev_or_null, 0, (size_t)K * sizeof(float), (cudaStream_t)stream) != cudaSuccess) { g_tc_err = "uhc_linear_dx_dact_tc: memset failed"; return -1; }
+    if (db_prev_or_null && cudaMemsetAsync(db_prev_or_null, 0, (size_t)K * sizeof(float), (cudaStream_t)stream) != cudaSuccess) { uhc_err() = "uhc_linear_dx_dact_tc: memset failed"; return -1; }
     dim3 grid((K + BN - 1) / BN, (M + BM - 1) / BM, 1);
     k_linear_tc<true><<<grid, NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(ma, mb, nullptr, nullptr, nullptr, nullptr, M, K, Np, ld_dz, act, 1, mz, mz, mdz, 0, mdzT, db_prev_or_null);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { g_tc_err = cudaGetErrorString(e); return -1; }
+    if (e != cudaSuccess) { uhc_err() = cudaGetErrorString(e); return -1; }
     return 0;
 }
 int uhc_transpose_bf16(const void *in, void *out, int R, int Cc, int ld_in, int ld_out, void *stream) {
@@ -816,16 +814,16 @@ int uhc_transpose_bf16(const void *in, void *out, int R, int Cc, int ld_in, int 
         k_transpose_bf16_v4<<<grid, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)in, (__nv_bfloat16 *)out, R, Cc, ld_in, ld_out);
     else
         k_transpose_bf16<<<grid, dim3(64, 8), 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)in, (__nv_bfloat16 *)out, R, Cc, ld_in, ld_out);
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+    CK(cudaGetLastError()); return 0;
 }
 int uhc_dact_bf16(const float *dh, const float *z_or_null, void *dz_bf16, void *dzT_bf16, float *db_or_null, int M, int N, int ld_dz, int ld_dzT, int act,
                   void *stream) {
-    if (db_or_null && cudaMemsetAsync(db_or_null, 0, N * sizeof(float), (cudaStream_t)stream) != cudaSuccess) { g_tc_err = "uhc_dact_bf16: memset failed"; return -1; }
+    if (db_or_null && cudaMemsetAsync(db_or_null, 0, N * sizeof(float), (cudaStream_t)stream) != cudaSuccess) { uhc_err() = "uhc_dact_bf16: memset failed"; return -1; }
     dim3 grid((N + 63) / 64, (M + 63) / 64);
     const bool v4 = N % 4 == 0 && (!dz_bf16 || (ld_dz % 4 == 0 && ((uintptr_t)dz_bf16 & 7) == 0)) && (!dzT_bf16 || (ld_dzT % 4 == 0 && ((uintptr_t)dzT_bf16 & 7) == 0)) &&
                     ((uintptr_t)dh & 15) == 0 && (!z_or_null || ((uintptr_t)z_or_null & 15) == 0);
     if (v4) k_dact_bf16_v4<<<grid, 256, 0, (cudaStream_t)stream>>>(dh, z_or_null, (__nv_bfloat16 *)dz_bf16, (__nv_bfloat16 *)dzT_bf16, db_or_null, M, N, ld_dz, ld_dzT, act);
     else k_dact_bf16<<<grid, dim3(64, 8), 0, (cudaStream_t)stream>>>(dh, z_or_null, (__nv_bfloat16 *)dz_bf16, (__nv_bfloat16 *)dzT_bf16, db_or_null, M, N, ld_dz, ld_dzT, act);
-    return cudaGetLastError() == cudaSuccess ? 0 : -1;
+    CK(cudaGetLastError()); return 0;
 }
 }

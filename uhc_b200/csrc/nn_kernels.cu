@@ -12,9 +12,7 @@
 #include <stdint.h>
 #include <string>
 #include "../../include/uhc_nn.h"
-
-static thread_local std::string g_nn_err;
-#define CKN(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_nn_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
+#include "errors.h"
 
 // ------------------------------------------------------------------------------------------------ activations
 __device__ __forceinline__ float act_fwd(float z, int act) {
@@ -104,7 +102,7 @@ static int launch_gemm(const float *A, const float *B, float *C, float *Z, const
     else if (ar && !bj) k_gemm<true, false><<<grid, 256, 0, st>>>(A, B, C, Z, bias, M, N, R, sai, sar, sbr, sbj, act, accumulate);
     else if (!ar && bj) k_gemm<false, true><<<grid, 256, 0, st>>>(A, B, C, Z, bias, M, N, R, sai, sar, sbr, sbj, act, accumulate);
     else k_gemm<false, false><<<grid, 256, 0, st>>>(A, B, C, Z, bias, M, N, R, sai, sar, sbr, sbj, act, accumulate);
-    CKN(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -347,8 +345,6 @@ __global__ void __launch_bounds__(256) k_mcp_backward(const float *__restrict__ 
 }
 
 extern "C" {
-const char *uhc_nn_last_error(void) { return g_nn_err.c_str(); }
-
 int uhc_linear_forward(const float *x, const float *W, const float *b, float *y, float *z_or_null, int M, int N, int K, int act, void *stream) {
     return launch_gemm(x, W, y, z_or_null, b, M, N, K, K, 1, 1, K, act, 0, (cudaStream_t)stream);   // y = act(x W^T + b)
 }
@@ -356,94 +352,94 @@ int uhc_linear_backward(const float *x, const float *W, const float *dz, float *
     cudaStream_t st = (cudaStream_t)stream;
     if (dx_or_null && launch_gemm(dz, W, dx_or_null, nullptr, nullptr, M, K, N, N, 1, K, 1, UHC_ACT_NONE, 0, st)) return -1;   // dx = dz W
     if (launch_gemm(dz, x, dW, nullptr, nullptr, N, K, M, 1, N, K, 1, UHC_ACT_NONE, 0, st)) return -1;                           // dW = dz^T x
-    if (db) { k_colsum<<<(N + 31) / 32, dim3(32, 32), 0, st>>>(dz, db, M, N); CKN(cudaGetLastError()); }
+    if (db) { k_colsum<<<(N + 31) / 32, dim3(32, 32), 0, st>>>(dz, db, M, N); CK(cudaGetLastError()); }
     return 0;
 }
 int uhc_act_backward(const float *dh, const float *z, float *dz, long n, int act, void *stream) {
-    k_act_bwd<<<1056, 256, 0, (cudaStream_t)stream>>>(dh, z, dz, (size_t)n, act); CKN(cudaGetLastError()); return 0;
+    k_act_bwd<<<1056, 256, 0, (cudaStream_t)stream>>>(dh, z, dz, (size_t)n, act); CK(cudaGetLastError()); return 0;
 }
 int uhc_gaussian_sample(const float *mean, const float *log_std, const unsigned char *mean_action, float *action, float *logp, int M, int A,
                         unsigned long long seed, unsigned long long step, void *stream) {
-    k_gauss_sample<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(mean, log_std, mean_action, action, logp, M, A, seed, step); CKN(cudaGetLastError()); return 0;
+    k_gauss_sample<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(mean, log_std, mean_action, action, logp, M, A, seed, step); CK(cudaGetLastError()); return 0;
 }
 int uhc_gaussian_logprob(const float *mean, const float *log_std, const float *action, float *logp, int M, int A, void *stream) {
-    k_gauss_logprob<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(mean, log_std, action, logp, M, A); CKN(cudaGetLastError()); return 0;
+    k_gauss_logprob<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(mean, log_std, action, logp, M, A); CK(cudaGetLastError()); return 0;
 }
 int uhc_ppo_policy_grad(const float *mean, const float *log_std, const float *action, const float *adv, const float *fixed_logp, const float *exps,
                         float clip_eps, float inv_count, float *dmean, float *loss_acc, int M, int A, void *stream) {
     k_ppo_grad<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(mean, log_std, action, adv, fixed_logp, exps, clip_eps, inv_count, dmean, loss_acc, M, A, nullptr);
-    CKN(cudaGetLastError()); return 0;
+    CK(cudaGetLastError()); return 0;
 }
 int uhc_ppo_policy_grad_dev(const float *mean, const float *log_std, const float *action, const float *adv, const float *fixed_logp, const float *exps,
                             float clip_eps, const float *inv_count_dev, float *dmean, float *loss_acc, int M, int A, void *stream) {
-    if (!inv_count_dev) { g_nn_err = "uhc_ppo_policy_grad_dev: inv_count_dev is null"; return -2; }
+    if (!inv_count_dev) { uhc_err() = "uhc_ppo_policy_grad_dev: inv_count_dev is null"; return -2; }
     k_ppo_grad<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(mean, log_std, action, adv, fixed_logp, exps, clip_eps, 0.f, dmean, loss_acc, M, A, inv_count_dev);
-    CKN(cudaGetLastError()); return 0;
+    CK(cudaGetLastError()); return 0;
 }
 int uhc_value_grad(const float *v, const float *ret, float *dv, float *loss_acc, int M, void *stream) {
-    k_value_grad<<<592, 256, 0, (cudaStream_t)stream>>>(v, ret, dv, loss_acc, M, (float)M); CKN(cudaGetLastError()); return 0;
+    k_value_grad<<<592, 256, 0, (cudaStream_t)stream>>>(v, ret, dv, loss_acc, M, (float)M); CK(cudaGetLastError()); return 0;
 }
 int uhc_value_grad_n(const float *v, const float *ret, float *dv, float *loss_acc, int M, long M_total, void *stream) {
-    k_value_grad<<<592, 256, 0, (cudaStream_t)stream>>>(v, ret, dv, loss_acc, M, (float)M_total); CKN(cudaGetLastError()); return 0;
+    k_value_grad<<<592, 256, 0, (cudaStream_t)stream>>>(v, ret, dv, loss_acc, M, (float)M_total); CK(cudaGetLastError()); return 0;
 }
 int uhc_sqsum(const float *x, long n, double *out_acc, void *stream) {
-    k_sqsum<<<592, 256, 0, (cudaStream_t)stream>>>(x, (size_t)n, out_acc); CKN(cudaGetLastError()); return 0;
+    k_sqsum<<<592, 256, 0, (cudaStream_t)stream>>>(x, (size_t)n, out_acc); CK(cudaGetLastError()); return 0;
 }
 int uhc_adam_step(float *p, const float *g, float *m, float *v, long n, float lr, float beta1, float beta2, float eps, int step,
                   const double *sqnorm_or_null, float max_norm, void *stream) {
     const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
     k_adam<<<1056, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (size_t)n, lr, beta1, beta2, eps, bc1, bc2, sqnorm_or_null, max_norm);
-    CKN(cudaGetLastError()); return 0;
+    CK(cudaGetLastError()); return 0;
 }
 int uhc_gae(const float *rew, const float *mask, const float *val, const float *last_val, float gamma, float tau, float *adv, float *ret, int T, int E,
             void *stream) {
-    k_gae<<<(E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(rew, mask, val, last_val, gamma, tau, adv, ret, T, E); CKN(cudaGetLastError()); return 0;
+    k_gae<<<(E + 127) / 128, 128, 0, (cudaStream_t)stream>>>(rew, mask, val, last_val, gamma, tau, adv, ret, T, E); CK(cudaGetLastError()); return 0;
 }
 int uhc_normalize_advantages(float *adv, long n, double *scratch2, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    CKN(cudaMemsetAsync(scratch2, 0, 2 * sizeof(double), st));
-    k_moments<<<592, 256, 0, st>>>(adv, (size_t)n, scratch2); CKN(cudaGetLastError());
-    k_normalize<<<592, 256, 0, st>>>(adv, (size_t)n, scratch2, nullptr); CKN(cudaGetLastError());
+    CK(cudaMemsetAsync(scratch2, 0, 2 * sizeof(double), st));
+    k_moments<<<592, 256, 0, st>>>(adv, (size_t)n, scratch2); CK(cudaGetLastError());
+    k_normalize<<<592, 256, 0, st>>>(adv, (size_t)n, scratch2, nullptr); CK(cudaGetLastError());
     return 0;
 }
 // the two halves of the same normalisation, for a batch sharded over GPUs: local (sum, sum of squares) -> [all-reduce] -> normalise with
 // the global moments and the global element count (both read from device memory: no host round trip between the collective and the kernel)
 int uhc_adv_moments(const float *adv, long n, double *out2, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    CKN(cudaMemsetAsync(out2, 0, 2 * sizeof(double), st));
-    k_moments<<<592, 256, 0, st>>>(adv, (size_t)n, out2); CKN(cudaGetLastError());
+    CK(cudaMemsetAsync(out2, 0, 2 * sizeof(double), st));
+    k_moments<<<592, 256, 0, st>>>(adv, (size_t)n, out2); CK(cudaGetLastError());
     return 0;
 }
 int uhc_adv_normalize(float *adv, long n, const double *mom2_dev, const double *ntotal_dev, void *stream) {
-    k_normalize<<<592, 256, 0, (cudaStream_t)stream>>>(adv, (size_t)n, mom2_dev, ntotal_dev); CKN(cudaGetLastError());
+    k_normalize<<<592, 256, 0, (cudaStream_t)stream>>>(adv, (size_t)n, mom2_dev, ntotal_dev); CK(cudaGetLastError());
     return 0;
 }
 int uhc_mcp_combine(const float *xall, const float *c, float *weight_or_null, float *mean, int M, int A, int P, void *stream) {
-    if (P < 1 || P > MCP_MAX_PRIM) { g_nn_err = "uhc_mcp_combine: 1..16 primitives"; return -2; }
-    k_mcp_combine<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(xall, c, weight_or_null, mean, M, A, P); CKN(cudaGetLastError()); return 0;
+    if (P < 1 || P > MCP_MAX_PRIM) { uhc_err() = "uhc_mcp_combine: 1..16 primitives"; return -2; }
+    k_mcp_combine<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(xall, c, weight_or_null, mean, M, A, P); CK(cudaGetLastError()); return 0;
 }
 int uhc_mcp_backward(const float *xall, const float *weight, const float *dmean, float *dxall, float *dc, int M, int A, int P, void *stream) {
-    if (P < 1 || P > MCP_MAX_PRIM) { g_nn_err = "uhc_mcp_backward: 1..16 primitives"; return -2; }
-    k_mcp_backward<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(xall, weight, dmean, dxall, dc, M, A, P); CKN(cudaGetLastError()); return 0;
+    if (P < 1 || P > MCP_MAX_PRIM) { uhc_err() = "uhc_mcp_backward: 1..16 primitives"; return -2; }
+    k_mcp_backward<<<(M + 7) / 8, 256, 0, (cudaStream_t)stream>>>(xall, weight, dmean, dxall, dc, M, A, P); CK(cudaGetLastError()); return 0;
 }
 int uhc_zfilter_workspace_doubles(int D) { return ZF_CHUNKS * D * 3; }
 int uhc_zfilter(const float *x, float *y, int M, int D, double *stats, float clip, int update, void *stream) {
     // without a caller workspace: one per (thread, D), allocated on first use (not legal inside a stream capture -- the rollout passes its own)
     static thread_local double *ws = nullptr; static thread_local int ws_d = 0, ws_dev = -1;
     int dev = 0; cudaGetDevice(&dev);
-    if (update && (!ws || ws_d < D || ws_dev != dev)) { if (ws && ws_dev == dev) cudaFree(ws); CKN(cudaMalloc((void **)&ws, (size_t)uhc_zfilter_workspace_doubles(D) * sizeof(double))); ws_d = D; ws_dev = dev; }
+    if (update && (!ws || ws_d < D || ws_dev != dev)) { if (ws && ws_dev == dev) cudaFree(ws); CK(cudaMalloc((void **)&ws, (size_t)uhc_zfilter_workspace_doubles(D) * sizeof(double))); ws_d = D; ws_dev = dev; }
     return uhc_zfilter_ws(x, y, M, D, stats, clip, update, ws, stream);
 }
 int uhc_zfilter_ws(const float *x, float *y, int M, int D, double *stats, float clip, int update, double *workspace, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (M < 0 || D <= 0) { g_nn_err = "uhc_zfilter_ws: M >= 0 and D > 0"; return -2; }
+    if (M < 0 || D <= 0) { uhc_err() = "uhc_zfilter_ws: M >= 0 and D > 0"; return -2; }
     if (update && M > 0) {     // an empty batch leaves the statistics as they are
-        if (!workspace) { g_nn_err = "uhc_zfilter_ws: workspace is null"; return -2; }
-        k_zfilter_partial<<<dim3((D + 31) / 32, ZF_CHUNKS), dim3(32, 32), 0, st>>>(x, M, D, workspace); CKN(cudaGetLastError());
-        k_zfilter_merge<<<(D + 127) / 128, 128, 0, st>>>(x, M, D, stats, workspace); CKN(cudaGetLastError());
-        k_zfilter_count<<<1, 1, 0, st>>>(stats, M); CKN(cudaGetLastError());
+        if (!workspace) { uhc_err() = "uhc_zfilter_ws: workspace is null"; return -2; }
+        k_zfilter_partial<<<dim3((D + 31) / 32, ZF_CHUNKS), dim3(32, 32), 0, st>>>(x, M, D, workspace); CK(cudaGetLastError());
+        k_zfilter_merge<<<(D + 127) / 128, 128, 0, st>>>(x, M, D, stats, workspace); CK(cudaGetLastError());
+        k_zfilter_count<<<1, 1, 0, st>>>(stats, M); CK(cudaGetLastError());
     }
-    if (y) { k_zfilter_apply<<<592, 256, 0, st>>>(x, y, M, D, stats, clip); CKN(cudaGetLastError()); }
+    if (y) { k_zfilter_apply<<<592, 256, 0, st>>>(x, y, M, D, stats, clip); CK(cudaGetLastError()); }
     return 0;
 }
 }  // extern "C"

@@ -19,12 +19,11 @@
 #include <vector>
 #include "../../include/uhc_nn.h"
 #include "../../include/uhc_ppo.h"
+#include "errors.h"
 
 namespace {
-thread_local std::string g_ppo_err;
 thread_local long g_launches = 0;      // kernels enqueued by the current uhc_ppo_update call (every CKU call below launches exactly one)
-#define CKP(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_ppo_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
-#define CKU(x, what) do { ++g_launches; if ((x) != 0) { const char *a_ = uhc_nn_last_error(), *b_ = uhc_tc_last_error(); g_ppo_err = std::string(what) + ": " + ((a_ && a_[0]) ? a_ : (b_ ? b_ : "")); return -1; } } while (0)
+#define CKU(x, what) do { ++g_launches; if ((x) != 0) return uhc_err_prefix(what); } while (0)
 
 inline long pad64(long n) { return (n + 63) / 64 * 64; }
 
@@ -133,15 +132,15 @@ struct UhcPpoTrainer {
 
 namespace {
 int check_net(const UhcNetDesc &n, const char *name) {
-    if (n.nlayers < 1 || n.nlayers > 8 || !n.flat || !n.gfull || !n.adam_m || !n.adam_v) { g_ppo_err = std::string(name) + ": bad UhcNetDesc"; return -2; }
+    if (n.nlayers < 1 || n.nlayers > 8 || !n.flat || !n.gfull || !n.adam_m || !n.adam_v) { uhc_err() = std::string(name) + ": bad UhcNetDesc"; return -2; }
     for (int i = 0; i < n.nlayers; i++)
-        if (n.dims[i] <= 0 || n.dims[i + 1] <= 0 || n.kp[i] != pad64(n.dims[i]) || !n.W_bf16[i]) { g_ppo_err = std::string(name) + ": kp[i] must be dims[i] rounded up to 64 and W_bf16[i] set"; return -2; }
+        if (n.dims[i] <= 0 || n.dims[i + 1] <= 0 || n.kp[i] != pad64(n.dims[i]) || !n.W_bf16[i]) { uhc_err() = std::string(name) + ": kp[i] must be dims[i] rounded up to 64 and W_bf16[i] set"; return -2; }
     return 0;
 }
 template <class T> int dalloc(UhcPpoTrainer *t, T **p, size_t bytes, bool zero) {
-    CKP(cudaMalloc((void **)p, bytes ? bytes : 16));
+    CK(cudaMalloc((void **)p, bytes ? bytes : 16));
     t->allocs.push_back((void *)*p);
-    if (zero) CKP(cudaMemset(*p, 0, bytes ? bytes : 16));
+    if (zero) CK(cudaMemset(*p, 0, bytes ? bytes : 16));
     return 0;
 }
 int alloc_net(UhcPpoTrainer *t, const UhcNetDesc &n, NetBuf &nb, long cap, bool own_out) {
@@ -194,7 +193,7 @@ int net_backward(UhcPpoTrainer *t, const UhcNetDesc &n, NetBuf &nb, const float 
         const int Kq = (K + 3) & ~3;
         if (K != Kq && t->dWpad && (long)N * Kq <= t->dWpad_n && uhc_linear_forward_tc_f32_pitched(dzT, hT, t->dWpad, Kq, N, K, (int)Mp, st) == 0) {
             g_launches += 2;          // the GEMM and the row copy
-            CKP(cudaMemcpy2DAsync(n.gfull + n.w_off[i], (size_t)K * 4, t->dWpad, (size_t)Kq * 4, (size_t)K * 4, N, cudaMemcpyDeviceToDevice, st));
+            CK(cudaMemcpy2DAsync(n.gfull + n.w_off[i], (size_t)K * 4, t->dWpad, (size_t)Kq * 4, (size_t)K * 4, N, cudaMemcpyDeviceToDevice, st));
         } else
             CKU(uhc_linear_forward_tc(dzT, hT, nullptr, nullptr, n.gfull + n.w_off[i], N, K, (int)Mp, 0, UHC_ACT_NONE, st), "dW GEMM");
         if (i > 0) {
@@ -235,19 +234,19 @@ int policy_backward(UhcPpoTrainer *t, const float *dmean, long M, cudaStream_t s
 }
 int start_all_reduce(UhcPpoTrainer *t, void *comm, float *buf, size_t n, cudaEvent_t done, cudaStream_t st) {
     AllReduceFn ar = nccl_all_reduce();
-    if (!ar) { g_ppo_err = "uhc_ppo_update: an ncclComm_t was passed but libnccl.so.2 / ncclAllReduce cannot be resolved"; return -1; }
-    CKP(cudaEventRecord(t->ev_ready, st));
-    CKP(cudaStreamWaitEvent(t->side, t->ev_ready, 0));
+    if (!ar) { uhc_err() = "uhc_ppo_update: an ncclComm_t was passed but libnccl.so.2 / ncclAllReduce cannot be resolved"; return -1; }
+    CK(cudaEventRecord(t->ev_ready, st));
+    CK(cudaStreamWaitEvent(t->side, t->ev_ready, 0));
     if (t->timing_used == t->timing.size()) {
-        cudaEvent_t a, b; CKP(cudaEventCreate(&a)); CKP(cudaEventCreate(&b));
+        cudaEvent_t a, b; CK(cudaEventCreate(&a)); CK(cudaEventCreate(&b));
         t->timing.push_back({a, b});
     }
     auto &tm = t->timing[t->timing_used++];
-    CKP(cudaEventRecord(tm.first, t->side));
+    CK(cudaEventRecord(tm.first, t->side));
     const int rc = ar(buf, buf, n, NCCL_FLOAT32, NCCL_SUM, comm, t->side);
-    if (rc != 0) { g_ppo_err = "ncclAllReduce failed with code " + std::to_string(rc); return -1; }
-    CKP(cudaEventRecord(tm.second, t->side));
-    CKP(cudaEventRecord(done, t->side));
+    if (rc != 0) { uhc_err() = "ncclAllReduce failed with code " + std::to_string(rc); return -1; }
+    CK(cudaEventRecord(tm.second, t->side));
+    CK(cudaEventRecord(done, t->side));
     t->comm_bytes += (long)(n * sizeof(float)); t->comm_calls++;
     return 0;
 }
@@ -269,30 +268,30 @@ static int run_epochs(UhcPpoTrainer *t, const float *actions, const float *exps,
 
     for (int ep = 0; ep < cfg->epochs; ++ep) {
         if ((ep > 0 || !value_forward_done) && net_forward(val, t->vb, t->xb, M, true, st)) return -1;
-        CKP(cudaMemsetAsync(losses_out, 0, 2 * sizeof(float), st));
+        CK(cudaMemsetAsync(losses_out, 0, 2 * sizeof(float), st));
         CKU(uhc_value_grad_n(t->vb.out, t->ret, t->dv, losses_out + 1, (int)M, M * world, st), "value gradient");
         if (net_backward(t, val, t->vb, t->dv, M, st)) return -1;
         const bool with_tail = stats_tail && ep == 0;
         if (comm && start_all_reduce(t, comm, val.gfull, (size_t)val.nflat + (with_tail ? (size_t)PLANES * nd : 0), t->ev_v, st)) return -1;
         if (with_tail) {    // the global statistics are needed before the first policy gradient
-            CKP(cudaStreamWaitEvent(st, t->ev_v, 0));
-            ++g_launches; k_stats_join<<<(nd + 255) / 256, 256, 0, st>>>(tail, D, t->mom, t->ntot, t->inv_count, zfilter_sync); CKP(cudaGetLastError());
+            CK(cudaStreamWaitEvent(st, t->ev_v, 0));
+            ++g_launches; k_stats_join<<<(nd + 255) / 256, 256, 0, st>>>(tail, D, t->mom, t->ntot, t->inv_count, zfilter_sync); CK(cudaGetLastError());
             CKU(uhc_adv_normalize(t->adv, M, t->mom, t->ntot, st), "advantage normalisation (global)");
-            ++g_launches; k_zfilter_from_sums<<<(2 * D + 1 + 255) / 256, 256, 0, st>>>(zfilter_sync, D, zfilter_stats); CKP(cudaGetLastError());
+            ++g_launches; k_zfilter_from_sums<<<(2 * D + 1 + 255) / 256, 256, 0, st>>>(zfilter_sync, D, zfilter_stats); CK(cudaGetLastError());
         }
         if (ep > 0 && policy_forward(t, M, &pmean, st)) return -1;
         CKU(uhc_ppo_policy_grad_dev(pmean, log_std, actions, t->adv, t->fixed, exps, cfg->clip_eps, t->inv_count, t->dmean, losses_out, (int)M, A, st), "policy gradient");
         if (policy_backward(t, t->dmean, M, st)) return -1;
         if (comm && start_all_reduce(t, comm, pol.gfull, (size_t)pol.nflat, t->ev_p, st)) return -1;
         // value step first, as the reference; the policy collective is still in flight
-        if (comm) CKP(cudaStreamWaitEvent(st, t->ev_v, 0));
+        if (comm) CK(cudaStreamWaitEvent(st, t->ev_v, 0));
         *adam_step_value += 1;
         CKU(uhc_adam_step(val.flat, val.gfull, val.adam_m, val.adam_v, val.nflat, val.lr, 0.9f, 0.999f, 1e-8f, *adam_step_value, nullptr, 0.f, st), "value Adam");
         if (refresh_bf16(val, st)) return -1;
-        if (comm) CKP(cudaStreamWaitEvent(st, t->ev_p, 0));
+        if (comm) CK(cudaStreamWaitEvent(st, t->ev_p, 0));
         const bool clip = cfg->grad_clip > 0.f && (!cfg->clip_first_step_only || *policy_steps_done == 0);
         if (clip) {
-            CKP(cudaMemsetAsync(t->sq, 0, sizeof(double), st));
+            CK(cudaMemsetAsync(t->sq, 0, sizeof(double), st));
             CKU(uhc_sqsum(pol.gfull, pol.nflat, t->sq, st), "gradient norm");
         }
         *adam_step_policy += 1; *policy_steps_done += 1;
@@ -303,22 +302,20 @@ static int run_epochs(UhcPpoTrainer *t, const float *actions, const float *exps,
 }
 
 extern "C" {
-const char *uhc_ppo_last_error(void) { return g_ppo_err.c_str(); }
-
 static int trainer_create(const UhcNetDesc *pnets, int nprim, const UhcNetDesc *value, long max_rows, int max_envs, int device, UhcPpoTrainer **out) {
     const int npn = nprim > 0 ? nprim + 1 : 1;
-    if (!pnets || !value || !out || max_rows <= 0 || max_envs <= 0 || nprim < 0 || nprim > 8) { g_ppo_err = "uhc_ppo_trainer_create: bad argument"; return -2; }
+    if (!pnets || !value || !out || max_rows <= 0 || max_envs <= 0 || nprim < 0 || nprim > 8) { uhc_err() = "uhc_ppo_trainer_create: bad argument"; return -2; }
     for (int j = 0; j < npn; j++) if (check_net(pnets[j], "policy")) return -2;
     if (check_net(*value, "value")) return -2;
     const int D = pnets[0].dims[0], A = pnets[0].dims[pnets[0].nlayers];
-    if (D != value->dims[0] || value->dims[value->nlayers] != 1) { g_ppo_err = "uhc_ppo_trainer_create: the nets must share the input width and the value head must be scalar"; return -2; }
+    if (D != value->dims[0] || value->dims[value->nlayers] != 1) { uhc_err() = "uhc_ppo_trainer_create: the nets must share the input width and the value head must be scalar"; return -2; }
     for (int j = 0; j < npn; j++) {
         const UhcNetDesc &n = pnets[j];
-        if (n.dims[0] != D || n.flat != pnets[0].flat || n.gfull != pnets[0].gfull || n.nflat != pnets[0].nflat) { g_ppo_err = "uhc_ppo_trainer_create: the policy's nets must share one flat parameter / gradient tensor and the observation"; return -2; }
-        if (nprim > 0 && j < nprim && n.dims[n.nlayers] != A) { g_ppo_err = "uhc_ppo_trainer_create: the primitives must share the action width"; return -2; }
-        if (nprim > 0 && j == nprim && n.dims[n.nlayers] != nprim) { g_ppo_err = "uhc_ppo_trainer_create: the composer's output width must be the number of primitives"; return -2; }
+        if (n.dims[0] != D || n.flat != pnets[0].flat || n.gfull != pnets[0].gfull || n.nflat != pnets[0].nflat) { uhc_err() = "uhc_ppo_trainer_create: the policy's nets must share one flat parameter / gradient tensor and the observation"; return -2; }
+        if (nprim > 0 && j < nprim && n.dims[n.nlayers] != A) { uhc_err() = "uhc_ppo_trainer_create: the primitives must share the action width"; return -2; }
+        if (nprim > 0 && j == nprim && n.dims[n.nlayers] != nprim) { uhc_err() = "uhc_ppo_trainer_create: the composer's output width must be the number of primitives"; return -2; }
     }
-    CKP(cudaSetDevice(device));
+    CK(cudaSetDevice(device));
     UhcPpoTrainer *t = new UhcPpoTrainer();
     t->device = device; t->cap = max_rows; t->cap_envs = max_envs; t->val = *value; t->nprim = nprim;
     t->pnets.assign(pnets, pnets + npn); t->pbufs.resize(npn);
@@ -347,8 +344,8 @@ static int trainer_create(const UhcNetDesc *pnets, int nprim, const UhcNetDesc *
          dalloc(t, &t->adv, (size_t)cap * 4, false) || dalloc(t, &t->ret, (size_t)cap * 4, false) || dalloc(t, &t->last_v, (size_t)max_envs * 4, false) ||
          dalloc(t, &t->inv_count, 4, true) || dalloc(t, &t->mom, 16, true) || dalloc(t, &t->cnt, 8, true) || dalloc(t, &t->ntot, 8, true) || dalloc(t, &t->sq, 8, true);
     if (rc) { uhc_ppo_trainer_destroy(t); return -1; }
-    CKP(cudaStreamCreateWithFlags(&t->side, cudaStreamNonBlocking));
-    CKP(cudaEventCreateWithFlags(&t->ev_ready, cudaEventDisableTiming)); CKP(cudaEventCreateWithFlags(&t->ev_v, cudaEventDisableTiming)); CKP(cudaEventCreateWithFlags(&t->ev_p, cudaEventDisableTiming));
+    CK(cudaStreamCreateWithFlags(&t->side, cudaStreamNonBlocking));
+    CK(cudaEventCreateWithFlags(&t->ev_ready, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&t->ev_v, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&t->ev_p, cudaEventDisableTiming));
     *out = t;
     return 0;
 }
@@ -356,7 +353,7 @@ int uhc_ppo_trainer_create(const UhcNetDesc *policy, const UhcNetDesc *value, lo
     return trainer_create(policy, 0, value, max_rows, max_envs, device, out);
 }
 int uhc_ppo_trainer_create_mcp(const UhcNetDesc *policy_nets, int nprim, const UhcNetDesc *value, long max_rows, int max_envs, int device, UhcPpoTrainer **out) {
-    if (nprim < 1) { g_ppo_err = "uhc_ppo_trainer_create_mcp: nprim >= 1"; return -2; }
+    if (nprim < 1) { uhc_err() = "uhc_ppo_trainer_create_mcp: nprim >= 1"; return -2; }
     return trainer_create(policy_nets, nprim, value, max_rows, max_envs, device, out);
 }
 
@@ -377,10 +374,10 @@ const float *uhc_ppo_advantages(const UhcPpoTrainer *t) { return t ? t->adv : nu
 const float *uhc_ppo_returns(const UhcPpoTrainer *t) { return t ? t->ret : nullptr; }
 
 int uhc_ppo_comm_stats(UhcPpoTrainer *t, double *ms, long *bytes, int *calls) {
-    if (!t) { g_ppo_err = "uhc_ppo_comm_stats: null trainer"; return -2; }
-    CKP(cudaStreamSynchronize(t->side));
+    if (!t) { uhc_err() = "uhc_ppo_comm_stats: null trainer"; return -2; }
+    CK(cudaStreamSynchronize(t->side));
     double tot = 0.0;
-    for (size_t i = 0; i < t->timing_used; i++) { float m = 0.f; CKP(cudaEventElapsedTime(&m, t->timing[i].first, t->timing[i].second)); tot += m; }
+    for (size_t i = 0; i < t->timing_used; i++) { float m = 0.f; CK(cudaEventElapsedTime(&m, t->timing[i].first, t->timing[i].second)); tot += m; }
     if (ms) *ms = tot;
     if (bytes) *bytes = t->comm_bytes;
     if (calls) *calls = t->comm_calls;
@@ -392,11 +389,11 @@ int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_stat
                    const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
                    int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out, void *stream) {
     if (!t || !states || !last_states || !actions || !rewards || !masks || !exps || !log_std || !cfg || !adam_step_policy || !adam_step_value || !policy_steps_done ||
-        !losses_out || T <= 0 || E <= 0 || world < 1) { g_ppo_err = "uhc_ppo_update: bad argument"; return -2; }
+        !losses_out || T <= 0 || E <= 0 || world < 1) { uhc_err() = "uhc_ppo_update: bad argument"; return -2; }
     const long M = (long)T * E;
-    if (M > t->cap || E > t->cap_envs) { g_ppo_err = "uhc_ppo_update: the rollout exceeds the trainer's capacity"; return -2; }
-    if (world > 1 && (!nccl_comm || !zfilter_stats || !zfilter_sync)) { g_ppo_err = "uhc_ppo_update: world > 1 needs an ncclComm_t and the ZFilter statistics"; return -2; }
-    CKP(cudaSetDevice(t->device));
+    if (M > t->cap || E > t->cap_envs) { uhc_err() = "uhc_ppo_update: the rollout exceeds the trainer's capacity"; return -2; }
+    if (world > 1 && (!nccl_comm || !zfilter_stats || !zfilter_sync)) { uhc_err() = "uhc_ppo_update: world > 1 needs an ncclComm_t and the ZFilter statistics"; return -2; }
+    CK(cudaSetDevice(t->device));
     cudaStream_t st = (cudaStream_t)stream;
     g_launches = 0;
     struct Tally { UhcPpoTrainer *t; ~Tally() { t->launches += g_launches; } } tally{t};
@@ -405,26 +402,26 @@ int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_stat
     const long Dp = pad64(D), Mp = pad64(M);
     void *comm = world > 1 ? nccl_comm : nullptr;
     const int nd = 4 + 1 + 2 * D;
-    if (comm && (long)PLANES * nd > val.gtail) { g_ppo_err = "uhc_ppo_update: the value net's gradient tail is too small for the statistics"; return -2; }
+    if (comm && (long)PLANES * nd > val.gtail) { uhc_err() = "uhc_ppo_update: the value net's gradient tail is too small for the statistics"; return -2; }
 
     // ---- V(s_T) of the state after the last step, V(s) of every row (also epoch 0's value forward), GAE
     CKU(uhc_f32_to_bf16_padded(last_states, t->lb, E, D, (int)Dp, st), "bf16 last states");
     if (net_forward(val, t->vb, t->lb, E, false, st)) return -1;
-    CKP(cudaMemcpyAsync(t->last_v, t->vb.out, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(t->last_v, t->vb.out, (size_t)E * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CKU(uhc_f32_to_bf16_padded(states, t->xb, (int)M, D, (int)Dp, st), "bf16 states");
     CKU(uhc_transpose_bf16(t->xb, t->xT, (int)M, D, (int)Dp, (int)Mp, st), "transpose states");
     if (net_forward(val, t->vb, t->xb, M, true, st)) return -1;
     CKU(uhc_gae(rewards, masks, t->vb.out, t->last_v, cfg->gamma, cfg->tau, t->adv, t->ret, T, E, st), "gae");
     CKU(uhc_adv_moments(t->adv, M, t->mom, st), "advantage moments");
-    CKP(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
-    ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CKP(cudaGetLastError());
+    CK(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
+    ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CK(cudaGetLastError());
     float *tail = val.gfull + val.nflat;
     if (!comm) {
         CKU(uhc_adv_normalize(t->adv, M, t->mom, nullptr, st), "advantage normalisation");
-        ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CKP(cudaGetLastError());
+        ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CK(cudaGetLastError());
     } else {
-        CKP(cudaMemsetAsync(tail, 0, (size_t)val.gtail * sizeof(float), st));
-        ++g_launches; k_stats_pack<<<(nd + 255) / 256, 256, 0, st>>>(t->mom, (double)M, t->cnt, zfilter_stats, zfilter_sync, D, tail); CKP(cudaGetLastError());
+        CK(cudaMemsetAsync(tail, 0, (size_t)val.gtail * sizeof(float), st));
+        ++g_launches; k_stats_pack<<<(nd + 255) / 256, 256, 0, st>>>(t->mom, (double)M, t->cnt, zfilter_stats, zfilter_sync, D, tail); CK(cudaGetLastError());
     }
     return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, zfilter_stats, zfilter_sync, comm, world, comm != nullptr,
                       true, losses_out, st);
@@ -435,21 +432,21 @@ int uhc_ppo_update_policy(UhcPpoTrainer *t, const float *states, const float *ac
                           const float *log_std, long M, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value, int *policy_steps_done,
                           void *nccl_comm, int world, float *losses_out, void *stream) {
     if (!t || !states || !actions || !returns || !advantages || !exps || !log_std || !cfg || !adam_step_policy || !adam_step_value || !policy_steps_done || !losses_out ||
-        M <= 0 || world < 1) { g_ppo_err = "uhc_ppo_update_policy: bad argument"; return -2; }
-    if (M > t->cap) { g_ppo_err = "uhc_ppo_update_policy: the batch exceeds the trainer's capacity"; return -2; }
-    if (world > 1 && !nccl_comm) { g_ppo_err = "uhc_ppo_update_policy: world > 1 needs an ncclComm_t"; return -2; }
-    CKP(cudaSetDevice(t->device));
+        M <= 0 || world < 1) { uhc_err() = "uhc_ppo_update_policy: bad argument"; return -2; }
+    if (M > t->cap) { uhc_err() = "uhc_ppo_update_policy: the batch exceeds the trainer's capacity"; return -2; }
+    if (world > 1 && !nccl_comm) { uhc_err() = "uhc_ppo_update_policy: world > 1 needs an ncclComm_t"; return -2; }
+    CK(cudaSetDevice(t->device));
     cudaStream_t st = (cudaStream_t)stream;
     g_launches = 0;
     struct Tally { UhcPpoTrainer *t; ~Tally() { t->launches += g_launches; } } tally{t};
     const int D = t->pnets[0].dims[0];
     CKU(uhc_f32_to_bf16_padded(states, t->xb, (int)M, D, (int)pad64(D), st), "bf16 states");
     CKU(uhc_transpose_bf16(t->xb, t->xT, (int)M, D, (int)pad64(D), (int)pad64(M), st), "transpose states");
-    CKP(cudaMemcpyAsync(t->adv, advantages, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    CKP(cudaMemcpyAsync(t->ret, returns, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    CKP(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
-    ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CKP(cudaGetLastError());
-    ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CKP(cudaGetLastError());      // (a sharded caller passes world = 1 per shard or pre-scales exps)
+    CK(cudaMemcpyAsync(t->adv, advantages, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(t->ret, returns, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
+    ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CK(cudaGetLastError());
+    ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CK(cudaGetLastError());      // (a sharded caller passes world = 1 per shard or pre-scales exps)
     return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, nullptr, nullptr, world > 1 ? nccl_comm : nullptr, world, false,
                       false, losses_out, st);
 }

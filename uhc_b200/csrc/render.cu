@@ -9,14 +9,12 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_render.h"
+#include "errors.h"
 #define UHC_RENDER_HOST 1
 #include "render_core.h"
 #include "track_glue.h"
 
 using namespace uhc;
-
-static thread_local std::string g_rd_err;
-#define CKR(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_rd_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
 
 namespace {
 
@@ -114,20 +112,20 @@ bool finite_cam(const UhcRenderCamera &c) {
 int check_variants(UhcEngine *e, long n, const int *variant_dev, cudaStream_t st, const char *who) {
     if (!variant_dev || n == 0) return 0;
     std::vector<int> v((size_t)n);
-    CKR(cudaMemcpyAsync(v.data(), variant_dev, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
-    CKR(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(v.data(), variant_dev, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     const int ns = trackx::num_shapes(e);
     for (long i = 0; i < n; i++)
-        if (v[(size_t)i] < 0 || v[(size_t)i] >= ns) { g_rd_err = std::string(who) + ": variant out of range"; return -2; }
+        if (v[(size_t)i] < 0 || v[(size_t)i] >= ns) { uhc_err() = std::string(who) + ": variant out of range"; return -2; }
     return 0;
 }
 
 int pose_args(UhcEngine *e, long n, const void *qpos, int precision, long pitch, const void *ghost, long ghost_pitch, const char *who) {
-    if (!e) { g_rd_err = std::string(who) + ": null engine"; return -2; }
-    if (n < 0) { g_rd_err = std::string(who) + ": n < 0"; return -2; }
-    if (precision != 32 && precision != 64) { g_rd_err = std::string(who) + ": precision must be 32 or 64"; return -2; }
-    if (pitch < motion::MQ || (ghost && ghost_pitch < motion::MQ)) { g_rd_err = std::string(who) + ": pitch < 76"; return -2; }
-    if (n > 0 && !qpos) { g_rd_err = std::string(who) + ": null qpos"; return -2; }
+    if (!e) { uhc_err() = std::string(who) + ": null engine"; return -2; }
+    if (n < 0) { uhc_err() = std::string(who) + ": n < 0"; return -2; }
+    if (precision != 32 && precision != 64) { uhc_err() = std::string(who) + ": precision must be 32 or 64"; return -2; }
+    if (pitch < motion::MQ || (ghost && ghost_pitch < motion::MQ)) { uhc_err() = std::string(who) + ": pitch < 76"; return -2; }
+    if (n > 0 && !qpos) { uhc_err() = std::string(who) + ": null qpos"; return -2; }
     return 0;
 }
 
@@ -142,21 +140,21 @@ int launch_pose(UhcEngine *e, long n, const void *qpos, int precision, long pitc
         k_render_pose<float><<<blocks, 128, 0, st>>>(m, n, nh, (const float *)qpos, pitch, (const float *)ghost, ghost_pitch, variant, pose);
     else
         k_render_pose<double><<<blocks, 128, 0, st>>>(m, n, nh, (const double *)qpos, pitch, (const double *)ghost, ghost_pitch, variant, pose);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
 // argument checks of a trace (-2 with nothing launched)
 int trace_args(UhcEngine *e, const UhcRenderCamera *cam, int W, int H, long n, int humanoids, const void *pose, const void *rgb, const char *who) {
-    if (!e) { g_rd_err = std::string(who) + ": null engine"; return -2; }
-    if (!find_ctx(e)) { g_rd_err = std::string(who) + ": no hull planes (uhc_render_init)"; return -2; }
-    if (!cam) { g_rd_err = std::string(who) + ": null camera"; return -2; }
-    if (n < 0) { g_rd_err = std::string(who) + ": n < 0"; return -2; }
-    if (W < 1 || H < 1 || W > 16384 || H > 16384) { g_rd_err = std::string(who) + ": W and H must be in 1 .. 16384"; return -2; }
-    if (humanoids != 1 && humanoids != 2) { g_rd_err = std::string(who) + ": humanoids must be 1 or 2"; return -2; }
-    if (n > 0 && (!pose || !rgb)) { g_rd_err = std::string(who) + ": null pose or rgb"; return -2; }
+    if (!e) { uhc_err() = std::string(who) + ": null engine"; return -2; }
+    if (!find_ctx(e)) { uhc_err() = std::string(who) + ": no hull planes (uhc_render_init)"; return -2; }
+    if (!cam) { uhc_err() = std::string(who) + ": null camera"; return -2; }
+    if (n < 0) { uhc_err() = std::string(who) + ": n < 0"; return -2; }
+    if (W < 1 || H < 1 || W > 16384 || H > 16384) { uhc_err() = std::string(who) + ": W and H must be in 1 .. 16384"; return -2; }
+    if (humanoids != 1 && humanoids != 2) { uhc_err() = std::string(who) + ": humanoids must be 1 or 2"; return -2; }
+    if (n > 0 && (!pose || !rgb)) { uhc_err() = std::string(who) + ": null pose or rgb"; return -2; }
     if (!finite_cam(*cam) || !(cam->distance > 0) || !(cam->fovy > 0 && cam->fovy < 180)) {
-        g_rd_err = std::string(who) + ": camera needs finite values, distance > 0 and 0 < fovy < 180"; return -2;
+        uhc_err() = std::string(who) + ": camera needs finite values, distance > 0 and 0 < fovy < 180"; return -2;
     }
     return 0;
 }
@@ -172,7 +170,7 @@ int launch_trace(RenderCtx *c, const UhcRenderCamera *cam, int W, int H, long n,
     a.rgb = rgb; a.depth = depth; a.label = label;
     const dim3 grid((unsigned)((W + TILE - 1) / TILE), (unsigned)((H + TILE - 1) / TILE), (unsigned)(n < 65535 ? n : 65535));
     k_render_trace<<<grid, dim3(TILE, TILE), trace_smem(c->nplane), st>>>(a);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -180,26 +178,24 @@ int launch_trace(RenderCtx *c, const UhcRenderCamera *cam, int W, int H, long n,
 
 extern "C" {
 
-const char *uhc_render_last_error(void) { return g_rd_err.c_str(); }
-
 int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
-    if (!e || !h || !h->plane || !h->plane_adr || !h->plane_num || !h->sphere) { g_rd_err = "uhc_render_init: null argument"; return -2; }
-    if (h->nshape != trackx::num_shapes(e)) { g_rd_err = "uhc_render_init: nshape differs from the engine's shape variants"; return -2; }
-    if (h->nplane < 4 || trace_smem(h->nplane) > 200 * 1024) { g_rd_err = "uhc_render_init: nplane out of range"; return -2; }
+    if (!e || !h || !h->plane || !h->plane_adr || !h->plane_num || !h->sphere) { uhc_err() = "uhc_render_init: null argument"; return -2; }
+    if (h->nshape != trackx::num_shapes(e)) { uhc_err() = "uhc_render_init: nshape differs from the engine's shape variants"; return -2; }
+    if (h->nplane < 4 || trace_smem(h->nplane) > 200 * 1024) { uhc_err() = "uhc_render_init: nplane out of range"; return -2; }
     for (int b = 0; b < render::NB; b++)
         if (h->plane_num[b] < 4 || h->plane_num[b] > UHC_RENDER_MAX_PLANES || h->plane_adr[b] < 0 || h->plane_adr[b] > h->nplane - h->plane_num[b]) {
-            g_rd_err = "uhc_render_init: plane_adr / plane_num of a body out of range"; return -2;
+            uhc_err() = "uhc_render_init: plane_adr / plane_num of a body out of range"; return -2;
         }
     const size_t np = (size_t)h->nshape * h->nplane, ns = (size_t)h->nshape * render::NB;
     std::vector<float4> pl(np), sp(ns);
     for (size_t i = 0; i < np; i++) {
         const double *p = h->plane + 4 * i;
-        if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && isfinite(p[3]))) { g_rd_err = "uhc_render_init: non-finite plane"; return -2; }
+        if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && isfinite(p[3]))) { uhc_err() = "uhc_render_init: non-finite plane"; return -2; }
         pl[i] = make_float4((float)p[0], (float)p[1], (float)p[2], (float)p[3]);
     }
     for (size_t i = 0; i < ns; i++) {
         const double *p = h->sphere + 4 * i;
-        if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && p[3] > 0 && isfinite(p[3]))) { g_rd_err = "uhc_render_init: bad bounding sphere"; return -2; }
+        if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && p[3] > 0 && isfinite(p[3]))) { uhc_err() = "uhc_render_init: bad bounding sphere"; return -2; }
         sp[i] = make_float4((float)p[0], (float)p[1], (float)p[2], (float)p[3]);
     }
     uhc_render_release(e);
@@ -207,12 +203,12 @@ int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
     c->eng = e; g_rd.push_back(c);
     c->nshape = h->nshape; c->nplane = h->nplane;
     for (int b = 0; b < render::NB; b++) { c->adr[b] = h->plane_adr[b]; c->num[b] = h->plane_num[b]; }
-    CKR(cudaMalloc((void **)&c->d_plane, np * sizeof(float4)));
-    CKR(cudaMalloc((void **)&c->d_sphere, ns * sizeof(float4)));
-    CKR(cudaMemcpy(c->d_plane, pl.data(), np * sizeof(float4), cudaMemcpyHostToDevice));
-    CKR(cudaMemcpy(c->d_sphere, sp.data(), ns * sizeof(float4), cudaMemcpyHostToDevice));
-    CKR(cudaFuncSetAttribute(k_render_trace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem(c->nplane)));
-    CKR(cudaDeviceSynchronize());
+    CK(cudaMalloc((void **)&c->d_plane, np * sizeof(float4)));
+    CK(cudaMalloc((void **)&c->d_sphere, ns * sizeof(float4)));
+    CK(cudaMemcpy(c->d_plane, pl.data(), np * sizeof(float4), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(c->d_sphere, sp.data(), ns * sizeof(float4), cudaMemcpyHostToDevice));
+    CK(cudaFuncSetAttribute(k_render_trace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem(c->nplane)));
+    CK(cudaDeviceSynchronize());
     return 0;
 }
 
@@ -223,7 +219,7 @@ void uhc_render_release(UhcEngine *e) {
 int uhc_render_pose(UhcEngine *e, long n, const void *qpos_dev, int precision, long pitch, const void *ghost_qpos_dev_or_null, long ghost_pitch,
                     const int *variant_dev_or_null, float *pose_dev, void *stream) {
     if (int rc = pose_args(e, n, qpos_dev, precision, pitch, ghost_qpos_dev_or_null, ghost_pitch, "uhc_render_pose")) return rc;
-    if (n > 0 && !pose_dev) { g_rd_err = "uhc_render_pose: null pose"; return -2; }
+    if (n > 0 && !pose_dev) { uhc_err() = "uhc_render_pose: null pose"; return -2; }
     cudaStream_t st = (cudaStream_t)stream;
     if (int rc = check_variants(e, n, variant_dev_or_null, st, "uhc_render_pose")) return rc;
     return launch_pose(e, n, qpos_dev, precision, pitch, ghost_qpos_dev_or_null, ghost_pitch, variant_dev_or_null, pose_dev, st);
@@ -248,9 +244,9 @@ int uhc_render_qpos(UhcEngine *e, const UhcRenderCamera *cam, int W, int H, long
     if (n == 0) return 0;
     RenderCtx *c = find_ctx(e);
     if ((size_t)n > c->pose_cap) {
-        CKR(cudaStreamSynchronize(st));                             // an earlier call on this stream may still read the old table
+        CK(cudaStreamSynchronize(st));                             // an earlier call on this stream may still read the old table
         cudaFree(c->d_pose); c->d_pose = nullptr; c->pose_cap = 0;
-        CKR(cudaMalloc((void **)&c->d_pose, (size_t)n * SLOTS * render::POSE * sizeof(float)));
+        CK(cudaMalloc((void **)&c->d_pose, (size_t)n * SLOTS * render::POSE * sizeof(float)));
         c->pose_cap = (size_t)n;
     }
     if (int rc = launch_pose(e, n, qpos_dev, precision, pitch, ghost_qpos_dev_or_null, ghost_pitch, variant_dev_or_null, c->d_pose, st)) return rc;

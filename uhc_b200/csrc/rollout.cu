@@ -22,15 +22,10 @@
 #include "../../include/uhc_b200.h"
 #include "../../include/uhc_nn.h"
 #include "../../include/uhc_rollout.h"
+#include "errors.h"
 #include "eval_glue.h"
 #include "graph_cache.h"
 #include "group_core.h"
-
-static thread_local std::string g_ro_err;
-#define CKR(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_ro_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
-#define CKC(x, msg) do { if ((x) != 0) { g_ro_err = std::string(msg) + ": " + (uhc_nn_last_error()[0] ? uhc_nn_last_error() : uhc_tc_last_error()); return -1; } } while (0)
-
-extern "C" const char *uhc_tc_last_error(void);
 
 namespace {
 
@@ -168,17 +163,17 @@ RolloutCtx *ctx_of(UhcEngine *e) {
 
 int check_policy(const Policy *pol) {
     const int P = pol->nprim;
-    if (P < 0 || P > UHC_MCP_MAX_PRIM) { g_ro_err = "UhcMcp: 1..8 primitives"; return -2; }
+    if (P < 0 || P > UHC_MCP_MAX_PRIM) { uhc_err() = "UhcMcp: 1..8 primitives"; return -2; }
     const UhcMlp *m0 = &pol->nets[0];
     for (int j = 0; j < num_nets(pol); j++) {
         const UhcMlp *m = &pol->nets[j];
-        if (m->nlayers < 1 || m->nlayers > 8) { g_ro_err = "UhcMlp: 1..8 layers"; return -2; }
-        if (m->dims[0] != m0->dims[0]) { g_ro_err = "UhcMcp: every net reads the same observation"; return -2; }
-        if (j < P && m->dims[m->nlayers] != m0->dims[m0->nlayers]) { g_ro_err = "UhcMcp: the primitives must share the action width"; return -2; }
-        if (P > 0 && j == P && m->dims[m->nlayers] != P) { g_ro_err = "UhcMcp: the composer's output width must be the number of primitives"; return -2; }
+        if (m->nlayers < 1 || m->nlayers > 8) { uhc_err() = "UhcMlp: 1..8 layers"; return -2; }
+        if (m->dims[0] != m0->dims[0]) { uhc_err() = "UhcMcp: every net reads the same observation"; return -2; }
+        if (j < P && m->dims[m->nlayers] != m0->dims[m0->nlayers]) { uhc_err() = "UhcMcp: the primitives must share the action width"; return -2; }
+        if (P > 0 && j == P && m->dims[m->nlayers] != P) { uhc_err() = "UhcMcp: the composer's output width must be the number of primitives"; return -2; }
         for (int i = 0; i < m->nlayers; i++) {
-            if (m->kp[i] != pad64(m->dims[i])) { g_ro_err = "UhcMlp: kp[i] must be dims[i] rounded up to 64"; return -2; }
-            if (!m->W_bf16[i]) { g_ro_err = "UhcMlp: null weights"; return -2; }
+            if (m->kp[i] != pad64(m->dims[i])) { uhc_err() = "UhcMlp: kp[i] must be dims[i] rounded up to 64"; return -2; }
+            if (!m->W_bf16[i]) { uhc_err() = "UhcMlp: null weights"; return -2; }
         }
     }
     return 0;
@@ -186,7 +181,7 @@ int check_policy(const Policy *pol) {
 
 int realloc_zero(void **p, size_t bytes) {
     if (*p) { cudaFree(*p); *p = nullptr; }
-    CKR(cudaMalloc(p, bytes)); CKR(cudaMemset(*p, 0, bytes));
+    CK(cudaMalloc(p, bytes)); CK(cudaMemset(*p, 0, bytes));
     return 0;
 }
 // validates pol (-2, nothing touched) and sizes s for it over E rows
@@ -222,10 +217,10 @@ void release(PolicyScratch *s) {
 // the step counter and the per-env arrays of the context: allocated once, never moved
 int ensure_ctx(RolloutCtx *c) {
     const size_t E = c->E;
-    if (!c->d_step) { CKR(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); CKR(cudaMemset(c->d_step, 0, sizeof(unsigned long long))); }
+    if (!c->d_step) { CK(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); CK(cudaMemset(c->d_step, 0, sizeof(unsigned long long))); }
     if (!c->d_mean_action) {
-        CKR(cudaMalloc((void **)&c->d_mean_action, E)); CKR(cudaMalloc((void **)&c->d_cinfo, E * 5 * 4)); CKR(cudaMalloc((void **)&c->d_pct, E * 4));
-        CKR(cudaMalloc((void **)&c->d_fail, E * 4)); CKR(cudaMalloc((void **)&c->d_end, E * 4));
+        CK(cudaMalloc((void **)&c->d_mean_action, E)); CK(cudaMalloc((void **)&c->d_cinfo, E * 5 * 4)); CK(cudaMalloc((void **)&c->d_pct, E * 4));
+        CK(cudaMalloc((void **)&c->d_fail, E * 4)); CK(cudaMalloc((void **)&c->d_end, E * 4));
     }
     return 0;
 }
@@ -269,7 +264,7 @@ int enqueue_layers(const PolicyScratch &s, const Policy *pol, int E, cudaStream_
         }
     }
     // the mixture head is row-wise: run over every row (a row no policy covers holds zeros or earlier values and is never read)
-    if (P > 0) { CKC(uhc_mcp_combine(s.d_xall, s.d_comp, nullptr, s.d_mean, E, A, P, st), "mixture head"); n++; }
+    if (P > 0) { if (uhc_mcp_combine(s.d_xall, s.d_comp, nullptr, s.d_mean, E, A, P, st)) return uhc_err_prefix("mixture head"); n++; }
     return n;
 }
 
@@ -278,13 +273,12 @@ int enqueue_policy(RolloutCtx *c, const float *obs, const Policy *pol, double *z
     const UhcMlp *m0 = &pol->nets[0];
     const int E = c->E, D = m0->dims[0];
     int n = 0;
-    if (update_filter) { CKC(uhc_zfilter_ws(obs, nullptr, E, D, zstats, zclip, 1, c->d_zws, st), "zfilter update"); n += 3; }
+    if (update_filter) { if (uhc_zfilter_ws(obs, nullptr, E, D, zstats, zclip, 1, c->d_zws, st)) return uhc_err_prefix("zfilter update"); n += 3; }
     k_zfilter_apply_bf16<<<1056, 256, 0, st>>>(obs, state_out, (unsigned short *)c->own.ns[0].acts[0], E, D, m0->kp[0], zstats, zclip);
-    CKR(cudaGetLastError()); n++;
+    CK(cudaGetLastError()); n++;
     const int nl = enqueue_layers(c->own, pol, E, st, [&](const Layer &l) {
         const UhcMlp *m = &pol->nets[l.net];
-        CKC(uhc_linear_forward_tc(l.in, m->W_bf16[l.i], m->bias[l.i], l.out_bf16, l.out_f32, E, l.N, l.Kp, l.ld, l.act, st), "policy GEMM");
-        return 0;
+        return uhc_linear_forward_tc(l.in, m->W_bf16[l.i], m->bias[l.i], l.out_bf16, l.out_f32, E, l.N, l.Kp, l.ld, l.act, st) ? uhc_err_prefix("policy GEMM") : 0;
     });
     return nl < 0 ? nl : n + nl;
 }
@@ -299,23 +293,23 @@ int enqueue_step(RolloutCtx *c, int row, const Policy *pol, const float *log_std
     int n = enqueue_policy(c, b->obs_cur, pol, zstats, zclip, update_filter, state_row, st);
     if (n < 0) return n;
     const bool mixed = noise_rate < 1.0f;
-    if (mixed) { k_mean_action<<<(c->E + 255) / 256, 256, 0, st>>>(c->d_mean_action, exps_row, c->E, 1.0f - noise_rate, seed, c->d_step); CKR(cudaGetLastError()); n++; }
+    if (mixed) { k_mean_action<<<(c->E + 255) / 256, 256, 0, st>>>(c->d_mean_action, exps_row, c->E, 1.0f - noise_rate, seed, c->d_step); CK(cudaGetLastError()); n++; }
     k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->own.d_mean, log_std, mixed ? c->d_mean_action : nullptr, act_row, logp_row, c->E, A, seed, c->d_step);
-    CKR(cudaGetLastError()); n++;
+    CK(cudaGetLastError()); n++;
     const bool timed = row < (int)c->ev0.size();
     // inside stream capture the record must be an EXTERNAL event-record node, or the event is owned by the graph and cannot be read from the host
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    if (timed) CKR(cudaStreamIsCapturing(st, &cap));
+    if (timed) CK(cudaStreamIsCapturing(st, &cap));
     const unsigned evflag = cap == cudaStreamCaptureStatusActive ? cudaEventRecordExternal : cudaEventRecordDefault;
-    if (timed) CKR(cudaEventRecordWithFlags(c->ev0[row], st, evflag));
-    if (uhc_env_step(c->eng, act_row, b->obs_cur, rew_row, c->d_cinfo, c->d_fail, c->d_end, c->d_pct, nullptr, st)) { g_ro_err = std::string("env step: ") + uhc_last_error(); return -1; }
-    if (timed) CKR(cudaEventRecordWithFlags(c->ev1[row], st, evflag));
+    if (timed) CK(cudaEventRecordWithFlags(c->ev0[row], st, evflag));
+    if (uhc_env_step(c->eng, act_row, b->obs_cur, rew_row, c->d_cinfo, c->d_fail, c->d_end, c->d_pct, nullptr, st)) return uhc_err_prefix("env step");
+    if (timed) CK(cudaEventRecordWithFlags(c->ev1[row], st, evflag));
     n++;
     const bool eplog = b->ep_clip && b->ep_pct;
     k_rollout_post<<<(c->E + 255) / 256, 256, 0, st>>>(c->d_fail, c->d_end, mask_row, fail_row, mixed ? nullptr : exps_row, c->E, c->d_step, uhc_episode_log_dev(c->eng),
                                                        eplog ? b->ep_clip + (size_t)row * E : nullptr, eplog ? b->ep_pct + (size_t)row * E : nullptr,
                                                        eplog && b->ep_start ? b->ep_start + (size_t)row * E : nullptr);
-    CKR(cudaGetLastError()); n++;
+    CK(cudaGetLastError()); n++;
     return n;
 }
 
@@ -323,34 +317,32 @@ int enqueue_step(RolloutCtx *c, int row, const Policy *pol, const float *log_std
 
 extern "C" {
 
-const char *uhc_rollout_last_error(void) { return g_ro_err.c_str(); }
-
 int uhc_rollout_set_step(UhcEngine *e, unsigned long long step) {
-    if (!e) { g_ro_err = "uhc_rollout_set_step: null engine"; return -2; }
+    if (!e) { uhc_err() = "uhc_rollout_set_step: null engine"; return -2; }
     RolloutCtx *c = ctx_of(e);
-    if (!c->d_step) { CKR(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); }
-    CKR(cudaMemcpy(c->d_step, &step, sizeof step, cudaMemcpyHostToDevice));
+    if (!c->d_step) { CK(cudaMalloc((void **)&c->d_step, sizeof(unsigned long long))); }
+    CK(cudaMemcpy(c->d_step, &step, sizeof step, cudaMemcpyHostToDevice));
     return 0;
 }
 int uhc_rollout_get_step(UhcEngine *e, unsigned long long *step) {
-    if (!e || !step) { g_ro_err = "uhc_rollout_get_step: bad argument"; return -2; }
+    if (!e || !step) { uhc_err() = "uhc_rollout_get_step: bad argument"; return -2; }
     RolloutCtx *c = ctx_of(e);
     *step = 0;
-    if (c->d_step) { CKR(cudaDeviceSynchronize()); CKR(cudaMemcpy(step, c->d_step, sizeof *step, cudaMemcpyDeviceToHost)); }
+    if (c->d_step) { CK(cudaDeviceSynchronize()); CK(cudaMemcpy(step, c->d_step, sizeof *step, cudaMemcpyDeviceToHost)); }
     return 0;
 }
 
 static int make_policy(Policy *pol, const UhcMlp *mlp, const UhcMcp *mcp, UhcEngine *e, const char *who) {
     memset(pol, 0, sizeof *pol);
     if (mcp) {
-        if (mcp->nprim < 1 || mcp->nprim > UHC_MCP_MAX_PRIM) { g_ro_err = std::string(who) + ": 1..8 primitives"; return -2; }
+        if (mcp->nprim < 1 || mcp->nprim > UHC_MCP_MAX_PRIM) { uhc_err() = std::string(who) + ": 1..8 primitives"; return -2; }
         pol->nprim = mcp->nprim;
         for (int k = 0; k < mcp->nprim; k++) pol->nets[k] = mcp->prim[k];
         pol->nets[mcp->nprim] = mcp->composer;
     } else pol->nets[0] = *mlp;
     const UhcMlp *m = &pol->nets[0];
     if (m->nlayers >= 1 && m->nlayers <= 8 && (m->dims[m->nlayers] != uhc_engine_act_dim(e) || m->dims[0] != uhc_engine_obs_dim(e))) {
-        g_ro_err = std::string(who) + ": the policy's input / output widths are not the engine's obs / action dims"; return -2;
+        uhc_err() = std::string(who) + ": the policy's input / output widths are not the engine's obs / action dims"; return -2;
     }
     return 0;
 }
@@ -364,7 +356,7 @@ static int policy_forward_impl(UhcEngine *e, const float *obs_dev, const Policy 
     if (enqueue_policy(c, obs_dev, pol, zfilter_stats, zclip, update_filter, state_out_or_null, st) < 0) return -1;
     const UhcMlp *m = &pol->nets[0];
     k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->own.d_mean, log_std, mean_action_or_null, action_out, logp_out_or_null, c->E, m->dims[m->nlayers], seed, c->d_step);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 static int rollout_impl(UhcEngine *e, int T, int row0, const Policy *pol, const float *log_std, double *zfilter_stats, float zclip, int update_filter,
@@ -387,41 +379,41 @@ static int rollout_impl(UhcEngine *e, int T, int row0, const Policy *pol, const 
         rc = GraphCache::capture([&](cudaStream_t cs) {
             for (int i = 0; i < T && n >= 0; i++) n = enqueue_step(c, row0 + i, pol, log_std, zfilter_stats, zclip, update_filter, seed, noise_rate, buf, cs);
             return n < 0 ? -1 : 0;
-        }, &exec, &g_ro_err);
+        }, &exec);
         if (rc) return rc;
         c->launches_per_step = n;
         c->graphs.insert(std::move(key), GraphCache::Gens{}, exec);   // nothing goes stale: the scratch drops them all, the rest is in the key
     }
-    CKR(cudaGraphLaunch(exec, st));
+    CK(cudaGraphLaunch(exec, st));
     return 0;
 }
 
 int uhc_policy_forward(UhcEngine *e, const float *obs_dev, const UhcMlp *mlp, const float *log_std, double *zfilter_stats, float zclip, int update_filter,
                        unsigned long long seed, const unsigned char *mean_action_or_null, float *state_out_or_null, float *action_out, float *logp_out_or_null,
                        void *stream) {
-    if (!e || !obs_dev || !mlp || !log_std || !zfilter_stats || !action_out) { g_ro_err = "uhc_policy_forward: bad argument"; return -2; }
+    if (!e || !obs_dev || !mlp || !log_std || !zfilter_stats || !action_out) { uhc_err() = "uhc_policy_forward: bad argument"; return -2; }
     Policy pol; if (make_policy(&pol, mlp, nullptr, e, "uhc_policy_forward")) return -2;
     return policy_forward_impl(e, obs_dev, &pol, log_std, zfilter_stats, zclip, update_filter, seed, mean_action_or_null, state_out_or_null, action_out, logp_out_or_null, stream);
 }
 int uhc_policy_forward_mcp(UhcEngine *e, const float *obs_dev, const UhcMcp *mcp, const float *log_std, double *zfilter_stats, float zclip, int update_filter,
                            unsigned long long seed, const unsigned char *mean_action_or_null, float *state_out_or_null, float *action_out, float *logp_out_or_null,
                            void *stream) {
-    if (!e || !obs_dev || !mcp || !log_std || !zfilter_stats || !action_out) { g_ro_err = "uhc_policy_forward_mcp: bad argument"; return -2; }
+    if (!e || !obs_dev || !mcp || !log_std || !zfilter_stats || !action_out) { uhc_err() = "uhc_policy_forward_mcp: bad argument"; return -2; }
     Policy pol; if (make_policy(&pol, nullptr, mcp, e, "uhc_policy_forward_mcp")) return -2;
     return policy_forward_impl(e, obs_dev, &pol, log_std, zfilter_stats, zclip, update_filter, seed, mean_action_or_null, state_out_or_null, action_out, logp_out_or_null, stream);
 }
 
 int uhc_rollout(UhcEngine *e, int T, int row0, const UhcMlp *mlp, const float *log_std, double *zfilter_stats, float zclip, int update_filter,
                 unsigned long long seed, float noise_rate, const UhcRolloutBuf *buf, int use_graph, void *stream) {
-    if (!e || !mlp || !log_std || !zfilter_stats || !buf || T <= 0 || row0 < 0 || row0 + T > buf->T_cap) { g_ro_err = "uhc_rollout: bad argument"; return -2; }
-    if (!buf->states || !buf->actions || !buf->rewards || !buf->masks || !buf->exps || !buf->obs_cur) { g_ro_err = "uhc_rollout: missing buffer"; return -2; }
+    if (!e || !mlp || !log_std || !zfilter_stats || !buf || T <= 0 || row0 < 0 || row0 + T > buf->T_cap) { uhc_err() = "uhc_rollout: bad argument"; return -2; }
+    if (!buf->states || !buf->actions || !buf->rewards || !buf->masks || !buf->exps || !buf->obs_cur) { uhc_err() = "uhc_rollout: missing buffer"; return -2; }
     Policy pol; if (make_policy(&pol, mlp, nullptr, e, "uhc_rollout")) return -2;
     return rollout_impl(e, T, row0, &pol, log_std, zfilter_stats, zclip, update_filter, seed, noise_rate, buf, use_graph, stream);
 }
 int uhc_rollout_mcp(UhcEngine *e, int T, int row0, const UhcMcp *mcp, const float *log_std, double *zfilter_stats, float zclip, int update_filter,
                     unsigned long long seed, float noise_rate, const UhcRolloutBuf *buf, int use_graph, void *stream) {
-    if (!e || !mcp || !log_std || !zfilter_stats || !buf || T <= 0 || row0 < 0 || row0 + T > buf->T_cap) { g_ro_err = "uhc_rollout_mcp: bad argument"; return -2; }
-    if (!buf->states || !buf->actions || !buf->rewards || !buf->masks || !buf->exps || !buf->obs_cur) { g_ro_err = "uhc_rollout_mcp: missing buffer"; return -2; }
+    if (!e || !mcp || !log_std || !zfilter_stats || !buf || T <= 0 || row0 < 0 || row0 + T > buf->T_cap) { uhc_err() = "uhc_rollout_mcp: bad argument"; return -2; }
+    if (!buf->states || !buf->actions || !buf->rewards || !buf->masks || !buf->exps || !buf->obs_cur) { uhc_err() = "uhc_rollout_mcp: missing buffer"; return -2; }
     Policy pol; if (make_policy(&pol, nullptr, mcp, e, "uhc_rollout_mcp")) return -2;
     return rollout_impl(e, T, row0, &pol, log_std, zfilter_stats, zclip, update_filter, seed, noise_rate, buf, use_graph, stream);
 }
@@ -429,22 +421,22 @@ int uhc_rollout_mcp(UhcEngine *e, int T, int row0, const UhcMcp *mcp, const floa
 // events around the env-step kernel of rows 0 .. nrows-1 (recorded on the launching stream, also inside graph replays); 0 disables.
 // Changing it drops the cached graphs.
 int uhc_rollout_time_env_step(UhcEngine *e, int nrows) {
-    if (!e || nrows < 0) { g_ro_err = "uhc_rollout_time_env_step: bad argument"; return -2; }
+    if (!e || nrows < 0) { uhc_err() = "uhc_rollout_time_env_step: bad argument"; return -2; }
     RolloutCtx *c = ctx_of(e);
-    CKR(cudaDeviceSynchronize());
+    CK(cudaDeviceSynchronize());
     c->graphs.clear();
     for (cudaEvent_t ev : c->ev0) cudaEventDestroy(ev);
     for (cudaEvent_t ev : c->ev1) cudaEventDestroy(ev);
     c->ev0.assign(nrows, nullptr); c->ev1.assign(nrows, nullptr);
-    for (int i = 0; i < nrows; i++) { CKR(cudaEventCreate(&c->ev0[i])); CKR(cudaEventCreate(&c->ev1[i])); }
+    for (int i = 0; i < nrows; i++) { CK(cudaEventCreate(&c->ev0[i])); CK(cudaEventCreate(&c->ev1[i])); }
     return 0;
 }
 int uhc_rollout_env_step_ms(UhcEngine *e, int row, float *ms) {
-    if (!e || !ms) { g_ro_err = "uhc_rollout_env_step_ms: bad argument"; return -2; }
+    if (!e || !ms) { uhc_err() = "uhc_rollout_env_step_ms: bad argument"; return -2; }
     RolloutCtx *c = ctx_of(e);
-    if (row < 0 || row >= (int)c->ev0.size()) { g_ro_err = "uhc_rollout_env_step_ms: row not timed"; return -2; }
-    CKR(cudaEventSynchronize(c->ev1[row]));
-    CKR(cudaEventElapsedTime(ms, c->ev0[row], c->ev1[row]));
+    if (row < 0 || row >= (int)c->ev0.size()) { uhc_err() = "uhc_rollout_env_step_ms: row not timed"; return -2; }
+    CK(cudaEventSynchronize(c->ev1[row]));
+    CK(cudaEventElapsedTime(ms, c->ev0[row], c->ev1[row]));
     return 0;
 }
 
@@ -465,7 +457,7 @@ void uhc_rollout_release(UhcEngine *e) {   // called by the binding before uhc_e
 }  // extern "C"
 
 // ---- the policy forward of the device evaluation and the tracker (eval_glue.h): the kernels of uhc_policy_forward(_mcp), enqueued from
-// eval.cu's and track.cu's graphs.  On failure the text is uhc_rollout_last_error()'s
+// eval.cu's and track.cu's graphs
 namespace uhc {
 namespace evalx {
 
@@ -483,7 +475,7 @@ int policy_enqueue(UhcEngine *e, const Policy &pol, const float *obs, const floa
     if (enqueue_policy(c, obs, &pol, zstats, zclip, 0, nullptr, st) < 0) return -1;
     const UhcMlp *m = &pol.nets[0];
     k_gauss_sample_dev<<<(c->E + 7) / 8, 256, 0, st>>>(c->own.d_mean, log_std, mean_action, action, nullptr, c->E, m->dims[m->nlayers], 0, c->d_step);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -509,8 +501,8 @@ int groups_prepare(UhcEngine *e, int G, const UhcMlp *mlps, const UhcMcp *mcps, 
     for (int g = 0; g < G; g++) {
         Policy *p = &(*pols)[g];
         if (make_policy(p, mlps ? mlps + g : nullptr, mcps ? mcps + g : nullptr, e, who)) return -2;
-        if (check_policy(p)) { g_ro_err = std::string(who) + ": " + g_ro_err; return -2; }
-        if (g > 0 && !same_arch(&(*pols)[0], p)) { g_ro_err = std::string(who) + ": every group's policy must have the same layer widths, K padding, activation and primitive count"; return -2; }
+        if (check_policy(p)) { uhc_err_prefix(who); return -2; }
+        if (g > 0 && !same_arch(&(*pols)[0], p)) { uhc_err() = std::string(who) + ": every group's policy must have the same layer widths, K padding, activation and primitive count"; return -2; }
     }
     RolloutCtx *c = ctx_of(e);
     int rc = ensure_ctx(c);
@@ -532,16 +524,15 @@ int groups_enqueue(UhcEngine *e, const std::vector<Policy> &pols, const int *row
     for (int g = 0; g <= G; g++) zg.row0[g] = row0[g];
     for (int g = 0; g < G; g++) { zg.stats[g] = zstats[g]; rows[g] = row0[g + 1] - row0[g]; }
     k_zfilter_apply_bf16_grouped<<<1056, 256, 0, st>>>(obs, nullptr, (unsigned short *)s.ns[0].acts[0], ntot, m0->dims[0], m0->kp[0], zg, zclip);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     const int nl = enqueue_layers(s, &pols[0], c->E, st, [&](const Layer &l) {
         const void *W[uhc::grp::MAX_GROUPS]; const float *b[uhc::grp::MAX_GROUPS];
         for (int g = 0; g < G; g++) { W[g] = pols[g].nets[l.net].W_bf16[l.i]; b[g] = pols[g].nets[l.net].bias[l.i]; }
-        CKC(uhc_linear_forward_tc_grouped(G, row0, rows, l.in, W, b, l.out_bf16, l.out_f32, c->E, l.N, l.Kp, l.ld, l.act, st), "grouped policy GEMM");
-        return 0;
+        return uhc_linear_forward_tc_grouped(G, row0, rows, l.in, W, b, l.out_bf16, l.out_f32, c->E, l.N, l.Kp, l.ld, l.act, st) ? uhc_err_prefix("grouped policy GEMM") : 0;
     });
     if (nl < 0) return -1;
     k_gauss_sample_dev<<<(ntot + 7) / 8, 256, 0, st>>>(s.d_mean, s.d_log_std0, mean_action, action, nullptr, ntot, m0->dims[m0->nlayers], 0, c->d_step);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 

@@ -9,6 +9,7 @@
 #include "../../include/uhc_b200.h"
 #include "../../include/uhc_rollout.h"
 #include "env_step.h"
+#include "errors.h"
 #include "motion_core.h"
 #include "eval_glue.h"
 #include "curriculum_core.h"
@@ -16,9 +17,6 @@
 #include "track_glue.h"
 
 using namespace uhc;
-
-static thread_local std::string g_err;
-#define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
 
 // the small per-model tables every solve walks (joint gains / armature, tree-level table) are staged once per CTA behind the
 // EPB work sets; the Model is pointed at the copies (sim_core.h reads them with shared-space loads)
@@ -285,10 +283,19 @@ static_assert(step_smem<float, EPB_F>() + 1024 + 64 <= 228 * 1024, "k_env_step<f
 
 extern "C" {
 
-const char *uhc_last_error(void) { return g_err.c_str(); }
+// the library's one error text (errors.h).  The per-header names are aliases of uhc_last_error, kept for the callers of earlier releases
+const char *uhc_last_error(void) { return uhc_err().c_str(); }
+const char *uhc_nn_last_error(void) { return uhc_last_error(); }
+const char *uhc_tc_last_error(void) { return uhc_last_error(); }
+const char *uhc_ppo_last_error(void) { return uhc_last_error(); }
+const char *uhc_rollout_last_error(void) { return uhc_last_error(); }
+const char *uhc_eval_last_error(void) { return uhc_last_error(); }
+const char *uhc_track_last_error(void) { return uhc_last_error(); }
+const char *uhc_render_last_error(void) { return uhc_last_error(); }
+const char *uhc_export_last_error(void) { return uhc_last_error(); }
 
 int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_envs, int device, int precision, UhcEngine **out) {
-    if (!model || !cfg || !out || num_envs <= 0 || (precision != 32 && precision != 64)) { g_err = "uhc_engine_create: bad argument"; return -2; }
+    if (!model || !cfg || !out || num_envs <= 0 || (precision != 32 && precision != 64)) { uhc_err() = "uhc_engine_create: bad argument"; return -2; }
     CK(cudaSetDevice(device));
     UhcEngine *e = new UhcEngine();
     e->E = num_envs; e->device = device; e->precision = precision; e->launches = 0; e->nshape = model->nshape > 0 ? model->nshape : 1;
@@ -313,7 +320,7 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
         CK(cudaFuncSetAttribute(k_eval_reseat<float, EPB_F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<float, EPB_F>()));
         int resident = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, k_env_step<float, EPB_F>, 32 * EPB_F, step_smem<float, EPB_F>()));
-        if (resident < 1) { g_err = "uhc_engine_create: k_env_step<float> with " + std::to_string(EPB_F) + " envs per block does not fit one SM"; delete e; return -3; }
+        if (resident < 1) { uhc_err() = "uhc_engine_create: k_env_step<float> with " + std::to_string(EPB_F) + " envs per block does not fit one SM"; delete e; return -3; }
     } else {
         CK(cudaFuncSetAttribute(k_env_step<double, EPB_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
         CK(cudaFuncSetAttribute(k_env_step<double, EPB_D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)step_smem<double, EPB_D>()));
@@ -371,13 +378,13 @@ static void cur_free(UhcEngine *e);
 static void cur_view(UhcEngine *e);
 
 int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg) {
-    if (!e || !cfg) { g_err = "uhc_engine_set_cfg: null"; return -2; }
+    if (!e || !cfg) { uhc_err() = "uhc_engine_set_cfg: null"; return -2; }
     e->view_gen++;
     CK(cudaSetDevice(e->device));
     const int old_tmax = e->precision == 32 ? e->evf.cfg.t_max : e->evd.cfg.t_max;
     const int old_obs_dim = uhc_engine_obs_dim(e);
     if (e->precision == 32) { fill_cfg(e->evf.cfg, cfg); e->evf.cfg.num_clips = e->num_clips; } else { fill_cfg(e->evd.cfg, cfg); e->evd.cfg.num_clips = e->num_clips; }
-    if (uhc_engine_obs_dim(e) != old_obs_dim) { g_err = "uhc_engine_set_cfg: the observation width cannot change on a live engine (buffers are sized at creation)"; return -2; }
+    if (uhc_engine_obs_dim(e) != old_obs_dim) { uhc_err() = "uhc_engine_set_cfg: the observation width cannot change on a live engine (buffers are sized at creation)"; return -2; }
     if (cfg->t_max != old_tmax && e->clip_w.empty()) { CK(cudaDeviceSynchronize()); return e->cur.M ? cur_weights(e) : upload_clip_cdf(e); }   // the sample_keys weights depend on t_max
     return 0;
 }
@@ -420,11 +427,11 @@ static int new_clip_table(UhcEngine *e, int nclips, const int *clip_len, const d
 }
 
 int uhc_load_clips(UhcEngine *e, int nclips, const int *clip_len, const double *frames_host, const double *shape_host) {
-    if (!e || nclips <= 0 || !clip_len || !frames_host || !shape_host) { g_err = "uhc_load_clips: bad argument"; return -2; }
+    if (!e || nclips <= 0 || !clip_len || !frames_host || !shape_host) { uhc_err() = "uhc_load_clips: bad argument"; return -2; }
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
     size_t nframes = 0;
-    for (int i = 0; i < nclips; i++) { if (clip_len[i] < 2) { g_err = "uhc_load_clips: clip shorter than 2 frames"; return -2; } nframes += clip_len[i]; }
+    for (int i = 0; i < nclips; i++) { if (clip_len[i] < 2) { uhc_err() = "uhc_load_clips: clip shorter than 2 frames"; return -2; } nframes += clip_len[i]; }
     if (new_clip_table(e, nclips, clip_len, shape_host)) return -1;
     const size_t nf = nframes * EX_SIZE;
     if (e->precision == 32) {
@@ -454,17 +461,17 @@ static void add_elapsed(float *acc, cudaEvent_t a, cudaEvent_t b) { float ms = 0
 
 int uhc_load_motions(UhcEngine *e, int nclips, const int *clip_len, int kind, int pose_dim, const double *rows_host, const double *shape_host,
                      const int *fk_model, int chunk_frames) {
-    if (!e || nclips <= 0 || !clip_len || !rows_host || !shape_host) { g_err = "uhc_load_motions: bad argument"; return -2; }
-    if (kind != UHC_MOTION_SMPL && kind != UHC_MOTION_QPOS) { g_err = "uhc_load_motions: kind must be UHC_MOTION_SMPL or UHC_MOTION_QPOS"; return -2; }
-    if (kind == UHC_MOTION_SMPL ? (pose_dim != 72 && pose_dim != 156) : pose_dim != NQ) { g_err = "uhc_load_motions: pose_dim must be 72 or 156 (UHC_MOTION_SMPL) or 76 (UHC_MOTION_QPOS)"; return -2; }
-    if (chunk_frames < 0) { g_err = "uhc_load_motions: chunk_frames < 0"; return -2; }
+    if (!e || nclips <= 0 || !clip_len || !rows_host || !shape_host) { uhc_err() = "uhc_load_motions: bad argument"; return -2; }
+    if (kind != UHC_MOTION_SMPL && kind != UHC_MOTION_QPOS) { uhc_err() = "uhc_load_motions: kind must be UHC_MOTION_SMPL or UHC_MOTION_QPOS"; return -2; }
+    if (kind == UHC_MOTION_SMPL ? (pose_dim != 72 && pose_dim != 156) : pose_dim != NQ) { uhc_err() = "uhc_load_motions: pose_dim must be 72 or 156 (UHC_MOTION_SMPL) or 76 (UHC_MOTION_QPOS)"; return -2; }
+    if (chunk_frames < 0) { uhc_err() = "uhc_load_motions: chunk_frames < 0"; return -2; }
     long long total = 0;
     for (int i = 0; i < nclips; i++) {
-        if (clip_len[i] < 2) { g_err = "uhc_load_motions: clip shorter than 2 frames"; return -2; }
+        if (clip_len[i] < 2) { uhc_err() = "uhc_load_motions: clip shorter than 2 frames"; return -2; }
         total += clip_len[i];
-        if (fk_model && (fk_model[i] < 0 || fk_model[i] >= e->nshape)) { g_err = "uhc_load_motions: fk_model index out of range"; return -2; }
+        if (fk_model && (fk_model[i] < 0 || fk_model[i] >= e->nshape)) { uhc_err() = "uhc_load_motions: fk_model index out of range"; return -2; }
     }
-    if (total > 0x7fffffffLL) { g_err = "uhc_load_motions: more than 2^31 - 1 frames"; return -2; }
+    if (total > 0x7fffffffLL) { uhc_err() = "uhc_load_motions: more than 2^31 - 1 frames"; return -2; }
     const int row_w = kind == UHC_MOTION_SMPL ? pose_dim + 3 : NQ;
     const int cap = chunk_frames > 0 ? chunk_frames : 32768;
     // chunks of whole clips, each of at most `cap` frames unless a single clip is longer
@@ -514,8 +521,8 @@ int uhc_load_motions(UhcEngine *e, int nclips, const int *clip_len, int kind, in
 }
 
 int uhc_get_clip_frames(UhcEngine *e, int clip, int first, int n, double *out_host) {
-    if (!e || !out_host || clip < 0 || clip >= e->num_clips || first < 0 || n < 0 || first + n > e->clip_len_h[clip]) { g_err = "uhc_get_clip_frames: bad argument"; return -2; }
-    if (!e->d_expert) { g_err = "uhc_get_clip_frames: no clips loaded"; return -3; }
+    if (!e || !out_host || clip < 0 || clip >= e->num_clips || first < 0 || n < 0 || first + n > e->clip_len_h[clip]) { uhc_err() = "uhc_get_clip_frames: bad argument"; return -2; }
+    if (!e->d_expert) { uhc_err() = "uhc_get_clip_frames: no clips loaded"; return -3; }
     if (n == 0) return 0;
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
@@ -531,13 +538,13 @@ int uhc_get_clip_frames(UhcEngine *e, int clip, int first, int n, double *out_ho
 }
 
 int uhc_load_motions_time(const UhcEngine *e, float *out2) {
-    if (!e || !out2) { g_err = "uhc_load_motions_time: bad argument"; return -2; }
+    if (!e || !out2) { uhc_err() = "uhc_load_motions_time: bad argument"; return -2; }
     out2[0] = e->mo_ms[0]; out2[1] = e->mo_ms[1];
     return 0;
 }
 
 int uhc_set_neutral_pose(UhcEngine *e, const double *qpos76, const double *qvel75) {
-    if (!e || !qpos76 || !qvel75) { g_err = "uhc_set_neutral_pose: bad argument"; return -2; }
+    if (!e || !qpos76 || !qvel75) { uhc_err() = "uhc_set_neutral_pose: bad argument"; return -2; }
     e->view_gen++;
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
@@ -549,14 +556,14 @@ int uhc_set_neutral_pose(UhcEngine *e, const double *qpos76, const double *qvel7
 }
 
 int uhc_set_clip_weights(UhcEngine *e, int nclips, const float *weights_host) {
-    if (!e || nclips != e->num_clips) { g_err = "uhc_set_clip_weights: call after uhc_load_clips with one weight per clip"; return -2; }
-    if (e->cur.M) { g_err = "uhc_set_clip_weights: the device curriculum owns the clip weights (uhc_curriculum_enable with max_freq 0 turns it off)"; return -2; }
+    if (!e || nclips != e->num_clips) { uhc_err() = "uhc_set_clip_weights: call after uhc_load_clips with one weight per clip"; return -2; }
+    if (e->cur.M) { uhc_err() = "uhc_set_clip_weights: the device curriculum owns the clip weights (uhc_curriculum_enable with max_freq 0 turns it off)"; return -2; }
     e->view_gen++;
     CK(cudaSetDevice(e->device));
     if (!weights_host) e->clip_w.clear();
     else {
-        double tot = 0; for (int i = 0; i < nclips; i++) { if (!(weights_host[i] >= 0.f)) { g_err = "uhc_set_clip_weights: negative / NaN weight"; return -2; } tot += weights_host[i]; }
-        if (!(tot > 0)) { g_err = "uhc_set_clip_weights: all weights are zero"; return -2; }
+        double tot = 0; for (int i = 0; i < nclips; i++) { if (!(weights_host[i] >= 0.f)) { uhc_err() = "uhc_set_clip_weights: negative / NaN weight"; return -2; } tot += weights_host[i]; }
+        if (!(tot > 0)) { uhc_err() = "uhc_set_clip_weights: all weights are zero"; return -2; }
         e->clip_w.assign(weights_host, weights_host + nclips);
     }
     CK(cudaDeviceSynchronize());
@@ -564,9 +571,9 @@ int uhc_set_clip_weights(UhcEngine *e, int nclips, const float *weights_host) {
 }
 
 int uhc_set_clip_models(UhcEngine *e, int nclips, const int *clip_model) {
-    if (!e || !clip_model || nclips != e->num_clips) { g_err = "uhc_set_clip_models: call after uhc_load_clips with one entry per clip"; return -2; }
+    if (!e || !clip_model || nclips != e->num_clips) { uhc_err() = "uhc_set_clip_models: call after uhc_load_clips with one entry per clip"; return -2; }
     e->view_gen++;
-    for (int i = 0; i < nclips; i++) if (clip_model[i] < 0 || clip_model[i] >= e->nshape) { g_err = "uhc_set_clip_models: shape index out of range"; return -2; }
+    for (int i = 0; i < nclips; i++) if (clip_model[i] < 0 || clip_model[i] >= e->nshape) { uhc_err() = "uhc_set_clip_models: shape index out of range"; return -2; }
     CK(cudaSetDevice(e->device));
     if (e->d_clip_model) cudaFree(e->d_clip_model);
     CK(cudaMalloc((void **)&e->d_clip_model, nclips * sizeof(int)));
@@ -577,15 +584,15 @@ int uhc_set_clip_models(UhcEngine *e, int nclips, const int *clip_model) {
 
 int uhc_env_reset(UhcEngine *e, int n, const int *env_ids_host, const int *clip_host, const int *start_host, const int *len_host,
                   const float *qpos_dev, const float *qvel_dev, float *obs_dev, void *stream) {
-    if (!e || n <= 0 || !env_ids_host || !clip_host || !start_host || !len_host) { g_err = "uhc_env_reset: bad argument"; return -2; }
-    if (!e->d_expert) { g_err = "uhc_env_reset: no clips loaded"; return -3; }
+    if (!e || n <= 0 || !env_ids_host || !clip_host || !start_host || !len_host) { uhc_err() = "uhc_env_reset: bad argument"; return -2; }
+    if (!e->d_expert) { uhc_err() = "uhc_env_reset: no clips loaded"; return -3; }
     CK(cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     for (int i = 0; i < n; i++) {
-        if (env_ids_host[i] < 0 || env_ids_host[i] >= e->E) { g_err = "uhc_env_reset: env id out of range"; return -2; }
+        if (env_ids_host[i] < 0 || env_ids_host[i] >= e->E) { uhc_err() = "uhc_env_reset: env id out of range"; return -2; }
         const int c = clip_host[i];
-        if (c < 0 || c >= e->num_clips) { g_err = "uhc_env_reset: clip index out of range"; return -2; }
-        if (start_host[i] < 0 || len_host[i] < 1 || start_host[i] + len_host[i] > e->clip_len_h[c]) { g_err = "uhc_env_reset: (start, length) outside the clip"; return -2; }
+        if (c < 0 || c >= e->num_clips) { uhc_err() = "uhc_env_reset: clip index out of range"; return -2; }
+        if (start_host[i] < 0 || len_host[i] < 1 || start_host[i] + len_host[i] > e->clip_len_h[c]) { uhc_err() = "uhc_env_reset: (start, length) outside the clip"; return -2; }
     }
     // the arguments travel through a pinned staging buffer owned by the engine, so the caller's arrays are free on return and the
     // call stays asynchronous: the only wait is for the PREVIOUS reset's kernel to have consumed the staging buffer
@@ -613,8 +620,8 @@ int uhc_env_reset(UhcEngine *e, int n, const int *env_ids_host, const int *clip_
 
 int uhc_env_step(UhcEngine *e, const float *actions_dev, float *obs_dev, float *reward_dev, float *cinfo_dev, int *fail_dev, int *end_dev,
                  float *percent_dev, float *torque_dev, void *stream) {
-    if (!e || !actions_dev) { g_err = "uhc_env_step: bad argument"; return -2; }
-    if (!e->d_expert) { g_err = "uhc_env_step: no clips loaded"; return -3; }
+    if (!e || !actions_dev) { uhc_err() = "uhc_env_step: bad argument"; return -2; }
+    if (!e->d_expert) { uhc_err() = "uhc_env_step: no clips loaded"; return -3; }
     CK(cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (e->d_order) { k_order_envs<<<1, 1024, 0, st>>>(e->precision == 32 ? e->evf.istate : e->evd.istate, e->E, e->d_order); e->launches++; }
@@ -630,7 +637,7 @@ int uhc_env_step(UhcEngine *e, const float *actions_dev, float *obs_dev, float *
 
 int uhc_env_step_host(UhcEngine *e, const float *actions_host, float *obs_host, float *reward_host, float *cinfo_host, int *fail_host,
                       int *end_host, float *percent_host) {
-    if (!e || !actions_host) { g_err = "uhc_env_step_host: bad argument"; return -2; }
+    if (!e || !actions_host) { uhc_err() = "uhc_env_step_host: bad argument"; return -2; }
     CK(cudaSetDevice(e->device));
     const size_t E = e->E;
     CK(cudaMemcpyAsync(e->d_act, actions_host, E * (size_t)uhc_engine_act_dim(e) * 4, cudaMemcpyHostToDevice, 0));
@@ -648,8 +655,8 @@ int uhc_env_step_host(UhcEngine *e, const float *actions_host, float *obs_host, 
 
 // state of n envs in one gather kernel + one copy: out = [n][319] doubles (qpos76 qvel75 xpos72 bquat96), iout = [n][8]
 int uhc_env_get_state_batch(UhcEngine *e, int n, const int *env_ids_host, double *out_host, int *istate_host) {
-    if (!e || n <= 0 || !env_ids_host || !out_host) { g_err = "uhc_env_get_state_batch: bad argument"; return -2; }
-    for (int i = 0; i < n; i++) if (env_ids_host[i] < 0 || env_ids_host[i] >= e->E) { g_err = "uhc_env_get_state_batch: env id out of range"; return -2; }
+    if (!e || n <= 0 || !env_ids_host || !out_host) { uhc_err() = "uhc_env_get_state_batch: bad argument"; return -2; }
+    for (int i = 0; i < n; i++) if (env_ids_host[i] < 0 || env_ids_host[i] >= e->E) { uhc_err() = "uhc_env_get_state_batch: env id out of range"; return -2; }
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
     if (e->gather_cap < n) {
@@ -668,7 +675,7 @@ int uhc_env_get_state_batch(UhcEngine *e, int n, const int *env_ids_host, double
 }
 
 int uhc_env_get_state(UhcEngine *e, int env, double *qpos76, double *qvel75, double *xpos72, double *bquat96, int *istate8) {
-    if (!e || env < 0 || env >= e->E) { g_err = "uhc_env_get_state: bad argument"; return -2; }
+    if (!e || env < 0 || env >= e->E) { uhc_err() = "uhc_env_get_state: bad argument"; return -2; }
     double out[319]; int is[SI_SIZE];
     int rc = uhc_env_get_state_batch(e, 1, &env, out, is);
     if (rc) return rc;
@@ -683,8 +690,8 @@ int uhc_env_get_state(UhcEngine *e, int env, double *qpos76, double *qvel75, dou
 // fail_safe (humanoid_im.py:902-905) for n envs at once: overwrite qpos/qvel, run sim.forward(), keep cur_t and the body quats.
 // One reset-with-override launch for all of them; no allocation in the steady state.
 int uhc_env_set_state_batch(UhcEngine *e, int n, const int *env_ids_host, const double *qpos_host, const double *qvel_host) {
-    if (!e || n <= 0 || !env_ids_host || !qpos_host || !qvel_host) { g_err = "uhc_env_set_state_batch: bad argument"; return -2; }
-    for (int i = 0; i < n; i++) if (env_ids_host[i] < 0 || env_ids_host[i] >= e->E) { g_err = "uhc_env_set_state_batch: env id out of range"; return -2; }
+    if (!e || n <= 0 || !env_ids_host || !qpos_host || !qvel_host) { uhc_err() = "uhc_env_set_state_batch: bad argument"; return -2; }
+    for (int i = 0; i < n; i++) if (env_ids_host[i] < 0 || env_ids_host[i] >= e->E) { uhc_err() = "uhc_env_set_state_batch: env id out of range"; return -2; }
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
     const size_t rs = e->precision == 32 ? 4 : 8;
@@ -703,7 +710,7 @@ int uhc_env_set_state_batch(UhcEngine *e, int n, const int *env_ids_host, const 
     if (rc) return rc;
     for (int i = 0; i < n; i++) {
         clip[i] = is[(size_t)i * SI_SIZE + SI_CLIP]; start[i] = is[(size_t)i * SI_SIZE + SI_START]; len[i] = is[(size_t)i * SI_SIZE + SI_LEN];
-        if (len[i] < 2 || clip[i] < 0 || clip[i] >= e->num_clips) { g_err = "uhc_env_set_state_batch: env has no valid episode (reset it first)"; return -2; }
+        if (len[i] < 2 || clip[i] < 0 || clip[i] >= e->num_clips) { uhc_err() = "uhc_env_set_state_batch: env has no valid episode (reset it first)"; return -2; }
     }
     int *d_idl = e->d_keep_t + n;
     CK(cudaMemcpy(d_idl, env_ids_host, n * sizeof(int), cudaMemcpyHostToDevice));
@@ -725,7 +732,7 @@ int uhc_env_set_state(UhcEngine *e, int env, const double *qpos76, const double 
 // device counters: out[0] = env-steps failed because a body's contacts did not fit the work set (MAXCON), out[1] = env-steps
 // skipped on an invalid (stale / never reset) env record
 int uhc_engine_counters(UhcEngine *e, int *out4) {
-    if (!e || !out4) { g_err = "uhc_engine_counters: bad argument"; return -2; }
+    if (!e || !out4) { uhc_err() = "uhc_engine_counters: bad argument"; return -2; }
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(out4, e->precision == 32 ? e->evf.counters : e->evd.counters, 4 * sizeof(int), cudaMemcpyDeviceToHost));
@@ -774,22 +781,22 @@ static int cur_scratch(UhcEngine *e, size_t N) {   // the update's count table a
     return 0;
 }
 static bool cur_check(UhcEngine *e, const char *who) {
-    if (!e) { g_err = std::string(who) + ": null engine"; return false; }
-    if (!e->cur.M) { g_err = std::string(who) + ": the device curriculum is not enabled"; return false; }
+    if (!e) { uhc_err() = std::string(who) + ": null engine"; return false; }
+    if (!e->cur.M) { uhc_err() = std::string(who) + ": the device curriculum is not enabled"; return false; }
     return true;
 }
 
 int uhc_curriculum_enable(UhcEngine *e, int max_freq, double temp, double freq, double prec_freq, int fit_clip) {
-    if (!e || max_freq < 0 || max_freq > cur::MAX_FREQ_CAP) { g_err = "uhc_curriculum_enable: max_freq must be 0 .. 4096"; return -2; }
+    if (!e || max_freq < 0 || max_freq > cur::MAX_FREQ_CAP) { uhc_err() = "uhc_curriculum_enable: max_freq must be 0 .. 4096"; return -2; }
     CK(cudaSetDevice(e->device));
     if (max_freq == 0) {
         if (e->cur.M) { cur_free(e); CK(cudaDeviceSynchronize()); if (upload_clip_cdf(e)) return -1; }
         return 0;
     }
-    if (!e->d_expert || e->num_clips <= 0) { g_err = "uhc_curriculum_enable: no clips loaded"; return -2; }
-    if (!(temp > 0.0) || !(temp < 1e300)) { g_err = "uhc_curriculum_enable: temp must be a positive number"; return -2; }
-    if (!(freq >= 0.0 && freq <= 1.0) || !(prec_freq >= 0.0 && prec_freq <= 1.0)) { g_err = "uhc_curriculum_enable: freq and prec_freq must lie in [0, 1]"; return -2; }
-    if (fit_clip < -1 || fit_clip >= e->num_clips) { g_err = "uhc_curriculum_enable: fit_clip must be -1 or a clip index"; return -2; }
+    if (!e->d_expert || e->num_clips <= 0) { uhc_err() = "uhc_curriculum_enable: no clips loaded"; return -2; }
+    if (!(temp > 0.0) || !(temp < 1e300)) { uhc_err() = "uhc_curriculum_enable: temp must be a positive number"; return -2; }
+    if (!(freq >= 0.0 && freq <= 1.0) || !(prec_freq >= 0.0 && prec_freq <= 1.0)) { uhc_err() = "uhc_curriculum_enable: freq and prec_freq must lie in [0, 1]"; return -2; }
+    if (fit_clip < -1 || fit_clip >= e->num_clips) { uhc_err() = "uhc_curriculum_enable: fit_clip must be -1 or a clip index"; return -2; }
     if (e->cur.M != max_freq) {
         if (e->cur.M) cur_free(e);
         const size_t C = e->num_clips, n = C * max_freq;
@@ -808,7 +815,7 @@ int uhc_curriculum_enable(UhcEngine *e, int max_freq, double temp, double freq, 
 }
 
 int uhc_get_clip_cdf(UhcEngine *e, float *out_host) {
-    if (!e || !out_host || !e->d_clip_cdf) { g_err = "uhc_get_clip_cdf: bad argument or no clips loaded"; return -2; }
+    if (!e || !out_host || !e->d_clip_cdf) { uhc_err() = "uhc_get_clip_cdf: bad argument or no clips loaded"; return -2; }
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(out_host, e->d_clip_cdf, e->num_clips * sizeof(float), cudaMemcpyDeviceToHost));
@@ -817,10 +824,10 @@ int uhc_get_clip_cdf(UhcEngine *e, float *out_host) {
 
 int uhc_curriculum_update(UhcEngine *e, const UhcRolloutBuf *buf, int T, void *stream) {
     if (!cur_check(e, "uhc_curriculum_update")) return -2;
-    if (!buf || !buf->ep_clip || !buf->ep_pct || !buf->ep_start || T <= 0 || T > buf->T_cap) { g_err = "uhc_curriculum_update: needs ep_clip, ep_pct and ep_start rows and 0 < T <= T_cap"; return -2; }
+    if (!buf || !buf->ep_clip || !buf->ep_pct || !buf->ep_start || T <= 0 || T > buf->T_cap) { uhc_err() = "uhc_curriculum_update: needs ep_clip, ep_pct and ep_start rows and 0 < T <= T_cap"; return -2; }
     CK(cudaSetDevice(e->device));
     const size_t N = (size_t)T * e->E;
-    if (N > 0x7fffffffu) { g_err = "uhc_curriculum_update: log too long"; return -2; }
+    if (N > 0x7fffffffu) { uhc_err() = "uhc_curriculum_update: log too long"; return -2; }
     if (cur_scratch(e, N)) return -1;
     cur_bind(e);
     CK(cur::launch_update(e->cur, buf->ep_clip, buf->ep_pct, buf->ep_start, (int)N, (cudaStream_t)stream));
@@ -846,8 +853,8 @@ static int cur_from_host(UhcEngine *e, const std::vector<int> &meta, const std::
 
 int uhc_curriculum_push(UhcEngine *e, int n, const int *clip, const float *pct, const int *start) {
     if (!cur_check(e, "uhc_curriculum_push")) return -2;
-    if (n < 0 || (n > 0 && (!clip || !pct || !start))) { g_err = "uhc_curriculum_push: bad argument"; return -2; }
-    for (int i = 0; i < n; i++) if (clip[i] < 0 || clip[i] >= e->num_clips || start[i] < 0 || !(pct[i] == pct[i])) { g_err = "uhc_curriculum_push: clip out of range, negative start or NaN percent"; return -2; }
+    if (n < 0 || (n > 0 && (!clip || !pct || !start))) { uhc_err() = "uhc_curriculum_push: bad argument"; return -2; }
+    for (int i = 0; i < n; i++) if (clip[i] < 0 || clip[i] >= e->num_clips || start[i] < 0 || !(pct[i] == pct[i])) { uhc_err() = "uhc_curriculum_push: clip out of range, negative start or NaN percent"; return -2; }
     if (n == 0) return 0;
     CK(cudaSetDevice(e->device));
     // the n outcomes are a log of their own: the update's kernels append them in order and rewrite the CDF (one copy, one synchronise)
@@ -869,7 +876,7 @@ int uhc_curriculum_push(UhcEngine *e, int n, const int *clip, const float *pct, 
 
 int uhc_curriculum_get(UhcEngine *e, int *len_host, float *pct_host, int *start_host) {
     if (!cur_check(e, "uhc_curriculum_get")) return -2;
-    if (!len_host || !pct_host || !start_host) { g_err = "uhc_curriculum_get: bad argument"; return -2; }
+    if (!len_host || !pct_host || !start_host) { uhc_err() = "uhc_curriculum_get: bad argument"; return -2; }
     CK(cudaSetDevice(e->device));
     std::vector<int> meta, st; std::vector<float> pc;
     if (cur_to_host(e, meta, pc, st)) return -1;
@@ -887,14 +894,14 @@ int uhc_curriculum_get(UhcEngine *e, int *len_host, float *pct_host, int *start_
 
 int uhc_curriculum_set(UhcEngine *e, const int *len_host, const float *pct_host, const int *start_host) {
     if (!cur_check(e, "uhc_curriculum_set")) return -2;
-    if (!len_host || !pct_host || !start_host) { g_err = "uhc_curriculum_set: bad argument"; return -2; }
+    if (!len_host || !pct_host || !start_host) { uhc_err() = "uhc_curriculum_set: bad argument"; return -2; }
     const int M = e->cur.M, C = e->num_clips;
     std::vector<int> meta(2 * (size_t)C), st((size_t)C * M, 0); std::vector<float> pc((size_t)C * M, 0.f);
     for (int c = 0; c < C; c++) {
-        if (len_host[c] < 0 || len_host[c] > M) { g_err = "uhc_curriculum_set: history length outside 0 .. max_freq"; return -2; }
+        if (len_host[c] < 0 || len_host[c] > M) { uhc_err() = "uhc_curriculum_set: history length outside 0 .. max_freq"; return -2; }
         for (int k = 0; k < len_host[c]; k++) {
             const float p = pct_host[(size_t)c * M + k]; const int s = start_host[(size_t)c * M + k];
-            if (s < 0 || !(p == p)) { g_err = "uhc_curriculum_set: negative start or NaN percent"; return -2; }
+            if (s < 0 || !(p == p)) { uhc_err() = "uhc_curriculum_set: negative start or NaN percent"; return -2; }
             pc[(size_t)c * M + k] = p; st[(size_t)c * M + k] = s;
         }
         meta[2 * c] = len_host[c] % M; meta[2 * c + 1] = len_host[c];
@@ -905,8 +912,8 @@ int uhc_curriculum_set(UhcEngine *e, const int *len_host, const float *pct_host,
 }
 
 int uhc_curriculum_reseed(UhcEngine *e, float *obs_dev, void *stream) {
-    if (!e) { g_err = "uhc_curriculum_reseed: null engine"; return -2; }
-    if (!e->d_expert) { g_err = "uhc_curriculum_reseed: no clips loaded"; return -3; }
+    if (!e) { uhc_err() = "uhc_curriculum_reseed: null engine"; return -2; }
+    if (!e->d_expert) { uhc_err() = "uhc_curriculum_reseed: no clips loaded"; return -3; }
     CK(cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (!e->d_reseed) CK(cudaMalloc((void **)&e->d_reseed, (size_t)4 * e->E * sizeof(int)));
@@ -965,20 +972,20 @@ const char *cfg_error(const UhcEngine *e, int H) {
     return nullptr;
 }
 
-int install_table(UhcEngine *e, int H, const int *fk_model, const double *shape, std::string *err) {
+int install_table(UhcEngine *e, int H, const int *fk_model, const double *shape) {
     const int E = e->E;
-    if (cudaSetDevice(e->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { *err = "cudaDeviceSynchronize failed"; return -1; }
+    if (cudaSetDevice(e->device) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) { uhc_err() = "cudaDeviceSynchronize failed"; return -1; }
     std::vector<int> lens(E, H);
     std::vector<double> shp;
     if (!shape) { shp.assign((size_t)E * 17, 0.0); shape = shp.data(); }
-    if (new_clip_table(e, E, lens.data(), shape)) { *err = g_err; return -1; }
-    if (fk_model && uhc_set_clip_models(e, E, fk_model)) { *err = g_err; return -1; }
+    if (new_clip_table(e, E, lens.data(), shape)) return -1;
+    if (fk_model && uhc_set_clip_models(e, E, fk_model)) return -1;
     const size_t rs = e->precision == 32 ? 4 : 8;
     cudaError_t ce = cudaMemset(e->d_expert, 0, (size_t)E * H * EX_SIZE * rs);
     if (ce == cudaSuccess)
         ce = e->precision == 32 ? cudaFuncSetAttribute(k_track_obs<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(EPB_OBS * sizeof(Work<float>)))
                                 : cudaFuncSetAttribute(k_track_obs<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(EPB_OBS * sizeof(Work<double>)));
-    if (ce != cudaSuccess) { *err = std::string("install_table: ") + cudaGetErrorString(ce); return -1; }
+    if (ce != cudaSuccess) { uhc_err() = std::string("install_table: ") + cudaGetErrorString(ce); return -1; }
     return 0;
 }
 

@@ -15,6 +15,7 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_track.h"
+#include "errors.h"
 #include "eval_glue.h"
 #include "graph_cache.h"
 #include "track_glue.h"
@@ -22,9 +23,6 @@
 #include "sim_core.h"
 
 using namespace uhc;
-
-static thread_local std::string g_tr_err;
-#define CKT(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { g_tr_err = std::string(#x) + ": " + cudaGetErrorString(e_); return -1; } } while (0)
 
 namespace {
 
@@ -131,12 +129,12 @@ void free_ctx(TrackCtx *c) {
     delete c;
 }
 
-// the tracker of e while its table is still the engine's table and its cfg can run the stream, else null with the reason in g_tr_err
+// the tracker of e while its table is still the engine's table and its cfg can run the stream, else null with the reason in uhc_err()
 TrackCtx *live_ctx(UhcEngine *e, const char *who) {
     TrackCtx *c = e ? find_ctx(e) : nullptr;
-    if (!c) { g_tr_err = std::string(who) + ": not tracking (uhc_track_begin)"; return nullptr; }
-    if (trackx::table_gen(e) != c->table_gen) { g_tr_err = std::string(who) + ": tracking ended: the clip table was replaced"; return nullptr; }
-    if (const char *why = trackx::cfg_error(e, c->H)) { g_tr_err = std::string(who) + ": " + why; return nullptr; }
+    if (!c) { uhc_err() = std::string(who) + ": not tracking (uhc_track_begin)"; return nullptr; }
+    if (trackx::table_gen(e) != c->table_gen) { uhc_err() = std::string(who) + ": tracking ended: the clip table was replaced"; return nullptr; }
+    if (const char *why = trackx::cfg_error(e, c->H)) { uhc_err() = std::string(who) + ": " + why; return nullptr; }
     return c;
 }
 
@@ -149,7 +147,7 @@ int enqueue_push(TrackCtx *c, const evalx::EngineRefs &R, const double *next, co
     else
         k_track_push<double><<<nb, 128, 0, st>>>(m, c->kind, c->pose_dim, c->row_w, c->H, E, next, mask, c->d_fk, (double *)R.expert, R.istate, c->d_raw,
                                                  c->d_have, c->d_dropped);
-    CKT(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
@@ -158,30 +156,30 @@ int enqueue_step(TrackCtx *c, const evalx::EngineRefs &R, const TrackKey &k, cud
     const int E = c->E, nb = (E + 127) / 128;
     if (k.has_next && enqueue_push(c, R, c->d_next, k.has_mask ? c->d_mask : nullptr, st)) return -1;
     k_track_gate<<<nb, 128, 0, st>>>(R.istate, c->d_have, c->H, E, R.num_clips, c->d_status);
-    CKT(cudaGetLastError());
-    CKT(trackx::launch_obs(e, R.obs, st));
+    CK(cudaGetLastError());
+    CK(trackx::launch_obs(e, R.obs, st));
     const int rc = evalx::policy_enqueue(e, k.pol, R.obs, k.log_std, (double *)k.zstats, k.zclip, c->d_ones, R.act, st);
-    if (rc) { g_tr_err = uhc_rollout_last_error(); return rc; }
-    if (uhc_env_step(e, R.act, nullptr, k.rew, R.cinfo, k.fail, R.end, R.pct, nullptr, st)) { g_tr_err = std::string("env step: ") + uhc_last_error(); return -1; }
+    if (rc) return rc;
+    if (uhc_env_step(e, R.act, nullptr, k.rew, R.cinfo, k.fail, R.end, R.pct, nullptr, st)) return uhc_err_prefix("env step");
     if (R.precision == 32)
         k_track_post<float><<<(E + 3) / 4, 128, 0, st>>>((const float *)R.state, R.istate, c->d_status, k.fail, k.fail_safe, E, c->d_steps, c->d_reseat, (float *)k.out);
     else
         k_track_post<double><<<(E + 3) / 4, 128, 0, st>>>((const double *)R.state, R.istate, c->d_status, k.fail, k.fail_safe, E, c->d_steps, c->d_reseat, (double *)k.out);
-    CKT(cudaGetLastError());
-    if (k.fail_safe) CKT(evalx::launch_reseat(e, E, c->d_reseat, st));
+    CK(cudaGetLastError());
+    if (k.fail_safe) CK(evalx::launch_reseat(e, E, c->d_reseat, st));
     return 0;
 }
 
 int track_step(UhcEngine *e, const double *next, const int *mask, const UhcMlp *mlp, const UhcMcp *mcp, const float *log_std, const double *zstats,
                float zclip, int fail_safe, void *out, float *rew, int *fail, void *stream) {
     const char *who = mcp ? "uhc_track_step_mcp" : "uhc_track_step";
-    if (!e || (!mlp && !mcp) || !log_std || !zstats || !out || !rew || !fail) { g_tr_err = std::string(who) + ": null argument"; return -2; }
+    if (!e || (!mlp && !mcp) || !log_std || !zstats || !out || !rew || !fail) { uhc_err() = std::string(who) + ": null argument"; return -2; }
     TrackCtx *c = live_ctx(e, who);
     if (!c) return -2;
     TrackKey k; memset(&k, 0, sizeof k);
     unsigned long long sgen = 0;
     int rc = evalx::policy_prepare(e, mlp, mcp, &k.pol, &sgen);
-    if (rc) { g_tr_err = uhc_rollout_last_error(); return rc; }
+    if (rc) return rc;
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     cudaStream_t st = (cudaStream_t)stream;
     k.has_next = next != nullptr; k.has_mask = next && mask; k.fail_safe = fail_safe ? 1 : 0; k.zclip = zclip;
@@ -191,15 +189,15 @@ int track_step(UhcEngine *e, const double *next, const int *mask, const UhcMlp *
     const GraphCache::Gens gens{sgen, c->gen, R.view_gen};
     c->graphs.drop_stale(gens);
     // the caller's frames and mask are copied into the tracker's own buffers, so a new tensor per step replays the same graph
-    if (next) CKT(cudaMemcpyAsync(c->d_next, next, (size_t)c->E * c->row_w * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if (next && mask) CKT(cudaMemcpyAsync(c->d_mask, mask, (size_t)c->E * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    if (next) CK(cudaMemcpyAsync(c->d_next, next, (size_t)c->E * c->row_w * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (next && mask) CK(cudaMemcpyAsync(c->d_mask, mask, (size_t)c->E * sizeof(int), cudaMemcpyDeviceToDevice, st));
     cudaGraphExec_t exec = c->graphs.find(key);
     if (!exec) {
-        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_step(c, R, k, cs); }, &exec, &g_tr_err);
+        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_step(c, R, k, cs); }, &exec);
         if (rc) return rc;
         c->graphs.insert(std::move(key), gens, exec);
     }
-    CKT(cudaGraphLaunch(exec, st));
+    CK(cudaGraphLaunch(exec, st));
     return 0;
 }
 
@@ -207,44 +205,41 @@ int track_step(UhcEngine *e, const double *next, const int *mask, const UhcMlp *
 
 extern "C" {
 
-const char *uhc_track_last_error(void) { return g_tr_err.c_str(); }
-
 int uhc_track_begin(UhcEngine *e, int window, int kind, int pose_dim, const int *fk_model_host, const double *shape_host) {
-    if (!e) { g_tr_err = "uhc_track_begin: null engine"; return -2; }
-    if (kind != UHC_MOTION_SMPL && kind != UHC_MOTION_QPOS) { g_tr_err = "uhc_track_begin: kind must be UHC_MOTION_SMPL or UHC_MOTION_QPOS"; return -2; }
-    if (kind == UHC_MOTION_SMPL ? (pose_dim != 72 && pose_dim != 156) : pose_dim != UHC_NQ) { g_tr_err = "uhc_track_begin: pose_dim must be 72 or 156 (UHC_MOTION_SMPL) or 76 (UHC_MOTION_QPOS)"; return -2; }
-    if (const char *why = trackx::cfg_error(e, window)) { g_tr_err = std::string("uhc_track_begin: ") + why; return -2; }
+    if (!e) { uhc_err() = "uhc_track_begin: null engine"; return -2; }
+    if (kind != UHC_MOTION_SMPL && kind != UHC_MOTION_QPOS) { uhc_err() = "uhc_track_begin: kind must be UHC_MOTION_SMPL or UHC_MOTION_QPOS"; return -2; }
+    if (kind == UHC_MOTION_SMPL ? (pose_dim != 72 && pose_dim != 156) : pose_dim != UHC_NQ) { uhc_err() = "uhc_track_begin: pose_dim must be 72 or 156 (UHC_MOTION_SMPL) or 76 (UHC_MOTION_QPOS)"; return -2; }
+    if (const char *why = trackx::cfg_error(e, window)) { uhc_err() = std::string("uhc_track_begin: ") + why; return -2; }
     const int E = uhc_num_envs(e);
-    if (fk_model_host) for (int i = 0; i < E; i++) if (fk_model_host[i] < 0 || fk_model_host[i] >= trackx::num_shapes(e)) { g_tr_err = "uhc_track_begin: fk_model index out of range"; return -2; }
-    if ((size_t)E * window * REC * 8 > ((size_t)1 << 40)) { g_tr_err = "uhc_track_begin: window too large"; return -2; }
+    if (fk_model_host) for (int i = 0; i < E; i++) if (fk_model_host[i] < 0 || fk_model_host[i] >= trackx::num_shapes(e)) { uhc_err() = "uhc_track_begin: fk_model index out of range"; return -2; }
+    if ((size_t)E * window * REC * 8 > ((size_t)1 << 40)) { uhc_err() = "uhc_track_begin: window too large"; return -2; }
     if (TrackCtx *old = find_ctx(e)) free_ctx(old);
-    std::string err;
-    if (trackx::install_table(e, window, fk_model_host, shape_host, &err)) { g_tr_err = err; return -1; }
+    if (trackx::install_table(e, window, fk_model_host, shape_host)) return -1;
     TrackCtx *c = new TrackCtx(); c->eng = e; g_tr.push_back(c);
     c->E = E; c->H = window; c->kind = kind; c->pose_dim = pose_dim; c->row_w = kind == UHC_MOTION_SMPL ? pose_dim + 3 : UHC_NQ;
     c->table_gen = trackx::table_gen(e); c->gen = ++g_tr_gen;
     const size_t En = E;
-    CKT(cudaMalloc((void **)&c->d_raw, En * 2 * c->row_w * sizeof(double))); CKT(cudaMalloc((void **)&c->d_next, En * c->row_w * sizeof(double)));
-    for (int **p : {&c->d_have, &c->d_steps, &c->d_dropped, &c->d_status, &c->d_reseat, &c->d_mask, &c->d_ids}) { CKT(cudaMalloc((void **)p, En * sizeof(int))); CKT(cudaMemset(*p, 0, En * sizeof(int))); }
-    CKT(cudaMalloc((void **)&c->d_ones, En));
+    CK(cudaMalloc((void **)&c->d_raw, En * 2 * c->row_w * sizeof(double))); CK(cudaMalloc((void **)&c->d_next, En * c->row_w * sizeof(double)));
+    for (int **p : {&c->d_have, &c->d_steps, &c->d_dropped, &c->d_status, &c->d_reseat, &c->d_mask, &c->d_ids}) { CK(cudaMalloc((void **)p, En * sizeof(int))); CK(cudaMemset(*p, 0, En * sizeof(int))); }
+    CK(cudaMalloc((void **)&c->d_ones, En));
     k_fill_ones<<<(E + 255) / 256, 256>>>(c->d_ones, E);
-    CKT(cudaGetLastError());
-    if (fk_model_host) { CKT(cudaMalloc((void **)&c->d_fk, En * sizeof(int))); CKT(cudaMemcpy(c->d_fk, fk_model_host, En * sizeof(int), cudaMemcpyHostToDevice)); }
-    CKT(cudaHostAlloc((void **)&c->h_ids, En * sizeof(int), cudaHostAllocDefault));
-    CKT(cudaEventCreateWithFlags(&c->ids_done, cudaEventDisableTiming));
-    CKT(cudaDeviceSynchronize());
+    CK(cudaGetLastError());
+    if (fk_model_host) { CK(cudaMalloc((void **)&c->d_fk, En * sizeof(int))); CK(cudaMemcpy(c->d_fk, fk_model_host, En * sizeof(int), cudaMemcpyHostToDevice)); }
+    CK(cudaHostAlloc((void **)&c->h_ids, En * sizeof(int), cudaHostAllocDefault));
+    CK(cudaEventCreateWithFlags(&c->ids_done, cudaEventDisableTiming));
+    CK(cudaDeviceSynchronize());
     return 0;
 }
 
 int uhc_track_reset(UhcEngine *e, int n, const int *env_ids_host, const double *frames_dev, const float *qpos_dev, const float *qvel_dev, void *stream) {
     TrackCtx *c = live_ctx(e, "uhc_track_reset");
     if (!c) return -2;
-    if (n < 1 || n > c->E || !env_ids_host || !frames_dev) { g_tr_err = "uhc_track_reset: needs 1 <= n <= E, env ids and frames"; return -2; }
-    for (int i = 0; i < n; i++) if (env_ids_host[i] < 0 || env_ids_host[i] >= c->E) { g_tr_err = "uhc_track_reset: env id out of range"; return -2; }
+    if (n < 1 || n > c->E || !env_ids_host || !frames_dev) { uhc_err() = "uhc_track_reset: needs 1 <= n <= E, env ids and frames"; return -2; }
+    for (int i = 0; i < n; i++) if (env_ids_host[i] < 0 || env_ids_host[i] >= c->E) { uhc_err() = "uhc_track_reset: env id out of range"; return -2; }
     cudaStream_t st = (cudaStream_t)stream;
-    CKT(cudaEventSynchronize(c->ids_done));            // the previous reset's kernel has consumed the staging buffer
+    CK(cudaEventSynchronize(c->ids_done));            // the previous reset's kernel has consumed the staging buffer
     memcpy(c->h_ids, env_ids_host, n * sizeof(int));
-    CKT(cudaMemcpyAsync(c->d_ids, c->h_ids, n * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_ids, c->h_ids, n * sizeof(int), cudaMemcpyHostToDevice, st));
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     const MotionModel &m = trackx::motion_model(e);
     if (R.precision == 32)
@@ -253,30 +248,28 @@ int uhc_track_reset(UhcEngine *e, int n, const int *env_ids_host, const double *
     else
         k_track_rows<double><<<(n + 127) / 128, 128, 0, st>>>(m, c->kind, c->pose_dim, c->row_w, c->H, n, c->d_ids, frames_dev, c->d_fk, (double *)R.expert,
                                                             c->d_raw, c->d_have, c->d_steps, c->d_dropped);
-    CKT(cudaGetLastError());
-    CKT(cudaEventRecord(c->ids_done, st));
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(c->ids_done, st));
     c->zeros.assign(n, 0); c->lens.assign(n, c->H);
-    if (uhc_env_reset(e, n, env_ids_host, env_ids_host, c->zeros.data(), c->lens.data(), qpos_dev, qvel_dev, nullptr, stream)) {
-        g_tr_err = std::string("uhc_track_reset: ") + uhc_last_error(); return -1;
-    }
+    if (uhc_env_reset(e, n, env_ids_host, env_ids_host, c->zeros.data(), c->lens.data(), qpos_dev, qvel_dev, nullptr, stream)) return uhc_err_prefix("uhc_track_reset");
     return 0;
 }
 
 int uhc_track_step(UhcEngine *e, const double *next_frames_dev, const int *mask_dev, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats,
                    float zclip, int fail_safe, void *state_out_dev, float *reward_dev, int *fail_dev, void *stream) {
-    if (!mlp) { g_tr_err = "uhc_track_step: null policy"; return -2; }
+    if (!mlp) { uhc_err() = "uhc_track_step: null policy"; return -2; }
     return track_step(e, next_frames_dev, mask_dev, mlp, nullptr, log_std, zfilter_stats, zclip, fail_safe, state_out_dev, reward_dev, fail_dev, stream);
 }
 int uhc_track_step_mcp(UhcEngine *e, const double *next_frames_dev, const int *mask_dev, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats,
                        float zclip, int fail_safe, void *state_out_dev, float *reward_dev, int *fail_dev, void *stream) {
-    if (!mcp) { g_tr_err = "uhc_track_step_mcp: null policy"; return -2; }
+    if (!mcp) { uhc_err() = "uhc_track_step_mcp: null policy"; return -2; }
     return track_step(e, next_frames_dev, mask_dev, nullptr, mcp, log_std, zfilter_stats, zclip, fail_safe, state_out_dev, reward_dev, fail_dev, stream);
 }
 
 int uhc_track_push(UhcEngine *e, const double *next_frames_dev, const int *mask_dev, void *stream) {
     TrackCtx *c = live_ctx(e, "uhc_track_push");
     if (!c) return -2;
-    if (!next_frames_dev) { g_tr_err = "uhc_track_push: null frames"; return -2; }
+    if (!next_frames_dev) { uhc_err() = "uhc_track_push: null frames"; return -2; }
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     return enqueue_push(c, R, next_frames_dev, mask_dev, (cudaStream_t)stream);
 }
@@ -284,29 +277,29 @@ int uhc_track_push(UhcEngine *e, const double *next_frames_dev, const int *mask_
 int uhc_track_obs(UhcEngine *e, float *obs_dev, void *stream) {
     TrackCtx *c = live_ctx(e, "uhc_track_obs");
     if (!c) return -2;
-    if (!obs_dev) { g_tr_err = "uhc_track_obs: null output"; return -2; }
+    if (!obs_dev) { uhc_err() = "uhc_track_obs: null output"; return -2; }
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     cudaStream_t st = (cudaStream_t)stream;
     const int nb = (c->E + 127) / 128;
     k_track_gate<<<nb, 128, 0, st>>>(R.istate, c->d_have, c->H, c->E, R.num_clips, c->d_status);
-    CKT(cudaGetLastError());
-    CKT(trackx::launch_obs(e, obs_dev, st));
+    CK(cudaGetLastError());
+    CK(trackx::launch_obs(e, obs_dev, st));
     k_track_ungate<<<nb, 128, 0, st>>>(R.istate, c->d_status, c->E);
-    CKT(cudaGetLastError());
+    CK(cudaGetLastError());
     return 0;
 }
 
 int uhc_track_state(UhcEngine *e, int *out_host) {
     TrackCtx *c = e ? find_ctx(e) : nullptr;
-    if (!c || !out_host) { g_tr_err = "uhc_track_state: not tracking or null output"; return -2; }
+    if (!c || !out_host) { uhc_err() = "uhc_track_state: not tracking or null output"; return -2; }
     const size_t E = c->E;
     evalx::EngineRefs R; evalx::engine_refs(e, &R);
     std::vector<int> steps(E), have(E), dropped(E), is(E * SI_SIZE);
-    CKT(cudaDeviceSynchronize());
-    CKT(cudaMemcpy(steps.data(), c->d_steps, E * sizeof(int), cudaMemcpyDeviceToHost));
-    CKT(cudaMemcpy(have.data(), c->d_have, E * sizeof(int), cudaMemcpyDeviceToHost));
-    CKT(cudaMemcpy(dropped.data(), c->d_dropped, E * sizeof(int), cudaMemcpyDeviceToHost));
-    CKT(cudaMemcpy(is.data(), R.istate, E * SI_SIZE * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaDeviceSynchronize());
+    CK(cudaMemcpy(steps.data(), c->d_steps, E * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(have.data(), c->d_have, E * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(dropped.data(), c->d_dropped, E * sizeof(int), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(is.data(), R.istate, E * SI_SIZE * sizeof(int), cudaMemcpyDeviceToHost));
     for (size_t i = 0; i < E; i++) {
         int *o = out_host + i * UHC_TRACK_STATE_COLS;
         o[0] = steps[i]; o[1] = is[i * SI_SIZE + SI_CUR_T]; o[2] = have[i]; o[3] = dropped[i];

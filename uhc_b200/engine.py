@@ -145,9 +145,10 @@ def load_library():
     return _lib
 
 
-def _chk(rc):
+def _chk(rc, who="uhc_b200", invalid=RuntimeError):
+    """raises `who: <the library's error text>` for a non-zero return code: `invalid` for -2 (a refused argument), RuntimeError otherwise"""
     if rc != 0:
-        raise RuntimeError("uhc_b200: " + load_library().uhc_last_error().decode())
+        raise (invalid if rc == -2 else RuntimeError)(f"{who}: " + load_library().uhc_last_error().decode())
 
 
 def _ip(a):
@@ -367,9 +368,7 @@ class Engine:
         fn = self.lib.uhc_eval_run_mcp_ex if isinstance(policy, UhcMcp) else self.lib.uhc_eval_run_ex
         rc = fn(self.h, C.c_int(n), _ip(clips), C.byref(policy), C.c_void_p(log_std.data_ptr()), C.c_void_p(zfilter_stats.data_ptr()), C.c_float(zclip),
                 C.c_int(int(bool(fail_safe))), C.c_int(int(window)), C.byref(out), self._stream())
-        if rc != 0:
-            self.lib.uhc_eval_last_error.restype = C.c_char_p
-            raise (ValueError if rc == -2 else RuntimeError)("uhc_eval_run: " + self.lib.uhc_eval_last_error().decode())
+        _chk(rc, "uhc_eval_run", ValueError)
         return self._eval_result(rec, 0, n, frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None)
 
     @staticmethod
@@ -412,9 +411,7 @@ class Engine:
         fn = self.lib.uhc_eval_run_groups_mcp_ex if mcp else self.lib.uhc_eval_run_groups_ex
         rc = fn(self.h, C.c_int(G), _ip(sizes), _ip(allc), pols, zs, C.c_float(zclip), C.c_int(int(bool(fail_safe))), C.c_int(int(window)),
                 C.byref(out), self._stream())
-        if rc != 0:
-            self.lib.uhc_eval_last_error.restype = C.c_char_p
-            raise (ValueError if rc == -2 else RuntimeError)("uhc_eval_run_groups: " + self.lib.uhc_eval_last_error().decode())
+        _chk(rc, "uhc_eval_run_groups", ValueError)
         fr, st, sm = frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None
         res, o = [], 0
         for k in sizes:
@@ -423,11 +420,6 @@ class Engine:
         return res
 
     # ---- the SMPL export (include/uhc_export.h)
-    def _exp_chk(self, rc, who):
-        if rc != 0:
-            self.lib.uhc_export_last_error.restype = C.c_char_p
-            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_export_last_error().decode())
-
     def qpos_to_smpl(self, qpos, variants=None):
         """qpos_to_smpl (uhc/smpllib/smpl_mujoco.py:738-752) on the device (uhc_qpos_to_smpl): qpos = a cuda tensor [n][>= 76] of float32 | float64
         whose rows are contiguous (its first 76 columns are read, in place) or anything numpy takes (copied to the device as float64); variants =
@@ -440,9 +432,9 @@ class Engine:
         n = q.shape[0]
         v = None if variants is None else t.as_tensor(np.array(np.broadcast_to(np.asarray(variants, np.int32), (n,))), device=dev)
         pose, trans = t.empty(n, 72, dtype=t.float64, device=dev), t.empty(n, 3, dtype=t.float64, device=dev)
-        self._exp_chk(self.lib.uhc_qpos_to_smpl(self.h, C.c_void_p(q.data_ptr()), C.c_int(32 if q.dtype == t.float32 else 64), C.c_long(n),
-                                                C.c_long(q.stride(0) if n > 1 else q.shape[1]), C.c_void_p(v.data_ptr() if v is not None else None),
-                                                C.c_void_p(pose.data_ptr()), C.c_void_p(trans.data_ptr()), self._stream()), "uhc_qpos_to_smpl")
+        _chk(self.lib.uhc_qpos_to_smpl(self.h, C.c_void_p(q.data_ptr()), C.c_int(32 if q.dtype == t.float32 else 64), C.c_long(n),
+                                       C.c_long(q.stride(0) if n > 1 else q.shape[1]), C.c_void_p(v.data_ptr() if v is not None else None),
+                                       C.c_void_p(pose.data_ptr()), C.c_void_p(trans.data_ptr()), self._stream()), "uhc_qpos_to_smpl", ValueError)
         return pose, trans
 
     def track_smpl(self, state_out, pose=None, trans=None):
@@ -454,20 +446,15 @@ class Engine:
         trans = t.empty(self.E, 3, dtype=t.float64, device=dev) if trans is None else trans
         assert state_out.is_cuda and state_out.is_contiguous() and tuple(state_out.shape) == (self.E, 223)
         assert state_out.dtype == (t.float32 if self.precision == 32 else t.float64)
-        self._exp_chk(self.lib.uhc_track_smpl(self.h, C.c_void_p(state_out.data_ptr()), C.c_void_p(pose.data_ptr()), C.c_void_p(trans.data_ptr()),
-                                              self._stream()), "uhc_track_smpl")
+        _chk(self.lib.uhc_track_smpl(self.h, C.c_void_p(state_out.data_ptr()), C.c_void_p(pose.data_ptr()), C.c_void_p(trans.data_ptr()),
+                                     self._stream()), "uhc_track_smpl", ValueError)
         return pose, trans
 
     # ---- the renderer (include/uhc_render.h)
-    def _rnd_chk(self, rc, who):
-        if rc != 0:
-            self.lib.uhc_render_last_error.restype = C.c_char_p
-            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_render_last_error().decode())
-
     def _render_init(self):
         if not self._render_ready:
             self._rhulls = self.model.render_struct(self.variants)
-            self._rnd_chk(self.lib.uhc_render_init(self.h, C.byref(self._rhulls)), "uhc_render_init")
+            _chk(self.lib.uhc_render_init(self.h, C.byref(self._rhulls)), "uhc_render_init", ValueError)
             self._render_ready = True
 
     def _rows(self, q, n=None):
@@ -494,8 +481,8 @@ class Engine:
         pose = t.zeros(n, 2, 24, 12, dtype=t.float32, device=self.obs.device)
         p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
         pitch = lambda x: C.c_long(x.stride(0) if x is not None and x.shape[0] > 1 else (x.shape[1] if x is not None else NQ))
-        self._rnd_chk(self.lib.uhc_render_pose(self.h, C.c_long(n), p(q), C.c_int(32 if q.dtype == t.float32 else 64), pitch(q), p(g), pitch(g), p(v),
-                                               p(pose), self._stream()), "uhc_render_pose")
+        _chk(self.lib.uhc_render_pose(self.h, C.c_long(n), p(q), C.c_int(32 if q.dtype == t.float32 else 64), pitch(q), p(g), pitch(g), p(v),
+                                      p(pose), self._stream()), "uhc_render_pose", ValueError)
         return pose
 
     def _render_out(self, n, size, depth, label):
@@ -523,8 +510,8 @@ class Engine:
         cam = make_camera(camera)
         p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
         pitch = lambda x: C.c_long(x.stride(0) if x is not None and x.shape[0] > 1 else (x.shape[1] if x is not None else NQ))
-        self._rnd_chk(self.lib.uhc_render_qpos(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(q), C.c_int(32 if q.dtype == t.float32 else 64),
-                                               pitch(q), p(g), pitch(g), p(v), p(rgb), p(dep), p(lab), self._stream()), "uhc_render_qpos")
+        _chk(self.lib.uhc_render_qpos(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(q), C.c_int(32 if q.dtype == t.float32 else 64),
+                                      pitch(q), p(g), pitch(g), p(v), p(rgb), p(dep), p(lab), self._stream()), "uhc_render_qpos", ValueError)
         return rgb, dep, lab
 
     def render_bodies(self, pose, humanoids=2, variants=None, camera=None, size=(640, 360), depth=False, label=False):
@@ -537,16 +524,11 @@ class Engine:
         W, H, rgb, dep, lab = self._render_out(n, size, depth, label)
         cam = make_camera(camera)
         p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
-        self._rnd_chk(self.lib.uhc_render_bodies(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(pose), C.c_int(int(humanoids)), p(v),
-                                                 p(rgb), p(dep), p(lab), self._stream()), "uhc_render_bodies")
+        _chk(self.lib.uhc_render_bodies(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(pose), C.c_int(int(humanoids)), p(v),
+                                        p(rgb), p(dep), p(lab), self._stream()), "uhc_render_bodies", ValueError)
         return rgb, dep, lab
 
     # ---- the batched physics tracker (include/uhc_track.h uhc_track_*)
-    def _trk_chk(self, rc, who):
-        if rc != 0:
-            self.lib.uhc_track_last_error.restype = C.c_char_p
-            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_track_last_error().decode())
-
     def track_begin(self, window=8, kind="qpos", pose_dim=None, fk_models=None, shapes=None):
         """tracking mode: env e follows a stream of raw target frames (kind "qpos": qpos rows of 76; "smpl": pose_aa (pose_dim 72 | 156) then
         trans) held in a window of `window` expert-table rows.  fk_models: shape variant per env (FK and simulated body), shapes: [E][17]."""
@@ -554,8 +536,8 @@ class Engine:
         pose_dim = (NQ if k == 1 else 72) if pose_dim is None else int(pose_dim)
         fk = None if fk_models is None else np.ascontiguousarray(fk_models, np.int32).reshape(self.E)
         shp = None if shapes is None else np.ascontiguousarray(np.asarray(shapes, np.float64).reshape(self.E, 17))
-        self._trk_chk(self.lib.uhc_track_begin(self.h, C.c_int(int(window)), C.c_int(k), C.c_int(pose_dim), None if fk is None else _ip_out(fk),
-                                               None if shp is None else shp.ctypes.data_as(C.POINTER(C.c_double))), "uhc_track_begin")
+        _chk(self.lib.uhc_track_begin(self.h, C.c_int(int(window)), C.c_int(k), C.c_int(pose_dim), None if fk is None else _ip_out(fk),
+                                      None if shp is None else shp.ctypes.data_as(C.POINTER(C.c_double))), "uhc_track_begin", ValueError)
         self.track_row_w = NQ if k == 1 else pose_dim + 3
         self._table_loaded(np.full(self.E, int(window), np.int32), fk)
 
@@ -566,9 +548,9 @@ class Engine:
         assert frames.is_cuda and frames.dtype == t.float64 and frames.is_contiguous() and tuple(frames.shape) == (len(ids), 2, self.track_row_w)
         for x, w in ((qpos, NQ), (qvel, NV)):
             assert x is None or (x.is_cuda and x.dtype == t.float32 and x.is_contiguous() and tuple(x.shape) == (len(ids), w))
-        self._trk_chk(self.lib.uhc_track_reset(self.h, C.c_int(len(ids)), _ip_out(ids), C.c_void_p(frames.data_ptr()),
-                                               C.c_void_p(qpos.data_ptr() if qpos is not None else None), C.c_void_p(qvel.data_ptr() if qvel is not None else None),
-                                               self._stream()), "uhc_track_reset")
+        _chk(self.lib.uhc_track_reset(self.h, C.c_int(len(ids)), _ip_out(ids), C.c_void_p(frames.data_ptr()),
+                                      C.c_void_p(qpos.data_ptr() if qpos is not None else None), C.c_void_p(qvel.data_ptr() if qvel is not None else None),
+                                      self._stream()), "uhc_track_reset", ValueError)
 
     def track_step(self, next_frames, mask, policy, log_std, zfilter_stats, zclip, fail_safe, state_out, reward_out, fail_out):
         """one tracker step of every env (uhc_track_step): next_frames float64 [E][row width] or None, mask int32 [E] or None; the outputs
@@ -581,27 +563,27 @@ class Engine:
         from .nn import UhcMcp
         fn = self.lib.uhc_track_step_mcp if isinstance(policy, UhcMcp) else self.lib.uhc_track_step
         p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
-        self._trk_chk(fn(self.h, p(next_frames), p(mask), C.byref(policy), p(log_std), p(zfilter_stats), C.c_float(zclip), C.c_int(int(bool(fail_safe))),
-                         p(state_out), p(reward_out), p(fail_out), self._stream()), "uhc_track_step")
+        _chk(fn(self.h, p(next_frames), p(mask), C.byref(policy), p(log_std), p(zfilter_stats), C.c_float(zclip), C.c_int(int(bool(fail_safe))),
+                p(state_out), p(reward_out), p(fail_out), self._stream()), "uhc_track_step", ValueError)
 
     def track_push(self, next_frames, mask=None):
         """append a frame to every (masked-in) env's stream without stepping (uhc_track_push)"""
         t = self.torch
         assert next_frames.is_cuda and next_frames.dtype == t.float64 and next_frames.is_contiguous() and tuple(next_frames.shape) == (self.E, self.track_row_w)
         assert mask is None or (mask.is_cuda and mask.dtype == t.int32 and mask.is_contiguous() and tuple(mask.shape) == (self.E,))
-        self._trk_chk(self.lib.uhc_track_push(self.h, C.c_void_p(next_frames.data_ptr()), C.c_void_p(mask.data_ptr() if mask is not None else None),
-                                              self._stream()), "uhc_track_push")
+        _chk(self.lib.uhc_track_push(self.h, C.c_void_p(next_frames.data_ptr()), C.c_void_p(mask.data_ptr() if mask is not None else None),
+                                     self._stream()), "uhc_track_push", ValueError)
 
     def track_obs(self, out=None):
         """the observation the next track_step feeds the policy (uhc_track_obs), [E][obs_dim] fp32"""
         out = self.torch.empty(self.E, self.obs_dim, device=self.obs.device) if out is None else out
-        self._trk_chk(self.lib.uhc_track_obs(self.h, C.c_void_p(out.data_ptr()), self._stream()), "uhc_track_obs")
+        _chk(self.lib.uhc_track_obs(self.h, C.c_void_p(out.data_ptr()), self._stream()), "uhc_track_obs", ValueError)
         return out
 
     def track_state(self):
         """per env: steps since its reset, cur_t in the window, rows held, pushes dropped on a full window (synchronises)"""
         out = np.zeros((self.E, 4), np.int32)
-        self._trk_chk(self.lib.uhc_track_state(self.h, _ip_out(out)), "uhc_track_state")
+        _chk(self.lib.uhc_track_state(self.h, _ip_out(out)), "uhc_track_state", ValueError)
         return dict(steps=out[:, 0], cur_t=out[:, 1], rows=out[:, 2], dropped=out[:, 3])
 
     def track_end(self):
@@ -616,15 +598,11 @@ class Engine:
             _chk(self.lib.uhc_set_clip_weights(self.h, C.c_int(len(w)), w.ctypes.data_as(C.POINTER(C.c_float))))
 
     # ---- the failure-weighted curriculum on the device (include/uhc_rollout.h uhc_curriculum_*)
-    def _cur_chk(self, rc, who):
-        if rc != 0:
-            raise (ValueError if rc == -2 else RuntimeError)(f"{who}: " + self.lib.uhc_last_error().decode())
-
     def curriculum_enable(self, max_freq=50, temp=0.2, freq=0.5, prec_freq=0.0, fit_clip=-1):
         """per-clip outcome rings of max_freq entries on the device; from here on the curriculum owns the clip CDF.  Called again with the
         same max_freq it keeps the history; max_freq = 0 turns it off."""
-        self._cur_chk(self.lib.uhc_curriculum_enable(self.h, C.c_int(int(max_freq)), C.c_double(float(temp)), C.c_double(float(freq)),
-                                                     C.c_double(float(prec_freq)), C.c_int(int(fit_clip))), "uhc_curriculum_enable")
+        _chk(self.lib.uhc_curriculum_enable(self.h, C.c_int(int(max_freq)), C.c_double(float(temp)), C.c_double(float(freq)),
+                                            C.c_double(float(prec_freq)), C.c_int(int(fit_clip))), "uhc_curriculum_enable", ValueError)
         self.cur_cfg = dict(max_freq=int(max_freq), temp=float(temp), freq=float(freq), prec_freq=float(prec_freq), fit_clip=int(fit_clip)) if max_freq else None
 
     def curriculum_update(self, buf, T):
@@ -632,21 +610,21 @@ class Engine:
         from .agent import UhcRolloutBuf
         b = UhcRolloutBuf()
         b.ep_clip, b.ep_pct, b.ep_start, b.T_cap = buf.ep_clip.data_ptr(), buf.ep_pct.data_ptr(), buf.ep_start.data_ptr(), buf.T
-        self._cur_chk(self.lib.uhc_curriculum_update(self.h, C.byref(b), C.c_int(int(T)), self._stream()), "uhc_curriculum_update")
+        _chk(self.lib.uhc_curriculum_update(self.h, C.byref(b), C.c_int(int(T)), self._stream()), "uhc_curriculum_update", ValueError)
 
     def curriculum_push(self, clips, pct, starts):
         clips = np.ascontiguousarray(clips, np.int32).reshape(-1)
         p = np.ascontiguousarray(pct, np.float32).reshape(-1)
         s = np.ascontiguousarray(starts, np.int32).reshape(-1)
         assert len(clips) == len(p) == len(s)
-        self._cur_chk(self.lib.uhc_curriculum_push(self.h, C.c_int(len(clips)), _ip(clips), p.ctypes.data_as(C.POINTER(C.c_float)), _ip(s)),
-                      "uhc_curriculum_push")
+        _chk(self.lib.uhc_curriculum_push(self.h, C.c_int(len(clips)), _ip(clips), p.ctypes.data_as(C.POINTER(C.c_float)), _ip(s)),
+             "uhc_curriculum_push", ValueError)
 
     def curriculum_get(self):
         """every clip's history, oldest first: (len [C], percent [C][max_freq], start [C][max_freq])"""
         n, M = len(self.clip_len), self.cur_cfg["max_freq"]
         ln, p, s = np.zeros(n, np.int32), np.zeros((n, M), np.float32), np.zeros((n, M), np.int32)
-        self._cur_chk(self.lib.uhc_curriculum_get(self.h, _ip_out(ln), p.ctypes.data_as(C.POINTER(C.c_float)), _ip_out(s)), "uhc_curriculum_get")
+        _chk(self.lib.uhc_curriculum_get(self.h, _ip_out(ln), p.ctypes.data_as(C.POINTER(C.c_float)), _ip_out(s)), "uhc_curriculum_get", ValueError)
         return ln, p, s
 
     def curriculum_set(self, lens, pct, starts):
@@ -654,7 +632,7 @@ class Engine:
         ln = np.ascontiguousarray(lens, np.int32).reshape(n)
         p = np.ascontiguousarray(pct, np.float32).reshape(n, M)
         s = np.ascontiguousarray(starts, np.int32).reshape(n, M)
-        self._cur_chk(self.lib.uhc_curriculum_set(self.h, _ip(ln), p.ctypes.data_as(C.POINTER(C.c_float)), _ip(s)), "uhc_curriculum_set")
+        _chk(self.lib.uhc_curriculum_set(self.h, _ip(ln), p.ctypes.data_as(C.POINTER(C.c_float)), _ip(s)), "uhc_curriculum_set", ValueError)
 
     def clip_cdf(self):
         """the sampler's cumulative clip weights [C] (fp32)"""
@@ -664,7 +642,7 @@ class Engine:
 
     def curriculum_reseed(self):
         """re-seed every env through the in-kernel sampler; returns the obs tensor with the reset rows"""
-        self._cur_chk(self.lib.uhc_curriculum_reseed(self.h, C.c_void_p(self.obs.data_ptr()), self._stream()), "uhc_curriculum_reseed")
+        _chk(self.lib.uhc_curriculum_reseed(self.h, C.c_void_p(self.obs.data_ptr()), self._stream()), "uhc_curriculum_reseed", ValueError)
         return self.obs
 
     @property

@@ -9,24 +9,13 @@ import math
 
 import numpy as np
 
-from .engine import load_library
+from .engine import _chk as _check, load_library as _lib
 
 ACT = {"none": 0, "gelu": 1, "tanh": 2, "relu": 3, "sigmoid": 4}
 
 
-def _lib():
-    L = load_library()
-    if not getattr(L, "_nn_ready", False):
-        L.uhc_nn_last_error.restype = C.c_char_p
-        L.uhc_tc_last_error.restype = C.c_char_p
-        L._nn_ready = True
-    return L
-
-
 def _chk(rc):
-    if rc != 0:
-        L = _lib()
-        raise RuntimeError("uhc_nn: " + (L.uhc_nn_last_error().decode() or L.uhc_tc_last_error().decode()))
+    _check(rc, "uhc_nn")
 
 
 def _p(t):
@@ -789,7 +778,6 @@ class CPpoTrainer:
 
     def __init__(self, policy, value, opt_p, opt_v, max_rows, max_envs, device):
         L = _lib()
-        L.uhc_ppo_last_error.restype = C.c_char_p
         L.uhc_ppo_advantages.restype = C.c_void_p
         L.uhc_ppo_returns.restype = C.c_void_p
         L.uhc_ppo_kernel_launches.restype = C.c_long
@@ -807,8 +795,7 @@ class CPpoTrainer:
         else:
             self.dp = net_desc(policy, opt_p)
             rc = L.uhc_ppo_trainer_create(C.byref(self.dp), C.byref(self.dv), C.c_long(max_rows), C.c_int(max_envs), C.c_int(dev or 0), C.byref(self.h))
-        if rc != 0:
-            raise RuntimeError("uhc_ppo_trainer_create: " + L.uhc_ppo_last_error().decode())
+        _check(rc, "uhc_ppo_trainer_create")
         self.max_rows, self.max_envs = max_rows, max_envs
 
     def close(self):
@@ -829,8 +816,7 @@ class CPpoTrainer:
         done = C.c_int(1 if getattr(self.opt_p, "_clip_consumed", False) else 0)
         rc = self.L.uhc_ppo_update(self.h, _p(states), _p(last_states), _p(actions), _p(rewards), _p(masks), _p(exps), _p(log_std), C.c_int(T), C.c_int(E),
                                    C.byref(cfg), C.byref(sp), C.byref(sv), C.byref(done), _p(zfilter), _p(z_sync), comm, C.c_int(world), _p(losses), _stream(states))
-        if rc != 0:
-            raise RuntimeError("uhc_ppo_update: " + self.L.uhc_ppo_last_error().decode())
+        _check(rc, "uhc_ppo_update")
         self.opt_p.step_n, self.opt_v.step_n = sp.value, sv.value
         self.opt_p._clip_consumed = done.value > 0
         # the C side refreshed the bf16 weight copies in place after every optimiser step
@@ -844,8 +830,7 @@ class CPpoTrainer:
         done = C.c_int(1 if getattr(self.opt_p, "_clip_consumed", False) else 0)
         rc = self.L.uhc_ppo_update_policy(self.h, _p(states), _p(actions), _p(returns), _p(advantages), _p(exps), _p(log_std), C.c_long(states.shape[0]), C.byref(cfg),
                                           C.byref(sp), C.byref(sv), C.byref(done), comm, C.c_int(world), _p(losses), _stream(states))
-        if rc != 0:
-            raise RuntimeError("uhc_ppo_update_policy: " + self.L.uhc_ppo_last_error().decode())
+        _check(rc, "uhc_ppo_update_policy")
         self.opt_p.step_n, self.opt_v.step_n = sp.value, sv.value
         self.opt_p._clip_consumed = done.value > 0
         self.policy._bf16 = getattr(self.policy, "_bf16_store", True)
@@ -857,8 +842,7 @@ class CPpoTrainer:
 
     def comm_stats(self):
         ms, by, calls = C.c_double(0), C.c_long(0), C.c_int(0)
-        if self.L.uhc_ppo_comm_stats(self.h, C.byref(ms), C.byref(by), C.byref(calls)) != 0:
-            raise RuntimeError("uhc_ppo_comm_stats: " + self.L.uhc_ppo_last_error().decode())
+        _check(self.L.uhc_ppo_comm_stats(self.h, C.byref(ms), C.byref(by), C.byref(calls)), "uhc_ppo_comm_stats")
         return ms.value, by.value, calls.value
 
     def advantages(self, M):
