@@ -42,6 +42,7 @@ typedef struct {
     UhcEvalClip *clips_host;       /* [n] */
     double *states_host_or_null;   /* [n][max(len) - 1][UHC_EVAL_STATE] */
     double *smpl_host_or_null;     /* [n][max(len) - 1][UHC_EVAL_SMPL] */
+    double *floor_host_or_null;    /* [n][max(len) - 1][UHC_FLOOR_NCOL] (include/uhc_floor.h) */
 } UhcEvalOut;
 
 const char *uhc_eval_last_error(void);   /* an alias of uhc_last_error (uhc_b200.h): the library keeps one error text */
@@ -76,7 +77,10 @@ int uhc_eval_run_groups_mcp(UhcEngine *e, int G, const int *group_n_host, const 
  * qpos -- the stepped state before any fail_safe re-seat, the state record's qpos -- is converted on the device by uhc_qpos_to_smpl's code with
  * the shape variant of the env's clip, and row [i][f] of smpl_host equals uhc_qpos_to_smpl of row [i][f] of states_host bit for bit.  Rows past
  * an env's `frames` are unspecified.  With smpl_host_or_null = NULL each is the call above (the same graph and outputs); the graphs with and
- * without the export are cached side by side. */
+ * without the export are cached side by side.
+ * With out->floor_host_or_null set (after uhc_floor_init, include/uhc_floor.h; -2 without it) each recorded frame's hulls are measured against
+ * the floor on the device from the same recorded state: row [i][f] of floor_host equals uhc_floor_qpos of rows f - 1, f of states_host[i]
+ * (row 0 without a previous frame) bit for bit.  NULL costs nothing: the graph, its outputs and its cache entry are those without the field. */
 int uhc_eval_run_ex(UhcEngine *e, int n, const int *clip_host, const UhcMlp *mlp, const float *log_std, const double *zfilter_stats, float zclip,
                     int fail_safe, int window, const UhcEvalOut *out, void *stream);
 int uhc_eval_run_mcp_ex(UhcEngine *e, int n, const int *clip_host, const UhcMcp *mcp, const float *log_std, const double *zfilter_stats, float zclip,
@@ -85,6 +89,7 @@ int uhc_eval_run_groups_ex(UhcEngine *e, int G, const int *group_n_host, const i
                            float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream);
 int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
                                float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream);
+int uhc_eval_graph_count(const UhcEngine *e);   /* graphs this engine's evaluation holds now, grouped ones included (read-only; tests) */
 void uhc_eval_release(UhcEngine *e);   /* frees the graphs / scratch of this engine (the grouped path's too); call before uhc_engine_destroy */
 
 #ifdef __cplusplus

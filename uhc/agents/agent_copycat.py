@@ -86,7 +86,9 @@ class AgentCopycat:
         self.test_data_loaders = [self.data_loader]
         if len(cfg.data_specs.get("test_file_path", [])) > 0:
             self.test_data_loaders.append(DatasetAMASSSingle(cfg.data_specs, data_mode="test", model=self.model_tables))
-        self.freq_dict = {k: [] for k in self.data_loader.data_keys}
+        self.logger = logging.getLogger(f"uhc_b200.{cfg.id}")
+        if not self.logger.handlers:
+            logging.basicConfig(level=logging.INFO, format="%(message)s")
         rw = cfg.reward_weights or {}
         w = [rw.get(k, d) for k, d in (("w_p", 0.6), ("w_v", 0.1), ("w_e", 0.2), ("w_c", 0.1), ("w_vf", 0.0))]
         kk = [rw.get(k, d) for k, d in (("k_p", 2), ("k_v", 0.005), ("k_e", 20), ("k_c", 1000), ("k_vf", 1))]
@@ -100,8 +102,13 @@ class AgentCopycat:
                 dist.init_process_group("nccl")
             sync = make_nccl_grad_sync(world)
         rfc_mode = supported_variant(cfg)       # refuses (AssertionError) what the batched engine does not implement instead of accepting it silently (ADVICE r1)
+        def fixed_motions(engine):
+            """data_specs.fix_height / drop_implausible (DatasetAMASSSingle.fix_floor): the raw motion is measured on the GPU, so it runs between
+            the engine's creation and the first table load; the clip table, the clip sampler and the history keys are all built from what is left"""
+            self.data_loader.fix_floor(engine, self.logger.info)
+            return self.data_loader.motions, self.data_loader.shapes
         self.agent = BatchedAgent(
-            self.num_envs, self.data_loader.motions if self._device_tables(self.data_loader) else self.data_loader.experts, self.data_loader.shapes, device=dev_index, seed=cfg.seed, policy_hsize=cfg.policy_hsize,
+            self.num_envs, fixed_motions if self._device_tables(self.data_loader) else self.data_loader.experts, self.data_loader.shapes, device=dev_index, seed=cfg.seed, policy_hsize=cfg.policy_hsize,
             value_hsize=cfg.value_hsize, htype=cfg.policy_htype, log_std=cfg.log_std, policy_lr=cfg.policy_lr, value_lr=cfg.value_lr,
             gamma=cfg.gamma, tau=cfg.tau, clip_epsilon=cfg.clip_epsilon, num_optim_epoch=cfg.num_optim_epoch, grad_clip=40.0,
             t_min=cfg.data_specs.get("t_min", 90), t_max=cfg.data_specs.get("t_max", -1), rank=rank, world=world, grad_sync=sync,
@@ -116,9 +123,9 @@ class AgentCopycat:
         self.state_dim, self.action_dim = self.agent.obs_dim, self.agent.act_dim
         self.expert_reward = reward_func[cfg.reward_id]
         self.env = None   # single-env facade, built lazily (eval_seq / visualisation code paths)
-        self.logger = logging.getLogger(f"uhc_b200.{cfg.id}")
-        if not self.logger.handlers:
-            logging.basicConfig(level=logging.INFO, format="%(message)s")
+        self.freq_dict = {k: [] for k in self.data_loader.data_keys}
+        for loader in self.test_data_loaders:                   # a separate test set: fixed here, before any evaluation reads its length
+            loader.fix_floor(self.agent.engine, self.logger.info)
         # the failure-weighted curriculum (freq_dict): on the host (default) or, with curriculum_on_device, in device rings updated after
         # every rollout (Engine.curriculum_*).  precision_mode and fit_single_key need the device curriculum and turn it on
         self._precision_mode = bool(cfg.get("precision_mode", False))
@@ -273,6 +280,7 @@ class AgentCopycat:
         cfg = self.cfg
         on_device = bool(cfg.get("eval_on_device", False))     # opt-in: BatchedAgent.evaluate (uhc_eval_run) instead of the host loop below
         motion = dump and bool(cfg.get("eval_dump_motion", False))   # opt-in: the dump also holds eval_seq's trajectories + SMPL per clip
+        floor = bool(cfg.get("eval_floor_metrics", False))           # opt-in: pentration / skate / float of the body hulls per clip (_add_floor)
         res_dicts = []
         eng = self.agent.engine
         E = self.num_envs
@@ -290,11 +298,14 @@ class AgentCopycat:
                 clips = (c0 + ids).astype(np.int32)
                 lens = eng.clip_len[clips]
                 if on_device:                                      # the same roll-out as the loop below, as CUDA-graph replays with the metrics on the device
-                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, **(dict(record_states=True, export_smpl=True) if motion else {}))
+                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, floor=floor, **(dict(record_states=True, export_smpl=True) if motion else {}))
                     last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
                     rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
                     self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec,
                                        lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs), pending)
+                    if floor:
+                        for i in ids:
+                            self._add_floor(res[loader.data_keys[c0 + i]], loader, int(clips[i]), dev[i]["floor"], np.arange(1, len(dev[i]["frames"]) + 1))
                     if motion:
                         for i in ids:
                             d = dev[i]
@@ -347,6 +358,12 @@ class AgentCopycat:
                     return compute_metrics({"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
                                             "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": pct, "fail_safe": fs})
                 self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics, pending)
+                if floor:                           # the host loop's recorded qpos through the device measurement
+                    for i in ids:
+                        if traj[i]["t"]:
+                            var = None if eng.clip_models is None else int(eng.clip_models[clips[i]])
+                            rows = eng.floor_qpos(np.array(traj[i]["pred"]).reshape(-1, 76), variants=var).cpu().numpy()
+                            self._add_floor(res[loader.data_keys[c0 + i]], loader, int(clips[i]), rows, np.array(traj[i]["t"], np.int64))
                 if motion:                          # the host loop's recorded qpos as SMPL through the device conversion
                     for i in ids:
                         pred = np.array(traj[i]["pred"]).reshape(-1, 76)
@@ -371,6 +388,8 @@ class AgentCopycat:
         """the coverage line and metric dict of one loader's results (and with dump its {epoch}_{loader}_coverage_full.pkl)"""
         n = loader.get_len()
         names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
+        if bool(self.cfg.get("eval_floor_metrics", False)):
+            names += ("pentration", "skate", "float", "pentration_gt", "skate_gt", "float_gt")
         metrics = {m: float(np.mean([np.mean(r[m]) for r in res.values() if m in r])) if any(m in r for r in res.values()) else float("nan") for m in names}
         coverage = int(round(metrics["succ"] * n))
         self.logger.info(f"Coverage {loader.name} of {coverage} out of {n} | " + " \t".join(f"{k}: {v:.3f}" for k, v in metrics.items()))
@@ -538,6 +557,20 @@ class AgentCopycat:
         eng.set_cfg(**self._env_cfg(test=False))
         self.agent.obs = None
         return out
+
+    def _add_floor(self, m, loader, clip, rows, t):
+        """eval_floor_metrics: pentration / skate / float (smpl_eval.compute_metrics' keys, from the body hulls instead of the SMPL mesh:
+        uhc_b200/metrics.py floor_summary) of a clip's simulated frames (rows = their [n][5] floor rows) and, as *_gt, of the expert frames
+        min(t, len - 1) they are paired with, measured by the same kernel"""
+        from uhc_b200.metrics import floor_summary
+        if not len(rows):
+            return
+        eng = self.agent.engine
+        gt = eng.clip_frames(clip) if self._device_tables(loader) else loader.experts[clip]
+        var = None if eng.clip_models is None else int(eng.clip_models[clip])
+        g = eng.floor_qpos(np.asarray(gt["qpos"])[np.minimum(t, int(eng.clip_len[clip]) - 1)], variants=var).cpu().numpy()
+        m.update(floor_summary(rows))
+        m.update({k + "_gt": v for k, v in floor_summary(g).items()})
 
     def _clip_result(self, L, last_t, fail_any, rsum, nrec, metrics_of):
         """res[key] of one evaluated clip of L frames, from either roll-out: the percent / succ rules of eval_seq and the reward average.

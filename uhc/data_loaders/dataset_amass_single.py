@@ -53,6 +53,48 @@ class DatasetAMASSSingle:
         else:
             self.experts = [motion_lib.make_expert(self.data["pose_aa"][k], self.data["trans"][k], model) for k in self.data_keys]
         self.shapes = [np.concatenate([self.data["beta"][k][0], [self.data["gender"][k][0]]]) for k in self.data_keys]
+        # opt-in height fix of raw motion against the floor (uhc_b200/motion_lib.py MotionSet.floor_audit / fix_height, on the GPU): it
+        # needs the raw rows and an engine, so it runs in fix_floor once the engine exists
+        self.fix_height = data_specs.get("fix_height", "off") or "off"
+        self.drop_implausible = bool(data_specs.get("drop_implausible", False))
+        assert self.fix_height in ("first_frame", "clip_min", "off"), "data_specs.fix_height: first_frame | clip_min | off"
+        if (self.fix_height != "off" or self.drop_implausible) and self.expert_tables != "device":
+            raise ValueError("data_specs.fix_height / data_specs.drop_implausible measure the raw motion on the GPU: they need "
+                             "data_specs.expert_tables: device")
+        self.floor_fixed = self.fix_height == "off" and not self.drop_implausible
+
+    def fix_floor(self, engine, log=print):
+        """data_specs.fix_height / drop_implausible, once: audits self.motions on the device, drops the clips the reference's rules drop
+        (printed as process_amass_db.py prints them) and lowers the rest.  Returns True when the motion changed."""
+        if self.floor_fixed:
+            return False
+        self.floor_fixed = True
+        audit = self.motions.floor_audit(engine)
+        drop = audit["implausible"] if self.drop_implausible else np.zeros(len(self.data_keys), bool)
+        for c in np.flatnonzero(drop):
+            k = self.data_keys[c]
+            if audit["start_high"][c]:
+                log(f"Starting too high: {k}")
+            elif audit["airborne_run"][c] > self.motions.AIRBORNE_RUN:
+                log(f"{k} too high sequence invalid for copycat: {audit['airborne_run'][c]}")
+            else:
+                log(f"{k} negative sequence invalid for copycat: {audit['deepest_toe'][c]}")
+        for c in np.flatnonzero(audit["crawling"] & ~drop):
+            log(f"Crawling: {self.data_keys[c]}")
+        fixed = self.motions.fix_height(audit, self.fix_height)
+        self.motions = fixed.drop(drop) if drop.any() else fixed
+        gone = {k for k, d in zip(self.data_keys, drop) if d}
+        self.data_keys = [k for k in self.data_keys if k not in gone]
+        self.sample_keys = [s for s in self.sample_keys if s[0] not in gone]
+        self.shapes = [s for s, d in zip(self.shapes, drop) if not d]
+        adr = np.concatenate([[0], np.cumsum(self.motions.lens)])
+        for c, k in enumerate(self.data_keys):          # the fixed translation, for get_sample_from_key
+            self.data["trans"][k] = self.motions.rows[adr[c]:adr[c + 1], self.motions.pose_dim:self.motions.pose_dim + 3].copy()
+        for k in gone:
+            for d in self.data.values():
+                d.pop(k)
+        self.seq_len = len(self.data_keys)
+        return True
 
     def get_len(self):
         return self.seq_len

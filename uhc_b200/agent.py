@@ -133,6 +133,8 @@ class BatchedAgent:
         self.auto_reset = bool(env_cfg.pop("auto_reset", True))
         self.engine = Engine(num_envs, model=model, device=device, precision=precision, variants=variants, auto_reset=int(self.auto_reset), t_min=t_min, t_max=t_max,
                              reset_seed=seed * 7919 + rank * 104729 + 1, **env_cfg)
+        if callable(clips):                                  # clips(engine) -> (MotionSet, shapes): raw motion that needs the engine before it is
+            clips, shapes = clips(self.engine)               # loaded (a height fix measured on the GPU); the sampler below sees what it returns
         if isinstance(clips, MotionSet):                     # raw motion: the expert tables are built on the GPU
             self.engine.load_motions(clips, shapes, clip_models)
         else:
@@ -404,21 +406,23 @@ class BatchedAgent:
     def curriculum_set(self, lens, pct, starts):
         self.engine.curriculum_set(lens, pct, starts)
 
-    def evaluate(self, clips, fail_safe, window=32, record_states=False, export_smpl=False):
+    def evaluate(self, clips, fail_safe, window=32, record_states=False, export_smpl=False, floor=False):
         """deterministic roll-out of every listed clip from frame 0 on the device (Engine.eval_run, one call per chunk of E clips) under
         the engine's current cfg.  Returns one dict per clip: frames = [nframes][6] per-frame rows (uhc_b200/metrics.py
         metrics_from_frames), last_t, fail_any, reward_sum (and states = [nframes][148] when record_states; pose_aa = [nframes][72] and
-        trans = [nframes][3], the simulated motion as SMPL, when export_smpl)."""
+        trans = [nframes][3], the simulated motion as SMPL, when export_smpl; floor = [nframes][5], the body hulls against the floor per frame
+        (include/uhc_floor.h; metrics.floor_summary), when floor)."""
         clips = np.asarray(clips, dtype=np.int32).reshape(-1)
         out = []
         for c0 in range(0, len(clips), self.E):
-            out += self._evaluate_call(clips[c0:c0 + self.E], fail_safe, window, record_states, export_smpl)
+            out += self._evaluate_call(clips[c0:c0 + self.E], fail_safe, window, record_states, export_smpl, floor)
         self.obs = None       # every env was reset onto an evaluation clip
         return out
 
-    def _evaluate_call(self, clips, fail_safe, window, record_states, export_smpl):
+    def _evaluate_call(self, clips, fail_safe, window, record_states, export_smpl, floor=False):
         pol = nn.mcp_struct(self.policy) if self.actor_type == "mcp" else nn.mlp_struct(self.policy)
-        r = self.engine.eval_run(clips, pol, self.log_std, self.running_state.stats, self.running_state.clip, fail_safe, window, record_states, export_smpl)
+        r = self.engine.eval_run(clips, pol, self.log_std, self.running_state.stats, self.running_state.clip, fail_safe, window, record_states, export_smpl,
+                                 floor)
         out = []
         for i, nf in enumerate(r["nframes"]):
             d = dict(frames=r["frames"][i, :nf].copy(), last_t=int(r["last_t"][i]), fail_any=bool(r["fail_any"][i]), reward_sum=float(r["reward_sum"][i]))
@@ -426,13 +430,15 @@ class BatchedAgent:
                 d["states"] = r["states"][i, :nf].copy()
             if export_smpl:
                 d["pose_aa"], d["trans"] = r["pose_aa"][i, :nf].copy(), r["trans"][i, :nf].copy()
+            if floor:
+                d["floor"] = r["floor"][i, :nf].copy()
             out.append(d)
         return out
 
-    def export_motion(self, clips, fail_safe, window=32, max_bytes=1 << 30):
+    def export_motion(self, clips, fail_safe, window=32, max_bytes=1 << 30, floor=False):
         """the simulated motion of every listed clip, as evaluate() rolls it out: per clip pred = [nframes][76] qpos, pred_jpos = [nframes][72]
         world body positions, pose_aa = [nframes][72] and trans = [nframes][3] (the qpos as SMPL, uhc_qpos_to_smpl on the device) and evaluate()'s
-        summary (frames, last_t, fail_any, reward_sum), in the caller's order.  Clips of similar length share a device call; a call takes at most
+        summary (frames, last_t, fail_any, reward_sum; floor = [nframes][5] with floor=True), in the caller's order.  Clips of similar length share a device call; a call takes at most
         E clips and as many as keep its pinned state and SMPL arrays, n * (max(len) - 1) * (148 + 75) * 8 bytes, within max_bytes (a clip that
         alone needs more runs on its own).  Every env is independent of the others, so a clip's result does not depend on the chunking.  Needs
         the engine's test-mode cfg (auto_reset off, as eval_policy sets it): with auto_reset an ended env would re-seed itself from the sampler,
@@ -449,7 +455,7 @@ class BatchedAgent:
             while k + m < len(clips) and m < self.E and (m + 1) * (int(self.engine.clip_len[clips[order[k + m]]]) - 1) * per_frame <= max_bytes:
                 m += 1
             idx = order[k:k + m]
-            for i, d in zip(idx, self._evaluate_call(clips[idx], fail_safe, window, True, True)):
+            for i, d in zip(idx, self._evaluate_call(clips[idx], fail_safe, window, True, True, floor)):
                 st = d.pop("states")
                 d["pred"], d["pred_jpos"] = st[:, :76], st[:, 76:]
                 out[i] = d
@@ -518,7 +524,7 @@ class BatchedAgent:
             zf.stats.copy_(self.running_state.stats)
         return net, zf
 
-    def evaluate_policies(self, checkpoints, clips, fail_safe, window=32, record_states=False):
+    def evaluate_policies(self, checkpoints, clips, fail_safe, window=32, record_states=False, floor=False):
         """evaluate() of every listed clip for each checkpoint ({"policy_dict", "running_state"}, what state_dicts writes), with the checkpoints
         side by side in each device call (Engine.eval_run_groups, packed by pack_groups).  Returns one list per checkpoint, each equal to
         what load_state_dicts(cp) + evaluate(clips, ...) returns.  The agent's own weights, log_std and running_state are not touched."""
@@ -532,12 +538,14 @@ class BatchedAgent:
         structs = [(nn.mcp_struct(net) if mcp else nn.mlp_struct(net), zf) for net, zf in pols]
         for call in pack_groups(K, n, self.E):
             groups = [(clips[c0:c1], structs[k][0], structs[k][1].stats) for k, c0, c1 in call]
-            res = self.engine.eval_run_groups(groups, self.running_state.clip, fail_safe, window, record_states)
+            res = self.engine.eval_run_groups(groups, self.running_state.clip, fail_safe, window, record_states, floor=floor)
             for (k, _, _), r in zip(call, res):
                 for i, nf in enumerate(r["nframes"]):
                     d = dict(frames=r["frames"][i, :nf].copy(), last_t=int(r["last_t"][i]), fail_any=bool(r["fail_any"][i]), reward_sum=float(r["reward_sum"][i]))
                     if record_states:
                         d["states"] = r["states"][i, :nf].copy()
+                    if floor:
+                        d["floor"] = r["floor"][i, :nf].copy()
                     out[k].append(d)
         self.obs = None       # every env was reset onto an evaluation clip
         return out

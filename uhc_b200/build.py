@@ -7,10 +7,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "libuhc_b200.so")
 SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_wgmma.cu", "rollout.cu", "ppo_update.cu"]
 # compiled on their own without multiply-add contraction: the motion library, the evaluation metrics, the curriculum weights and the tracker's
-# streamed rows and the SMPL export restate numpy / scipy's fp64 arithmetic operation for operation; the renderer's pixel path must give the bits
-# of its host emulation
-NO_FMA_SRCS = ["motion_lib.cu", "eval.cu", "curriculum.cu", "track.cu", "export.cu", "render.cu"]
-DEPS = ["errors.h", "sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "graph_cache.h", "group_core.h", "curriculum_core.h", "track_core.h", "track_obs.h", "track_glue.h", "smpl_export_core.h", "render_core.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h", "../../include/uhc_track.h", "../../include/uhc_export.h", "../../include/uhc_render.h"]
+# streamed rows and the SMPL export restate numpy / scipy's fp64 arithmetic operation for operation; the renderer's pixel path and the floor
+# measurements must give the bits of their host emulations
+NO_FMA_SRCS = ["motion_lib.cu", "eval.cu", "curriculum.cu", "track.cu", "export.cu", "render.cu", "floor.cu"]
+DEPS = ["errors.h", "sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "graph_cache.h", "group_core.h", "curriculum_core.h", "track_core.h", "track_obs.h", "track_glue.h", "smpl_export_core.h", "render_core.h", "floor_core.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h", "../../include/uhc_track.h", "../../include/uhc_export.h", "../../include/uhc_render.h", "../../include/uhc_floor.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 

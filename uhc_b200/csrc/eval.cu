@@ -8,6 +8,7 @@
 //   k_eval_frame                                                                 per env still alive: the frame's metrics into a window buffer,
 //                                                                                the reward sum, fail / end, the fail_safe flag
 //   k_eval_export (SMPL export only)                                               per env that recorded a frame: its qpos as SMPL (export.cu)
+//   k_eval_floor (floor rows only)                                                 per env that recorded a frame: its hulls against the floor (floor.cu)
 //   k_eval_reseat (fail_safe only)                                               uhc_env_set_state_batch's re-seat of the flagged envs
 // `window` steps are captured once per argument set into a CUDA graph (graph_cache.h); after each replay one 2-D copy moves the window's frame rows
 // into the caller's (pinned) array and one 4-byte copy returns the number of envs still alive, the host loop's early exit.
@@ -23,6 +24,7 @@
 #include "errors.h"
 #include "eval_core.h"
 #include "eval_glue.h"
+#include "floor_core.h"
 #include "graph_cache.h"
 #include "sim_core.h"
 #include "smpl_export_core.h"
@@ -95,11 +97,12 @@ struct EvalPolicies { bool grouped; std::vector<evalx::Policy> pols; std::vector
 struct EvalCtx {
     UhcEngine *eng = nullptr;
     int E = 0, n_cap = 0, win_cap = 0, states_cap = 0;
-    size_t smpl_cap = 0;                          // rows (env x slot) of d_wsmpl
+    size_t smpl_cap = 0, floor_cap = 0;           // rows (env x slot) of d_wsmpl, d_wfloor
     unsigned long long gen = 0;                   // bumped when the scratch below is reallocated
     UhcEvalClip *d_clips = nullptr; int *d_alive = nullptr, *d_reseat = nullptr, *d_count = nullptr; unsigned char *d_ones = nullptr;
     double *d_ring = nullptr, *d_win = nullptr, *d_wstates = nullptr;
     double *d_wsmpl = nullptr; int *d_xdone = nullptr;   // SMPL export: window rows [n][window][UHC_EVAL_SMPL], frames exported per env
+    double *d_wfloor = nullptr, *d_fprev = nullptr; int *d_fdone = nullptr;   // floor rows: window rows [n][window][NCOL], per env the qpos last measured, frames measured
     int *h_count = nullptr;                       // pinned
     cudaEvent_t ev = nullptr;
     std::vector<int> ids, clip0, start, len;      // reset arguments (kept: no allocation in the steady state)
@@ -115,7 +118,7 @@ EvalCtx *ev_ctx(UhcEngine *e) {
 }
 // per-env arrays sized by E once; the window buffers grow with n * window (and the state record and the SMPL export with it when requested).
 // Called before any capture: a graph holds these pointers, so they never change while one of them can be replayed (gen)
-int ensure(EvalCtx *c, int n, int window, bool states, bool smpl) {
+int ensure(EvalCtx *c, int n, int window, bool states, bool smpl, bool floor) {
     const size_t E = c->E;
     if (!c->d_clips) {
         CK(cudaMalloc((void **)&c->d_clips, E * sizeof(UhcEvalClip))); CK(cudaMalloc((void **)&c->d_alive, E * 4)); CK(cudaMalloc((void **)&c->d_reseat, E * 4));
@@ -138,11 +141,19 @@ int ensure(EvalCtx *c, int n, int window, bool states, bool smpl) {
         CK(cudaMalloc((void **)&c->d_wsmpl, (size_t)need * UHC_EVAL_SMPL * sizeof(double))); c->smpl_cap = (size_t)need;
     }
     if (smpl && !c->d_xdone) { CK(cudaMalloc((void **)&c->d_xdone, E * sizeof(int))); c->gen++; }
+    if (floor && (size_t)need > c->floor_cap) {
+        if (c->d_wfloor) cudaFree(c->d_wfloor);
+        c->d_wfloor = nullptr; c->floor_cap = 0; c->gen++;
+        CK(cudaMalloc((void **)&c->d_wfloor, (size_t)need * floorm::NCOL * sizeof(double))); c->floor_cap = (size_t)need;
+    }
+    if (floor && !c->d_fdone) {
+        CK(cudaMalloc((void **)&c->d_fdone, E * sizeof(int))); CK(cudaMalloc((void **)&c->d_fprev, E * motion::MQ * sizeof(double))); c->gen++;
+    }
     return 0;
 }
 
 int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const EvalPolicies &P, float zclip, int n, int nrec_max, int fail_safe, int window, bool states,
-                   bool smpl, cudaStream_t st) {
+                   bool smpl, bool floor, cudaStream_t st) {
     for (int s = 0; s < window; s++) {
         const int rc = P.grouped ? evalx::groups_enqueue(c->eng, P.pols, P.row0.data(), P.zstats, zclip, R.obs, c->d_ones, R.act, st)
                                  : evalx::policy_enqueue(c->eng, P.pols[0], R.obs, P.log_std, (double *)P.zstats[0], zclip, c->d_ones, R.act, st);
@@ -161,6 +172,8 @@ int enqueue_window(EvalCtx *c, const evalx::EngineRefs &R, const EvalPolicies &P
         CK(cudaGetLastError());
         if (smpl) CK(smplx::launch_eval_export(R.precision, R.state, R.istate, trackx::clip_models(c->eng), trackx::motion_model(c->eng).body, c->d_clips,
                                                 c->d_xdone, n, window, s, c->d_wsmpl, st));
+        if (floor) CK(floorm::launch_eval_floor(c->eng, R.precision, R.state, R.istate, trackx::clip_models(c->eng), c->d_clips, c->d_fdone, c->d_fprev, n,
+                                                window, s, c->d_wfloor, st));
         if (fail_safe) CK(evalx::launch_reseat(c->eng, n, c->d_reseat, st));
     }
     return 0;
@@ -184,7 +197,7 @@ int reset_envs(EvalCtx *c, UhcEngine *e, const evalx::EngineRefs &R, int n, cons
 
 // replays until every env has stopped or nrec_max steps have run; after each, the window's rows of envs 0..n-1 go to the caller's arrays
 int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, const UhcEvalOut &o, cudaStream_t st) {
-    double *frames_host = o.frames_host, *states_host = o.states_host_or_null, *smpl_host = o.smpl_host_or_null;
+    double *frames_host = o.frames_host, *states_host = o.states_host_or_null, *smpl_host = o.smpl_host_or_null, *floor_host = o.floor_host_or_null;
     if (smpl_host && (!c->d_wsmpl || c->smpl_cap < (size_t)n * (size_t)window)) { uhc_err() = "SMPL export: the window buffer is smaller than n * window rows"; return -1; }
     for (int s0 = 0; s0 < nrec_max; s0 += window) {
         CK(cudaGraphLaunch(exec, st));
@@ -197,6 +210,9 @@ int replay(EvalCtx *c, cudaGraphExec_t exec, int n, int nrec_max, int window, co
         if (smpl_host)
             CK(cudaMemcpy2DAsync(smpl_host + (size_t)s0 * UHC_EVAL_SMPL, (size_t)nrec_max * UHC_EVAL_SMPL * sizeof(double), c->d_wsmpl,
                                   (size_t)window * UHC_EVAL_SMPL * sizeof(double), (size_t)rows * UHC_EVAL_SMPL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
+        if (floor_host)
+            CK(cudaMemcpy2DAsync(floor_host + (size_t)s0 * floorm::NCOL, (size_t)nrec_max * floorm::NCOL * sizeof(double), c->d_wfloor,
+                                  (size_t)window * floorm::NCOL * sizeof(double), (size_t)rows * floorm::NCOL * sizeof(double), n, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(c->h_count, c->d_count, 4, cudaMemcpyDeviceToHost, st));
         CK(cudaEventRecord(c->ev, st));
         CK(cudaEventSynchronize(c->ev));
@@ -236,20 +252,23 @@ int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *c
     int rc = grouped ? evalx::groups_prepare(e, G, mlps, mcps, &P.pols, &pgen) : evalx::policy_prepare(e, mlps, mcps, &P.pols[0], &pgen);
     if (rc) return rc;
     EvalCtx *c = ev_ctx(e);
-    const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr;
-    if (ensure(c, n, window, states, smpl)) return -1;
+    const bool states = o.states_host_or_null != nullptr, smpl = o.smpl_host_or_null != nullptr, floor = o.floor_host_or_null != nullptr;
+    const unsigned long long fgen = floor ? floorm::floor_gen(e) : 0;
+    if (floor && !fgen) return refuse("floor rows need the hull vertices (uhc_floor_init)");
+    if (ensure(c, n, window, states, smpl, floor)) return -1;
     cudaStream_t st = (cudaStream_t)stream;
     const int nrec_max = max_len - 1;
     if (reset_envs(c, e, R, n, clip_host, st)) return -1;
     if (smpl) CK(cudaMemsetAsync(c->d_xdone, 0, (size_t)n * sizeof(int), st));
+    if (floor) CK(cudaMemsetAsync(c->d_fdone, 0, (size_t)n * sizeof(int), st));
     // no grouped policy covers the parked envs: they step with zero actions (the graph writes action rows 0 .. n-1 only)
     if (grouped && n < R.E) CK(cudaMemsetAsync(R.act + (size_t)n * R.act_dim, 0, (size_t)(R.E - n) * R.act_dim * sizeof(float), st));
 
     // the key: every argument the graph's kernels got.  The generations: the graph also holds the policy scratch, the window buffers and
     // the engine view (cfg, clip table) of its capture, and is dropped once any of them has changed
-    struct { int n, nrec_max, window, fail_safe, states, smpl; float zclip; const float *log_std; } head;
+    struct { int n, nrec_max, window, fail_safe, states, smpl; float zclip; unsigned long long floor; const float *log_std; } head;
     memset(&head, 0, sizeof head);
-    head.n = n; head.nrec_max = nrec_max; head.window = window; head.fail_safe = fail_safe ? 1 : 0; head.states = states; head.smpl = smpl; head.zclip = zclip;
+    head.n = n; head.nrec_max = nrec_max; head.window = window; head.fail_safe = fail_safe ? 1 : 0; head.states = states; head.smpl = smpl; head.floor = fgen; head.zclip = zclip;
     head.log_std = log_std;
     std::string key;
     GraphCache::append(&key, &head); GraphCache::append(&key, group_n, G); GraphCache::append(&key, zstats, G); GraphCache::append(&key, P.pols.data(), G);
@@ -258,7 +277,7 @@ int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *c
     cache.drop_stale(gens);
     cudaGraphExec_t exec = cache.find(key);
     if (!exec) {
-        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_window(c, R, P, zclip, n, nrec_max, head.fail_safe, window, states, smpl, cs); }, &exec);
+        rc = GraphCache::capture([&](cudaStream_t cs) { return enqueue_window(c, R, P, zclip, n, nrec_max, head.fail_safe, window, states, smpl, floor, cs); }, &exec);
         if (rc) return rc;
         cache.insert(std::move(key), gens, exec);
     }
@@ -270,7 +289,7 @@ int eval_run(UhcEngine *e, bool grouped, int G, const int *group_n, const int *c
 extern "C" {
 
 static UhcEvalOut eval_out(double *frames_host, UhcEvalClip *clips_host, double *states_host_or_null) {
-    UhcEvalOut o; o.frames_host = frames_host; o.clips_host = clips_host; o.states_host_or_null = states_host_or_null; o.smpl_host_or_null = nullptr;
+    UhcEvalOut o; o.frames_host = frames_host; o.clips_host = clips_host; o.states_host_or_null = states_host_or_null; o.smpl_host_or_null = nullptr; o.floor_host_or_null = nullptr;
     return o;
 }
 
@@ -321,12 +340,17 @@ int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, con
     return eval_run(e, true, G, group_n_host, clip_host, nullptr, mcps, nullptr, zfilter_stats_host, zclip, fail_safe, window, *out, stream);
 }
 
+int uhc_eval_graph_count(const UhcEngine *e) {
+    for (const EvalCtx *c : g_ev) if (c->eng == e) return (int)(c->graphs.size() + c->ggraphs.size());
+    return 0;
+}
+
 void uhc_eval_release(UhcEngine *e) {
     for (size_t i = 0; i < g_ev.size(); i++) if (g_ev[i]->eng == e) {
         EvalCtx *c = g_ev[i];
         c->graphs.clear(); c->ggraphs.clear();
         for (void *p : {(void *)c->d_clips, (void *)c->d_alive, (void *)c->d_reseat, (void *)c->d_count, (void *)c->d_ones, (void *)c->d_ring,
-                        (void *)c->d_win, (void *)c->d_wstates, (void *)c->d_wsmpl, (void *)c->d_xdone}) if (p) cudaFree(p);
+                        (void *)c->d_win, (void *)c->d_wstates, (void *)c->d_wsmpl, (void *)c->d_xdone, (void *)c->d_wfloor, (void *)c->d_fprev, (void *)c->d_fdone}) if (p) cudaFree(p);
         if (c->h_count) cudaFreeHost(c->h_count);
         if (c->ev) cudaEventDestroy(c->ev);
         delete c; g_ev.erase(g_ev.begin() + i); return;

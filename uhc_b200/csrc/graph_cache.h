@@ -21,6 +21,7 @@ public:
     explicit GraphCache(size_t cap) : cap_(cap) {}
     template <class T> static void append(std::string *key, const T *p, size_t count = 1) { key->append((const char *)p, count * sizeof(T)); }
 
+    size_t size() const { return entries_.size(); }
     void clear() { for (Entry &g : entries_) cudaGraphExecDestroy(g.exec); entries_.clear(); }
     void drop_stale(const Gens &gens) {
         for (size_t i = 0; i < entries_.size();) {

@@ -31,10 +31,18 @@ class UhcEvalClip(C.Structure):
 
 class UhcEvalOut(C.Structure):
     """include/uhc_eval.h UhcEvalOut"""
-    _fields_ = [("frames_host", C.c_void_p), ("clips_host", C.c_void_p), ("states_host_or_null", C.c_void_p), ("smpl_host_or_null", C.c_void_p)]
+    _fields_ = [("frames_host", C.c_void_p), ("clips_host", C.c_void_p), ("states_host_or_null", C.c_void_p), ("smpl_host_or_null", C.c_void_p),
+                ("floor_host_or_null", C.c_void_p)]
+
+
+class UhcFloorHulls(C.Structure):
+    """include/uhc_floor.h UhcFloorHulls"""
+    _fields_ = [("nshape", C.c_int), ("nvert", C.c_int), ("hull", C.POINTER(C.c_double)), ("hull_adr", C.POINTER(C.c_int)), ("hull_num", C.POINTER(C.c_int))]
 
 
 EVAL_SMPL = 75      # include/uhc_eval.h UHC_EVAL_SMPL: pose 72, trans 3
+FLOOR_NCOL = 5      # include/uhc_floor.h UHC_FLOOR_NCOL: min_z (m), pen_mm, skate_mm, float_mm, n_below
+FLOOR_NFEET = 4     # UHC_FLOOR_NFEET: z of L_Ankle, R_Ankle, L_Toe, R_Toe
 
 
 class UhcRenderCamera(C.Structure):
@@ -190,7 +198,7 @@ class Engine:
         self.fail = torch.zeros(self.E, device=dev, dtype=torch.int32)
         self.end = torch.zeros(self.E, device=dev, dtype=torch.int32)
         self.clip_len = self.clip_models = None
-        self._render_ready = False
+        self._render_ready = self._floor_ready = False
         self.cur_cfg = None            # device curriculum parameters while it is enabled (curriculum_enable)
         if int(cfg.get("reactive_v", 0)) == 1:
             self.set_neutral_pose()
@@ -209,6 +217,7 @@ class Engine:
             self.lib.uhc_eval_release(self.h)
             self.lib.uhc_track_end(self.h)
             self.lib.uhc_render_release(self.h)
+            self.lib.uhc_floor_release(self.h)
             self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
             self.h = None
@@ -348,12 +357,13 @@ class Engine:
         v = np.ascontiguousarray(qvel, np.float64).reshape(len(ids), NV)
         _chk(self.lib.uhc_env_set_state_batch(self.h, C.c_int(len(ids)), _ip(ids), q.ctypes.data_as(C.POINTER(C.c_double)), v.ctypes.data_as(C.POINTER(C.c_double))))
 
-    def eval_run(self, clips, policy, log_std, zfilter_stats, zclip=5.0, fail_safe=False, window=32, record_states=False, export_smpl=False):
+    def eval_run(self, clips, policy, log_std, zfilter_stats, zclip=5.0, fail_safe=False, window=32, record_states=False, export_smpl=False, floor=False):
         """device evaluation of up to E clips (uhc_eval_run, include/uhc_eval.h): envs 0..n-1 roll out clips[i] from frame 0 with the mean
         action under the current cfg.  policy: nn.mlp_struct / nn.mcp_struct of the policy; zfilter_stats: the ZFilter's device statistics.
         Returns dict(frames=[n][max(len)-1][6] per-frame rows (rows past `nframes` unspecified), nframes, last_t, fail_any, reward_sum,
         states=[n][max(len)-1][148] recorded qpos + xpos when record_states, else None, and with export_smpl pose_aa=[n][max(len)-1][72] and
-        trans=[n][max(len)-1][3], every recorded qpos as SMPL (uhc_eval_run_ex), else None)."""
+        trans=[n][max(len)-1][3], every recorded qpos as SMPL (uhc_eval_run_ex), else None, and with floor floor=[n][max(len)-1][5], every recorded
+        frame's hulls against the floor (include/uhc_floor.h: min_z, pen_mm, skate_mm, float_mm, n_below), else None)."""
         t = self.torch
         clips = np.ascontiguousarray(clips, dtype=np.int32).reshape(-1)
         n = len(clips)
@@ -362,35 +372,43 @@ class Engine:
         frames = t.empty((max(n, 1), T, 6), dtype=t.float64, pin_memory=True)
         states = t.empty((max(n, 1), T, 148), dtype=t.float64, pin_memory=True) if record_states else None
         smpl = t.empty((max(n, 1), T, EVAL_SMPL), dtype=t.float64, pin_memory=True) if export_smpl else None
+        fl = self._floor_buf(max(n, 1), T) if floor else None
         rec = (UhcEvalClip * max(n, 1))()
-        out = self._eval_out(frames, rec, states, smpl)
+        out = self._eval_out(frames, rec, states, smpl, fl)
         from .nn import UhcMcp
         fn = self.lib.uhc_eval_run_mcp_ex if isinstance(policy, UhcMcp) else self.lib.uhc_eval_run_ex
         rc = fn(self.h, C.c_int(n), _ip(clips), C.byref(policy), C.c_void_p(log_std.data_ptr()), C.c_void_p(zfilter_stats.data_ptr()), C.c_float(zclip),
                 C.c_int(int(bool(fail_safe))), C.c_int(int(window)), C.byref(out), self._stream())
         _chk(rc, "uhc_eval_run", ValueError)
-        return self._eval_result(rec, 0, n, frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None)
+        return self._eval_result(rec, 0, n, frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None,
+                                 fl.numpy() if fl is not None else None)
+
+    def _floor_buf(self, n, T):
+        self._floor_init()
+        return self.torch.empty((n, T, FLOOR_NCOL), dtype=self.torch.float64, pin_memory=True)
 
     @staticmethod
-    def _eval_out(frames, rec, states, smpl):
+    def _eval_out(frames, rec, states, smpl, floor=None):
         o = UhcEvalOut()
         o.frames_host, o.clips_host = frames.data_ptr(), C.addressof(rec)
         o.states_host_or_null = states.data_ptr() if states is not None else None
         o.smpl_host_or_null = smpl.data_ptr() if smpl is not None else None
+        o.floor_host_or_null = floor.data_ptr() if floor is not None else None
         return o
 
     @staticmethod
-    def _eval_result(rec, o, k, fr, st, sm):
+    def _eval_result(rec, o, k, fr, st, sm, fl=None):
         r = rec[o:o + k]
         return dict(frames=fr[o:o + k], nframes=np.array([x.frames for x in r]), last_t=np.array([x.last_t for x in r]),
                     fail_any=np.array([bool(x.fail_any) for x in r]), reward_sum=np.array([x.reward_sum for x in r]),
                     states=st[o:o + k] if st is not None else None,
-                    pose_aa=sm[o:o + k, :, :72] if sm is not None else None, trans=sm[o:o + k, :, 72:] if sm is not None else None)
+                    pose_aa=sm[o:o + k, :, :72] if sm is not None else None, trans=sm[o:o + k, :, 72:] if sm is not None else None,
+                    floor=fl[o:o + k] if fl is not None else None)
 
-    def eval_run_groups(self, groups, zclip=5.0, fail_safe=False, window=32, record_states=False, export_smpl=False):
+    def eval_run_groups(self, groups, zclip=5.0, fail_safe=False, window=32, record_states=False, export_smpl=False, floor=False):
         """several policies of one architecture in one device evaluation (uhc_eval_run_groups): groups = [(clips, policy, zfilter_stats)], group g
         on the envs after those of groups 0 .. g-1.  Returns one eval_run dict per group, bit-identical to eval_run(clips, policy, ...) of that
-        group alone (any finite log_std).  export_smpl: as eval_run's."""
+        group alone (any finite log_std).  export_smpl, floor: as eval_run's."""
         t = self.torch
         from .nn import UhcMcp, UhcMlp
         G = len(groups)
@@ -403,8 +421,9 @@ class Engine:
         frames = t.empty((max(n, 1), T, 6), dtype=t.float64, pin_memory=True)
         states = t.empty((max(n, 1), T, 148), dtype=t.float64, pin_memory=True) if record_states else None
         smpl = t.empty((max(n, 1), T, EVAL_SMPL), dtype=t.float64, pin_memory=True) if export_smpl else None
+        fl = self._floor_buf(max(n, 1), T) if floor else None
         rec = (UhcEvalClip * max(n, 1))()
-        out = self._eval_out(frames, rec, states, smpl)
+        out = self._eval_out(frames, rec, states, smpl, fl)
         mcp = G > 0 and isinstance(groups[0][1], UhcMcp)
         pols = ((UhcMcp if mcp else UhcMlp) * max(G, 1))(*[p for _, p, _ in groups])
         zs = (C.c_void_p * max(G, 1))(*[z.data_ptr() for _, _, z in groups])
@@ -413,9 +432,10 @@ class Engine:
                 C.byref(out), self._stream())
         _chk(rc, "uhc_eval_run_groups", ValueError)
         fr, st, sm = frames.numpy(), states.numpy() if states is not None else None, smpl.numpy() if smpl is not None else None
+        fl = fl.numpy() if fl is not None else None
         res, o = [], 0
         for k in sizes:
-            res.append(self._eval_result(rec, o, int(k), fr, st, sm))
+            res.append(self._eval_result(rec, o, int(k), fr, st, sm, fl))
             o += int(k)
         return res
 
@@ -450,6 +470,69 @@ class Engine:
                                      self._stream()), "uhc_track_smpl", ValueError)
         return pose, trans
 
+    # ---- the floor measurements (include/uhc_floor.h)
+    def _floor_init(self):
+        if not self._floor_ready:
+            models = self.variants or [self.model]
+            m = self.model
+            keep = self._fkeep = dict(hull=np.ascontiguousarray(np.stack([v.hull for v in models]), np.float64),
+                                      adr=np.ascontiguousarray(m.hull_adr, np.int32), num=np.ascontiguousarray(m.hull_num, np.int32))
+            h = UhcFloorHulls()
+            h.nshape, h.nvert = len(models), len(m.hull)
+            h.hull = keep["hull"].ctypes.data_as(C.POINTER(C.c_double))
+            h.hull_adr, h.hull_num = _ip_out(keep["adr"]), _ip_out(keep["num"])
+            _chk(self.lib.uhc_floor_init(self.h, C.byref(h)), "uhc_floor_init", ValueError)
+            self._floor_ready = True
+
+    def floor_qpos(self, qpos, variants=None, first=None):
+        """the body hulls against the floor z = 0 on the device (uhc_floor_qpos): qpos = a cuda tensor [n][>= 76] of float32 | float64 whose rows
+        are contiguous (its first 76 columns are read, in place: a state record of 148 or the tracker's state_out of 223 as they are) or anything
+        numpy takes (copied as float64); variants = shape variant per row (None: 0); first = per row, 1 where the row has no previous frame
+        (None: the rows are one clip).  Returns [n][5] float64 on the device: min_z (m), pen_mm, skate_mm, float_mm, n_below."""
+        t = self.torch
+        self._floor_init()
+        q = self._rows(qpos, who="floor_qpos")
+        n = q.shape[0]
+        v = self._variant_arg(variants, n)
+        f = self._variant_arg(first, n)
+        out = t.empty(n, FLOOR_NCOL, dtype=t.float64, device=self.obs.device)
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        _chk(self.lib.uhc_floor_qpos(self.h, p(q), C.c_int(32 if q.dtype == t.float32 else 64), C.c_long(n), C.c_long(q.stride(0) if n > 1 else q.shape[1]),
+                                     p(v), p(f), p(out), self._stream()), "uhc_floor_qpos", ValueError)
+        return out
+
+    def track_floor(self, state_out, out=None):
+        """the tracker's state_out [E][223] against the floor (uhc_track_floor), env e with the shape variant of uhc_track_begin's fk_models and no
+        previous frame; stream-ordered, no synchronise.  Returns [E][5] float64 on the device (written into out when given)."""
+        t = self.torch
+        self._floor_init()
+        out = t.empty(self.E, FLOOR_NCOL, dtype=t.float64, device=self.obs.device) if out is None else out
+        assert state_out.is_cuda and state_out.is_contiguous() and tuple(state_out.shape) == (self.E, 223)
+        assert state_out.dtype == (t.float32 if self.precision == 32 else t.float64)
+        _chk(self.lib.uhc_track_floor(self.h, C.c_void_p(state_out.data_ptr()), C.c_void_p(out.data_ptr()), self._stream()), "uhc_track_floor", ValueError)
+        return out
+
+    def motion_floor(self, motions, fk_models=None, chunk_frames=0):
+        """uhc_floor_qpos' reduction over the raw rows of a motion_lib.MotionSet (uhc_motion_floor), before any table is built: returns
+        (rows [frames][5], feet [frames][4] = z of L_Ankle, R_Ankle, L_Toe, R_Toe), float64 cuda tensors; fk_models: shape variant per clip."""
+        t = self.torch
+        self._floor_init()
+        n = len(motions)
+        lens = np.ascontiguousarray(motions.lens, np.int32)
+        rows = np.ascontiguousarray(motions.rows, np.float64)
+        fk = None if fk_models is None else np.ascontiguousarray(fk_models, np.int32).reshape(n)
+        out = t.empty(int(lens.sum()), FLOOR_NCOL, dtype=t.float64, device=self.obs.device)
+        feet = t.empty(int(lens.sum()), FLOOR_NFEET, dtype=t.float64, device=self.obs.device)
+        _chk(self.lib.uhc_motion_floor(self.h, C.c_int(n), _ip(lens), C.c_int(motions.kind), C.c_int(motions.pose_dim),
+                                       rows.ctypes.data_as(C.POINTER(C.c_double)), None if fk is None else _ip(fk), C.c_int(int(chunk_frames)),
+                                       C.c_void_p(out.data_ptr()), C.c_void_p(feet.data_ptr())), "uhc_motion_floor", ValueError)
+        return out, feet
+
+    @property
+    def eval_graph_count(self):
+        """CUDA graphs the evaluation holds for this engine now (uhc_eval_graph_count)"""
+        return int(self.lib.uhc_eval_graph_count(self.h))
+
     # ---- the renderer (include/uhc_render.h)
     def _render_init(self):
         if not self._render_ready:
@@ -457,17 +540,20 @@ class Engine:
             _chk(self.lib.uhc_render_init(self.h, C.byref(self._rhulls)), "uhc_render_init", ValueError)
             self._render_ready = True
 
-    def _rows(self, q, n=None):
+    def _rows(self, q, n=None, who="render"):
         """a cuda tensor [n][>= 76] of float32 | float64 with contiguous rows (read in place), or anything numpy takes (copied as float64)"""
         t = self.torch
         q = q if t.is_tensor(q) and q.is_cuda else t.as_tensor(np.ascontiguousarray(q, np.float64), device=self.obs.device)
         if q.dim() != 2 or q.dtype not in (t.float32, t.float64) or q.shape[1] < NQ or q.stride(1) != 1 or (n is not None and q.shape[0] != n):
-            raise ValueError("render: qpos rows must be [n][>= 76] contiguous rows of float32 | float64 (the ghost as many as qpos)")
+            raise ValueError(who + ": qpos rows must be [n][>= 76] contiguous rows of float32 | float64 (the ghost as many as qpos)")
         return q
 
     def _variant_arg(self, variants, n):
         if variants is None:
             return None
+        t = self.torch
+        if t.is_tensor(variants) and variants.is_cuda and variants.dtype == t.int32 and variants.is_contiguous() and tuple(variants.shape) == (n,):
+            return variants                        # already on the device: used in place
         return self.torch.as_tensor(np.array(np.broadcast_to(np.asarray(variants, np.int32), (n,))), device=self.obs.device)
 
     def render_pose(self, qpos, ghost=None, variants=None):

@@ -66,6 +66,16 @@ def compute_metrics(res):
     return out
 
 
+def floor_summary(rows):
+    """the floor metrics of a clip from its per-frame rows [T][5] (include/uhc_floor.h: min_z, pen_mm, skate_mm, float_mm, n_below), as
+    smpl_eval.compute_metrics reports them: pentration (the reference's key) = mean pen_mm, skate = mean skate_mm over the T - 1 frame pairs
+    (row 0 has no previous frame), float = mean float_mm.  The rows come from the body hulls, not the SMPL mesh."""
+    r = np.asarray(rows, dtype=np.float64).reshape(-1, 5)
+    T = len(r)
+    return {"pentration": float(r[:, 1].mean()) if T else 0.0, "skate": float(r[1:, 2].mean()) if T > 1 else 0.0,
+            "float": float(r[:, 3].mean()) if T else 0.0}
+
+
 def metrics_from_frames(frames, percent, fail_safe):
     """compute_metrics' dict from the per-frame rows [T][6] the device evaluation writes (uhc_b200/csrc/eval_core.h; T >= 3):
     mpjpe_g, mpjpe, pa_mpjpe, vel (valid from frame 1), accel (from frame 2), |I - X_pred X_gt^-1|_F, which root_dist_mm divides by T."""

@@ -165,6 +165,70 @@ class MotionSet:
     def num_frames(self):
         return int(self.lens.sum())
 
+    @classmethod
+    def _from_rows(cls, kind, pose_dim, rows, lens):
+        ms = object.__new__(cls)
+        ms.kind, ms.pose_dim = kind, pose_dim
+        ms.rows, ms.lens = np.ascontiguousarray(rows, np.float64), np.asarray(lens, np.int32)
+        return ms
+
+    # ---- height against the floor, before the tables are built (include/uhc_floor.h uhc_motion_floor).  The reference fixes the height off
+    # line with the SMPL mesh (uhc/data_process/process_amass_db.py:126-219); here the surface is the body hulls, which are coarser.
+    START_HIGH, AIRBORNE_Z, AIRBORNE_RUN, TOE_DEPTH, CRAWL_ROOT, CRAWL_FEET = 0.1, 0.2, 30, -0.15, 0.3, -0.1
+
+    def floor_audit(self, engine, fk_models=None):
+        """Per clip, from one device pass over the raw rows (Engine.motion_floor; fk_models = shape variant per clip), arrays [C]:
+          dz_first      lowest hull vertex of frame 0 (m): fix_height_smpl_vanilla's gp
+          dz_clip       lowest hull vertex of the whole clip
+          start_high    dz_first > 0.1 (fix_height_smpl drops these)
+          airborne_run  longest run of frames with both feet above 0.2 m once the clip is lowered by dz_first (fix_height_smpl drops runs
+                        above 30; it reads SMPL joints 10 and 11, which this model names L_Toe and R_Toe)
+          deepest_toe   lowest toe of the clip once lowered by dz_first (fix_height drops clips below -0.15)
+          crawling      root below 0.3 m with both toes above -0.1 m at frame 0 (fix_height leaves these clips alone)
+          implausible   start_high, or airborne_run > 30, or deepest_toe < -0.15: the clips drop_implausible removes"""
+        rows, feet = engine.motion_floor(self, fk_models)
+        rows, feet = (np.asarray(x.cpu() if hasattr(x, "cpu") else x, dtype=np.float64) for x in (rows, feet))
+        C = len(self)
+        adr = np.concatenate([[0], np.cumsum(self.lens)])
+        models = getattr(engine, "variants", None) or [engine.model]
+        fk = np.zeros(C, np.int32) if fk_models is None else np.asarray(fk_models, np.int32).reshape(C)
+        out = {k: np.zeros(C) for k in ("dz_first", "dz_clip", "deepest_toe")}
+        out.update(airborne_run=np.zeros(C, np.int64), crawling=np.zeros(C, bool))
+        for c in range(C):
+            a, b = int(adr[c]), int(adr[c + 1])
+            dz = rows[a, 0]
+            toes = feet[a:b, 2:4] - dz
+            up = np.concatenate([[0], (toes > self.AIRBORNE_Z).all(1).astype(np.int64), [0]])
+            edges = np.flatnonzero(np.diff(up))
+            root_z = self.rows[a, 2] if self.kind == self.QPOS else self.rows[a, self.pose_dim + 2] + models[fk[c]].root_offset[2]
+            out["dz_first"][c], out["dz_clip"][c], out["deepest_toe"][c] = dz, rows[a:b, 0].min(), toes.min()
+            out["airborne_run"][c] = (edges[1::2] - edges[::2]).max() if len(edges) else 0
+            out["crawling"][c] = root_z < self.CRAWL_ROOT and feet[a, 2:4].min() > self.CRAWL_FEET
+        out["start_high"] = out["dz_first"] > self.START_HIGH
+        out["implausible"] = out["start_high"] | (out["airborne_run"] > self.AIRBORNE_RUN) | (out["deepest_toe"] < self.TOE_DEPTH)
+        return out
+
+    def fix_height(self, audit, mode="first_frame", offset=0.0):
+        """a new set with every clip's translation z (trans of SMPL rows, qpos[2] of qpos rows) lowered so that the lowest hull vertex of
+        frame 0 (mode "first_frame", fix_height_smpl_vanilla; crawling clips are left alone, as fix_height does) or of the whole clip
+        ("clip_min") sits at `offset` above the floor; "off" returns the rows unchanged.  audit: floor_audit's result for this set."""
+        if mode not in ("first_frame", "clip_min", "off"):
+            raise ValueError(f"fix_height: mode must be first_frame, clip_min or off, not {mode!r}")
+        rows = self.rows.copy()
+        if mode != "off":
+            dz = np.asarray(audit["dz_first" if mode == "first_frame" else "dz_clip"], np.float64) - float(offset)
+            if mode == "first_frame":
+                dz = np.where(audit["crawling"], 0.0, dz)
+            assert len(dz) == len(self), "fix_height: the audit is of another set"
+            rows[:, 2 if self.kind == self.QPOS else self.pose_dim + 2] -= np.repeat(dz, self.lens)
+        return self._from_rows(self.kind, self.pose_dim, rows, self.lens.copy())
+
+    def drop(self, mask):
+        """a new set without the clips where mask is true"""
+        keep = ~np.asarray(mask, bool).reshape(len(self))
+        assert keep.any(), "MotionSet.drop: no clip left"
+        return self._from_rows(self.kind, self.pose_dim, self.rows[np.repeat(keep, self.lens)], self.lens[keep])
+
 
 def synthetic_clip(T, rng, model=None, kind="normal"):
     """AMASS-shaped synthetic motion (SURVEY.md section 8d config 5): 30 fps, joint angles = sum of 3 low-frequency sinusoids

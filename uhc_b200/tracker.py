@@ -71,6 +71,15 @@ class Tracker:
             self._smpl = (t.empty(self.E, 72, device=self.state.device, dtype=t.float64), t.empty(self.E, 3, device=self.state.device, dtype=t.float64))
         return self.engine.track_smpl(self.state, *self._smpl)
 
+    def floor(self):
+        """the body hulls of the last step's state against the floor (uhc_floor_qpos' kernel at pitch 223, each env with its fk_models shape variant
+        and no previous frame: the envs are unrelated rows, so skate_mm is 0).  Returns [E][5] float64 on the device: min_z (m), pen_mm,
+        skate_mm, float_mm, n_below, a tensor overwritten by the next call.  The variants were range-checked by track_begin, so nothing synchronises
+        (as smpl())."""
+        if getattr(self, "_floor", None) is None:
+            self._floor = self.torch.empty(self.E, 5, device=self.state.device, dtype=self.torch.float64)
+        return self.engine.track_floor(self.state, self._floor)
+
     def steps(self):
         """control steps each env has taken since its reset (synchronises)"""
         return self.engine.track_state()["steps"]
