@@ -22,7 +22,9 @@ int uhc_linear_backward(const float *x, const float *W, const float *dz, float *
 int uhc_act_backward(const float *dh, const float *z, float *dz, long n, int act, void *stream);
 
 /* tensor-core forward of the same layer for the rollout path (wgmma, bf16 operands, fp32 accumulate): see mlp_wgmma.cu.
- * x_bf16 [M][Kp], W_bf16 [N][Kp] with Kp a multiple of 64 (zero padded); y_bf16 [M][Np] (next layer's input) and/or y_f32 [M][N]. */
+ * x_bf16 [M][Kp], W_bf16 [N][Kp] with Kp a multiple of 64 (zero padded); y_bf16 [M][Np] (next layer's input) and/or y_f32 [M][N].
+ * A bf16 y needs a 16-byte aligned base and a pitch ldy_bf16 >= N that is a multiple of 8 (every tensor-core entry point returns -2 otherwise,
+ * the grouped one included); its columns N .. min(ldy, N rounded up to 128) are written as zeros. */
 int uhc_linear_forward_tc(const void *x_bf16, const void *W_bf16, const float *b, void *y_bf16_or_null, float *y_f32_or_null,
                           int M, int N, int Kp, int ldy_bf16, int act, void *stream);
 /* the same for G <= UHC_TC_MAX_GROUPS weight sets in one launch: rows [row0_host[g], row0_host[g] + rows_host[g]) of x and y use W_bf16_host[g]

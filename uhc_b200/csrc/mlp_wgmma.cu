@@ -685,6 +685,9 @@ static int linear_tc_impl(const void *x_bf16, const void *W_bf16, const float *b
     if (ld_yf <= 0) ld_yf = N;      // row pitch of the fp32 y in floats (only a plain fp32 product through the TMA engine takes a pitch other than N)
     if (Kp % BK != 0 || M <= 0 || N <= 0) { uhc_err() = "uhc_linear_forward_tc: Kp must be a positive multiple of 64"; return -2; }
     if (y_bf16_or_null && (ldy_bf16 % 8 != 0)) { uhc_err() = "uhc_linear_forward_tc: ldy must be a multiple of 8"; return -2; }
+    // the per-thread epilogue writes bf16 rows as 16-byte vectors, and a pitch below N would drop the columns past it
+    if (y_bf16_or_null && ((uintptr_t)y_bf16_or_null & 15)) { uhc_err() = "uhc_linear_forward_tc: the bf16 y must be 16-byte aligned"; return -2; }
+    if (y_bf16_or_null && ldy_bf16 < N) { uhc_err() = "uhc_linear_forward_tc: ldy must be >= N"; return -2; }
     int dev = 0; cudaGetDevice(&dev);
     if (set_smem_attr(dev)) return -1;
     CUtensorMap ma, mb;
@@ -761,6 +764,7 @@ int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_h
     if (!x_bf16 || !W_bf16_host || (!y_bf16_or_null && !y_f32_or_null)) { uhc_err() = "uhc_linear_forward_tc_grouped: null argument"; return -2; }
     if (Kp % BK != 0 || Kp <= 0 || M <= 0 || N <= 0) { uhc_err() = "uhc_linear_forward_tc_grouped: M, N > 0 and Kp a positive multiple of 64"; return -2; }
     if (y_bf16_or_null && (ldy_bf16 % 8 != 0 || ldy_bf16 < N)) { uhc_err() = "uhc_linear_forward_tc_grouped: ldy must be a multiple of 8 and >= N"; return -2; }
+    if (y_bf16_or_null && ((uintptr_t)y_bf16_or_null & 15)) { uhc_err() = "uhc_linear_forward_tc_grouped: the bf16 y must be 16-byte aligned"; return -2; }
     GroupedArgs ga;
     memset(&ga, 0, sizeof ga);
     if (uhc::grp::plan_tiles(G, row0_host, rows_host, M, &ga.plan)) {
