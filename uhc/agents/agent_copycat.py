@@ -487,14 +487,20 @@ class AgentCopycat:
             self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
         return out
 
-    def render_motion(self, epoch=0, loaders=None, out_dir=None, size=(1920, 1080)):
+    def render_motion(self, epoch=0, loaders=None, out_dir=None, size=(1920, 1080), video="mp4"):
         """CopycatVisualizer's render_video without MuJoCo: every clip of the test loaders (or `loaders`) evaluated on the device and drawn
         there (BatchedAgent.render_motion), the simulated `pred` beside the expert `gt` as eval_seq pairs them, one mp4 per clip written by
         write_frames_to_video to {out_dir or cfg.output}/{take_key}_{cfg.id}_{epoch}_0.mp4 (the visualizer's video_path).  The view follows cfg's
         hide_im / hide_expert / shift_expert / focus as update_pose does.  Returns {loader name: {take_key: path}}; clips of two loaders with
         the same key share a file name, as in the visualizer, so such loaders want one call each with their own out_dir.  Like export_motion it is
-        not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored."""
+        not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored.  video="mjpeg"
+        compresses the frames on the device (BatchedAgent.render_motion's encode="jpeg") and writes {take_key}_{cfg.id}_{epoch}_0.avi, a
+        Motion-JPEG AVI (uhc_b200.video.write_mjpeg_avi), instead."""
         from uhc.utils.image_utils import write_frames_to_video
+        from uhc_b200.video import write_mjpeg_avi
+        if video not in ("mp4", "mjpeg"):
+            raise ValueError('render_motion: video must be "mp4" or "mjpeg"')
+        ext, W, H = ("mp4" if video == "mp4" else "avi"), int(size[0]), int(size[1])
         cfg, eng = self.cfg, self.agent.engine
         out_dir = out_dir or getattr(cfg, "output", None) or cfg.output_dir
         os.makedirs(out_dir, exist_ok=True)
@@ -507,12 +513,16 @@ class AgentCopycat:
                 saved = self._freq_dict_from_device() if self.curriculum_on_device else None
                 self._load_tables(loader)
             eng.set_cfg(**self._env_cfg(test=True))
-            paths = {k: osp.join(out_dir, f"{k}_{cfg.id}_{epoch}_0.mp4") for k in loader.data_keys}
+            paths = {k: osp.join(out_dir, f"{k}_{cfg.id}_{epoch}_0.{ext}") for k in loader.data_keys}
 
             def writer(i, chunks, keys=loader.data_keys, paths=paths):
-                write_frames_to_video((f for ch in chunks for f in ch), paths[keys[i]])
+                if video == "mp4":
+                    write_frames_to_video((f for ch in chunks for f in ch), paths[keys[i]])
+                else:
+                    write_mjpeg_avi(paths[keys[i]], (f for ch in chunks for f in ch), W, H)
 
-            self.agent.render_motion(np.arange(loader.get_len(), dtype=np.int32), bool(cfg.fail_safe), size, cam, writer=writer)
+            self.agent.render_motion(np.arange(loader.get_len(), dtype=np.int32), bool(cfg.fail_safe), size, cam, writer=writer,
+                                     encode=None if video == "mp4" else "jpeg")
             if loader is not self.data_loader:
                 self._load_tables(self.data_loader)
                 if saved is not None:

@@ -463,18 +463,25 @@ class BatchedAgent:
         self.obs = None
         return out
 
-    def render_motion(self, clips, fail_safe, size=(640, 360), camera=None, ghost=True, max_bytes=1 << 30, writer=None, window=32):
+    def render_motion(self, clips, fail_safe, size=(640, 360), camera=None, ghost=True, max_bytes=1 << 30, writer=None, window=32, encode=None,
+                      quality=90):
         """export_motion's evaluation of every listed clip, drawn on the device (Engine.render): frame k of clip i shows the simulated qpos
         pred[k] (grey) and, with ghost, the expert frame eval_seq pairs it with, gt[k] = qpos[min(k + 1, len - 1)] (red), with the clip's
         shape variant.  Frames come to the host in chunks of at most max_bytes of rgb (at least one frame).  writer(i, chunks) is called once
         per clip, in the caller's order, with an iterator over its uint8 chunks [k][H][W][3], rendered as it is consumed; without a writer
         the frames are returned.  Returns per clip export_motion's dict plus gt (and frames without a writer).  self.render_times holds the
-        seconds spent in evaluation, rendering, device-to-host copies and the writer."""
+        seconds spent in evaluation, rendering, device-to-host copies and the writer.  With encode="jpeg" every chunk is compressed on the
+        device (Engine.encode_jpeg at `quality`) and only the JPEG files come to the host: a chunk, and frames, are then lists of bytes, one
+        file per frame, and render_times also holds the seconds of encoding."""
+        if encode not in (None, "jpeg"):
+            raise ValueError('render_motion: encode must be None or "jpeg"')
         W, H = (int(x) for x in size)
         step = max(1, int(max_bytes) // (W * H * 3))
         t0 = time.perf_counter()
         mot = self.export_motion(clips, fail_safe, window, max_bytes)
         times = self.render_times = dict(evaluation=time.perf_counter() - t0, rendering=0.0, copy=0.0, writer=0.0)
+        if encode:
+            times["encoding"] = 0.0
         eng, clips = self.engine, np.asarray(clips, dtype=np.int32).reshape(-1)
 
         def chunks(d, var):
@@ -483,10 +490,17 @@ class BatchedAgent:
                 rgb = eng.render(d["pred"][k0:k0 + step], d["gt"][k0:k0 + step] if ghost else None, var, camera, (W, H))[0]
                 self.torch.cuda.synchronize(self.dev)
                 t2 = time.perf_counter()
-                host = rgb.cpu().numpy()
-                t3 = time.perf_counter()
                 times["rendering"] += t2 - t1
-                times["copy"] += t3 - t2
+                if encode:
+                    data, offsets = eng.encode_jpeg(rgb, quality)        # synchronises
+                    t3 = time.perf_counter()
+                    times["encoding"] += t3 - t2
+                    data, o = data.cpu().numpy(), offsets.cpu().numpy()
+                    host = [data[o[i]:o[i + 1]].tobytes() for i in range(len(o) - 1)]
+                else:
+                    t3 = t2
+                    host = rgb.cpu().numpy()
+                times["copy"] += time.perf_counter() - t3
                 yield host
 
         for i, (c, d) in enumerate(zip(clips, mot)):
@@ -494,11 +508,15 @@ class BatchedAgent:
             d["gt"] = eng.clip_frames(int(c))["qpos"][np.minimum(np.arange(1, nf + 1), L - 1)]
             var = None if eng.clip_models is None else int(eng.clip_models[c])
             if writer is None:
-                d["frames"] = np.concatenate(list(chunks(d, var))) if nf else np.zeros((0, H, W, 3), np.uint8)
+                if encode:
+                    d["frames"] = [f for ch in chunks(d, var) for f in ch]
+                else:
+                    d["frames"] = np.concatenate(list(chunks(d, var))) if nf else np.zeros((0, H, W, 3), np.uint8)
             else:
-                t1, inner = time.perf_counter(), times["rendering"] + times["copy"]
+                inside = lambda: times["rendering"] + times["copy"] + times.get("encoding", 0.0)
+                t1, inner = time.perf_counter(), inside()
                 writer(i, chunks(d, var))
-                times["writer"] += time.perf_counter() - t1 - (times["rendering"] + times["copy"] - inner)
+                times["writer"] += time.perf_counter() - t1 - (inside() - inner)
         return mot
 
     def _checkpoint_policy(self, k, cp):

@@ -217,6 +217,7 @@ class Engine:
             self.lib.uhc_eval_release(self.h)
             self.lib.uhc_track_end(self.h)
             self.lib.uhc_render_release(self.h)
+            self.lib.uhc_video_release(self.h)
             self.lib.uhc_floor_release(self.h)
             self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
@@ -613,6 +614,33 @@ class Engine:
         _chk(self.lib.uhc_render_bodies(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(pose), C.c_int(int(humanoids)), p(v),
                                         p(rgb), p(dep), p(lab), self._stream()), "uhc_render_bodies", ValueError)
         return rgb, dep, lab
+
+    # ---- the JPEG encoder (include/uhc_video.h)
+    def encode_jpeg(self, rgb, quality=90):
+        """frames rgb [n][H][W][3] (a contiguous cuda uint8 tensor, render()'s layout) -> (data, offsets): one baseline JPEG file per frame
+        (uhc_jpeg_encode), packed in the cuda uint8 tensor data, file i = data[offsets[i]:offsets[i + 1]] with offsets a cuda int64 tensor [n + 1]"""
+        t = self.torch
+        if not (t.is_tensor(rgb) and rgb.is_cuda and rgb.dtype == t.uint8 and rgb.dim() == 4 and rgb.shape[3] == 3 and rgb.is_contiguous()):
+            raise ValueError("encode_jpeg: rgb must be a contiguous cuda uint8 tensor [n][H][W][3]")
+        n, H, W = (int(x) for x in rgb.shape[:3])
+        dev = rgb.device
+        offsets = t.empty(n + 1, dtype=t.int64, device=dev)
+        hints = self.__dict__.setdefault("_jpeg_hint", {})
+        key = (W, H, int(quality))
+        cap = max(1, n * hints.get(key, W * H // 4 + 1024))           # bytes per frame seen so far at this size and quality, with a margin
+        total = C.c_size_t(0)
+        for _ in range(2):
+            data = t.empty(cap, dtype=t.uint8, device=dev)
+            rc = self.lib.uhc_jpeg_encode(self.h, C.c_void_p(rgb.data_ptr()), C.c_long(n), C.c_int(W), C.c_int(H), C.c_int(int(quality)),
+                                          C.c_void_p(data.data_ptr()), C.c_size_t(cap), C.c_void_p(offsets.data_ptr()), C.byref(total),
+                                          self._stream())
+            if rc != -3:
+                break
+            cap = int(total.value)                                     # too small: the call reported the size it needs
+        _chk(rc, "uhc_jpeg_encode", ValueError)
+        if n:
+            hints[key] = max(hints.get(key, 0), int(total.value) * 5 // (4 * n) + 1)
+        return data[:int(total.value)], offsets
 
     # ---- the batched physics tracker (include/uhc_track.h uhc_track_*)
     def track_begin(self, window=8, kind="qpos", pose_dim=None, fk_models=None, shapes=None):
