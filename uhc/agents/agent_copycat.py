@@ -281,6 +281,11 @@ class AgentCopycat:
         on_device = bool(cfg.get("eval_on_device", False))     # opt-in: BatchedAgent.evaluate (uhc_eval_run) instead of the host loop below
         motion = dump and bool(cfg.get("eval_dump_motion", False))   # opt-in: the dump also holds eval_seq's trajectories + SMPL per clip
         floor = bool(cfg.get("eval_floor_metrics", False))           # opt-in: pentration / skate / float of the body hulls per clip (_add_floor)
+        full = self._full_eval()                                     # opt-in: the SMPL mesh of every clip, pentration / skate from it (_add_mesh)
+        if full and floor:
+            raise ValueError("full_eval and eval_floor_metrics both write pentration / skate: enable one of them")
+        if full:
+            self._mesh_model()
         res_dicts = []
         eng = self.agent.engine
         E = self.num_envs
@@ -298,7 +303,8 @@ class AgentCopycat:
                 clips = (c0 + ids).astype(np.int32)
                 lens = eng.clip_len[clips]
                 if on_device:                                      # the same roll-out as the loop below, as CUDA-graph replays with the metrics on the device
-                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, floor=floor, **(dict(record_states=True, export_smpl=True) if motion else {}))
+                    kw = dict(record_states=True, export_smpl=True) if motion else (dict(record_states=True) if full else {})
+                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, floor=floor, **kw)
                     last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
                     rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
                     self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec,
@@ -306,6 +312,9 @@ class AgentCopycat:
                     if floor:
                         for i in ids:
                             self._add_floor(res[loader.data_keys[c0 + i]], loader, int(clips[i]), dev[i]["floor"], np.arange(1, len(dev[i]["frames"]) + 1))
+                    if full:
+                        self._add_mesh(res, loader, c0, ids, clips, [dev[i]["states"][:, :76] for i in ids],
+                                       [np.arange(1, len(dev[i]["frames"]) + 1) for i in ids], dump)
                     if motion:
                         for i in ids:
                             d = dev[i]
@@ -364,6 +373,9 @@ class AgentCopycat:
                             var = None if eng.clip_models is None else int(eng.clip_models[clips[i]])
                             rows = eng.floor_qpos(np.array(traj[i]["pred"]).reshape(-1, 76), variants=var).cpu().numpy()
                             self._add_floor(res[loader.data_keys[c0 + i]], loader, int(clips[i]), rows, np.array(traj[i]["t"], np.int64))
+                if full:
+                    self._add_mesh(res, loader, c0, ids, clips, [np.array(traj[i]["pred"]).reshape(-1, 76) for i in ids],
+                                   [np.array(traj[i]["t"], np.int64) for i in ids], dump)
                 if motion:                          # the host loop's recorded qpos as SMPL through the device conversion
                     for i in ids:
                         pred = np.array(traj[i]["pred"]).reshape(-1, 76)
@@ -390,6 +402,8 @@ class AgentCopycat:
         names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
         if bool(self.cfg.get("eval_floor_metrics", False)):
             names += ("pentration", "skate", "float", "pentration_gt", "skate_gt", "float_gt")
+        elif self._full_eval():
+            names += ("pentration", "skate", "pentration_gt", "skate_gt")
         metrics = {m: float(np.mean([np.mean(r[m]) for r in res.values() if m in r])) if any(m in r for r in res.values()) else float("nan") for m in names}
         coverage = int(round(metrics["succ"] * n))
         self.logger.info(f"Coverage {loader.name} of {coverage} out of {n} | " + " \t".join(f"{k}: {v:.3f}" for k, v in metrics.items()))
@@ -581,6 +595,64 @@ class AgentCopycat:
         g = eng.floor_qpos(np.asarray(gt["qpos"])[np.minimum(t, int(eng.clip_len[clip]) - 1)], variants=var).cpu().numpy()
         m.update(floor_summary(rows))
         m.update({k + "_gt": v for k, v in floor_summary(g).items()})
+
+    def _full_eval(self):
+        """full_eval (the reference's --full_eval flag or full_eval: true in the yml)"""
+        return bool(self.cfg.get("full_eval", False) or getattr(self.cfg, "full_eval", False))
+
+    def _mesh_model(self):
+        """full_eval's model: SMPL_NEUTRAL.{pkl,npz} in data/smpl relative to the working directory, where the reference's
+        SMPL_Robot(data_dir="data/smpl") reads it (convert_2_smpl_params passes no gender), uploaded once"""
+        if not getattr(self, "_mesh_ready", False):
+            path = osp.join("data", "smpl")
+            if not any(osp.exists(osp.join(path, "SMPL_NEUTRAL." + e)) for e in ("pkl", "npz")):
+                raise FileNotFoundError(f"full_eval needs the SMPL model {osp.join(path, 'SMPL_NEUTRAL.pkl')} (or .npz), relative to the working directory")
+            self.agent.engine.mesh_init(path)
+            self._mesh_ready = True
+
+    def _add_mesh(self, res, loader, c0, ids, clips, preds, ts, dump, max_bytes=1 << 30):
+        """full_eval: convert_2_smpl_params (humanoid_im.py:127-150) and compute_metrics' mesh keys (smpl_eval.py:113-121) for one evaluation
+        chunk.  Every clip's simulated rows preds[k] and the expert rows min(t, len - 1) they are paired with go qpos -> SMPL -> mesh on the
+        device (Engine.qpos_mesh) through the neutral model (_mesh_model), with the clip's beta[:10] when has_shape and zeros otherwise; pentration / skate (and *_gt for the expert rows)
+        come from the mesh against the floor (metrics.floor_summary).  With dump, pred_vertices / gt_vertices [T][V][3] float32 and
+        pred_joints / gt_joints [T][24][3] join the result, computed in device calls of at most max_bytes of vertices."""
+        from uhc_b200.metrics import floor_summary
+        eng = self.agent.engine
+        segs = []                                      # (result dict, key prefix, qpos rows, beta, variant)
+        for i, q, t in zip(ids, preds, ts):
+            if not len(t):
+                continue
+            c = int(clips[i])
+            gt = eng.clip_frames(c) if self._device_tables(loader) else loader.experts[c]
+            beta = np.asarray(loader.shapes[c], np.float64)[:10] if self.cfg.get("has_shape", False) else np.zeros(10)
+            var = 0 if eng.clip_models is None else int(eng.clip_models[c])
+            tt = np.minimum(np.asarray(t, np.int64), int(eng.clip_len[c]) - 1)
+            r = res[loader.data_keys[c0 + i]]
+            segs += [(r, "pred", np.asarray(q, np.float64).reshape(-1, 76), beta, var), (r, "gt", np.asarray(gt["qpos"], np.float64)[tt], beta, var)]
+        if not segs:
+            return
+        betas, bseg = np.unique(np.stack([s[3] for s in segs]), axis=0, return_inverse=True)
+        lens = [len(s[2]) for s in segs]
+        q = np.concatenate([s[2] for s in segs])
+        bidx = np.repeat(bseg.reshape(-1), lens).astype(np.int32)
+        var = np.repeat([s[4] for s in segs], lens).astype(np.int32)
+        first = np.zeros(len(q), np.int32)
+        first[np.cumsum([0] + lens[:-1])] = 1
+        rows = eng.qpos_mesh(q, betas, bidx, variants=var, floor=True, first=first).cpu().numpy()
+        o = 0
+        for (r, who, qs, _, _), n in zip(segs, lens):
+            f = floor_summary(rows[o:o + n])
+            sfx = "" if who == "pred" else "_gt"
+            r["pentration" + sfx], r["skate" + sfx] = f["pentration"], f["skate"]
+            if dump:
+                verts, joints = np.empty((n, eng.smpl_nvert, 3), np.float32), np.empty((n, 24, 3))
+                step = max(1, max_bytes // (eng.smpl_nvert * 12))
+                for a in range(0, n, step):
+                    v, j = eng.qpos_mesh(q[o + a:o + min(n, a + step)], betas, bidx[o + a:o + min(n, a + step)], variants=var[o + a:o + min(n, a + step)],
+                                         first=None)
+                    verts[a:a + step], joints[a:a + step] = v.cpu().numpy(), j.cpu().numpy()
+                r[who + "_vertices"], r[who + "_joints"] = verts, joints
+            o += n
 
     def _clip_result(self, L, last_t, fail_any, rsum, nrec, metrics_of):
         """res[key] of one evaluated clip of L frames, from either roll-out: the percent / succ rules of eval_seq and the reward average.

@@ -40,6 +40,12 @@ class UhcFloorHulls(C.Structure):
     _fields_ = [("nshape", C.c_int), ("nvert", C.c_int), ("hull", C.POINTER(C.c_double)), ("hull_adr", C.POINTER(C.c_int)), ("hull_num", C.POINTER(C.c_int))]
 
 
+class UhcSmplModel(C.Structure):
+    """include/uhc_mesh.h UhcSmplModel"""
+    _fields_ = [("nvert", C.c_int), ("v_template", C.POINTER(C.c_double)), ("shapedirs", C.POINTER(C.c_double)), ("posedirs", C.POINTER(C.c_double)),
+                ("J_regressor", C.POINTER(C.c_double)), ("weights", C.POINTER(C.c_double)), ("parents", C.POINTER(C.c_int))]
+
+
 EVAL_SMPL = 75      # include/uhc_eval.h UHC_EVAL_SMPL: pose 72, trans 3
 FLOOR_NCOL = 5      # include/uhc_floor.h UHC_FLOOR_NCOL: min_z (m), pen_mm, skate_mm, float_mm, n_below
 FLOOR_NFEET = 4     # UHC_FLOOR_NFEET: z of L_Ankle, R_Ankle, L_Toe, R_Toe
@@ -219,6 +225,7 @@ class Engine:
             self.lib.uhc_render_release(self.h)
             self.lib.uhc_video_release(self.h)
             self.lib.uhc_floor_release(self.h)
+            self.lib.uhc_mesh_release(self.h)
             self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
             self.h = None
@@ -528,6 +535,68 @@ class Engine:
                                        rows.ctypes.data_as(C.POINTER(C.c_double)), None if fk is None else _ip(fk), C.c_int(int(chunk_frames)),
                                        C.c_void_p(out.data_ptr()), C.c_void_p(feet.data_ptr())), "uhc_motion_floor", ValueError)
         return out, feet
+
+    # ---- the SMPL mesh (include/uhc_mesh.h)
+    def mesh_init(self, model):
+        """uploads an SMPL model (uhc_mesh_init): a dict as uhc_b200.smpl_model.load_smpl_model returns it, or a path it reads.  A later call
+        replaces the model; a failed one leaves the previous model in place."""
+        from uhc_b200.smpl_model import load_smpl_model, validate
+        m = load_smpl_model(model) if isinstance(model, (str, os.PathLike)) else validate({k: np.asarray(v) for k, v in model.items()})
+        keep = {k: np.ascontiguousarray(m[k], np.float64) for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "weights")}
+        keep["parents"] = np.ascontiguousarray(m["parents"], np.int32)
+        d = lambda k: keep[k].ctypes.data_as(C.POINTER(C.c_double))
+        h = UhcSmplModel(len(keep["v_template"]), d("v_template"), d("shapedirs"), d("posedirs"), d("J_regressor"), d("weights"), _ip_out(keep["parents"]))
+        _chk(self.lib.uhc_mesh_init(self.h, C.byref(h)), "uhc_mesh_init", ValueError)
+        self.smpl_nvert = len(keep["v_template"])
+
+    def _smpl_args(self, pose, trans, betas, beta_idx):
+        t = self.torch
+        dev = self.obs.device
+        f64 = lambda x: x if t.is_tensor(x) and x.is_cuda and x.dtype == t.float64 and x.is_contiguous() else \
+            t.as_tensor(np.ascontiguousarray(x.cpu().numpy() if t.is_tensor(x) else x, np.float64), device=dev)
+        pose, trans, betas = f64(pose), f64(trans), f64(betas)
+        n = pose.shape[0]
+        betas = betas[None] if betas.dim() == 1 else betas
+        if pose.dim() != 2 or pose.shape[1] != 72 or tuple(trans.shape) != (n, 3) or betas.dim() != 2 or betas.shape[1] != 10:
+            raise ValueError("smpl_mesh: pose [n][72], trans [n][3] and betas [nb][10] float64")
+        return pose, trans, betas, self._variant_arg(beta_idx, n)
+
+    def smpl_mesh(self, pose, trans, betas, beta_idx=None, vertices=True, joints=True):
+        """SMPL linear blend skinning on the device (uhc_smpl_mesh) after mesh_init: pose [n][72] axis-angles and trans [n][3] (qpos_to_smpl's
+        outputs, used in place when they are float64 cuda tensors), betas [nb][10], beta_idx = the betas row of each row (None: row 0).
+        Returns (vertices [n][V][3] float32, joints [n][24][3] float64) cuda tensors, None for what is not asked for."""
+        t = self.torch
+        pose, trans, betas, bi = self._smpl_args(pose, trans, betas, beta_idx)
+        n = pose.shape[0]
+        dev = self.obs.device
+        V = getattr(self, "smpl_nvert", 0)
+        vo = t.empty(n, V, 3, dtype=t.float32, device=dev) if vertices else None
+        jo = t.empty(n, 24, 3, dtype=t.float64, device=dev) if joints else None
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        _chk(self.lib.uhc_smpl_mesh(self.h, C.c_long(n), p(pose), p(trans), C.c_int(betas.shape[0]), p(betas), p(bi), p(vo), p(jo), self._stream()),
+             "uhc_smpl_mesh", ValueError)
+        return vo, jo
+
+    def smpl_floor(self, pose, trans, betas, beta_idx=None, first=None):
+        """the SMPL mesh of the same rows against the floor z = 0 (uhc_smpl_floor), no vertex written: first = per row, 1 where it has no
+        previous row (None: one clip).  Returns [n][5] float64 on the device: min_z (m), pen_mm, skate_mm, float_mm, n_below."""
+        t = self.torch
+        pose, trans, betas, bi = self._smpl_args(pose, trans, betas, beta_idx)
+        n = pose.shape[0]
+        f = self._variant_arg(first, n)
+        out = t.empty(n, FLOOR_NCOL, dtype=t.float64, device=self.obs.device)
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        _chk(self.lib.uhc_smpl_floor(self.h, C.c_long(n), p(pose), p(trans), C.c_int(betas.shape[0]), p(betas), p(bi), p(f), p(out), self._stream()),
+             "uhc_smpl_floor", ValueError)
+        return out
+
+    def qpos_mesh(self, qpos, betas, beta_idx=None, variants=None, vertices=True, joints=True, floor=False, first=None):
+        """qpos rows -> SMPL (qpos_to_smpl with `variants`) -> the mesh, without leaving the device: smpl_mesh's (vertices, joints), or with
+        floor=True smpl_floor's rows"""
+        pose, trans = self.qpos_to_smpl(qpos, variants)
+        if floor:
+            return self.smpl_floor(pose, trans, betas, beta_idx, first)
+        return self.smpl_mesh(pose, trans, betas, beta_idx, vertices, joints)
 
     @property
     def eval_graph_count(self):
