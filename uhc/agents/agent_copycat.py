@@ -102,6 +102,7 @@ class AgentCopycat:
                 dist.init_process_group("nccl")
             sync = make_nccl_grad_sync(world)
         rfc_mode = supported_variant(cfg)       # refuses (AssertionError) what the batched engine does not implement instead of accepting it silently (ADVICE r1)
+        self._subjects = self._subject_bodies(dev_index) if cfg.get("subject_bodies", False) else None
         def fixed_motions(engine):
             """data_specs.fix_height / drop_implausible (DatasetAMASSSingle.fix_floor): the raw motion is measured on the GPU, so it runs between
             the engine's creation and the first table load; the clip table, the clip sampler and the history keys are all built from what is left"""
@@ -118,7 +119,8 @@ class AgentCopycat:
             obs_v=int(cfg.obs_v), fut_frames=int(cfg.get("fut_frames", 10)), fut_skip=int(cfg.get("skip", 10)),
             has_shape=bool(cfg.get("has_shape", False)) and bool(cfg.get("has_shape_obs", True)), actor_type=cfg.actor_type, num_primitive=int(cfg.get("num_primitive", 8)), composer_dim=tuple(cfg.get("composer_dim", [300, 200])),
             reactive_v=int(cfg.get("reactive_v", 0)), reactive_rate=float(cfg.get("reactive_rate", 0.3)),
-            term_body=cfg.get("env_term_body", "body"), head_body=self.model_tables.body_names.index("Head"), reward_mul=cfg.reward_id == "world_rfc_implicit_v1_mul")
+            term_body=cfg.get("env_term_body", "body"), head_body=self.model_tables.body_names.index("Head"), reward_mul=cfg.reward_id == "world_rfc_implicit_v1_mul",
+            variants=self._subjects and self._subjects[0], subject_of=self._subjects and self._subject_of)
         self.policy_net, self.value_net, self.running_state = self.agent.policy, self.agent.value, self.agent.running_state
         self.state_dim, self.action_dim = self.agent.obs_dim, self.agent.act_dim
         self.expert_reward = reward_func[cfg.reward_id]
@@ -686,8 +688,37 @@ class AgentCopycat:
         """data_specs.expert_tables: device -- the loader keeps the raw motion and the engine builds the expert tables on the GPU"""
         return getattr(loader, "expert_tables", "host") == "device"
 
+    def _subject_bodies(self, device):
+        """subject_bodies: every clip is simulated with its own subject's body, as the reference's reset_robot rebuilds the humanoid per clip
+        (humanoid_im.py:154-180).  Loads data/smpl/SMPL_{NEUTRAL,MALE,FEMALE}.{pkl,npz} from the working directory, where the reference's
+        Robot reads all three, and builds one shape variant per distinct (beta[:10], gender) of every loader's clips on the GPU
+        (uhc_b200/subject_body.py).  Returns (variants, {subject key: variant})."""
+        from uhc_b200.smpl_model import load_smpl_model
+        from uhc_b200.subject_body import SubjectBasis, subject_key
+        assert all(self._device_tables(l) for l in self.test_data_loaders), \
+            "subject_bodies needs data_specs.expert_tables: device (the expert FK then runs on each clip's own body); expert_tables: host builds neutral-body tables"
+        path, models = osp.join("data", "smpl"), []
+        for g in ("NEUTRAL", "MALE", "FEMALE"):
+            f = [osp.join(path, f"SMPL_{g}.{e}") for e in ("pkl", "npz") if osp.exists(osp.join(path, f"SMPL_{g}.{e}"))]
+            if not f:
+                raise FileNotFoundError(f"subject_bodies needs the SMPL model {osp.join(path, f'SMPL_{g}.pkl')} (or .npz), relative to the working directory")
+            models.append(load_smpl_model(f[0]))
+        basis = SubjectBasis.from_models(self.model_tables, *models)
+        shapes = np.concatenate([np.asarray(l.shapes, np.float64).reshape(-1, 17) for l in self.test_data_loaders])
+        variants, idx = basis.build(shapes[:, :10], shapes[:, 16], device=device)
+        self.logger.info(f"subject_bodies: {len(variants)} bodies for {len(shapes)} clips")
+        return variants, {subject_key(r[:10], r[16]): int(v) for r, v in zip(shapes, idx)}
+
+    def _subject_of(self, shapes):
+        """the shape variant of every clip of a loader (subject_bodies), from its shape rows [C][17]"""
+        from uhc_b200.subject_body import subject_key
+        return np.array([self._subjects[1][subject_key(r[:10], r[16])] for r in np.asarray(shapes, np.float64).reshape(-1, 17)], np.int32)
+
     def _load_tables(self, loader):
-        if self._device_tables(loader):
+        if self._device_tables(loader) and self._subjects is not None:
+            v = self._subject_of(loader.shapes)
+            self.agent.engine.load_motions(loader.motions, loader.shapes, v, fk_models=v)
+        elif self._device_tables(loader):
             self.agent.engine.load_motions(loader.motions, loader.shapes)
         else:
             self.agent.engine.load_clips(loader.experts, loader.shapes)

@@ -124,7 +124,7 @@ class BatchedAgent:
                  value_hsize=(2048, 1024, 512), htype="gelu", log_std=-2.3, policy_lr=5e-5, value_lr=3e-4, gamma=0.95, tau=0.95,
                  clip_epsilon=0.2, num_optim_epoch=10, grad_clip=40.0, t_min=5, t_max=300, noise_rate=1.0, rank=0, world=1,
                  grad_sync=None, model=None, update_tc=True, variants=None, clip_models=None, c_update=True, actor_type="gauss", num_primitive=8,
-                 composer_dim=(300, 200), **env_cfg):
+                 composer_dim=(300, 200), subject_of=None, **env_cfg):
         import torch
         self.torch = torch
         self.dev = torch.device("cuda", device)
@@ -135,8 +135,12 @@ class BatchedAgent:
                              reset_seed=seed * 7919 + rank * 104729 + 1, **env_cfg)
         if callable(clips):                                  # clips(engine) -> (MotionSet, shapes): raw motion that needs the engine before it is
             clips, shapes = clips(self.engine)               # loaded (a height fix measured on the GPU); the sampler below sees what it returns
+        fk_models = None
+        if subject_of is not None:                           # subject_of(shapes [C][17]) -> the variant of each clip: its simulated body and the
+            assert isinstance(clips, MotionSet), "subject_of needs raw motion: the expert FK runs on each clip's body on the GPU"
+            clip_models = fk_models = subject_of(shapes)     # body of its expert FK (AgentCopycat's subject_bodies)
         if isinstance(clips, MotionSet):                     # raw motion: the expert tables are built on the GPU
-            self.engine.load_motions(clips, shapes, clip_models)
+            self.engine.load_motions(clips, shapes, clip_models, fk_models=fk_models)
         else:
             self.engine.load_clips(clips, shapes, clip_models)   # clip_models: body-shape variant per clip (the reference rebuilds the robot per clip)
         self.sampler = ClipSampler(self.engine.clip_len, t_min, t_max, seed=seed * 9973 + rank)

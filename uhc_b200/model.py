@@ -76,6 +76,26 @@ class HumanoidModel:
             self.invw = self._invweight0()
         self._pack()
 
+    @classmethod
+    def from_tables(cls, base, body_f, hull, maps):
+        """a shape variant of `base` from its tables (uhc_b200/subject_body.py): body_f [24][20] and hull [nvert][3] taken as they are (invweight0
+        and the bounding spheres included), maps [24][3][4] the per-body affine maps (A | t) that carry base's hulls onto this one.  Shares the
+        base's topology, dof tables and joint limits."""
+        m = cls.__new__(cls)
+        m.__dict__.update({k: v for k, v in base.__dict__.items() if k not in ("_keep", "_rkeep")})
+        bf = np.array(body_f, np.float64).reshape(NB, BODYF)
+        m.hull = np.array(hull, np.float64).reshape(len(base.hull), 3)
+        m.maps = np.array(maps, np.float64).reshape(NB, 3, 4)
+        m.offset, m.ipos, m.mass, m.invw = bf[:, 0:3].copy(), bf[:, 3:6].copy(), bf[:, 6].copy(), bf[:, 13].copy()
+        q = bf[:, 7:13]
+        m.inertia = np.stack([np.stack([q[:, 0], q[:, 3], q[:, 4]], 1), np.stack([q[:, 3], q[:, 1], q[:, 5]], 1),
+                              np.stack([q[:, 4], q[:, 5], q[:, 2]], 1)], 1)
+        m.body_f = np.ascontiguousarray(bf)
+        m.root_offset = bf[0, 0:3].copy()            # the root body's offset: where smpl_to_qpos puts the pelvis, as the device FK does
+        m.qpos0 = base.qpos0.copy()
+        m.qpos0[:3] = m.root_offset
+        return m
+
     def _topology(self):
         p = self.parent
         self.depth = np.zeros(NB, np.int32)
@@ -204,12 +224,27 @@ class HumanoidModel:
             num.append(len(keep))
         return np.concatenate(planes), np.concatenate([[0], np.cumsum(num)[:-1]]).astype(np.int32), np.array(num, np.int32)
 
+    def mapped_planes(self, planes):
+        """hull_planes() of a variant built by from_tables, as the images of its base's `planes` under the body maps instead of a hull per
+        body: x -> A x + t takes n . x + d <= 0 to (A^-T n) . x' + d - (A^-T n) . t <= 0, renormalised"""
+        pl, adr, num = planes
+        out = np.empty_like(pl)
+        for b in range(NB):
+            A, t = self.maps[b, :, :3], self.maps[b, :, 3]
+            rows = pl[adr[b]:adr[b] + num[b]]
+            n = np.linalg.solve(A.T, rows[:, :3].T).T
+            d = rows[:, 3] - n @ t
+            s = np.linalg.norm(n, axis=1)
+            out[adr[b]:adr[b] + num[b]] = np.hstack([n / s[:, None], (d / s)[:, None]])
+        return out, adr, num
+
     def render_struct(self, variants=None):
         """ctypes UhcRenderHulls of the shape variants host_struct(variants) builds, in the same order (arrays kept alive on self).  Variants
         share plane_adr / plane_num: a body whose hull has fewer merged faces in one variant repeats its last plane, which clips nothing more."""
         models = variants or [self]
         assert models[0] is self
-        per = [m.hull_planes() for m in models]
+        own = self.hull_planes()
+        per = [own if s == 0 else m.mapped_planes(own) if getattr(m, "maps", None) is not None else m.hull_planes() for s, m in enumerate(models)]
         num = np.max([p[2] for p in per], axis=0).astype(np.int32)
         adr = np.concatenate([[0], np.cumsum(num)[:-1]]).astype(np.int32)
         plane = np.zeros((len(models), int(num.sum()), 4))
