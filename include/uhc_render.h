@@ -1,5 +1,6 @@
 /* uhc_render.h -- C ABI of the offline renderer (part of libuhc_b200.so): the simulated and the reference humanoid drawn on the GPU as an exact
- * ray cast of the 24 convex body hulls the contact pass collides with, over a checkered floor.
+ * ray cast of the 24 convex body hulls the contact pass collides with, over a checkered floor; or, with uhc_render_mesh, as a ray cast of the
+ * skinned SMPL mesh (include/uhc_mesh.h's vertices) under the same camera, floor, shading and outputs.
  *
  * Reference interface replaced: CopycatVisualizer (uhc/utils/copycat_visualizer.py) with render_video, which replays eval_seq's `pred` beside
  * `gt` in one MuJoCo scene and reads 1920x1080 frames back from the GL viewer.  The camera is MuJoCo's free camera as the visualizer sets it
@@ -42,7 +43,7 @@ const char *uhc_render_last_error(void);   /* an alias of uhc_last_error (uhc_b2
 /* Uploads the plane tables (as fp32) once per engine; a second call replaces them.  -2 unless nshape equals the engine's shape variants,
  * every body has 4 .. UHC_RENDER_MAX_PLANES planes inside 0 .. nplane - 1, and every value is finite.  Synchronises the device. */
 int uhc_render_init(UhcEngine *e, const UhcRenderHulls *hulls);
-/* Frees what uhc_render_init and the pose scratch hold (also safe without them). */
+/* Frees what uhc_render_init, uhc_render_mesh_init and their scratch hold (also safe without them). */
 void uhc_render_release(UhcEngine *e);
 
 /* The pose table [n][2][24][UHC_RENDER_POSE] fp32 of n frames: humanoid 0 = qpos row i, humanoid 1 = ghost row i (left untouched without a
@@ -61,6 +62,39 @@ int uhc_render_bodies(UhcEngine *e, const UhcRenderCamera *cam, int W, int H, lo
 int uhc_render_qpos(UhcEngine *e, const UhcRenderCamera *cam, int W, int H, long n, const void *qpos_dev, int precision, long pitch,
                     const void *ghost_qpos_dev_or_null, long ghost_pitch, const int *variant_dev_or_null, unsigned char *rgb_dev,
                     float *depth_dev_or_null, unsigned char *label_dev_or_null, void *stream);
+
+/* ---- the skinned SMPL mesh (uhc_render_mesh): the same camera, floor, shading and outputs, with the posed mesh instead of the hulls.
+ * The mesh is traced through a fixed two-level hierarchy, body -> leaves of at most UHC_RENDER_MESH_LEAF faces -> triangles, whose topology
+ * uhc_b200/render_mesh.py builds once per model: face f belongs to the body whose SMPL joint has the largest summed skinning weight over its
+ * three vertices, and every body's faces are split by a recursive median split of their rest-pose centroids.  Per frame only the boxes are
+ * refitted. */
+#define UHC_RENDER_MESH_LEAF 32
+
+/* The topology, host pointers read during uhc_render_mesh_init only.  The faces are permuted so that leaf l holds faces leaf_first[l] ..
+ * leaf_first[l + 1] - 1 and body b holds leaves body_leaf[b] .. body_leaf[b + 1] - 1 (leaves body-major); face_body[f] = the model body
+ * (0 .. 23) of permuted face f. */
+typedef struct {
+    int nvert, nface, nleaf;
+    const int *face;            /* [nface][3] vertex indices, 0 .. nvert - 1 */
+    const int *face_body;       /* [nface] */
+    const int *leaf_first;      /* [nleaf + 1] */
+    const int *body_leaf;       /* [25] */
+} UhcRenderMesh;
+
+/* Uploads the topology once per engine; a second call replaces it, a failed call leaves the previous one.  -2 with nothing uploaded unless
+ * every index lies in 0 .. nvert - 1, every face lies in exactly one leaf and that leaf belongs to the face's body, every leaf holds 1 ..
+ * UHC_RENDER_MESH_LEAF faces, every body's leaves are one contiguous range, and the leaf boxes of two humanoids fit the trace kernel's
+ * shared memory.  uhc_render_release frees it too.  Synchronises the device. */
+int uhc_render_mesh_init(UhcEngine *e, const UhcRenderMesh *mesh);
+/* n frames of W x H pixels of the mesh: verts_dev = [n][V][3] fp32 (uhc_smpl_mesh's vertices) of the grey humanoid, ghost_verts_dev_or_null
+ * the same of the red one (shifted by shift_expert in x), root_dev_or_null = [n][3] fp32, the first humanoid's root, where a camera with focus
+ * looks (required then).  Outputs, labels (2 + b / 26 + b: the body b a face belongs to) and the camera as uhc_render_bodies.  Shading is flat:
+ * the face normal, turned towards the viewer, with one shadow ray towards the light.  Boxes are refitted into the engine's scratch, which
+ * grows with n.  Bad arguments (-2): uhc_render_bodies' (but no uhc_render_init is needed), no uhc_render_mesh_init, nvert != the
+ * topology's, a null verts with n > 0, a null root with focus on. */
+int uhc_render_mesh(UhcEngine *e, const UhcRenderCamera *cam, int W, int H, long n, const float *verts_dev, const float *ghost_verts_dev_or_null,
+                    const float *root_dev_or_null, int nvert, unsigned char *rgb_dev, float *depth_dev_or_null, unsigned char *label_dev_or_null,
+                    void *stream);
 
 #ifdef __cplusplus
 }

@@ -503,7 +503,7 @@ class AgentCopycat:
             self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
         return out
 
-    def render_motion(self, epoch=0, loaders=None, out_dir=None, size=(1920, 1080), video="mp4"):
+    def render_motion(self, epoch=0, loaders=None, out_dir=None, size=(1920, 1080), video="mp4", body="hulls"):
         """CopycatVisualizer's render_video without MuJoCo: every clip of the test loaders (or `loaders`) evaluated on the device and drawn
         there (BatchedAgent.render_motion), the simulated `pred` beside the expert `gt` as eval_seq pairs them, one mp4 per clip written by
         write_frames_to_video to {out_dir or cfg.output}/{take_key}_{cfg.id}_{epoch}_0.mp4 (the visualizer's video_path).  The view follows cfg's
@@ -511,7 +511,9 @@ class AgentCopycat:
         the same key share a file name, as in the visualizer, so such loaders want one call each with their own out_dir.  Like export_motion it is
         not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored.  video="mjpeg"
         compresses the frames on the device (BatchedAgent.render_motion's encode="jpeg") and writes {take_key}_{cfg.id}_{epoch}_0.avi, a
-        Motion-JPEG AVI (uhc_b200.video.write_mjpeg_avi), instead."""
+        Motion-JPEG AVI (uhc_b200.video.write_mjpeg_avi), instead.  body="mesh" draws the skinned SMPL mesh instead of the body hulls:
+        the neutral model data/smpl/SMPL_NEUTRAL.{pkl,npz} (as full_eval loads it, and it must hold the faces `f`), each clip shaped by its
+        beta[:10] under has_shape and zeros otherwise."""
         from uhc.utils.image_utils import write_frames_to_video
         from uhc_b200.video import write_mjpeg_avi
         if video not in ("mp4", "mjpeg"):
@@ -520,6 +522,8 @@ class AgentCopycat:
         cfg, eng = self.cfg, self.agent.engine
         out_dir = out_dir or getattr(cfg, "output", None) or cfg.output_dir
         os.makedirs(out_dir, exist_ok=True)
+        if body == "mesh":
+            self._mesh_model(render=True)
         cam = {k: bool(getattr(cfg, k, False)) for k in ("hide_im", "hide_expert", "focus")}
         cam["shift_expert"] = 1.0 if getattr(cfg, "shift_expert", False) else 0.0
         out = {}
@@ -537,8 +541,12 @@ class AgentCopycat:
                 else:
                     write_mjpeg_avi(paths[keys[i]], (f for ch in chunks for f in ch), W, H)
 
-            self.agent.render_motion(np.arange(loader.get_len(), dtype=np.int32), bool(cfg.fail_safe), size, cam, writer=writer,
-                                     encode=None if video == "mp4" else "jpeg")
+            ids = np.arange(loader.get_len(), dtype=np.int32)
+            betas = None
+            if body == "mesh" and self.cfg.get("has_shape", False):
+                betas = np.stack([np.asarray(loader.shapes[c], np.float64)[:10] for c in ids])
+            self.agent.render_motion(ids, bool(cfg.fail_safe), size, cam, writer=writer, encode=None if video == "mp4" else "jpeg", body=body,
+                                     betas=betas)
             if loader is not self.data_loader:
                 self._load_tables(self.data_loader)
                 if saved is not None:
@@ -602,15 +610,19 @@ class AgentCopycat:
         """full_eval (the reference's --full_eval flag or full_eval: true in the yml)"""
         return bool(self.cfg.get("full_eval", False) or getattr(self.cfg, "full_eval", False))
 
-    def _mesh_model(self):
+    def _mesh_model(self, render=False):
         """full_eval's model: SMPL_NEUTRAL.{pkl,npz} in data/smpl relative to the working directory, where the reference's
-        SMPL_Robot(data_dir="data/smpl") reads it (convert_2_smpl_params passes no gender), uploaded once"""
+        SMPL_Robot(data_dir="data/smpl") reads it (convert_2_smpl_params passes no gender), uploaded once; with render also the mesh
+        renderer's topology of it (render_motion(body="mesh"))"""
+        path = osp.join("data", "smpl")
         if not getattr(self, "_mesh_ready", False):
-            path = osp.join("data", "smpl")
             if not any(osp.exists(osp.join(path, "SMPL_NEUTRAL." + e)) for e in ("pkl", "npz")):
-                raise FileNotFoundError(f"full_eval needs the SMPL model {osp.join(path, 'SMPL_NEUTRAL.pkl')} (or .npz), relative to the working directory")
+                raise FileNotFoundError(f"the SMPL mesh (full_eval, render_motion(body='mesh')) needs the model {osp.join(path, 'SMPL_NEUTRAL.pkl')} (or .npz), relative to the working directory")
             self.agent.engine.mesh_init(path)
             self._mesh_ready = True
+        if render and not getattr(self, "_render_mesh_ready", False):
+            self.agent.engine.render_mesh_init(path)
+            self._render_mesh_ready = True
 
     def _add_mesh(self, res, loader, c0, ids, clips, preds, ts, dump, max_bytes=1 << 30):
         """full_eval: convert_2_smpl_params (humanoid_im.py:127-150) and compute_metrics' mesh keys (smpl_eval.py:113-121) for one evaluation

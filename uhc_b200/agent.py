@@ -468,7 +468,7 @@ class BatchedAgent:
         return out
 
     def render_motion(self, clips, fail_safe, size=(640, 360), camera=None, ghost=True, max_bytes=1 << 30, writer=None, window=32, encode=None,
-                      quality=90):
+                      quality=90, body="hulls", betas=None):
         """export_motion's evaluation of every listed clip, drawn on the device (Engine.render): frame k of clip i shows the simulated qpos
         pred[k] (grey) and, with ghost, the expert frame eval_seq pairs it with, gt[k] = qpos[min(k + 1, len - 1)] (red), with the clip's
         shape variant.  Frames come to the host in chunks of at most max_bytes of rgb (at least one frame).  writer(i, chunks) is called once
@@ -476,11 +476,24 @@ class BatchedAgent:
         the frames are returned.  Returns per clip export_motion's dict plus gt (and frames without a writer).  self.render_times holds the
         seconds spent in evaluation, rendering, device-to-host copies and the writer.  With encode="jpeg" every chunk is compressed on the
         device (Engine.encode_jpeg at `quality`) and only the JPEG files come to the host: a chunk, and frames, are then lists of bytes, one
-        file per frame, and render_times also holds the seconds of encoding."""
+        file per frame, and render_times also holds the seconds of encoding.  body="mesh" draws the skinned SMPL mesh instead of the hulls
+        (Engine.render_smpl, after the engine's mesh_init and render_mesh_init): clip i's pred and gt are both shaped by betas[i] (betas =
+        [len(clips)][10] in the caller's order; None: zeros), and the vertices of a chunk count against max_bytes beside its rgb."""
         if encode not in (None, "jpeg"):
             raise ValueError('render_motion: encode must be None or "jpeg"')
+        if body not in ("hulls", "mesh"):
+            raise ValueError('render_motion: body must be "hulls" or "mesh"')
         W, H = (int(x) for x in size)
-        step = max(1, int(max_bytes) // (W * H * 3))
+        per_frame = W * H * 3
+        if body == "mesh":
+            if getattr(self.engine, "smpl_nvert", None) is None:
+                raise ValueError('render_motion: body="mesh" needs the engine\'s mesh_init and render_mesh_init')
+            nclip = len(np.atleast_1d(clips))
+            betas = np.zeros((nclip, 10)) if betas is None else np.asarray(betas, np.float64)
+            if betas.shape != (nclip, 10):
+                raise ValueError(f"render_motion: betas must be [len(clips)][10] = [{nclip}][10], got {list(betas.shape)}")
+            per_frame += (2 if ghost else 1) * self.engine.smpl_nvert * 12
+        step = max(1, int(max_bytes) // per_frame)
         t0 = time.perf_counter()
         mot = self.export_motion(clips, fail_safe, window, max_bytes)
         times = self.render_times = dict(evaluation=time.perf_counter() - t0, rendering=0.0, copy=0.0, writer=0.0)
@@ -488,10 +501,14 @@ class BatchedAgent:
             times["encoding"] = 0.0
         eng, clips = self.engine, np.asarray(clips, dtype=np.int32).reshape(-1)
 
-        def chunks(d, var):
+        def chunks(d, var, beta):
             for k0 in range(0, len(d["pred"]), step):
                 t1 = time.perf_counter()
-                rgb = eng.render(d["pred"][k0:k0 + step], d["gt"][k0:k0 + step] if ghost else None, var, camera, (W, H))[0]
+                pred, gt = d["pred"][k0:k0 + step], d["gt"][k0:k0 + step] if ghost else None
+                if body == "mesh":
+                    rgb = eng.render_smpl(pred, gt, beta, variants=var, camera=camera, size=(W, H))[0]
+                else:
+                    rgb = eng.render(pred, gt, var, camera, (W, H))[0]
                 self.torch.cuda.synchronize(self.dev)
                 t2 = time.perf_counter()
                 times["rendering"] += t2 - t1
@@ -511,15 +528,16 @@ class BatchedAgent:
             nf, L = len(d["pred"]), int(eng.clip_len[c])
             d["gt"] = eng.clip_frames(int(c))["qpos"][np.minimum(np.arange(1, nf + 1), L - 1)]
             var = None if eng.clip_models is None else int(eng.clip_models[c])
+            beta = None if betas is None else betas[i]
             if writer is None:
                 if encode:
-                    d["frames"] = [f for ch in chunks(d, var) for f in ch]
+                    d["frames"] = [f for ch in chunks(d, var, beta) for f in ch]
                 else:
-                    d["frames"] = np.concatenate(list(chunks(d, var))) if nf else np.zeros((0, H, W, 3), np.uint8)
+                    d["frames"] = np.concatenate(list(chunks(d, var, beta))) if nf else np.zeros((0, H, W, 3), np.uint8)
             else:
                 inside = lambda: times["rendering"] + times["copy"] + times.get("encoding", 0.0)
                 t1, inner = time.perf_counter(), inside()
-                writer(i, chunks(d, var))
+                writer(i, chunks(d, var, beta))
                 times["writer"] += time.perf_counter() - t1 - (inside() - inner)
         return mot
 

@@ -16,9 +16,12 @@
 
 using namespace uhc;
 
+namespace uhc { void render_mesh_release(UhcEngine *e); }   // render_mesh.cu: the mesh tables and their scratch
+
 namespace {
 
 constexpr int TILE = 16, SLOTS = 2 * render::NB;
+constexpr size_t SMEM_MAX = 200 * 1024;                // dynamic shared memory of a trace, at most
 
 struct RenderCtx {
     UhcEngine *eng = nullptr;
@@ -102,12 +105,6 @@ __global__ void __launch_bounds__(TILE * TILE) k_render_trace(const __grid_const
 
 size_t trace_smem(int nplane) { return (size_t)nplane * sizeof(float4) + (size_t)SLOTS * (render::POSE + 4) * sizeof(float); }
 
-bool finite_cam(const UhcRenderCamera &c) {
-    double v[8] = {c.lookat[0], c.lookat[1], c.lookat[2], c.azimuth, c.elevation, c.distance, c.fovy, c.shift_expert};
-    for (double x : v) if (!isfinite(x)) return false;
-    return true;
-}
-
 // the variant array on the host, range-checked (-2), or -1 on a CUDA error
 int check_variants(UhcEngine *e, long n, const int *variant_dev, cudaStream_t st, const char *who) {
     if (!variant_dev || n == 0) return 0;
@@ -148,14 +145,9 @@ int launch_pose(UhcEngine *e, long n, const void *qpos, int precision, long pitc
 int trace_args(UhcEngine *e, const UhcRenderCamera *cam, int W, int H, long n, int humanoids, const void *pose, const void *rgb, const char *who) {
     if (!e) { uhc_err() = std::string(who) + ": null engine"; return -2; }
     if (!find_ctx(e)) { uhc_err() = std::string(who) + ": no hull planes (uhc_render_init)"; return -2; }
-    if (!cam) { uhc_err() = std::string(who) + ": null camera"; return -2; }
-    if (n < 0) { uhc_err() = std::string(who) + ": n < 0"; return -2; }
-    if (W < 1 || H < 1 || W > 16384 || H > 16384) { uhc_err() = std::string(who) + ": W and H must be in 1 .. 16384"; return -2; }
+    if (const char *why = render::frame_args_error(cam, W, H, n)) { uhc_err() = std::string(who) + ": " + why; return -2; }
     if (humanoids != 1 && humanoids != 2) { uhc_err() = std::string(who) + ": humanoids must be 1 or 2"; return -2; }
     if (n > 0 && (!pose || !rgb)) { uhc_err() = std::string(who) + ": null pose or rgb"; return -2; }
-    if (!finite_cam(*cam) || !(cam->distance > 0) || !(cam->fovy > 0 && cam->fovy < 180)) {
-        uhc_err() = std::string(who) + ": camera needs finite values, distance > 0 and 0 < fovy < 180"; return -2;
-    }
     return 0;
 }
 
@@ -181,7 +173,7 @@ extern "C" {
 int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
     if (!e || !h || !h->plane || !h->plane_adr || !h->plane_num || !h->sphere) { uhc_err() = "uhc_render_init: null argument"; return -2; }
     if (h->nshape != trackx::num_shapes(e)) { uhc_err() = "uhc_render_init: nshape differs from the engine's shape variants"; return -2; }
-    if (h->nplane < 4 || trace_smem(h->nplane) > 200 * 1024) { uhc_err() = "uhc_render_init: nplane out of range"; return -2; }
+    if (h->nplane < 4 || trace_smem(h->nplane) > SMEM_MAX) { uhc_err() = "uhc_render_init: nplane out of range"; return -2; }
     for (int b = 0; b < render::NB; b++)
         if (h->plane_num[b] < 4 || h->plane_num[b] > UHC_RENDER_MAX_PLANES || h->plane_adr[b] < 0 || h->plane_adr[b] > h->nplane - h->plane_num[b]) {
             uhc_err() = "uhc_render_init: plane_adr / plane_num of a body out of range"; return -2;
@@ -198,7 +190,7 @@ int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
         if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && p[3] > 0 && isfinite(p[3]))) { uhc_err() = "uhc_render_init: bad bounding sphere"; return -2; }
         sp[i] = make_float4((float)p[0], (float)p[1], (float)p[2], (float)p[3]);
     }
-    uhc_render_release(e);
+    if (RenderCtx *old = find_ctx(e)) free_ctx(old);             // the mesh tables (uhc_render_mesh_init) stay
     RenderCtx *c = new RenderCtx();
     c->eng = e; g_rd.push_back(c);
     c->nshape = h->nshape; c->nplane = h->nplane;
@@ -207,13 +199,15 @@ int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
     CK(cudaMalloc((void **)&c->d_sphere, ns * sizeof(float4)));
     CK(cudaMemcpy(c->d_plane, pl.data(), np * sizeof(float4), cudaMemcpyHostToDevice));
     CK(cudaMemcpy(c->d_sphere, sp.data(), ns * sizeof(float4), cudaMemcpyHostToDevice));
-    CK(cudaFuncSetAttribute(k_render_trace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)trace_smem(c->nplane)));
+    // the init's limit, not these planes' need: the attribute is per function, and fewer planes on another engine must not lower it
+    CK(cudaFuncSetAttribute(k_render_trace, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX));
     CK(cudaDeviceSynchronize());
     return 0;
 }
 
 void uhc_render_release(UhcEngine *e) {
     if (RenderCtx *c = e ? find_ctx(e) : nullptr) free_ctx(c);
+    uhc::render_mesh_release(e);
 }
 
 int uhc_render_pose(UhcEngine *e, long n, const void *qpos_dev, int precision, long pitch, const void *ghost_qpos_dev_or_null, long ghost_pitch,

@@ -5,6 +5,9 @@
 // (render.cu: -fmad=false, IEEE division and square root) and a host build with -ffp-contract=off give the same bits.  The camera basis is
 // built on the host in fp64 (camera_setup) and handed over in fp32: no trigonometric function runs per pixel.
 //
+// shade_pixel is templated on the scene: the hulls (Scene, cast below) or the skinned mesh (render_mesh_core.h's MeshScene and its cast), so
+// both renderers share the camera, floor, checker, colours, shading and to_u8.
+//
 // A pose table row holds, per body, R (row-major 3x3, body -> world) and the body origin p: world = R v + p.  Hull planes are in body
 // frame, n . v + d <= 0 inside.
 #pragma once
@@ -69,6 +72,18 @@ inline void camera_setup(const CamIn &c, int W, int H, int humanoids, Cam *out) 
     out->shift = (float)c.shift_expert;
     out->focus = c.focus != 0;
     out->visible = (c.hide_im ? 0 : 1) | ((humanoids > 1 && !c.hide_expert) ? 2 : 0);
+}
+
+// host only: the argument checks every trace shares (nullptr: none fails)
+template <class CamIn>
+inline const char *frame_args_error(const CamIn *c, int W, int H, long n) {
+    if (!c) return "null camera";
+    if (n < 0) return "n < 0";
+    if (W < 1 || H < 1 || W > 16384 || H > 16384) return "W and H must be in 1 .. 16384";
+    const double v[8] = {c->lookat[0], c->lookat[1], c->lookat[2], c->azimuth, c->elevation, c->distance, c->fovy, c->shift_expert};
+    for (double x : v) if (!isfinite(x)) return "camera needs finite values, distance > 0 and 0 < fovy < 180";
+    if (!(c->distance > 0) || !(c->fovy > 0 && c->fovy < 180)) return "camera needs finite values, distance > 0 and 0 < fovy < 180";
+    return nullptr;
 }
 #endif
 
@@ -165,10 +180,15 @@ UHC_RDEV int cast(const Scene &s, const float *o, const float *d, float t_lo, fl
 
 UHC_RDEV unsigned char to_u8(float c) { return (unsigned char)((c > 1.0f ? 1.0f : (c < 0.0f ? 0.0f : c)) * 255.0f + 0.5f); }
 
-// pixel (x, y) of a W x H frame: rgb, depth (+inf on sky), label
-UHC_RDEV void shade_pixel(const Cam &cam, const Scene &s, int x, int y, int W, int H, unsigned char *rgb, float *depth, unsigned char *label) {
+// the first humanoid's root x, y (before any shift), where a focused camera looks
+UHC_RDEV void focus_xy(const Scene &s, float *look) { look[0] = s.pose[9]; look[1] = s.pose[10]; }
+
+// pixel (x, y) of a W x H frame: rgb, depth (+inf on sky), label.  S is the frame's scene: Scene (the hulls) or, through the overloads of
+// cast and focus_xy that render_mesh_core.h adds, MeshScene (the skinned mesh); camera, floor, checker, colours and shading are shared.
+template <class S>
+UHC_RDEV void shade_pixel(const Cam &cam, const S &s, int x, int y, int W, int H, unsigned char *rgb, float *depth, unsigned char *label) {
     float look[3] = {cam.look[0], cam.look[1], cam.look[2]};
-    if (cam.focus) { look[0] = s.pose[9]; look[1] = s.pose[10]; }     // the first humanoid's root (before any shift)
+    if (cam.focus) focus_xy(s, look);
     const float o[3] = {look[0] + cam.off[0], look[1] + cam.off[1], look[2] + cam.off[2]};
     const float a = 2.0f * ((float)x + 0.5f) / (float)W - 1.0f, b = 1.0f - 2.0f * ((float)y + 0.5f) / (float)H;
     float d[3];

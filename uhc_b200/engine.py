@@ -57,6 +57,20 @@ class UhcRenderCamera(C.Structure):
                 ("focus", C.c_int), ("hide_im", C.c_int), ("hide_expert", C.c_int), ("shift_expert", C.c_double)]
 
 
+class UhcRenderMesh(C.Structure):
+    """include/uhc_render.h UhcRenderMesh"""
+    _fields_ = [("nvert", C.c_int), ("nface", C.c_int), ("nleaf", C.c_int), ("face", C.POINTER(C.c_int)), ("face_body", C.POINTER(C.c_int)),
+                ("leaf_first", C.POINTER(C.c_int)), ("body_leaf", C.POINTER(C.c_int))]
+
+    @classmethod
+    def of(cls, tables, nvert):
+        """over the arrays of uhc_b200.render_mesh.build_tables (kept alive by the struct)"""
+        keep = {k: np.ascontiguousarray(tables[k], np.int32) for k in ("face", "face_body", "leaf_first", "body_leaf")}
+        m = cls(int(nvert), len(keep["face"]), len(keep["leaf_first"]) - 1, *(_ip_out(keep[k]) for k in ("face", "face_body", "leaf_first", "body_leaf")))
+        m._keep = keep
+        return m
+
+
 def make_camera(camera=None):
     """UhcRenderCamera from a dict (or None): CopycatVisualizer.setup_viewing_angle's view by default -- lookat (0, 0, 1), azimuth 45,
     elevation -8, distance 5, fovy 45 (MuJoCo's default) -- with focus / hide_im / hide_expert (bools) and shift_expert (x offset of the
@@ -540,8 +554,8 @@ class Engine:
     def mesh_init(self, model):
         """uploads an SMPL model (uhc_mesh_init): a dict as uhc_b200.smpl_model.load_smpl_model returns it, or a path it reads.  A later call
         replaces the model; a failed one leaves the previous model in place."""
-        from uhc_b200.smpl_model import load_smpl_model, validate
-        m = load_smpl_model(model) if isinstance(model, (str, os.PathLike)) else validate({k: np.asarray(v) for k, v in model.items()})
+        from uhc_b200.smpl_model import as_model
+        m = as_model(model)
         keep = {k: np.ascontiguousarray(m[k], np.float64) for k in ("v_template", "shapedirs", "posedirs", "J_regressor", "weights")}
         keep["parents"] = np.ascontiguousarray(m["parents"], np.int32)
         d = lambda k: keep[k].ctypes.data_as(C.POINTER(C.c_double))
@@ -683,6 +697,54 @@ class Engine:
         _chk(self.lib.uhc_render_bodies(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(pose), C.c_int(int(humanoids)), p(v),
                                         p(rgb), p(dep), p(lab), self._stream()), "uhc_render_bodies", ValueError)
         return rgb, dep, lab
+
+    # ---- the mesh renderer (include/uhc_render.h uhc_render_mesh*)
+    def render_mesh_init(self, model):
+        """uploads the mesh renderer's topology (uhc_render_mesh_init) of an SMPL model with faces: a dict as
+        uhc_b200.smpl_model.load_smpl_model returns it, or a path it reads.  The tables are built on the host (uhc_b200.render_mesh); a later
+        call replaces them, a failed one leaves the previous ones."""
+        from uhc_b200.render_mesh import build_tables
+        from uhc_b200.smpl_model import as_model
+        m = as_model(model)
+        if m.get("faces") is None:
+            raise ValueError("render_mesh_init: the SMPL model has no faces (key f)")
+        self._rmesh = UhcRenderMesh.of(build_tables(m["faces"], m["weights"], m["v_template"], self.model.body_names), len(m["v_template"]))
+        _chk(self.lib.uhc_render_mesh_init(self.h, C.byref(self._rmesh)), "uhc_render_mesh_init", ValueError)
+
+    def render_mesh(self, verts, ghost_verts=None, root=None, camera=None, size=(640, 360), depth=False, label=False):
+        """n frames of W x H pixels of the skinned mesh (uhc_render_mesh) after render_mesh_init: verts / ghost_verts = [n][V][3] (smpl_mesh's
+        vertices: contiguous float32 cuda tensors are read in place, anything else is copied as float32), root = [n][3] where a camera with focus looks (the first humanoid's root).  Outputs, labels
+        and the camera as render()."""
+        t = self.torch
+        dev = self.obs.device
+        verts = t.as_tensor(verts, dtype=t.float32, device=dev).contiguous()          # in place when already a contiguous float32 cuda tensor
+        ghost_verts = None if ghost_verts is None else t.as_tensor(ghost_verts, dtype=t.float32, device=dev).contiguous()
+        if verts.dim() != 3 or verts.shape[2] != 3 or (ghost_verts is not None and ghost_verts.shape != verts.shape):
+            raise ValueError("render_mesh: verts and ghost_verts must be [n][V][3] of one shape")
+        n, V = int(verts.shape[0]), int(verts.shape[1])
+        if root is not None:
+            root = t.as_tensor(root, dtype=t.float32, device=self.obs.device).contiguous()
+            if tuple(root.shape) != (n, 3):
+                raise ValueError("render_mesh: root must be [n][3]")
+        W, H, rgb, dep, lab = self._render_out(n, size, depth, label)
+        cam = make_camera(camera)
+        p = lambda x: C.c_void_p(x.data_ptr() if x is not None else None)
+        _chk(self.lib.uhc_render_mesh(self.h, C.byref(cam), C.c_int(W), C.c_int(H), C.c_long(n), p(verts), p(ghost_verts), p(root), C.c_int(V),
+                                      p(rgb), p(dep), p(lab), self._stream()), "uhc_render_mesh", ValueError)
+        return rgb, dep, lab
+
+    def render_smpl(self, qpos, ghost=None, betas=None, beta_idx=None, variants=None, camera=None, size=(640, 360), depth=False, label=False):
+        """qpos rows (and the ghost's) -> SMPL (qpos_to_smpl with `variants`) -> the skinned mesh (smpl_mesh with betas [nb][10] and beta_idx per
+        row, shared by both humanoids) -> render_mesh, without leaving the device; needs mesh_init and render_mesh_init of the same model.  The
+        focus root is qpos[:, :3], the hull renderer's root, so a mesh frame is framed exactly like render()'s frame of the same qpos."""
+        if betas is None:
+            raise ValueError("render_smpl: betas [nb][10] are required")
+        q = self._rows(qpos, who="render_smpl")
+        g = None if ghost is None else self._rows(ghost, q.shape[0], who="render_smpl")
+        verts = self.qpos_mesh(q, betas, beta_idx, variants, joints=False)[0]
+        gverts = None if g is None else self.qpos_mesh(g, betas, beta_idx, variants, joints=False)[0]
+        root = q[:, :3].to(self.torch.float32).contiguous()
+        return self.render_mesh(verts, gverts, root, camera, size, depth, label)
 
     # ---- the JPEG encoder (include/uhc_video.h)
     def encode_jpeg(self, rgb, quality=90):

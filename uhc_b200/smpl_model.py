@@ -94,14 +94,30 @@ def validate(m):
     bad = np.abs(m["weights"].sum(1) - 1.0) > 1e-6
     if bad.any():
         raise ValueError(f"SMPL model: weights of vertex {int(np.argmax(bad))} do not sum to 1")
+    if m.get("faces") is not None:
+        f = np.asarray(m["faces"])
+        if f.ndim != 2 or f.shape[1] != 3 or len(f) < 1 or not (np.issubdtype(f.dtype, np.integer) or (np.isfinite(f).all() and (f == np.round(f)).all())):
+            raise ValueError(f"SMPL model: f (the faces) has shape {f.shape}, expected (F, 3) integer vertex indices with F >= 1")
+        if f.min() < 0 or f.max() >= V:
+            raise ValueError(f"SMPL model: f (the faces) holds a vertex index outside 0 .. {V - 1}")
+        m["faces"] = f.astype(np.int32)
     return m
+
+
+def as_model(model):
+    """a model argument as Engine.mesh_init / render_mesh_init take it -- a path (load_smpl_model) or a dict in load_smpl_model's layout, whose
+    arrays are checked by validate (a faces value of None, as load_smpl_model returns for a file without `f`, stays absent)"""
+    if isinstance(model, (str, os.PathLike)):
+        return load_smpl_model(model)
+    return validate({k: None if v is None else np.asarray(v) for k, v in model.items()})
 
 
 def load_smpl_model(path):
     """the SMPL model at `path` (.pkl, .npz, or a directory with SMPL_NEUTRAL.{pkl,npz}) as fp64 arrays: v_template [V][3], shapedirs
     [V][3][10] (the first 10 components, smplx's default num_betas), posedirs [V][3][207], J_regressor [24][V] dense, weights [V][24],
-    parents [24] (kintree_table[0] with the root -1).  ValueError naming the key for a missing key, inconsistent shapes, parents[i] >= i,
-    non-finite values or a weight row whose sum is not 1 within 1e-6."""
+    parents [24] (kintree_table[0] with the root -1), and faces [F][3] int32 when the file has `f` (None otherwise; only mesh rendering needs
+    them).  ValueError naming the key for a missing key, inconsistent shapes, parents[i] >= i, non-finite values, a weight row whose sum is
+    not 1 within 1e-6, or faces that are not F >= 1 rows of vertex indices in 0 .. V - 1."""
     raw = _read(os.fspath(path))
     if not isinstance(raw, dict):
         raise ValueError("SMPL model: the file does not hold a dict of arrays")
@@ -114,5 +130,6 @@ def load_smpl_model(path):
     parents = kt[0].astype(np.int64)
     parents[0] = -1
     m = dict(v_template=vt, shapedirs=np.ascontiguousarray(sd[:, :, :NBETA]), posedirs=_as(raw, "posedirs", (V, 3, NPOSE)),
-             J_regressor=_as(raw, "J_regressor", (NJ, V)), weights=_as(raw, "weights", (V, NJ)), parents=parents.astype(np.int32))
+             J_regressor=_as(raw, "J_regressor", (NJ, V)), weights=_as(raw, "weights", (V, NJ)), parents=parents.astype(np.int32),
+             faces=_dense(raw["f"]) if "f" in raw else None)
     return validate(m)
