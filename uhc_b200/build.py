@@ -17,14 +17,24 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
-def build(force=False, verbose=False):
+def build(force=False, verbose=False, so=SO, defines=()):
+    """so: the library to write (default: the in-tree one the package loads); defines: extra preprocessor macros ("NAME" or "NAME=VALUE"),
+    e.g. build(so="/tmp/x/libuhc_b200.so", defines=["UHC_PHASE_CLOCKS"]) for an instrumented variant beside the production library."""
     csrc = os.path.join(HERE, "csrc")
     srcs = [os.path.join(csrc, s) for s in SRCS]
     nofma = [os.path.join(csrc, s) for s in NO_FMA_SRCS]
     deps = srcs + nofma + [os.path.join(csrc, d) for d in DEPS] + [os.path.abspath(__file__)]
-    if not force and os.path.exists(SO) and os.path.getmtime(SO) >= max(os.path.getmtime(d) for d in deps if os.path.exists(d)):
-        return SO
-    flags = [f for f in NVCC_FLAGS if f != "--use_fast_math=false"] + os.environ.get("UHC_NVCC_EXTRA", "").split()
+    extra = os.environ.get("UHC_NVCC_EXTRA", "").split() + ["-D" + d for d in defines]
+    # the extra flags the library at `so` was built with live in a stamp beside it (no stamp: none), so a library built with other
+    # defines or UHC_NVCC_EXTRA is never taken for an up-to-date one
+    stamp = so + ".flags"
+    built_with = open(stamp).read() if os.path.exists(stamp) else ""
+    if (not force and built_with == " ".join(extra) and os.path.exists(so)
+            and os.path.getmtime(so) >= max(os.path.getmtime(d) for d in deps if os.path.exists(d))):
+        return so
+    if os.path.exists(stamp):
+        os.remove(stamp)
+    flags = [f for f in NVCC_FLAGS if f != "--use_fast_math=false"] + extra
     with tempfile.TemporaryDirectory() as tmp:
         objs = []
         for s in nofma:
@@ -36,13 +46,16 @@ def build(force=False, verbose=False):
             if r.returncode:
                 raise RuntimeError("nvcc failed")
             objs.append(o)
-        cmd = ["nvcc"] + flags + ["-o", SO] + srcs + objs + ["-ldl"]
+        cmd = ["nvcc"] + flags + ["-o", so] + srcs + objs + ["-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or r.returncode:
         print(r.stdout[-6000:], r.stderr[-12000:])
     if r.returncode:
         raise RuntimeError("nvcc failed")
-    return SO
+    if extra:
+        with open(stamp, "w") as f:
+            f.write(" ".join(extra))
+    return so
 
 
 if __name__ == "__main__":

@@ -37,6 +37,9 @@ struct EngineView {
     int *ep_start_log;      // [E] the start frame of that episode, written by the curriculum variant of the step kernel
     int *counters;          // [4] device counters: 0 = env-steps failed because a body's contacts did not fit MAXCON, 1 = env-steps skipped on an invalid env record
     CurView cur;
+#if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
+    long long *phase_cyc;   // [E][NPHASE] cycles per phase summed over control steps (null = not collected); UHC_PHASE_CLOCKS builds only
+#endif
 };
 
 // an env record the step kernel can run: a clip of the CURRENT clip table and at least two frames (uhc_load_clips invalidates every
@@ -263,6 +266,7 @@ UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, co
     Real *st = ev.state + (size_t)env * ST_SIZE;
     const int clip = is[SI_CLIP], start = is[SI_START], len = is[SI_LEN];
     int cur_t = is[SI_CUR_T];
+    PCLK_START(w);
     load_state(ev, env, w, 0);     // the warp's mbarrier completes exactly one phase per kernel launch
     // action = [NU joint targets | vf_dim residual-force dims | 30 meta-PD scales]: the work set keeps the joint targets, the implicit root
     // wrench and the meta-PD scales at the fixed slots the PD code reads; the explicit per-body forces are read from global memory where used
@@ -280,13 +284,16 @@ UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, co
     LANES_END
     const Model<Real> &mdl = w.mdl;
     TOPO_DECL(mdl);
+    PCLK(true, w, PC_LOAD);
 #pragma unroll 1
     for (int it = 0; it < NSUB; ++it) {
         UHC_CTA_SYNC(true);   // see substep_dynamics: the CTA's warps run each substep's straight-line code together
+        PCLK(true, w, PC_SYNC_SUBSTEP);
         iters += substep_dynamics<Real, ObsT>(mdl, w.cfg, w, tp, target, it, true, torque_out, true, action);
         if (w.ncon > maxcon) maxcon = w.ncon;
-        if (it == NSUB - 1) world_quat(mdl, w.q, w);  // pose of the last forward pass (what data.body_xquat holds)
+        if (it == NSUB - 1) { world_quat(mdl, w.q, w); PCLK(true, w, PC_EPILOGUE); }  // pose of the last forward pass (what data.body_xquat holds)
         integrate(mdl, w);
+        PCLK(true, w, PC_INTEGRATE);
     }
     cur_t += 1;
     // body quats: prev <- stored, current from the new qpos (humanoid_im.py:1196, :1219)
@@ -362,6 +369,10 @@ UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, co
         if (lane == 0) is[SI_EPISODE] = episode;
         LANES_END
     }
+#if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
+    PCLK(true, w, PC_EPILOGUE);
+    if (ev.phase_cyc && (threadIdx.x & 31) == 0) for (int i = 0; i < NPHASE; i++) ev.phase_cyc[(size_t)env * NPHASE + i] += w.pc[i];
+#endif
     return fail || end;
 }
 

@@ -115,6 +115,10 @@ struct EnvCfg {
 };
 constexpr int VF_BODY_DIM = 9, MAX_ACT_DIM = NU + VF_BODY_DIM * NB + 30;
 
+// phases of a control step for the cycle accounting of UHC_PHASE_CLOCKS builds (PCLK below, scripts/step_phase_cycles.py)
+enum { PC_LOAD, PC_PD, PC_KIN, PC_COLLIDE, PC_SMOOTH, PC_CSETUP, PC_NEWTON_ABA, PC_NEWTON_ROWS, PC_SYNC_SUBSTEP, PC_SYNC_PD, PC_SYNC_SMOOTH,
+       PC_INTEGRATE, PC_EPILOGUE, NPHASE };
+
 // per-environment working set (lives in shared memory on the GPU)
 template <class Real>
 struct Work {
@@ -157,7 +161,21 @@ struct Work {
     // instead of a per-thread local-memory copy
     alignas(8) Model<Real> mdl;
     alignas(8) EnvCfg<Real> cfg;
+#if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
+    long long pc_t, pc[NPHASE];   // clock64 of the last phase boundary, cycles per phase of this control step
+#endif
 };
+
+// Phase cycle accounting, compiled in only with -DUHC_PHASE_CLOCKS: lane 0 of a warp reads clock64() at every phase boundary of the
+// control step and adds the interval since the previous boundary to that phase; env_step_warp adds the totals to EngineView::phase_cyc.
+// PCLK(on, w, ph) closes phase ph when `on` (the in-kernel reset runs substep_dynamics without it).  Without the switch both are empty.
+#if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
+#define PCLK_START(w) do { __syncwarp(); if ((threadIdx.x & 31) == 0) { for (int i_ = 0; i_ < NPHASE; i_++) (w).pc[i_] = 0; (w).pc_t = clock64(); } } while (0)
+#define PCLK(on, w, ph) do { if (on) { __syncwarp(); if ((threadIdx.x & 31) == 0) { const long long t_ = clock64(); (w).pc[ph] += t_ - (w).pc_t; (w).pc_t = t_; } } } while (0)
+#else
+#define PCLK_START(w) do { } while (0)
+#define PCLK(on, w, ph) do { (void)sizeof(on); } while (0)
+#endif
 
 // ------------------------------------------------------------------------------------------------ scalar helpers
 // reciprocal: hardware approximation + one Newton step on the GPU (within 1 ulp; no slow-path branch), exact division elsewhere
@@ -474,11 +492,13 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
     LVARA(Real, Ur, 3);
     Real *arm = w.Mp;     // joint-space diagonal (armature + arm_scale kd)
     LVAR(int, body); LVAR(int, src); LVAR(int, act); LVAR(int, rr); LVAR(int, ent); LVAR(int, entn);
-    const int nlvl = (UHC_LDT(m.lvl_pack) >> 26) & 15;
+    const int *lp = m.lvl_pack;   // once: for the compiler the stores of the sweeps may alias the Model, and every level would reload the pointer
+    const int nlvl = (UHC_LDT(lp) >> 26) & 15;
+    int nslot_n = (UHC_LDT(lp + (nlvl - 1) * LVL_G) >> 18) & 3;   // uniform: most children any body of the level has (fetched one level ahead)
     LANES_BEGIN
     for (int i = 0; i < 3; i++) { LVA(row)[i] = pbc(Real(0)); LVA(pA)[i] = pbc(Real(0)); }
     LV(rr) = lane - 6 * (lane / 6);
-    LV(entn) = lane < 6 * LVL_G ? UHC_LDT(m.lvl_pack + (nlvl - 1) * LVL_G + lane / 6) : 0;
+    LV(entn) = lane < 6 * LVL_G ? UHC_LDT(lp + (nlvl - 1) * LVL_G + lane / 6) : 0;
     const bool limits = use_contacts && w.nlim > 0;     // an active joint-limit row (J = +-e_i) adds its D to the joint-space diagonal of the Hessian
     for (int i = lane; i < NV; i += 32) {
         Real d = UHC_LDT(m.dof_f + 4 * i) + arm_scale * UHC_LDT(m.dof_f + 4 * i + 2);   // joint-space diagonal
@@ -488,10 +508,12 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
     LANES_END
 #pragma unroll 1
     for (int lvl = nlvl - 1; lvl >= 0; --lvl) {
+        const int nslot = nslot_n;
+        if (lvl > 0) nslot_n = (UHC_LDT(lp + (lvl - 1) * LVL_G) >> 18) & 3;
         LANES_BEGIN
         const int g = lane / 6, r = LV(rr);
         const int e = LV(entn);            // this level's table entry was fetched one level ahead
-        LV(entn) = (g < LVL_G && lvl > 0) ? UHC_LDT(m.lvl_pack + (lvl - 1) * LVL_G + g) : 0;
+        LV(entn) = (g < LVL_G && lvl > 0) ? UHC_LDT(lp + (lvl - 1) * LVL_G + g) : 0;
         const int b = (e & 63) - 1;
         LV(ent) = e; LV(body) = b;
         Real ri[6] = {0, 0, 0, 0, 0, 0}, pi[6] = {0, 0, 0, 0, 0, 0};
@@ -507,7 +529,6 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
         }
         for (int i = 0; i < 3; i++) { LVA(nrow)[i].x = ri[2 * i]; LVA(nrow)[i].y = ri[2 * i + 1]; LVA(npA)[i].x = pi[2 * i]; LVA(npA)[i].y = pi[2 * i + 1]; }
         LANES_END_R
-        const int nslot = (UHC_LDT(m.lvl_pack + lvl * LVL_G) >> 18) & 3;   // uniform: most children any body of this level has
 #pragma unroll 1
         for (int k = 0; k < nslot; ++k) {  // children of this level's bodies: they sit one level deeper, their results are still in row / pA
             LANES_BEGIN
@@ -531,9 +552,12 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
         {
             LANES_BEGIN   // this lane's entries of U = IA S
             const int b = LV(body), d0 = 3 * ((LV(ent) >> 20) & 31);
+            P Sk[3][3];                    // S of the joint in registers first: a store to aU may alias S for the compiler
+#pragma unroll
+            for (int k = 0; k < 3; k++) for (int i = 0; i < 3; i++) Sk[k][i] = as_pairs(w.S[d0 + k])[i];
 #pragma unroll
             for (int k = 0; k < 3; k++) {
-                const Real u = pdot6(LVA(row), as_pairs(w.S[d0 + k]));
+                const Real u = pdot6(LVA(row), Sk[k]);
                 LVA(Ur)[k] = u;
                 if (b >= 0) w.aU[d0 + k][LV(rr)] = u;
             }
@@ -541,10 +565,12 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
             LANES_BEGIN
             const int b = LV(body), d0 = 3 * ((LV(ent) >> 20) & 31), r = LV(rr);
             const Real sg = ((LV(ent) >> 25) & 1) ? Real(-1) : Real(1);   // joint crossed against its kinematic direction
-            P U0[3], U1[3], U2[3];
-            const P *S0 = as_pairs(w.S[d0]), *S1 = as_pairs(w.S[d0 + 1]), *S2 = as_pairs(w.S[d0 + 2]);
+            P U0[3], U1[3], U2[3], S0[3], S1[3], S2[3];
 #pragma unroll
-            for (int i = 0; i < 3; i++) { U0[i] = as_pairs(w.aU[d0])[i]; U1[i] = as_pairs(w.aU[d0 + 1])[i]; U2[i] = as_pairs(w.aU[d0 + 2])[i]; }
+            for (int i = 0; i < 3; i++) {
+                U0[i] = as_pairs(w.aU[d0])[i]; U1[i] = as_pairs(w.aU[d0 + 1])[i]; U2[i] = as_pairs(w.aU[d0 + 2])[i];
+                S0[i] = as_pairs(w.S[d0])[i]; S1[i] = as_pairs(w.S[d0 + 1])[i]; S2[i] = as_pairs(w.S[d0 + 2])[i];
+            }
             // D = S^T U + arm (symmetric), u = b - S^T pA
             const Real D00 = pdot6(S0, U0) + arm[d0], D11 = pdot6(S1, U1) + arm[d0 + 1], D22 = pdot6(S2, U2) + arm[d0 + 2];
             const Real D01 = pdot6(S0, U1), D02 = pdot6(S0, U2), D12 = pdot6(S1, U2);
@@ -598,16 +624,16 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
     WSHFL1(LVA(pacc)[3], sol, 3); WSHFL1(LVA(pacc)[4], sol, 4); WSHFL1(LVA(pacc)[5], sol, 5);
     // centre -> leaves (the spatial acceleration a is replicated in the 6 lanes of a group; every lane starts from the centre body's)
     LANES_BEGIN
-    const int bc = (UHC_LDT(m.lvl_pack) & 63) - 1;
+    const int bc = (UHC_LDT(lp) & 63) - 1;
     if (use_contacts && lane < 6) w.Ab[bc][lane] = LV(sol);
-    LV(entn) = (lane < 6 * LVL_G && nlvl > 1) ? UHC_LDT(m.lvl_pack + LVL_G + lane / 6) : 0;
+    LV(entn) = (lane < 6 * LVL_G && nlvl > 1) ? UHC_LDT(lp + LVL_G + lane / 6) : 0;
     LANES_END
 #pragma unroll 1
     for (int lvl = 1; lvl < nlvl; ++lvl) {
         LANES_BEGIN
         const int g = lane / 6;
         const int e = LV(entn);
-        LV(entn) = (g < LVL_G && lvl + 1 < nlvl) ? UHC_LDT(m.lvl_pack + (lvl + 1) * LVL_G + g) : 0;
+        LV(entn) = (g < LVL_G && lvl + 1 < nlvl) ? UHC_LDT(lp + (lvl + 1) * LVL_G + g) : 0;
         const int b = (e & 63) - 1;
         LV(body) = b; LV(ent) = e;
         LV(src) = b >= 0 ? ((e >> 6) & 7) * 6 : lane;
@@ -620,10 +646,17 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
         if (b >= 0) {
             const Real sg = ((LV(ent) >> 25) & 1) ? Real(-1) : Real(1);
             const int d0 = 3 * ((LV(ent) >> 20) & 31);
-            const Real x0 = w.au[d0] - pdot6(as_pairs(w.aU[d0]), a), x1 = w.au[d0 + 1] - pdot6(as_pairs(w.aU[d0 + 1]), a),
-                       x2 = w.au[d0 + 2] - pdot6(as_pairs(w.aU[d0 + 2]), a);
+            // every operand of the level in registers first: for the compiler the stores to x below may alias S, and each S load would wait for them
+            P U0[3], U1[3], U2[3], S0[3], S1[3], S2[3];
+#pragma unroll
+            for (int i = 0; i < 3; i++) {
+                U0[i] = as_pairs(w.aU[d0])[i]; U1[i] = as_pairs(w.aU[d0 + 1])[i]; U2[i] = as_pairs(w.aU[d0 + 2])[i];
+                S0[i] = as_pairs(w.S[d0])[i]; S1[i] = as_pairs(w.S[d0 + 1])[i]; S2[i] = as_pairs(w.S[d0 + 2])[i];
+            }
+            const Real au0 = w.au[d0], au1 = w.au[d0 + 1], au2 = w.au[d0 + 2];
+            const Real x0 = au0 - pdot6(U0, a), x1 = au1 - pdot6(U1, a), x2 = au2 - pdot6(U2, a);
             if (r == 0) { x[d0] = sg * x0; x[d0 + 1] = sg * x1; x[d0 + 2] = sg * x2; }
-            paxpy6(x0, as_pairs(w.S[d0]), a); paxpy6(x1, as_pairs(w.S[d0 + 1]), a); paxpy6(x2, as_pairs(w.S[d0 + 2]), a);
+            paxpy6(x0, S0, a); paxpy6(x1, S1, a); paxpy6(x2, S2, a);
             if (b == 0 && r == 0) {   // free-joint accelerations from the Pelvis spatial acceleration: qacc_0 = S_0^-1 a = S_0^T a
                 x[0] = a[1].y; x[1] = a[2].x; x[2] = a[2].y;
                 for (int k = 0; k < 3; k++) x[3 + k] = w.S[3 + k][0] * a[0].x + w.S[3 + k][1] * a[0].y + w.S[3 + k][2] * a[1].x;
@@ -1323,7 +1356,9 @@ UHC_DEVNI int substep_dynamics(const Model<Real> &m, const EnvCfg<Real> &cfg, Wo
             else if (with_pd && cfg.rfc_mode == 0) rfc_implicit(cfg, w, fapp);
             kin_rne_forward(m, w, tp);
             project_force(m, w, w.Fb, w.C, Real(1), (const Real *)nullptr);
+            PCLK(cta_sync, w, PC_KIN);
             collide(m, w, tp);
+            PCLK(cta_sync, w, PC_COLLIDE);
             LANES_BEGIN
             for (int i = lane; i < NV; i += 32) {  // smooth acceleration a_s = M^-1 (tau + f_applied - C)
                 Real f = -w.C[i];
@@ -1344,9 +1379,15 @@ UHC_DEVNI int substep_dynamics(const Model<Real> &m, const EnvCfg<Real> &cfg, Wo
         //      Newton starts from the warm start and only needs f_s, not a_s = M^-1 f_s)
         if (!(phase == PH_SMOOTH && (w.ncon > 0 || w.nlim > 0))) aba_solve(m, w, arm_scale, phase == PH_NEWTON, rhs);
         // ---- phase post-processing
-        if (phase == PH_PD) { pd_finish(m, cfg, w, it, torque_out); phase = PH_SMOOTH; UHC_CTA_SYNC(cta_sync); }
-        else if (phase == PH_SMOOTH) {
+        if (phase == PH_PD) {
+            pd_finish(m, cfg, w, it, torque_out); phase = PH_SMOOTH;
+            PCLK(cta_sync, w, PC_PD);
             UHC_CTA_SYNC(cta_sync);
+            PCLK(cta_sync, w, PC_SYNC_PD);
+        } else if (phase == PH_SMOOTH) {
+            PCLK(cta_sync, w, PC_SMOOTH);
+            UHC_CTA_SYNC(cta_sync);
+            PCLK(cta_sync, w, PC_SYNC_SMOOTH);
             if (w.ncon == 0 && w.nlim == 0) {
                 LANES_BEGIN
                 for (int i = lane; i < NV; i += 32) w.a[i] = w.as_[i];
@@ -1356,8 +1397,13 @@ UHC_DEVNI int substep_dynamics(const Model<Real> &m, const EnvCfg<Real> &cfg, Wo
                 constraint_setup(m, w);
                 scale = newton_init(m, w, tp, &gn2);
             }
+            PCLK(cta_sync, w, PC_CSETUP);
             phase = PH_NEWTON;
-        } else if (newton_advance(m, w, tp, &gn2)) done = true;
+        } else {
+            PCLK(cta_sync, w, PC_NEWTON_ABA);
+            if (newton_advance(m, w, tp, &gn2)) done = true;
+            PCLK(cta_sync, w, PC_NEWTON_ROWS);
+        }
     }
     return iters;
 }

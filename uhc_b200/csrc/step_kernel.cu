@@ -270,6 +270,9 @@ template <class Real> static int build_view(UhcEngine *e, EngineView<Real> &ev, 
     ev.ep_log = el; ev.ep_start_log = el + (size_t)2 * e->E;
     ev.cur.pct = nullptr; ev.cur.start = nullptr; ev.cur.meta = nullptr; ev.cur.max_freq = 0; ev.cur.fit_clip = -1; ev.cur.prec_freq = 0.f;
     ev.state = st; ev.istate = is; ev.expert = nullptr; ev.clip_adr = nullptr; ev.clip_shape = nullptr; ev.clip_model = nullptr; ev.clip_cdf = nullptr;
+#ifdef UHC_PHASE_CLOCKS
+    ev.phase_cyc = nullptr;
+#endif
     return 0;
 }
 
@@ -617,6 +620,18 @@ int uhc_env_reset(UhcEngine *e, int n, const int *env_ids_host, const int *clip_
     e->launches++;
     return 0;
 }
+
+#ifdef UHC_PHASE_CLOCKS
+// Builds with -DUHC_PHASE_CLOCKS only (scripts/step_phase_cycles.py; not part of the library's API): from the next launch on, every warp of
+// k_env_step adds the clock64() cycles of each phase of its control step (sim_core.h, PC_*) to buf[env][phase] -- device memory of
+// E x NPHASE int64 the caller zeroes; null stops the accounting.  Returns NPHASE.  Graphs captured before this call keep the old view.
+int uhc_phase_clocks(UhcEngine *e, long long *buf) {
+    if (!e) { uhc_err() = "uhc_phase_clocks: bad argument"; return -2; }
+    e->evf.phase_cyc = buf; e->evd.phase_cyc = buf;
+    e->view_gen++;
+    return NPHASE;
+}
+#endif
 
 int uhc_env_step(UhcEngine *e, const float *actions_dev, float *obs_dev, float *reward_dev, float *cinfo_dev, int *fail_dev, int *end_dev,
                  float *percent_dev, float *torque_dev, void *stream) {
