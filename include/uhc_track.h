@@ -14,6 +14,7 @@
 #define UHC_TRACK_H
 #include "uhc_b200.h"
 #include "uhc_rollout.h"
+#include "uhc_subject.h"
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -53,6 +54,30 @@ int uhc_track_obs(UhcEngine *e, float *obs_dev, void *stream);
 int uhc_track_state(UhcEngine *e, int *out_host);
 /* frees the stream buffers and graphs; the clip table stays loaded (its rows are whatever the windows held) */
 void uhc_track_end(UhcEngine *e);
+/* CUDA graphs the tracker of this engine holds now (read-only; tests) */
+int uhc_track_graph_count(const UhcEngine *e);
+
+/* Run-time subjects: each env simulates and follows its own body, built on the device from SMPL beta and gender (include/uhc_subject.h), as
+ * the reference rebuilds its humanoid for every sequence (HumanoidEnv.load_expert -> reset_robot).
+ *
+ * uhc_track_subjects_enable uploads `basis` (for the engine's variant 0) and, on the first call, reserves one extra shape variant per env,
+ * slot nshape + env, in every per-variant table of the engine: body_f and hull in the engine's precision, the FK's fp64 body table, and the
+ * hull in fp64 for the floor measurements.  Each slot starts as a copy of variant 0.  Memory: per env 24 x 20 + nvert x 3 values of the
+ * engine's precision, 24 x 6 + nvert x 3 doubles.  The tables move, so the graphs of the rollout, the evaluation and the tracker captured
+ * before are dropped, never replayed.  Call it before uhc_track_begin: -2 while tracking is active, or for a basis uhc_subject_bodies
+ * refuses (nothing changes then); a later call replaces the basis and keeps the slots. */
+int uhc_track_subjects_enable(UhcEngine *e, const UhcSubjectBasis *basis);
+/* While tracking on an enabled engine: for each listed env, its body from beta[:10] and the gender (shape_host [n][17] = beta 16, gender code
+ * 0 neutral / 1 male / 2 female), by uhc_subject_bodies' code, written into its slot of every table (the engine-precision values rounded as
+ * uhc_engine_create rounds them); its clip model and FK variant become the slot, its shape observation the row, and its record is
+ * invalidated: it is not stepped until uhc_track_reset builds its rows with the new body's FK.  The other envs are untouched, and tracker
+ * steps replay the same graphs (the tables keep their addresses).  The call synchronises `stream` once, after the build: -2 with every table
+ * as before for an inverted body (det A <= 0), and, with nothing launched, for env ids out of range or listed twice, a non-finite value, a
+ * gender without a basis, or an engine that is not tracking or not enabled. */
+int uhc_track_set_subjects(UhcEngine *e, int n, const int *env_ids_host, const double *shape_host, void *stream);
+/* env's slot as the engine holds it, each output optional (NULL: skipped): body_f [24][20] and hull [nvert][3] in the engine's precision widened
+ * to fp64, the FK's body rows [24][6] (offset, ipos) and the fp64 hull of the floor measurements [nvert][3].  Synchronises the device. */
+int uhc_track_subject_tables(UhcEngine *e, int env, double *body_f_host, double *hull_host, double *fk_body_host, double *hull64_host);
 
 #ifdef __cplusplus
 }

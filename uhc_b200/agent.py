@@ -592,7 +592,8 @@ class BatchedAgent:
 
     def tracker(self, window=8, kind="qpos", fail_safe=True, **kw):
         """this agent's policy as a batched physics tracker of streamed target frames (uhc_b200/tracker.py); it takes over the engine's
-        clip table until the next load_clips / load_motions.  The cfg must be a test-mode one: auto_reset off, trail_steps >= 1."""
+        clip table until the next load_clips / load_motions.  The cfg must be a test-mode one: auto_reset off, trail_steps >= 1.  subjects=
+        a subject_body.SubjectBasis lets Tracker.set_subjects give each env its own body at run time."""
         from .tracker import Tracker
         return Tracker(self, window, kind, fail_safe, **kw)
 

@@ -25,6 +25,8 @@ cudaError_t launch_reseat(UhcEngine *e, int n, const int *reseat, cudaStream_t s
 // changes whenever the sampler's curriculum view (rings, fit_clip, prec_freq, CDF pointer under the curriculum) changes; the rollout's
 // graphs are keyed on it                                                                                                   // step_kernel.cu
 unsigned long long curriculum_gen(const UhcEngine *e);
+// destroys the rollout's cached graphs (their keys do not cover the engine view): for a change that moves the engine's model tables
+void drop_rollout_graphs(UhcEngine *e);                                                      // rollout.cu
 // the policy of a rollout as a flat net list: one MLP (PolicyGaussian, nprim = 0: nets[0]) or a PolicyMCP mixture (nets[0 .. nprim-1] =
 // primitives, nets[nprim] = composer).  Zeroed before it is filled, so its bytes can go into a graph key
 struct Policy { int nprim; int pad; UhcMlp nets[UHC_MCP_MAX_PRIM + 1]; };

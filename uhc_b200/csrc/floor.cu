@@ -26,7 +26,8 @@ namespace {
 constexpr int WARPS = 4;   // frames per block
 constexpr unsigned FULL = 0xffffffffu;
 
-struct FloorDev { const double *vert; const unsigned char *vbody; int nvert; };   // vert = [nshape][nvert][3]
+// vert = [nshape][nvert][3]; variant nshape + env is env's run-time subject (uhc_track_set_subjects), whose vertices are slot [env][nvert][3]
+struct FloorDev { const double *vert; const unsigned char *vbody; int nvert, nshape; const double *slot; };
 
 struct FloorCtx {
     UhcEngine *eng = nullptr;
@@ -43,9 +44,13 @@ FloorCtx *find_ctx(const UhcEngine *e) {
     return nullptr;
 }
 
+// the hulls of a launch whose variants may be the engine's clip models, which point the tracker's envs at their run-time subjects
+FloorDev with_slots(const FloorCtx *c, const UhcEngine *e) { FloorDev d = c->dev; d.slot = trackx::slot_hulls(e); return d; }
+
 // steps 2 - 4 of floor_core.h for the warp's frame: cur / prev = the poses lanes 0 / 1 placed (prev null: no previous frame)
 __device__ __forceinline__ void warp_frame(const FloorDev &d, int variant, const double *cur, const double *prev, int lane, double *out) {
-    const floorm::Hull h{d.vert + (size_t)variant * d.nvert * 3, d.vbody, d.nvert};
+    const double *v = variant < d.nshape ? d.vert + (size_t)variant * d.nvert * 3 : d.slot + (size_t)(variant - d.nshape) * d.nvert * 3;
+    const floorm::Hull h{v, d.vbody, d.nvert};
     floorm::Part p;
     floorm::lane_part(h, cur, prev, lane, &p);
     for (int off = floorm::LANES / 2; off > 0; off >>= 1) {
@@ -156,9 +161,9 @@ cudaError_t launch_eval_floor(UhcEngine *e, int precision, const void *state, co
     const motion::MotionModel &m = trackx::motion_model(e);
     const unsigned blocks = (unsigned)((n + WARPS - 1) / WARPS);
     if (precision == 32)
-        k_eval_floor<float><<<blocks, 32 * WARPS, 0, st>>>(m, c->dev, (const float *)state, istate, clip_model, clips, done, prev, n, window, slot, win_floor);
+        k_eval_floor<float><<<blocks, 32 * WARPS, 0, st>>>(m, with_slots(c, e), (const float *)state, istate, clip_model, clips, done, prev, n, window, slot, win_floor);
     else
-        k_eval_floor<double><<<blocks, 32 * WARPS, 0, st>>>(m, c->dev, (const double *)state, istate, clip_model, clips, done, prev, n, window, slot, win_floor);
+        k_eval_floor<double><<<blocks, 32 * WARPS, 0, st>>>(m, with_slots(c, e), (const double *)state, istate, clip_model, clips, done, prev, n, window, slot, win_floor);
     return cudaGetLastError();
 }
 
@@ -197,7 +202,7 @@ int uhc_floor_init(UhcEngine *e, const UhcFloorHulls *h) {
     uhc_floor_release(e);
     FloorCtx *c = new FloorCtx();
     c->eng = e; c->nshape = h->nshape; c->gen = ++g_fl_gen; c->d_vert = d_vert; c->d_vbody = d_vbody;
-    c->dev = FloorDev{d_vert, d_vbody, h->nvert};
+    c->dev = FloorDev{d_vert, d_vbody, h->nvert, h->nshape, nullptr};
     g_fl.push_back(c);
     return 0;
 }
@@ -249,9 +254,9 @@ int uhc_track_floor(UhcEngine *e, const void *state_out_dev, double *out_dev, vo
     const unsigned blocks = (unsigned)((R.E + WARPS - 1) / WARPS);
     cudaStream_t st = (cudaStream_t)stream;
     if (R.precision == 32)
-        k_floor_qpos<float><<<blocks, 32 * WARPS, 0, st>>>(m, c->dev, (const float *)state_out_dev, R.E, UHC_TRACK_OUT, trackx::clip_models(e), nullptr, false, out_dev);
+        k_floor_qpos<float><<<blocks, 32 * WARPS, 0, st>>>(m, with_slots(c, e), (const float *)state_out_dev, R.E, UHC_TRACK_OUT, trackx::clip_models(e), nullptr, false, out_dev);
     else
-        k_floor_qpos<double><<<blocks, 32 * WARPS, 0, st>>>(m, c->dev, (const double *)state_out_dev, R.E, UHC_TRACK_OUT, trackx::clip_models(e), nullptr, false, out_dev);
+        k_floor_qpos<double><<<blocks, 32 * WARPS, 0, st>>>(m, with_slots(c, e), (const double *)state_out_dev, R.E, UHC_TRACK_OUT, trackx::clip_models(e), nullptr, false, out_dev);
     CK(cudaGetLastError());
     return 0;
 }

@@ -442,6 +442,14 @@ int uhc_rollout_env_step_ms(UhcEngine *e, int row, float *ms) {
 
 int uhc_rollout_launches_per_step(UhcEngine *e) { return e ? ctx_of(e)->launches_per_step : -1; }
 
+}  // extern "C"
+
+void uhc::evalx::drop_rollout_graphs(UhcEngine *e) {
+    for (RolloutCtx *c : g_ctx) if (c->eng == e) c->graphs.clear();
+}
+
+extern "C" {
+
 void uhc_rollout_release(UhcEngine *e) {   // called by the binding before uhc_engine_destroy
     for (size_t i = 0; i < g_ctx.size(); i++) if (g_ctx[i]->eng == e) {
         RolloutCtx *c = g_ctx[i];

@@ -15,6 +15,7 @@
 #include "curriculum_core.h"
 #include "track_obs.h"
 #include "track_glue.h"
+#include "subject_glue.h"
 
 using namespace uhc;
 
@@ -210,6 +211,12 @@ struct UhcEngine {
     size_t cur_cnt_cap = 0, cur_rank_cap = 0;
     int *d_reseed = nullptr;       // [4][E] ids / clip / start / len of uhc_curriculum_reseed
     int *d_push = nullptr; int push_cap = 0;   // [3][n] clip / percent bits / start of uhc_curriculum_push
+    // variant 0 of the model in fp64 on the host: the base of the run-time subject builder
+    std::vector<double> base_bf, base_hull, base_dof; std::vector<int> base_hull_adr, base_hull_num, base_parent, base_sub_end;
+    // run-time subjects (uhc_track_subjects_enable): nslot = E once enabled, and variant nshape + env of body_f / hull / mo_model.body is env's
+    // own body; d_slot_hull holds the same hulls in fp64 ([E][nvert][3], the floor measurements' vertices)
+    subjx::Builder *subj = nullptr; int nslot = 0;
+    double *d_slot_hull = nullptr;
 };
 
 template <class T> static int dev_copy(UhcEngine *e, T **dst, const T *src, size_t n) {
@@ -304,6 +311,10 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
     e->E = num_envs; e->device = device; e->precision = precision; e->launches = 0; e->nshape = model->nshape > 0 ? model->nshape : 1;
     int rc = precision == 32 ? build_view<float>(e, e->evf, model, cfg) : build_view<double>(e, e->evd, model, cfg);
     if (rc) { delete e; return rc; }
+    e->base_bf.assign(model->body_f, model->body_f + NB * BODYF); e->base_hull.assign(model->hull, model->hull + (size_t)model->nvert * 3);
+    e->base_dof.assign(model->dof_f, model->dof_f + NV * 4);
+    e->base_hull_adr.assign(model->hull_adr, model->hull_adr + NB); e->base_hull_num.assign(model->hull_num, model->hull_num + NB);
+    e->base_parent.assign(model->parent, model->parent + NB); e->base_sub_end.assign(model->body_sub_end, model->body_sub_end + NB);
     {   // the motion library's FK reads the bone offsets / com positions of every shape variant in fp64, whatever the engine's precision
         std::vector<double> body((size_t)e->nshape * NB * motion::BODY6);
         motion::motion_body_table(model->body_f, BODYF, e->nshape, body.data());
@@ -356,6 +367,8 @@ void uhc_engine_destroy(UhcEngine *e) {
     if (e->d_gather) cudaFree(e->d_gather);
     if (e->d_gather_i) cudaFree(e->d_gather_i);
     for (void *p : {(void *)e->cur.pct, (void *)e->cur.start, (void *)e->cur.meta, (void *)e->cur.p, (void *)e->cur.cnt, (void *)e->cur.rank, (void *)e->cur.ncl, (void *)e->d_reseed, (void *)e->d_push}) if (p) cudaFree(p);
+    if (e->d_slot_hull) cudaFree(e->d_slot_hull);
+    subjx::builder_free(e->subj);
     delete e;
 }
 
@@ -995,6 +1008,10 @@ int install_table(UhcEngine *e, int H, const int *fk_model, const double *shape)
     if (!shape) { shp.assign((size_t)E * 17, 0.0); shape = shp.data(); }
     if (new_clip_table(e, E, lens.data(), shape)) return -1;
     if (fk_model && uhc_set_clip_models(e, E, fk_model)) return -1;
+    if (!fk_model && e->nslot) {                // uhc_track_set_subjects points single envs at their slots
+        const std::vector<int> zero(E, 0);
+        if (uhc_set_clip_models(e, E, zero.data())) return -1;
+    }
     const size_t rs = e->precision == 32 ? 4 : 8;
     cudaError_t ce = cudaMemset(e->d_expert, 0, (size_t)E * H * EX_SIZE * rs);
     if (ce == cudaSuccess)
@@ -1008,6 +1025,79 @@ unsigned long long table_gen(const UhcEngine *e) { return e->table_gen; }
 int num_shapes(const UhcEngine *e) { return e->nshape; }
 const motion::MotionModel &motion_model(const UhcEngine *e) { return e->mo_model; }
 const int *clip_models(const UhcEngine *e) { return e->d_clip_model; }
+
+UhcModelHost base_model(const UhcEngine *e) {
+    UhcModelHost m;
+    memset(&m, 0, sizeof m);
+    m.body_f = e->base_bf.data(); m.hull = e->base_hull.data(); m.dof_f = e->base_dof.data(); m.nvert = (int)(e->base_hull.size() / 3);
+    m.hull_adr = e->base_hull_adr.data(); m.hull_num = e->base_hull_num.data(); m.parent = e->base_parent.data(); m.body_sub_end = e->base_sub_end.data();
+    m.nshape = 1;
+    return m;
+}
+
+// rows first .. first + n - 1 of a table of `row`-wide rows become copies of row 0
+template <class T>
+__global__ void k_repeat_row(T *__restrict__ t, size_t row, size_t first, int n) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)n * row; i += (size_t)gridDim.x * blockDim.x) t[first * row + i] = t[i % row];
+}
+
+// *tab (an engine allocation of nold rows) -> a new allocation of nold + extra rows, the extra ones copies of row 0; the old one is freed
+template <class T>
+static int grow_table(UhcEngine *e, const T **tab, size_t row, int nold, int extra) {
+    T *d = nullptr;
+    CK(cudaMalloc((void **)&d, row * (nold + extra) * sizeof(T)));
+    e->allocs.push_back(d);
+    CK(cudaMemcpy(d, *tab, row * nold * sizeof(T), cudaMemcpyDeviceToDevice));
+    k_repeat_row<T><<<1024, 256>>>(d, row, nold, extra);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    for (size_t i = 0; i < e->allocs.size(); i++)
+        if (e->allocs[i] == (const void *)*tab) { cudaFree(e->allocs[i]); e->allocs.erase(e->allocs.begin() + i); break; }
+    *tab = d;
+    return 0;
+}
+
+template <class Real>
+static int grow_model(UhcEngine *e, Model<Real> &M) {
+    if (grow_table<Real>(e, &M.body_f, NB * BODYF, e->nshape, e->E) || grow_table<Real>(e, &M.hull, (size_t)M.nvert * 3, e->nshape, e->E)) return -1;
+    M.nshape = e->nshape + e->E;
+    return 0;
+}
+
+int enable_subjects(UhcEngine *e, subjx::Builder *b) {
+    subjx::builder_free(e->subj);
+    e->subj = b;
+    if (e->nslot) return 0;                     // the slots exist: only the basis changes
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());
+    e->view_gen++;                              // the tables move: no graph may replay the old pointers
+    evalx::drop_rollout_graphs(e);
+    if (e->precision == 32 ? grow_model<float>(e, e->evf.model) : grow_model<double>(e, e->evd.model)) return -1;
+    const double *body = e->mo_model.body;
+    if (grow_table<double>(e, &body, NB * motion::BODY6, e->nshape, e->E)) return -1;
+    e->mo_model.body = body;
+    const size_t hv = e->base_hull.size();
+    CK(cudaMalloc((void **)&e->d_slot_hull, hv * e->E * sizeof(double)));
+    CK(cudaMemcpy(e->d_slot_hull, e->base_hull.data(), hv * sizeof(double), cudaMemcpyHostToDevice));
+    k_repeat_row<double><<<1024, 256>>>(e->d_slot_hull, hv, 1, e->E - 1);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    e->nslot = e->E;
+    return 0;
+}
+
+const subjx::Builder *subject_builder(const UhcEngine *e) { return e->nslot ? e->subj : nullptr; }
+
+void slots(UhcEngine *e, Slots *s) {
+    const bool f32 = e->precision == 32;
+    s->nshape = e->nshape; s->nvert = f32 ? e->evf.model.nvert : e->evd.model.nvert; s->precision = e->precision;
+    s->body_f = f32 ? (void *)e->evf.model.body_f : (void *)e->evd.model.body_f;
+    s->hull = f32 ? (void *)e->evf.model.hull : (void *)e->evd.model.hull;
+    s->body6 = const_cast<double *>(e->mo_model.body); s->hull64 = e->d_slot_hull;
+    s->clip_model = e->d_clip_model; s->shape = e->d_shape; s->istate = f32 ? e->evf.istate : e->evd.istate;
+}
+
+const double *slot_hulls(const UhcEngine *e) { return e->d_slot_hull; }
 
 cudaError_t launch_obs(UhcEngine *e, float *obs, cudaStream_t st) {
     const int E = e->E;

@@ -10,6 +10,7 @@
 #include "../../include/uhc_subject.h"
 #include "errors.h"
 #include "subject_core.h"
+#include "subject_glue.h"
 
 using namespace uhc;
 
@@ -131,44 +132,53 @@ struct DeviceScope {                   // the caller's current device is restore
     ~DeviceScope() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
-int run(int device, const UhcModelHost *base, const UhcSubjectBasis *basis, int n, const double *betas, const int *gender, double *body_f,
-        double *hull, double *maps) {
+// the builder's inputs on the current device: variant 0 of base and every gender's basis.  -2 when the hull does not tile into bodies
+int prepare(const UhcModelHost *base, const UhcSubjectBasis *basis, const char *who, SubDev *d, Bufs &B) {
     using namespace subj;
     const int V = base->nvert;
     std::vector<int> vbody((size_t)V, -1);
     for (int b = 0; b < NB; b++)
         for (int k = 0; k < base->hull_num[b]; k++) {
             const long v = (long)base->hull_adr[b] + k;
-            if (v < 0 || v >= V) { uhc_err() = "uhc_subject_bodies: hull_adr / hull_num outside the hull"; return -2; }
+            if (v < 0 || v >= V) { uhc_err() = std::string(who) + ": hull_adr / hull_num outside the hull"; return -2; }
             vbody[(size_t)v] = b;
         }
     for (int v = 0; v < V; v++)
-        if (vbody[(size_t)v] < 0) { uhc_err() = "uhc_subject_bodies: a hull vertex belongs to no body"; return -2; }
+        if (vbody[(size_t)v] < 0) { uhc_err() = std::string(who) + ": a hull vertex belongs to no body"; return -2; }
     std::vector<double> arm(NV);
     for (int i = 0; i < NV; i++) arm[(size_t)i] = base->dof_f[4 * i];
-    DeviceScope scope;
-    CK(cudaGetDevice(&scope.prev));
-    CK(cudaSetDevice(device));
-    Bufs B;
-    SubDev d{};
-    d.nvert = V;
+    *d = SubDev{};
+    d->nvert = V;
     for (int b = 0; b < NB; b++) {
-        d.parent[b] = base->parent[b]; d.sub_end[b] = base->body_sub_end[b]; d.hull_adr[b] = base->hull_adr[b]; d.hull_num[b] = base->hull_num[b];
+        d->parent[b] = base->parent[b]; d->sub_end[b] = base->body_sub_end[b]; d->hull_adr[b] = base->hull_adr[b]; d->hull_num[b] = base->hull_num[b];
     }
     double *bf0, *hull0, *armd; int *vb;
     CK(B.up(&bf0, base->body_f, (size_t)NB * BODYF));
     CK(B.up(&hull0, base->hull, (size_t)V * 3));
     CK(B.up(&armd, arm.data(), arm.size()));
     CK(B.up(&vb, vbody.data(), vbody.size()));
-    d.bf0 = bf0; d.hull0 = hull0; d.armature = armd; d.vbody = vb;
+    d->bf0 = bf0; d->hull0 = hull0; d->armature = armd; d->vbody = vb;
     for (int g = 0; g < 3; g++) {
-        d.map[g] = d.off[g] = nullptr;
+        d->map[g] = d->off[g] = nullptr;
         if (!basis->map[g]) continue;
         double *m, *o;
         CK(B.up(&m, basis->map[g], (size_t)NB * NTERM * MAPW));
         CK(B.up(&o, basis->offset[g], (size_t)NB * NTERM * 3));
-        d.map[g] = m; d.off[g] = o;
+        d->map[g] = m; d->off[g] = o;
     }
+    return 0;
+}
+
+int run(int device, const UhcModelHost *base, const UhcSubjectBasis *basis, int n, const double *betas, const int *gender, double *body_f,
+        double *hull, double *maps) {
+    using namespace subj;
+    const int V = base->nvert;
+    DeviceScope scope;
+    CK(cudaGetDevice(&scope.prev));
+    CK(cudaSetDevice(device));
+    Bufs B;
+    SubDev d;
+    if (const int rc = prepare(base, basis, "uhc_subject_bodies", &d, B)) return rc;
     const int cap = n < CHUNK ? n : CHUNK;
     double *be, *bfo, *hu, *mp = nullptr; int *ge, *bad;
     CK(B.alloc(&be, (size_t)cap * NBETA));
@@ -224,4 +234,33 @@ extern "C" int uhc_subject_bodies(int device, const UhcModelHost *base, const Uh
             if (!isfinite(betas_host[(size_t)r * NBETA + l])) { uhc_err() = "uhc_subject_bodies: subject " + std::to_string(r) + ": non-finite beta"; return -2; }
     }
     return run(device, base, basis, n, betas_host, gender_host, body_f_host, hull_host, maps_host_or_null);
+}
+
+// ---- the builder of the tracker's run-time subjects (subject_glue.h): k_subject over rows already on the device
+struct uhc::subjx::Builder {
+    SubDev d;
+    Bufs B;
+};
+
+int uhc::subjx::builder_create(const UhcModelHost *base, const UhcSubjectBasis *basis, const char *who, Builder **out) {
+    if (!base || !basis || !base->body_f || !base->hull || !base->dof_f || !base->hull_adr || !base->hull_num || !base->parent ||
+        !base->body_sub_end || base->nvert < 1) {
+        uhc_err() = std::string(who) + ": null pointer"; return -2;
+    }
+    for (int g = 0; g < 3; g++)
+        if (!basis->map[g] != !basis->offset[g]) { uhc_err() = std::string(who) + ": gender " + std::to_string(g) + " has one of its two bases"; return -2; }
+    if (!basis->map[0] && !basis->map[1] && !basis->map[2]) { uhc_err() = std::string(who) + ": the basis has no gender"; return -2; }
+    Builder *b = new Builder();
+    if (const int rc = prepare(base, basis, who, &b->d, b->B)) { delete b; return rc; }
+    *out = b;
+    return 0;
+}
+
+void uhc::subjx::builder_free(Builder *b) { delete b; }
+bool uhc::subjx::has_gender(const Builder *b, int g) { return g >= 0 && g < 3 && b->d.map[g] != nullptr; }
+int uhc::subjx::nvert(const Builder *b) { return b->d.nvert; }
+
+cudaError_t uhc::subjx::launch(const Builder *b, int n, const double *betas, const int *gender, double *body_f, double *hull, int *bad, cudaStream_t st) {
+    k_subject<<<(unsigned)n, NT, 0, st>>>(b->d, betas, gender, body_f, hull, nullptr, bad);
+    return cudaGetLastError();
 }

@@ -8,6 +8,9 @@
 //   k_track_post                             per env: the gated record restored, step count, fail_safe flag, the state gathered
 //   k_eval_reseat (fail_safe only)           uhc_eval_run's re-seat on row cur_t
 //
+// Run-time subjects (uhc_track_set_subjects): k_subject (subject.cu) builds the bodies into a staging area, the host reads the inverted-body
+// flags once, then k_subject_install writes each env's slot of the engine's tables (track_glue.h Slots) and points the env at it.
+//
 // Compiled on its own with -fmad=false (uhc_b200/build.py) like motion_lib.cu: the rows restate motion_lib.py's fp64 arithmetic and
 // must equal uhc_load_motions' rows bit for bit.
 #include <cuda_runtime.h>
@@ -21,6 +24,8 @@
 #include "track_glue.h"
 #include "track_core.h"
 #include "sim_core.h"
+#include "subject_core.h"
+#include "subject_glue.h"
 
 using namespace uhc;
 
@@ -98,6 +103,24 @@ __global__ void __launch_bounds__(128) k_track_post(const Real *__restrict__ sta
 
 __global__ void k_fill_ones(unsigned char *p, int n) { const int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = 1; }
 
+// one block per staged subject i: env ids[i]'s slot v = nshape + env of every table gets body i (the engine-precision tables rounded as
+// uhc_engine_create's upload rounds, the FK table = body_f columns 0:6 as motion_body_table takes them), the env's clip model and FK variant
+// become v, its shape row shape[i], and its record is invalidated until uhc_track_reset
+template <class Real>
+__global__ void k_subject_install(int n, const int *__restrict__ ids, int nshape, int nvert, const double *__restrict__ bf, const double *__restrict__ hull,
+                                  const double *__restrict__ shape, Real *__restrict__ body_f, Real *__restrict__ hull_t, double *__restrict__ body6,
+                                  double *__restrict__ hull64, int *__restrict__ clip_model, int *__restrict__ fk, Real *__restrict__ clip_shape,
+                                  int *__restrict__ istate) {
+    using subj::BODYF; using subj::NB;
+    const int i = blockIdx.x, env = ids[i], v = nshape + env;
+    const double *b = bf + (size_t)i * NB * BODYF, *h = hull + (size_t)i * nvert * 3;
+    for (int k = threadIdx.x; k < NB * BODYF; k += blockDim.x) body_f[(size_t)v * NB * BODYF + k] = (Real)b[k];
+    for (int k = threadIdx.x; k < NB * motion::BODY6; k += blockDim.x) body6[(size_t)v * NB * motion::BODY6 + k] = b[k / motion::BODY6 * BODYF + k % motion::BODY6];
+    for (int k = threadIdx.x; k < nvert * 3; k += blockDim.x) { hull_t[(size_t)v * nvert * 3 + k] = (Real)h[k]; hull64[(size_t)env * nvert * 3 + k] = h[k]; }
+    if (threadIdx.x < 17) clip_shape[(size_t)env * 17 + threadIdx.x] = (Real)shape[(size_t)i * 17 + threadIdx.x];
+    if (threadIdx.x == 0) { clip_model[env] = v; fk[env] = v; istate[(size_t)env * SI_SIZE + SI_LEN] = 0; }
+}
+
 // every argument of a step that reaches a kernel; zeroed, then filled: its bytes are the graph's key
 struct TrackKey {
     int has_next, has_mask, fail_safe; float zclip; evalx::Policy pol; const float *log_std; const double *zstats; void *out; float *rew; int *fail;
@@ -113,6 +136,9 @@ struct TrackCtx {
     cudaEvent_t ids_done = nullptr;                // the last k_track_rows that read d_ids has been enqueued before it
     std::vector<int> zeros, lens;                  // reset arguments of uhc_env_reset (start 0, length H)
     GraphCache graphs{32};                         // one step each (graph_cache.h)
+    // staging of uhc_track_set_subjects, grown to the largest call: betas [n][10], shape rows [n][17], built body_f / hull, flags, ids, genders
+    double *d_sbeta = nullptr, *d_sshape = nullptr, *d_sbf = nullptr, *d_shull = nullptr; int *d_sbad = nullptr, *d_sids = nullptr, *d_sgender = nullptr;
+    int s_cap = 0;
 };
 std::vector<TrackCtx *> g_tr;
 unsigned long long g_tr_gen = 0;                   // distinct per begin: graphs never outlive the buffers they hold
@@ -122,7 +148,8 @@ void free_ctx(TrackCtx *c) {
     cudaDeviceSynchronize();
     c->graphs.clear();
     for (void *p : {(void *)c->d_raw, (void *)c->d_next, (void *)c->d_have, (void *)c->d_steps, (void *)c->d_dropped, (void *)c->d_status, (void *)c->d_reseat,
-                    (void *)c->d_mask, (void *)c->d_fk, (void *)c->d_ids, (void *)c->d_ones}) if (p) cudaFree(p);
+                    (void *)c->d_mask, (void *)c->d_fk, (void *)c->d_ids, (void *)c->d_ones, (void *)c->d_sbeta, (void *)c->d_sshape, (void *)c->d_sbf,
+                    (void *)c->d_shull, (void *)c->d_sbad, (void *)c->d_sids, (void *)c->d_sgender}) if (p) cudaFree(p);
     if (c->h_ids) cudaFreeHost(c->h_ids);
     if (c->ids_done) cudaEventDestroy(c->ids_done);
     for (size_t i = 0; i < g_tr.size(); i++) if (g_tr[i] == c) { g_tr.erase(g_tr.begin() + i); break; }
@@ -224,7 +251,11 @@ int uhc_track_begin(UhcEngine *e, int window, int kind, int pose_dim, const int 
     CK(cudaMalloc((void **)&c->d_ones, En));
     k_fill_ones<<<(E + 255) / 256, 256>>>(c->d_ones, E);
     CK(cudaGetLastError());
-    if (fk_model_host) { CK(cudaMalloc((void **)&c->d_fk, En * sizeof(int))); CK(cudaMemcpy(c->d_fk, fk_model_host, En * sizeof(int), cudaMemcpyHostToDevice)); }
+    if (fk_model_host || trackx::subject_builder(e)) {     // with run-time subjects every env's FK variant can change, at a fixed address
+        CK(cudaMalloc((void **)&c->d_fk, En * sizeof(int)));
+        if (fk_model_host) CK(cudaMemcpy(c->d_fk, fk_model_host, En * sizeof(int), cudaMemcpyHostToDevice));
+        else CK(cudaMemset(c->d_fk, 0, En * sizeof(int)));
+    }
     CK(cudaHostAlloc((void **)&c->h_ids, En * sizeof(int), cudaHostAllocDefault));
     CK(cudaEventCreateWithFlags(&c->ids_done, cudaEventDisableTiming));
     CK(cudaDeviceSynchronize());
@@ -309,6 +340,97 @@ int uhc_track_state(UhcEngine *e, int *out_host) {
 
 void uhc_track_end(UhcEngine *e) {
     if (TrackCtx *c = e ? find_ctx(e) : nullptr) free_ctx(c);
+}
+
+int uhc_track_graph_count(const UhcEngine *e) {
+    for (const TrackCtx *c : g_tr) if (c->eng == e) return (int)c->graphs.size();
+    return 0;
+}
+
+int uhc_track_subjects_enable(UhcEngine *e, const UhcSubjectBasis *basis) {
+    if (!e || !basis) { uhc_err() = "uhc_track_subjects_enable: null argument"; return -2; }
+    if (trackx::tracking(e)) { uhc_err() = "uhc_track_subjects_enable: tracking is active (call it before uhc_track_begin, or after uhc_track_end)"; return -2; }
+    const UhcModelHost base = trackx::base_model(e);
+    subjx::Builder *b = nullptr;
+    if (const int rc = subjx::builder_create(&base, basis, "uhc_track_subjects_enable", &b)) return rc;
+    return trackx::enable_subjects(e, b);
+}
+
+int uhc_track_subject_tables(UhcEngine *e, int env, double *body_f_host, double *hull_host, double *fk_body_host, double *hull64_host) {
+    if (!e || !trackx::subject_builder(e)) { uhc_err() = "uhc_track_subject_tables: run-time subjects are not enabled"; return -2; }
+    if (env < 0 || env >= uhc_num_envs(e)) { uhc_err() = "uhc_track_subject_tables: env id out of range"; return -2; }
+    trackx::Slots s; trackx::slots(e, &s);
+    const size_t v = (size_t)s.nshape + env, nb = (size_t)subj::NB * subj::BODYF, nh = (size_t)s.nvert * 3, rs = s.precision == 32 ? 4 : 8;
+    std::vector<unsigned char> tmp(nh * rs);
+    auto widen = [&](const void *src, size_t n, double *out) -> int {
+        CK(cudaMemcpy(tmp.data(), src, n * rs, cudaMemcpyDeviceToHost));
+        for (size_t k = 0; k < n; k++) out[k] = rs == 4 ? (double)((const float *)tmp.data())[k] : ((const double *)tmp.data())[k];
+        return 0;
+    };
+    CK(cudaDeviceSynchronize());
+    if (body_f_host && widen((const char *)s.body_f + v * nb * rs, nb, body_f_host)) return -1;
+    if (hull_host && widen((const char *)s.hull + v * nh * rs, nh, hull_host)) return -1;
+    if (fk_body_host) CK(cudaMemcpy(fk_body_host, s.body6 + v * subj::NB * motion::BODY6, (size_t)subj::NB * motion::BODY6 * sizeof(double), cudaMemcpyDeviceToHost));
+    if (hull64_host) CK(cudaMemcpy(hull64_host, s.hull64 + (size_t)env * nh, nh * sizeof(double), cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int uhc_track_set_subjects(UhcEngine *e, int n, const int *env_ids_host, const double *shape_host, void *stream) {
+    TrackCtx *c = live_ctx(e, "uhc_track_set_subjects");
+    if (!c) return -2;
+    const subjx::Builder *b = trackx::subject_builder(e);
+    if (!b) { uhc_err() = "uhc_track_set_subjects: run-time subjects are not enabled (uhc_track_subjects_enable before uhc_track_begin)"; return -2; }
+    if (n < 1 || n > c->E || !env_ids_host || !shape_host) { uhc_err() = "uhc_track_set_subjects: needs 1 <= n <= E, env ids and shape rows"; return -2; }
+    std::vector<char> seen(c->E, 0);
+    std::vector<double> beta((size_t)n * subj::NBETA);
+    std::vector<int> gender(n);
+    for (int i = 0; i < n; i++) {
+        const int env = env_ids_host[i];
+        if (env < 0 || env >= c->E || seen[env]) { uhc_err() = "uhc_track_set_subjects: env id out of range or listed twice"; return -2; }
+        seen[env] = 1;
+        const double *r = shape_host + (size_t)i * 17;
+        for (int k = 0; k < 17; k++)
+            if (!isfinite(r[k])) { uhc_err() = "uhc_track_set_subjects: row " + std::to_string(i) + ": non-finite beta or gender"; return -2; }
+        const double g = r[16];
+        if (!(g == 0.0 || g == 1.0 || g == 2.0) || !subjx::has_gender(b, (int)g)) {
+            uhc_err() = "uhc_track_set_subjects: row " + std::to_string(i) + ": gender code " + std::to_string(g) + " has no basis"; return -2;
+        }
+        gender[i] = (int)g;
+        for (int l = 0; l < subj::NBETA; l++) beta[(size_t)i * subj::NBETA + l] = r[l];
+    }
+    const int V = subjx::nvert(b);
+    if (c->s_cap < n) {
+        for (void *p : {(void *)c->d_sbeta, (void *)c->d_sshape, (void *)c->d_sbf, (void *)c->d_shull, (void *)c->d_sbad, (void *)c->d_sids, (void *)c->d_sgender}) if (p) cudaFree(p);
+        c->d_sbeta = c->d_sshape = c->d_sbf = c->d_shull = nullptr; c->d_sbad = c->d_sids = c->d_sgender = nullptr; c->s_cap = 0;
+        const size_t N = n;
+        CK(cudaMalloc((void **)&c->d_sbeta, N * subj::NBETA * sizeof(double))); CK(cudaMalloc((void **)&c->d_sshape, N * 17 * sizeof(double)));
+        CK(cudaMalloc((void **)&c->d_sbf, N * subj::NB * subj::BODYF * sizeof(double))); CK(cudaMalloc((void **)&c->d_shull, N * V * 3 * sizeof(double)));
+        for (int **p : {&c->d_sbad, &c->d_sids, &c->d_sgender}) CK(cudaMalloc((void **)p, N * sizeof(int)));
+        c->s_cap = n;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    CK(cudaMemcpyAsync(c->d_sbeta, beta.data(), beta.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_sgender, gender.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_sshape, shape_host, (size_t)n * 17 * sizeof(double), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_sids, env_ids_host, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+    CK(subjx::launch(b, n, c->d_sbeta, c->d_sgender, c->d_sbf, c->d_shull, c->d_sbad, st));
+    std::vector<int> bad(n);
+    CK(cudaMemcpyAsync(bad.data(), c->d_sbad, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));         // the one synchronise: an inverted body is refused before any table is written
+    for (int i = 0; i < n; i++)
+        if (bad[i]) {
+            uhc_err() = "uhc_track_set_subjects: row " + std::to_string(i) + ": the map of body " + std::to_string(bad[i] - 1) + " inverts it (det A <= 0)";
+            return -2;
+        }
+    trackx::Slots s; trackx::slots(e, &s);
+    if (s.precision == 32)
+        k_subject_install<float><<<n, 256, 0, st>>>(n, c->d_sids, s.nshape, s.nvert, c->d_sbf, c->d_shull, c->d_sshape, (float *)s.body_f, (float *)s.hull,
+                                                     s.body6, s.hull64, s.clip_model, c->d_fk, (float *)s.shape, s.istate);
+    else
+        k_subject_install<double><<<n, 256, 0, st>>>(n, c->d_sids, s.nshape, s.nvert, c->d_sbf, c->d_shull, c->d_sshape, (double *)s.body_f, (double *)s.hull,
+                                                      s.body6, s.hull64, s.clip_model, c->d_fk, (double *)s.shape, s.istate);
+    CK(cudaGetLastError());
+    return 0;
 }
 
 }  // extern "C"

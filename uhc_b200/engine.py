@@ -834,6 +834,34 @@ class Engine:
     def track_end(self):
         self.lib.uhc_track_end(self.h)
 
+    @property
+    def track_graph_count(self):
+        """CUDA graphs the tracker holds for this engine now (uhc_track_graph_count)"""
+        return int(self.lib.uhc_track_graph_count(self.h))
+
+    def track_subjects_enable(self, basis):
+        """run-time subjects (uhc_track_subjects_enable): one extra shape variant per env, filled by track_set_subjects; basis = a
+        subject_body.SubjectBasis of this engine's model.  Before track_begin."""
+        s = basis.struct()
+        _chk(self.lib.uhc_track_subjects_enable(self.h, C.byref(s)), "uhc_track_subjects_enable", ValueError)
+
+    def track_subject_tables(self, env):
+        """env's run-time subject slot (uhc_track_subject_tables): dict(body_f [24][20], hull [nvert][3]) in the engine's precision widened to
+        float64, fk_body [24][6] and hull64 [nvert][3] in float64"""
+        nv = len(self.model.hull)
+        out = dict(body_f=np.zeros((24, 20)), hull=np.zeros((nv, 3)), fk_body=np.zeros((24, 6)), hull64=np.zeros((nv, 3)))
+        d = lambda k: out[k].ctypes.data_as(C.POINTER(C.c_double))
+        _chk(self.lib.uhc_track_subject_tables(self.h, C.c_int(int(env)), d("body_f"), d("hull"), d("fk_body"), d("hull64")),
+             "uhc_track_subject_tables", ValueError)
+        return out
+
+    def track_set_subjects(self, env_ids, shapes):
+        """each listed env's own body from its shape row [17] = beta 16, gender code (uhc_track_set_subjects); track_reset those envs next"""
+        ids = np.ascontiguousarray(env_ids, np.int32).reshape(-1)
+        shp = np.ascontiguousarray(np.asarray(shapes, np.float64).reshape(len(ids), 17))
+        _chk(self.lib.uhc_track_set_subjects(self.h, C.c_int(len(ids)), _ip_out(ids), shp.ctypes.data_as(C.POINTER(C.c_double)), self._stream()),
+             "uhc_track_set_subjects", ValueError)
+
     def set_clip_weights(self, weights=None):
         """sampling weights of the in-kernel re-seeding (None = the reference's sample_keys rule)."""
         if weights is None:

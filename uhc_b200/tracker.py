@@ -9,6 +9,13 @@ previous step has run, the role the UHC policy plays inside HumanoidKinEnv.step 
 
 Each step is one CUDA-graph replay on the device: the new frame's expert record, the observation against it, the policy mean, the
 physics step and fail_safe.  The returned tensors are the tracker's own buffers, overwritten by the next step.
+
+With subjects= (a subject_body.SubjectBasis, e.g. SubjectBasis.from_models over the user's SMPL files) every env can be given its own body
+while the tracker runs, as the reference's reset_robot rebuilds the humanoid for each sequence:
+
+    trk = agent.tracker(window=8, kind="smpl", subjects=basis)
+    trk.set_subjects([3], betas=[beta], genders=["female"])   # env 3's body, built on the GPU
+    trk.reset(f0[3:4], f1[3:4], env_ids=[3])                  # its rows from the new body's FK; the other envs keep stepping
 """
 import numpy as np
 
@@ -16,10 +23,12 @@ from . import nn
 
 
 class Tracker:
-    def __init__(self, agent, window=8, kind="qpos", fail_safe=True, pose_dim=None, fk_models=None, shapes=None):
+    def __init__(self, agent, window=8, kind="qpos", fail_safe=True, pose_dim=None, fk_models=None, shapes=None, subjects=None):
         import torch
         self.torch, self.agent, self.engine = torch, agent, agent.engine
         self.E, self.fail_safe = agent.E, bool(fail_safe)
+        if subjects is not None:
+            self.engine.track_subjects_enable(subjects)
         self.engine.track_begin(window, kind, pose_dim, fk_models, shapes)
         self.row_w = self.engine.track_row_w
         dev = agent.dev
@@ -39,6 +48,20 @@ class Tracker:
         cvt = lambda x: None if x is None else t.as_tensor(x).to(device=self.state.device, dtype=t.float32).contiguous()
         self.engine.track_reset(ids, frames, cvt(qpos), cvt(qvel))
         self.agent.obs = None          # the envs left whatever episode they were on
+
+    def set_subjects(self, env_ids, betas, genders):
+        """gives each listed env its own body, built on the device from betas [n][10 .. 16] (the first 10 shape the body, all of them up to 16
+        go into the shape observation) and genders [n] (0 / "neutral", 1 / "male", 2 / "female", DatasetAMASSSingle's codes).  Needs subjects=
+        at construction.  The envs do not step again until reset(..., env_ids=...) gives them frames; the others are untouched."""
+        from uhc.data_loaders.dataset_amass_single import _gender_code
+        ids = np.asarray(env_ids, np.int32).reshape(-1)
+        b = np.asarray(betas, np.float64).reshape(len(ids), -1)
+        if b.shape[1] < 10 or b.shape[1] > 16:
+            raise ValueError("set_subjects: betas must be [n][10 .. 16]")
+        g = [x if isinstance(x, (int, np.integer)) else _gender_code(x) for x in np.asarray(genders, object).reshape(-1)]
+        shapes = np.zeros((len(ids), 17))
+        shapes[:, :b.shape[1]], shapes[:, 16] = b, g
+        self.engine.track_set_subjects(ids, shapes)
 
     def step(self, next_frames=None, mask=None):
         """next_frames: target frame t + 1 of every env ([E][row width], None on the first step after a reset); mask: int32 [E], 0 = this
@@ -64,7 +87,7 @@ class Tracker:
         return self.state[:, 151:223].reshape(self.E, 24, 3)
 
     def smpl(self):
-        """the state of the last step as SMPL (qpos_to_smpl on the device, each env with its fk_models shape variant), enqueued on the tracker's
+        """the state of the last step as SMPL (qpos_to_smpl on the device, each env with its fk_models shape variant or its set_subjects body), enqueued on the tracker's
         stream with no host synchronise.  Returns (pose_aa [E][72], trans [E][3]), float64 tensors overwritten by the next call."""
         if getattr(self, "_smpl", None) is None:
             t = self.torch
@@ -73,6 +96,7 @@ class Tracker:
 
     def floor(self):
         """the body hulls of the last step's state against the floor (uhc_floor_qpos' kernel at pitch 223, each env with its fk_models shape variant
+        or its set_subjects body
         and no previous frame: the envs are unrelated rows, so skate_mm is 0).  Returns [E][5] float64 on the device: min_z (m), pen_mm,
         skate_mm, float_mm, n_below, a tensor overwritten by the next call.  The variants were range-checked by track_begin, so nothing synchronises
         (as smpl())."""
