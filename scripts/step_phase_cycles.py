@@ -15,6 +15,8 @@ library UHC_B200_SO names) on the bench's rollout: the bench's clip, agent and s
           one whose cycles grow in proportion to k is bound by instruction issue or a shared pipe.
   nosync  the table and the k = 16 probe again with the substep alignment barriers compiled out
   production  the table's workload on the production library: kernel time only (it has no clocks)
+  groups  the table's workload on production builds with other substep alignment: one 16-warp group per CTA (-DUHC_SYNC_GROUP=16) and no
+          barriers (-DUHC_NO_CTA_SYNC), kernel time only, against the production library's two 8-warp groups
 
 Writes DIR/step_phase_cycles.json and prints the phase table.  The card's name, power limit and SM clock are read in the same call.
 """
@@ -114,7 +116,8 @@ def main():
         tmp = tempfile.TemporaryDirectory()
         bdir = tmp.name
     libs = {}
-    for name, defs in (("clocks", ["UHC_PHASE_CLOCKS"]), ("clocks_nosync", ["UHC_PHASE_CLOCKS", "UHC_NO_CTA_SYNC"])):
+    for name, defs in (("clocks", ["UHC_PHASE_CLOCKS"]), ("clocks_nosync", ["UHC_PHASE_CLOCKS", "UHC_NO_CTA_SYNC"]),
+                       ("sync16", ["UHC_SYNC_GROUP=16"]), ("nosync", ["UHC_NO_CTA_SYNC"])):
         os.makedirs(os.path.join(bdir, name), exist_ok=True)
         libs[name] = build.build(so=os.path.join(bdir, name, "libuhc_b200.so"), defines=defs)
     prod = build.build()
@@ -124,6 +127,7 @@ def main():
     res["table"], *res["probe"] = run_variant(libs["clocks"], [(full, EPB)] + [(wave, k) for k in (4, 8, 12, 16)], a.steps, a.warmup, True)
     res["nosync"] = run_variant(libs["clocks_nosync"], [(full, EPB), (wave, EPB)], a.steps, a.warmup, True)
     res["production"] = run_variant(prod, [(full, EPB), (wave, EPB)], a.steps, a.warmup, False)
+    res["groups"] = {name: run_variant(libs[name], [(full, EPB)], a.steps, a.warmup, False)[0] for name in ("sync16", "nosync")}
     res["card_after"] = card()
     os.makedirs(a.out, exist_ok=True)
     with open(os.path.join(a.out, "step_phase_cycles.json"), "w") as f:
@@ -138,6 +142,8 @@ def main():
     print("kernel ms: instrumented %.3f, production %.3f, production one wave %.3f, no alignment barriers %.3f" % (
         res["table"]["kernel_ms_median"], res["production"][0]["kernel_ms_median"], res["production"][1]["kernel_ms_median"], res["nosync"][0]["kernel_ms_median"]))
     print("probe kernel ms at k = 4 8 12 16:", " ".join("%.3f" % r["kernel_ms_median"] for r in res["probe"]))
+    print("kernel ms at 4096 envs: two 8-warp groups %.3f, one 16-warp group %.3f, no barriers %.3f" % (
+        res["production"][0]["kernel_ms_median"], res["groups"]["sync16"]["kernel_ms_median"], res["groups"]["nosync"]["kernel_ms_median"]))
     if tmp:
         tmp.cleanup()
 

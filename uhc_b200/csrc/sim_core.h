@@ -293,7 +293,11 @@ template <class R> UHC_DEV const Pr<R> *as_pairs(const R *p) { return reinterpre
 
 // ------------------------------------------------------------------------------------------------ warp primitives
 #ifndef UHC_EMU
-template <class R> UHC_DEV R warp_sum(R x) { for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o); return x; }
+template <class R> UHC_DEV R warp_sum(R x) {
+#pragma unroll 1
+    for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+}
 template <class R> UHC_DEV R warp_max(R x) { for (int o = 16; o; o >>= 1) { R y = __shfl_xor_sync(0xffffffffu, x, o); x = x > y ? x : y; } return x; }
 template <class R> UHC_DEV void warp_argmin(R &x, int &i) {
     for (int o = 16; o; o >>= 1) { R y = __shfl_xor_sync(0xffffffffu, x, o); int j = __shfl_xor_sync(0xffffffffu, i, o); if (y < x || (y == x && j < i)) { x = y; i = j; } }
@@ -305,13 +309,16 @@ template <class R> UHC_DEV void warp_argmin(R &x, int &i) {
 UHC_DEV int warp_excl_scan(int x, int lane) { int p = x; for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, p, o); if (lane >= o) p += t; } return p - x; }
 #define WEXSCAN(dst, src) { dst = warp_excl_scan(src, (int)(threadIdx.x & 31)); }
 // bodies are numbered depth-first, so subtree(b) = lanes [b, sub_end]: subtree sum = difference of an inclusive warp prefix sum
+// The scan steps are a rolled loop over the offsets with the K components inside: the same additions per component, a fifth of the code
 template <class R, int K> UHC_DEV void subtree_sum(R (&x)[K], int sub_end, int lane) {
+#pragma unroll 1
+    for (int o = 1; o < 32; o <<= 1) {
+#pragma unroll
+        for (int i = 0; i < K; i++) { const R t = __shfl_up_sync(0xffffffffu, x[i], o); if (lane >= o) x[i] += t; }
+    }
 #pragma unroll
     for (int i = 0; i < K; i++) {
-        R p = x[i];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { R t = __shfl_up_sync(0xffffffffu, p, o); if (lane >= o) p += t; }
-        const R hi = __shfl_sync(0xffffffffu, p, sub_end), lo = __shfl_up_sync(0xffffffffu, p, 1);
+        const R hi = __shfl_sync(0xffffffffu, x[i], sub_end), lo = __shfl_up_sync(0xffffffffu, x[i], 1);
         x[i] = hi - (lane > 0 ? lo : R(0));
     }
 }
@@ -319,7 +326,7 @@ template <class R, int K> UHC_DEV void subtree_sum(R (&x)[K], int sub_end, int l
 // its 2^(k+1) nearest ancestors-or-self (chains are at most MAXLEVEL + 1 = 9 bodies long -> 4 rounds instead of one per level)
 template <class R, int K> UHC_DEV void ancestor_sum(R (&x)[K], int a1, int a2, int a4, int a8) {
     static_assert(MAXLEVEL + 1 <= 16, "four pointer-jumping rounds cover chains of 16 bodies");
-#pragma unroll
+#pragma unroll 1
     for (int rnd = 0; rnd < 4; ++rnd) {
         const int src = rnd == 0 ? a1 : (rnd == 1 ? a2 : (rnd == 2 ? a4 : a8));
 #pragma unroll
@@ -327,13 +334,11 @@ template <class R, int K> UHC_DEV void ancestor_sum(R (&x)[K], int a1, int a2, i
     }
 }
 #define WSUBTREE(n, K, tp) subtree_sum<Real, K>(n, tp.sub_end, tp.lane)
-template <class R, int K> UHC_DEV void prefix_sum(R (&x)[K], int lane) {   // inclusive, over the 32 lanes
+template <class R, int K> UHC_DEV void prefix_sum(R (&x)[K], int lane) {   // inclusive, over the 32 lanes (rolled like subtree_sum)
+#pragma unroll 1
+    for (int o = 1; o < 32; o <<= 1) {
 #pragma unroll
-    for (int i = 0; i < K; i++) {
-        R p = x[i];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const R t = __shfl_up_sync(0xffffffffu, p, o); if (lane >= o) p += t; }
-        x[i] = p;
+        for (int i = 0; i < K; i++) { const R t = __shfl_up_sync(0xffffffffu, x[i], o); if (lane >= o) x[i] += t; }
     }
 }
 #define WPREFIX(n, K) prefix_sum<Real, K>(n, (int)(threadIdx.x & 31))
@@ -500,6 +505,7 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
     LV(rr) = lane - 6 * (lane / 6);
     LV(entn) = lane < 6 * LVL_G ? UHC_LDT(lp + (nlvl - 1) * LVL_G + lane / 6) : 0;
     const bool limits = use_contacts && w.nlim > 0;     // an active joint-limit row (J = +-e_i) adds its D to the joint-space diagonal of the Hessian
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) {
         Real d = UHC_LDT(m.dof_f + 4 * i) + arm_scale * UHC_LDT(m.dof_f + 4 * i + 2);   // joint-space diagonal
         if (limits && w.tau[i] != 0 && w.as_[i] < 0) d += abs_(w.tau[i]);
@@ -814,6 +820,7 @@ UHC_DEVNI void tree_vel(const Model<Real> &m, Work<Real> &w, const Real *x, Real
 template <class Real>
 UHC_DEV void project_force(const Model<Real> &m, Work<Real> &w, const Real (*F)[6], Real *y, Real scale, const Real *add) {
     LANES_BEGIN
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) {
         const int b = i < 6 ? 0 : 1 + (i - 6) / 3;
         y[i] = scale * pdot6(as_pairs(w.S[i]), as_pairs(F[b])) + (add ? add[i] : Real(0));
@@ -913,6 +920,7 @@ template <class Real>
 UHC_DEV void constraint_setup(const Model<Real> &m, Work<Real> &w) {
     const Real kk = Real(1) / (m.simp1 * m.simp1 * m.solref0 * m.solref0 * m.solref1 * m.solref1), bb = Real(2) / (m.simp1 * m.solref0);
     LANES_BEGIN
+#pragma unroll 1
     for (int c = lane; c < w.ncon; c += 32) {
         const int b = w.cbody[c];
         const Real pos = w.cdist[c] - m.margin;
@@ -942,12 +950,14 @@ UHC_DEV void limit_setup(const Model<Real> &m, Work<Real> &w) {
     LVAR(int, viol);
     LANES_BEGIN
     int f = 0;
+#pragma unroll 1
     for (int i = 6 + lane; i < NV; i += 32) { const Real q = w.q[i + 1]; f |= (q < UHC_LDT(m.dof_lim + 4 * i)) | (q > UHC_LDT(m.dof_lim + 4 * i + 1)); }
     LV(viol) = f;
     LANES_END_R
     if (!WBALLOT(viol)) { w.nlim = 0; return; }
     const Real kk = Real(1) / (m.simp1 * m.simp1 * m.solref0 * m.solref0 * m.solref1 * m.solref1), bb = Real(2) / (m.simp1 * m.solref0);
     LANES_BEGIN
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) {
         Real sD = 0;
         if (i >= 6) {
@@ -980,6 +990,7 @@ UHC_DEV void limit_setup(const Model<Real> &m, Work<Real> &w) {
 template <class Real>
 UHC_DEVNI void contact_rows(const Model<Real> &m, Work<Real> &w, const Real (*X)[6], Real (*out)[4], const Real (*sub)[4]) {
     LANES_BEGIN
+#pragma unroll 1
     for (int c = lane; c < w.ncon; c += 32) {
         const int b = w.cbody[c]; Real u[3], t[3];
         cross3(X[b], w.cr[c], t);
@@ -1081,6 +1092,7 @@ UHC_DEV Real newton_init(const Model<Real> &m, Work<Real> &w, const TPT &tp, Rea
     LVAR(Real, part); LVAR(Real, gs);
     LANES_BEGIN
     Real s = 0;
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) {
         const int b = i < 6 ? 0 : 1 + (i - 6) / 3;
         Real gi = pdot6(as_pairs(w.S[i]), as_pairs(w.Fb[b])) + UHC_LDT(m.dof_f + 4 * i) * w.aw[i] - w.fs[i];
@@ -1106,16 +1118,19 @@ UHC_DEV bool newton_advance(const Model<Real> &m, Work<Real> &w, const TPT &tp, 
     LVAR(Real, pa);
     LANES_BEGIN
     Real sA = 0;
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) sA += w.g[i] * w.p[i];
     LV(pa) = sA;
     LANES_END_R
     const Real gp = WSUM(pa);           // directional derivative at al = 0 (negative: p is a descent direction)
     Real lo = 0, hi = -1, al = 1;
     bool exact = false;
+#pragma unroll 1
     for (int ls = 0; ls < 12; ++ls) {
         LVAR(Real, d1); LVAR(Real, d2); LVAR(int, chg);
         LANES_BEGIN
         Real s1 = 0, s2 = 0; int ch = 0;
+#pragma unroll 1
         for (int c = lane; c < w.ncon; c += 32) for (int e = 0; e < 4; e++) {
             const Real r0 = w.cres[c][e], jp = w.cjp[c][e], r = r0 + al * jp;
             if ((r0 < 0) != (r < 0)) { const Real dj = w.cD[c] * jp; s1 -= dj * abs_(r); s2 += (r < 0) ? dj * jp : -dj * jp; ch = 1; }
@@ -1138,8 +1153,10 @@ UHC_DEV bool newton_advance(const Model<Real> &m, Work<Real> &w, const TPT &tp, 
     // a, residuals; multipliers D delta of the rows that switched between 0 and al (the others carry none) into cjp
     LVAR(int, chg2);
     LANES_BEGIN
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) w.a[i] += al * w.p[i];
     int ch = 0;
+#pragma unroll 1
     for (int c = lane; c < w.ncon; c += 32) for (int e = 0; e < 4; e++) {
         const Real r0 = w.cres[c][e], r = r0 + al * w.cjp[c][e];
         const bool sw = (r0 < 0) != (r < 0);
@@ -1159,6 +1176,7 @@ UHC_DEV bool newton_advance(const Model<Real> &m, Work<Real> &w, const TPT &tp, 
     const bool any2 = WBALLOT(chg2) != 0;
     if (exact && !any2) {
         LANES_BEGIN
+#pragma unroll 1
         for (int i = lane; i < NV; i += 32) { w.g[i] = 0; w.p[i] = 0; }
         LANES_END
         *gn2 = 0;
@@ -1168,6 +1186,7 @@ UHC_DEV bool newton_advance(const Model<Real> &m, Work<Real> &w, const TPT &tp, 
     LVAR(Real, gs);
     LANES_BEGIN
     Real s = 0;
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) {
         const int b = i < 6 ? 0 : 1 + (i - 6) / 3;
         Real gi = (1 - al) * w.g[i];
@@ -1214,6 +1233,7 @@ UHC_DEV void pd_setup(const Model<Real> &m, const EnvCfg<Real> &cfg, Work<Real> 
     const Real dt = m.dt;
     Real sp, sd; pd_gains(cfg, w, it, &sp, &sd);
     LANES_BEGIN
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) {
         Real rhs = -w.C[i];
         if (i >= 6) {
@@ -1238,6 +1258,7 @@ UHC_DEV void pd_finish(const Model<Real> &m, const EnvCfg<Real> &cfg, Work<Real>
     const Real dt = m.dt;
     Real sp, sd; pd_gains(cfg, w, it, &sp, &sd);
     LANES_BEGIN
+#pragma unroll 1
     for (int i = 6 + lane; i < NV; i += 32) {
         const Real kp = UHC_LDT(m.dof_f + 4 * i + 1) * sp, kd = UHC_LDT(m.dof_f + 4 * i + 2) * sd, lim = UHC_LDT(m.dof_f + 4 * i + 3);
         const Real t = clamp_(-kp * w.g[i] - kd * (w.v[i] + w.p[i] * dt), -lim, lim);
@@ -1302,6 +1323,7 @@ template <class Real>
 UHC_DEV void integrate(const Model<Real> &m, Work<Real> &w) {
     const Real dt = m.dt;
     LANES_BEGIN
+#pragma unroll 1
     for (int i = lane; i < NV; i += 32) { const Real vn = w.v[i] + dt * w.a[i]; w.v[i] = vn; w.aw[i] = w.a[i]; if (i >= 6) w.q[i + 1] += dt * vn; }
     LANES_END
     LANES_BEGIN
@@ -1324,7 +1346,7 @@ UHC_DEV void integrate(const Model<Real> &m, Work<Real> &w) {
 // exposes to the Python side (SURVEY.md section 7 "stale dynamics").  with_pd = false: reset path (sim.forward with ctrl = 0).
 enum { PH_PD = 0, PH_SMOOTH = 1, PH_NEWTON = 2 };
 // The warps of a CTA are re-aligned at points every warp passes exactly once per substep: they then run the same code at
-// the same time and share instruction-cache lines (the per-substep code is ~3x the 32 KB instruction cache).
+// the same time and share instruction-cache lines (the per-substep code is 112 KB of SASS: scripts/step_sass_footprint.py).
 // The fp32 kernel runs one 16-warp CTA per SM aligned as two groups of 8 warps (one named barrier each): on an H100 at 4096 envs that
 // was ~1 % faster than two 8-warp CTAs per SM aligned as a whole (k_env_step 3.06 vs 3.08 ms).  On the GPU the kernel was first tuned
 // on, aligning 7 warps was faster than groups of 2 / 3 / 4 warps and than aligning every 2nd / 3rd substep or each Newton iteration.
@@ -1360,6 +1382,7 @@ UHC_DEVNI int substep_dynamics(const Model<Real> &m, const EnvCfg<Real> &cfg, Wo
             collide(m, w, tp);
             PCLK(cta_sync, w, PC_COLLIDE);
             LANES_BEGIN
+#pragma unroll 1
             for (int i = lane; i < NV; i += 32) {  // smooth acceleration a_s = M^-1 (tau + f_applied - C)
                 Real f = -w.C[i];
                 if (explicit_rf) f += w.as_[i];
@@ -1390,6 +1413,7 @@ UHC_DEVNI int substep_dynamics(const Model<Real> &m, const EnvCfg<Real> &cfg, Wo
             PCLK(cta_sync, w, PC_SYNC_SMOOTH);
             if (w.ncon == 0 && w.nlim == 0) {
                 LANES_BEGIN
+#pragma unroll 1
                 for (int i = lane; i < NV; i += 32) w.a[i] = w.as_[i];
                 LANES_END
                 done = true;

@@ -34,8 +34,13 @@ __device__ __forceinline__ void stage_tables(EngineView<Real> &ev, unsigned char
     ev.model.dof_f = s_dof; ev.model.dof_lim = s_lim; ev.model.lvl_pack = s_lvl; ev.model.topo_s = s_topo;
 }
 
-// warps per substep alignment group (sim_core.h, UHC_CTA_SYNC): the fp32 kernel's 16-warp CTA is two groups, the fp64 kernel's one
-constexpr int SYNC_GROUP = 8;
+// warps per substep alignment group (sim_core.h, UHC_CTA_SYNC): the fp32 kernel's 16-warp CTA is two groups, the fp64 kernel's one.
+// -DUHC_SYNC_GROUP=n builds other group sizes beside the production library (scripts/step_phase_cycles.py)
+#ifndef UHC_SYNC_GROUP
+#define UHC_SYNC_GROUP 8
+#endif
+constexpr int SYNC_GROUP = UHC_SYNC_GROUP;
+static_assert(SYNC_GROUP >= 1 && SYNC_GROUP <= 16, "an alignment group is 1 to 16 warps");
 #ifdef UHC_MAXNREG     /* experiment knob: cap registers without changing the CTA shape */
 #define UHC_STEP_BOUNDS(EPB, Real) __maxnreg__(UHC_MAXNREG)
 #else
