@@ -84,6 +84,8 @@ const char *uhc_last_error(void);
 
 /* precision: 32 (product) or 64 (fp64 debug build of the same kernels). */
 int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_envs, int device, int precision, UhcEngine **out);
+/* frees the engine and everything any uhc_* call attached to it (evaluation, tracker, rollout, renderers, SMPL mesh, floor hulls, JPEG
+ * encoder), on the engine's device; the uhc_*_release calls and uhc_track_end before it are optional */
 void uhc_engine_destroy(UhcEngine *e);
 int uhc_engine_set_cfg(UhcEngine *e, const UhcEnvCfg *cfg);
 

@@ -90,7 +90,7 @@ int uhc_eval_run_groups_ex(UhcEngine *e, int G, const int *group_n_host, const i
 int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, const int *clip_host, const UhcMcp *mcps, const double *const *zfilter_stats_host,
                                float zclip, int fail_safe, int window, const UhcEvalOut *out, void *stream);
 int uhc_eval_graph_count(const UhcEngine *e);   /* graphs this engine's evaluation holds now, grouped ones included (read-only; tests) */
-void uhc_eval_release(UhcEngine *e);   /* frees the graphs / scratch of this engine (the grouped path's too); call before uhc_engine_destroy */
+void uhc_eval_release(UhcEngine *e);   /* frees the graphs / scratch of this engine (the grouped path's too); optional: uhc_engine_destroy frees it too */
 
 #ifdef __cplusplus
 }

@@ -39,7 +39,7 @@ const char *uhc_floor_last_error(void);   /* an alias of uhc_last_error (uhc_b20
  * them: evaluation graphs captured with the earlier copy are keyed on it and are not replayed.  A failed call leaves what was there.
  * -2: a null pointer, nshape other than the engine's shape variants, nvert < 1, bodies whose ranges do not tile 0 .. nvert - 1 in order */
 int uhc_floor_init(UhcEngine *e, const UhcFloorHulls *h);
-void uhc_floor_release(UhcEngine *e);     /* call before uhc_engine_destroy */
+void uhc_floor_release(UhcEngine *e);     /* optional: uhc_engine_destroy frees it too */
 
 /* n frames, frame i's qpos (76 values) at qpos_dev + i * qpos_pitch elements, fp32 (precision 32) or fp64 (64): a pitch of 223 reads the
  * tracker's state_out rows, 148 the evaluation's state record, 76 a plain qpos array.  variant_dev_or_null = [n] shape variant per frame

@@ -38,7 +38,7 @@ const char *uhc_mesh_last_error(void);   /* an alias of uhc_last_error (uhc_b200
  * the model; a failed call leaves the previous one in place.  -2: a null pointer, nvert < 1, a parent table that is not a tree in order,
  * a non-finite value */
 int uhc_mesh_init(UhcEngine *e, const UhcSmplModel *m);
-void uhc_mesh_release(UhcEngine *e);     /* call before uhc_engine_destroy */
+void uhc_mesh_release(UhcEngine *e);     /* optional: uhc_engine_destroy frees it too */
 
 /* n rows of SMPL pose_dev [n][72] (axis-angles of the 24 joints) and trans_dev [n][3] in fp64, exactly what uhc_qpos_to_smpl writes (so
  * qpos -> SMPL -> mesh stays on the device); betas_dev = [nbetas][10] shapes, row i takes betas_dev[beta_idx[i]] (beta_idx_dev_or_null

@@ -43,7 +43,7 @@ const char *uhc_render_last_error(void);   /* an alias of uhc_last_error (uhc_b2
 /* Uploads the plane tables (as fp32) once per engine; a second call replaces them.  -2 unless nshape equals the engine's shape variants,
  * every body has 4 .. UHC_RENDER_MAX_PLANES planes inside 0 .. nplane - 1, and every value is finite.  Synchronises the device. */
 int uhc_render_init(UhcEngine *e, const UhcRenderHulls *hulls);
-/* Frees what uhc_render_init, uhc_render_mesh_init and their scratch hold (also safe without them). */
+/* Frees what uhc_render_init, uhc_render_mesh_init and their scratch hold (also safe without them); optional: uhc_engine_destroy frees it too. */
 void uhc_render_release(UhcEngine *e);
 
 /* The pose table [n][2][24][UHC_RENDER_POSE] fp32 of n frames: humanoid 0 = qpos row i, humanoid 1 = ghost row i (left untouched without a

@@ -99,7 +99,7 @@ int uhc_rollout_mcp(UhcEngine *e, int T, int row0, const UhcMcp *mcp, const floa
 int uhc_rollout_time_env_step(UhcEngine *e, int nrows);
 int uhc_rollout_env_step_ms(UhcEngine *e, int row, float *ms);
 int uhc_rollout_launches_per_step(UhcEngine *e);   /* kernels per control step of the last uhc_rollout (bench `gpu_launches`) */
-void uhc_rollout_release(UhcEngine *e);            /* frees graphs / scratch of this engine; call before uhc_engine_destroy */
+void uhc_rollout_release(UhcEngine *e);            /* frees graphs / scratch of this engine; optional: uhc_engine_destroy frees it too */
 
 #ifdef __cplusplus
 }

@@ -52,7 +52,8 @@ int uhc_track_push(UhcEngine *e, const double *next_frames_dev, const int *mask_
 int uhc_track_obs(UhcEngine *e, float *obs_dev, void *stream);
 /* out_host = [E][UHC_TRACK_STATE_COLS] (synchronises the device) */
 int uhc_track_state(UhcEngine *e, int *out_host);
-/* frees the stream buffers and graphs; the clip table stays loaded (its rows are whatever the windows held) */
+/* frees the stream buffers and graphs; the clip table stays loaded (its rows are whatever the windows held); optional:
+ * uhc_engine_destroy frees them too */
 void uhc_track_end(UhcEngine *e);
 /* CUDA graphs the tracker of this engine holds now (read-only; tests) */
 int uhc_track_graph_count(const UhcEngine *e);

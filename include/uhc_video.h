@@ -27,7 +27,7 @@ size_t uhc_jpeg_bound(int W, int H);
 int uhc_jpeg_encode(UhcEngine *e, const unsigned char *rgb_dev, long n, int W, int H, int quality, unsigned char *out_dev, size_t out_cap,
                     size_t *offsets_dev, size_t *total_host, void *stream);
 
-/* Frees the encoder's scratch of this engine (also safe without any). */
+/* Frees the encoder's scratch of this engine (also safe without any); optional: uhc_engine_destroy frees it too. */
 void uhc_video_release(UhcEngine *e);
 
 #ifdef __cplusplus

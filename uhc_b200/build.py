@@ -12,7 +12,7 @@ SRCS = ["step_kernel.cu", "nn_kernels.cu", "mlp_wgmma.cu", "rollout.cu", "ppo_up
 # are the same bits in every kernel that computes them; the subject
 # body builder's derived columns restate model.py's numpy arithmetic and must give the bits of its host emulation
 NO_FMA_SRCS = ["motion_lib.cu", "eval.cu", "curriculum.cu", "track.cu", "export.cu", "render.cu", "render_mesh.cu", "floor.cu", "mesh.cu", "subject.cu"]
-DEPS = ["errors.h", "sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "graph_cache.h", "group_core.h", "curriculum_core.h", "track_core.h", "track_obs.h", "track_glue.h", "smpl_export_core.h", "render_core.h", "render_mesh_core.h", "floor_core.h", "video_core.h", "mesh_core.h", "subject_core.h", "subject_glue.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h", "../../include/uhc_track.h", "../../include/uhc_export.h", "../../include/uhc_render.h", "../../include/uhc_floor.h", "../../include/uhc_video.h", "../../include/uhc_mesh.h", "../../include/uhc_subject.h"]
+DEPS = ["errors.h", "engine_slots.h", "sim_core.h", "env_step.h", "motion_core.h", "eval_core.h", "eval_glue.h", "graph_cache.h", "group_core.h", "curriculum_core.h", "track_core.h", "track_obs.h", "track_glue.h", "smpl_export_core.h", "render_core.h", "render_mesh_core.h", "floor_core.h", "video_core.h", "mesh_core.h", "subject_core.h", "subject_glue.h", "../../include/uhc_b200.h", "../../include/uhc_nn.h", "../../include/uhc_rollout.h", "../../include/uhc_ppo.h", "../../include/uhc_eval.h", "../../include/uhc_track.h", "../../include/uhc_export.h", "../../include/uhc_render.h", "../../include/uhc_floor.h", "../../include/uhc_video.h", "../../include/uhc_mesh.h", "../../include/uhc_subject.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math=false",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 

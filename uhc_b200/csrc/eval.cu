@@ -21,6 +21,7 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_eval.h"
+#include "engine_slots.h"
 #include "errors.h"
 #include "eval_core.h"
 #include "eval_glue.h"
@@ -108,13 +109,10 @@ struct EvalCtx {
     std::vector<int> ids, clip0, start, len;      // reset arguments (kept: no allocation in the steady state)
     GraphCache graphs{32}, ggraphs{16};           // of uhc_eval_run and of uhc_eval_run_groups (graph_cache.h)
 };
-std::vector<EvalCtx *> g_ev;
-
 EvalCtx *ev_ctx(UhcEngine *e) {
-    for (EvalCtx *c : g_ev) if (c->eng == e) return c;
-    EvalCtx *c = new EvalCtx(); c->eng = e; c->E = uhc_num_envs(e);
-    g_ev.push_back(c);
-    return c;
+    void *&s = engine_slot(e, SLOT_EVAL);
+    if (!s) { EvalCtx *c = new EvalCtx(); c->eng = e; c->E = uhc_num_envs(e); s = c; }
+    return (EvalCtx *)s;
 }
 // per-env arrays sized by E once; the window buffers grow with n * window (and the state record and the SMPL export with it when requested).
 // Called before any capture: a graph holds these pointers, so they never change while one of them can be replayed (gen)
@@ -341,20 +339,19 @@ int uhc_eval_run_groups_mcp_ex(UhcEngine *e, int G, const int *group_n_host, con
 }
 
 int uhc_eval_graph_count(const UhcEngine *e) {
-    for (const EvalCtx *c : g_ev) if (c->eng == e) return (int)(c->graphs.size() + c->ggraphs.size());
-    return 0;
+    const EvalCtx *c = e ? (const EvalCtx *)engine_slot(e, SLOT_EVAL) : nullptr;
+    return c ? (int)(c->graphs.size() + c->ggraphs.size()) : 0;
 }
 
 void uhc_eval_release(UhcEngine *e) {
-    for (size_t i = 0; i < g_ev.size(); i++) if (g_ev[i]->eng == e) {
-        EvalCtx *c = g_ev[i];
-        c->graphs.clear(); c->ggraphs.clear();
-        for (void *p : {(void *)c->d_clips, (void *)c->d_alive, (void *)c->d_reseat, (void *)c->d_count, (void *)c->d_ones, (void *)c->d_ring,
-                        (void *)c->d_win, (void *)c->d_wstates, (void *)c->d_wsmpl, (void *)c->d_xdone, (void *)c->d_wfloor, (void *)c->d_fprev, (void *)c->d_fdone}) if (p) cudaFree(p);
-        if (c->h_count) cudaFreeHost(c->h_count);
-        if (c->ev) cudaEventDestroy(c->ev);
-        delete c; g_ev.erase(g_ev.begin() + i); return;
-    }
+    EvalCtx *c = e ? (EvalCtx *)engine_slot(e, SLOT_EVAL) : nullptr;
+    if (!c) return;
+    c->graphs.clear(); c->ggraphs.clear();
+    for (void *p : {(void *)c->d_clips, (void *)c->d_alive, (void *)c->d_reseat, (void *)c->d_count, (void *)c->d_ones, (void *)c->d_ring,
+                    (void *)c->d_win, (void *)c->d_wstates, (void *)c->d_wsmpl, (void *)c->d_xdone, (void *)c->d_wfloor, (void *)c->d_fprev, (void *)c->d_fdone}) if (p) cudaFree(p);
+    if (c->h_count) cudaFreeHost(c->h_count);
+    if (c->ev) cudaEventDestroy(c->ev);
+    delete c; engine_slot(e, SLOT_EVAL) = nullptr;
 }
 
 }  // extern "C"

@@ -13,6 +13,7 @@
 #include <vector>
 #include "../../include/uhc_floor.h"
 #include "../../include/uhc_track.h"
+#include "engine_slots.h"
 #include "errors.h"
 #include "eval_glue.h"
 #include "floor_core.h"
@@ -30,19 +31,14 @@ constexpr unsigned FULL = 0xffffffffu;
 struct FloorDev { const double *vert; const unsigned char *vbody; int nvert, nshape; const double *slot; };
 
 struct FloorCtx {
-    UhcEngine *eng = nullptr;
     int nshape = 0;
     unsigned long long gen = 0;        // of this upload: graphs that hold `dev` carry it in their key
     double *d_vert = nullptr; unsigned char *d_vbody = nullptr;
     FloorDev dev{};
 };
-std::vector<FloorCtx *> g_fl;
 unsigned long long g_fl_gen = 0;
 
-FloorCtx *find_ctx(const UhcEngine *e) {
-    for (FloorCtx *c : g_fl) if (c->eng == e) return c;
-    return nullptr;
-}
+FloorCtx *find_ctx(const UhcEngine *e) { return (FloorCtx *)engine_slot(e, SLOT_FLOOR); }
 
 // the hulls of a launch whose variants may be the engine's clip models, which point the tracker's envs at their run-time subjects
 FloorDev with_slots(const FloorCtx *c, const UhcEngine *e) { FloorDev d = c->dev; d.slot = trackx::slot_hulls(e); return d; }
@@ -201,19 +197,18 @@ int uhc_floor_init(UhcEngine *e, const UhcFloorHulls *h) {
     }
     uhc_floor_release(e);
     FloorCtx *c = new FloorCtx();
-    c->eng = e; c->nshape = h->nshape; c->gen = ++g_fl_gen; c->d_vert = d_vert; c->d_vbody = d_vbody;
+    c->nshape = h->nshape; c->gen = ++g_fl_gen; c->d_vert = d_vert; c->d_vbody = d_vbody;
     c->dev = FloorDev{d_vert, d_vbody, h->nvert, h->nshape, nullptr};
-    g_fl.push_back(c);
+    engine_slot(e, SLOT_FLOOR) = c;
     return 0;
 }
 
 void uhc_floor_release(UhcEngine *e) {
-    for (size_t i = 0; i < g_fl.size(); i++) if (g_fl[i]->eng == e) {
-        FloorCtx *c = g_fl[i];
-        if (c->d_vert) cudaFree(c->d_vert);
-        if (c->d_vbody) cudaFree(c->d_vbody);
-        delete c; g_fl.erase(g_fl.begin() + i); return;
-    }
+    FloorCtx *c = e ? find_ctx(e) : nullptr;
+    if (!c) return;
+    if (c->d_vert) cudaFree(c->d_vert);
+    if (c->d_vbody) cudaFree(c->d_vbody);
+    delete c; engine_slot(e, SLOT_FLOOR) = nullptr;
 }
 
 int uhc_floor_qpos(UhcEngine *e, const void *qpos_dev, int precision, long n, long qpos_pitch, const int *variant_dev_or_null,

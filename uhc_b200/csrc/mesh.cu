@@ -14,6 +14,7 @@
 #include <vector>
 #include "../../include/uhc_floor.h"
 #include "../../include/uhc_mesh.h"
+#include "engine_slots.h"
 #include "errors.h"
 #include "floor_core.h"
 #include "mesh_core.h"
@@ -39,7 +40,6 @@ struct MeshDev {
 };
 
 struct MeshCtx {
-    UhcEngine *eng = nullptr;
     MeshDev dev{};
     void *own[7] = {};                 // the model's device arrays
     float *vs = nullptr; double *J = nullptr; int cap_nb = 0;        // shape scratch: [nb][V][3], [nb][24][3]
@@ -52,12 +52,7 @@ struct MeshCtx {
         if (A) cudaFree(A);
     }
 };
-std::vector<MeshCtx *> g_mesh;
-
-MeshCtx *find_ctx(const UhcEngine *e) {
-    for (MeshCtx *c : g_mesh) if (c->eng == e) return c;
-    return nullptr;
-}
+MeshCtx *find_ctx(const UhcEngine *e) { return (MeshCtx *)engine_slot(e, SLOT_MESH); }
 
 __device__ __forceinline__ double shaped(const MeshDev &d, long v, int c, const double *beta) {
     const double *s = d.sd + ((size_t)v * 3 + c) * meshm::NBETA;
@@ -327,18 +322,16 @@ int uhc_mesh_init(UhcEngine *e, const UhcSmplModel *m) {
         uhc_err() = std::string("uhc_mesh_init: ") + cudaGetErrorString(ce); return -1;
     }
     uhc_mesh_release(e);
-    c->eng = e;
     c->dev.V = m->nvert;
     for (int k = 0; k < meshm::NJ; k++) c->dev.parents[k] = m->parents[k];
     c->dev.vt = vt; c->dev.sd = sd; c->dev.jreg = jr; c->dev.pd = pdd; c->dev.w_adr = w_adr; c->dev.w_j = w_j; c->dev.w_w = w_w;
-    g_mesh.push_back(c);
+    engine_slot(e, SLOT_MESH) = c;
     return 0;
 }
 
 void uhc_mesh_release(UhcEngine *e) {
-    for (size_t i = 0; i < g_mesh.size(); i++) if (g_mesh[i]->eng == e) {
-        delete g_mesh[i]; g_mesh.erase(g_mesh.begin() + i); return;
-    }
+    if (!e) return;
+    delete find_ctx(e); engine_slot(e, SLOT_MESH) = nullptr;
 }
 
 int uhc_smpl_mesh(UhcEngine *e, long n, const double *pose_dev, const double *trans_dev, int nbetas, const double *betas_dev,

@@ -9,6 +9,7 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_render.h"
+#include "engine_slots.h"
 #include "errors.h"
 #define UHC_RENDER_HOST 1
 #include "render_core.h"
@@ -24,22 +25,17 @@ constexpr int TILE = 16, SLOTS = 2 * render::NB;
 constexpr size_t SMEM_MAX = 200 * 1024;                // dynamic shared memory of a trace, at most
 
 struct RenderCtx {
-    UhcEngine *eng = nullptr;
     int nshape = 0, nplane = 0;
     int adr[render::NB], num[render::NB];
     float4 *d_plane = nullptr, *d_sphere = nullptr;    // [nshape][nplane], [nshape][24]
     float *d_pose = nullptr; size_t pose_cap = 0;      // uhc_render_qpos' pose table, frames
 };
-std::vector<RenderCtx *> g_rd;
-
-RenderCtx *find_ctx(const UhcEngine *e) {
-    for (RenderCtx *c : g_rd) if (c->eng == e) return c;
-    return nullptr;
-}
-void free_ctx(RenderCtx *c) {
+RenderCtx *find_ctx(const UhcEngine *e) { return (RenderCtx *)engine_slot(e, SLOT_RENDER); }
+void free_ctx(UhcEngine *e) {
+    RenderCtx *c = find_ctx(e);
+    if (!c) return;
     cudaFree(c->d_plane); cudaFree(c->d_sphere); cudaFree(c->d_pose);
-    for (size_t i = 0; i < g_rd.size(); i++) if (g_rd[i] == c) { g_rd.erase(g_rd.begin() + i); break; }
-    delete c;
+    delete c; engine_slot(e, SLOT_RENDER) = nullptr;
 }
 
 template <class Real>
@@ -190,9 +186,9 @@ int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
         if (!(isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && p[3] > 0 && isfinite(p[3]))) { uhc_err() = "uhc_render_init: bad bounding sphere"; return -2; }
         sp[i] = make_float4((float)p[0], (float)p[1], (float)p[2], (float)p[3]);
     }
-    if (RenderCtx *old = find_ctx(e)) free_ctx(old);             // the mesh tables (uhc_render_mesh_init) stay
+    free_ctx(e);                                                  // the mesh tables (uhc_render_mesh_init) stay
     RenderCtx *c = new RenderCtx();
-    c->eng = e; g_rd.push_back(c);
+    engine_slot(e, SLOT_RENDER) = c;
     c->nshape = h->nshape; c->nplane = h->nplane;
     for (int b = 0; b < render::NB; b++) { c->adr[b] = h->plane_adr[b]; c->num[b] = h->plane_num[b]; }
     CK(cudaMalloc((void **)&c->d_plane, np * sizeof(float4)));
@@ -206,7 +202,8 @@ int uhc_render_init(UhcEngine *e, const UhcRenderHulls *h) {
 }
 
 void uhc_render_release(UhcEngine *e) {
-    if (RenderCtx *c = e ? find_ctx(e) : nullptr) free_ctx(c);
+    if (!e) return;
+    free_ctx(e);
     uhc::render_mesh_release(e);
 }
 

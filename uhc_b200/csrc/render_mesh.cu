@@ -8,8 +8,8 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <string>
-#include <vector>
 #include "../../include/uhc_render.h"
+#include "engine_slots.h"
 #include "errors.h"
 #define UHC_RENDER_HOST 1
 #include "render_mesh_core.h"
@@ -22,17 +22,11 @@ constexpr int TILE = 16, SLOTS = 2 * render::NB, REFIT_THREADS = 128;
 constexpr size_t SMEM_MAX = 200 * 1024;
 
 struct MeshCtx {
-    UhcEngine *eng = nullptr;
     int nvert = 0, nface = 0, nleaf = 0;
     int *d_face = nullptr, *d_leaf_first = nullptr, *d_body_leaf = nullptr;
     float *d_box = nullptr; size_t box_cap = 0;        // refitted boxes, frames: [n][SLOTS + 2 nleaf][6]
 };
-std::vector<MeshCtx *> g_mc;
-
-MeshCtx *find_ctx(const UhcEngine *e) {
-    for (MeshCtx *c : g_mc) if (c->eng == e) return c;
-    return nullptr;
-}
+MeshCtx *find_ctx(const UhcEngine *e) { return (MeshCtx *)engine_slot(e, SLOT_RENDER_MESH); }
 
 __host__ __device__ size_t frame_boxes(int nleaf) { return (size_t)(SLOTS + 2 * nleaf) * 6; }     // floats per frame
 size_t trace_smem(int nleaf) { return frame_boxes(nleaf) * sizeof(float) + (size_t)(nleaf + 1 + render::NB + 1) * sizeof(int); }
@@ -99,17 +93,14 @@ __global__ void __launch_bounds__(TILE * TILE) k_render_mesh_trace(const __grid_
     }
 }
 
-void free_ctx(MeshCtx *c) {
-    cudaFree(c->d_face); cudaFree(c->d_leaf_first); cudaFree(c->d_body_leaf); cudaFree(c->d_box);
-    for (size_t i = 0; i < g_mc.size(); i++) if (g_mc[i] == c) { g_mc.erase(g_mc.begin() + i); break; }
-    delete c;
-}
-
 }  // namespace
 
 namespace uhc {
 void render_mesh_release(UhcEngine *e) {
-    if (MeshCtx *c = e ? find_ctx(e) : nullptr) free_ctx(c);
+    MeshCtx *c = e ? find_ctx(e) : nullptr;
+    if (!c) return;
+    cudaFree(c->d_face); cudaFree(c->d_leaf_first); cudaFree(c->d_body_leaf); cudaFree(c->d_box);
+    delete c; engine_slot(e, SLOT_RENDER_MESH) = nullptr;
 }
 }  // namespace uhc
 
@@ -122,7 +113,7 @@ int uhc_render_mesh_init(UhcEngine *e, const UhcRenderMesh *m) {
     if (trace_smem(m->nleaf) > SMEM_MAX) { uhc_err() = "uhc_render_mesh_init: the leaf boxes of two humanoids do not fit the trace's shared memory"; return -2; }
     uhc::render_mesh_release(e);
     MeshCtx *c = new MeshCtx();
-    c->eng = e; g_mc.push_back(c);
+    engine_slot(e, SLOT_RENDER_MESH) = c;
     c->nvert = m->nvert; c->nface = m->nface; c->nleaf = m->nleaf;
     CK(cudaMalloc((void **)&c->d_face, (size_t)m->nface * 3 * sizeof(int)));
     CK(cudaMalloc((void **)&c->d_leaf_first, (size_t)(m->nleaf + 1) * sizeof(int)));

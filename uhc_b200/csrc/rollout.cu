@@ -22,6 +22,7 @@
 #include "../../include/uhc_b200.h"
 #include "../../include/uhc_nn.h"
 #include "../../include/uhc_rollout.h"
+#include "engine_slots.h"
 #include "errors.h"
 #include "eval_glue.h"
 #include "graph_cache.h"
@@ -152,13 +153,10 @@ struct RolloutCtx {
     int launches_per_step = 0;
     std::vector<cudaEvent_t> ev0, ev1;    // optional: events around the env-step kernel of buffer row r (bench roofline: the dominant kernel's live duration)
 };
-std::vector<RolloutCtx *> g_ctx;
-
 RolloutCtx *ctx_of(UhcEngine *e) {
-    for (RolloutCtx *c : g_ctx) if (c->eng == e) return c;
-    RolloutCtx *c = new RolloutCtx(); c->eng = e; c->E = uhc_num_envs(e);
-    g_ctx.push_back(c);
-    return c;
+    void *&s = engine_slot(e, SLOT_ROLLOUT);
+    if (!s) { RolloutCtx *c = new RolloutCtx(); c->eng = e; c->E = uhc_num_envs(e); s = c; }
+    return (RolloutCtx *)s;
 }
 
 int check_policy(const Policy *pol) {
@@ -445,21 +443,20 @@ int uhc_rollout_launches_per_step(UhcEngine *e) { return e ? ctx_of(e)->launches
 }  // extern "C"
 
 void uhc::evalx::drop_rollout_graphs(UhcEngine *e) {
-    for (RolloutCtx *c : g_ctx) if (c->eng == e) c->graphs.clear();
+    if (RolloutCtx *c = (RolloutCtx *)engine_slot(e, SLOT_ROLLOUT)) c->graphs.clear();
 }
 
 extern "C" {
 
-void uhc_rollout_release(UhcEngine *e) {   // called by the binding before uhc_engine_destroy
-    for (size_t i = 0; i < g_ctx.size(); i++) if (g_ctx[i]->eng == e) {
-        RolloutCtx *c = g_ctx[i];
-        c->graphs.clear();
-        for (cudaEvent_t ev : c->ev0) cudaEventDestroy(ev);
-        for (cudaEvent_t ev : c->ev1) cudaEventDestroy(ev);
-        release(&c->own); release(&c->grouped);
-        for (void *p : {(void *)c->d_zws, (void *)c->d_step, (void *)c->d_mean_action, (void *)c->d_cinfo, (void *)c->d_pct, (void *)c->d_fail, (void *)c->d_end}) if (p) cudaFree(p);
-        delete c; g_ctx.erase(g_ctx.begin() + i); return;
-    }
+void uhc_rollout_release(UhcEngine *e) {
+    RolloutCtx *c = e ? (RolloutCtx *)engine_slot(e, SLOT_ROLLOUT) : nullptr;
+    if (!c) return;
+    c->graphs.clear();
+    for (cudaEvent_t ev : c->ev0) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : c->ev1) cudaEventDestroy(ev);
+    release(&c->own); release(&c->grouped);
+    for (void *p : {(void *)c->d_zws, (void *)c->d_step, (void *)c->d_mean_action, (void *)c->d_cinfo, (void *)c->d_pct, (void *)c->d_fail, (void *)c->d_end}) if (p) cudaFree(p);
+    delete c; engine_slot(e, SLOT_ROLLOUT) = nullptr;
 }
 
 }  // extern "C"

@@ -7,7 +7,14 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_b200.h"
+#include "../../include/uhc_eval.h"
+#include "../../include/uhc_floor.h"
+#include "../../include/uhc_mesh.h"
+#include "../../include/uhc_render.h"
 #include "../../include/uhc_rollout.h"
+#include "../../include/uhc_track.h"
+#include "../../include/uhc_video.h"
+#include "engine_slots.h"
 #include "env_step.h"
 #include "errors.h"
 #include "motion_core.h"
@@ -222,7 +229,11 @@ struct UhcEngine {
     // own body; d_slot_hull holds the same hulls in fp64 ([E][nvert][3], the floor measurements' vertices)
     subjx::Builder *subj = nullptr; int nslot = 0;
     double *d_slot_hull = nullptr;
+    void *slot[SLOT_COUNT] = {};   // the subsystems' contexts (engine_slots.h)
 };
+
+void *&engine_slot(UhcEngine *e, EngineSlot s) { return e->slot[s]; }
+void *engine_slot(const UhcEngine *e, EngineSlot s) { return e->slot[s]; }
 
 template <class T> static int dev_copy(UhcEngine *e, T **dst, const T *src, size_t n) {
     CK(cudaMalloc((void **)dst, n * sizeof(T))); e->allocs.push_back(*dst);
@@ -357,6 +368,14 @@ int uhc_engine_create(const UhcModelHost *model, const UhcEnvCfg *cfg, int num_e
 void uhc_engine_destroy(UhcEngine *e) {
     if (!e) return;
     cudaSetDevice(e->device);
+    // the evaluation's graphs hold the rollout's policy scratch, so the evaluation goes first and the rollout last
+    uhc_eval_release(e);
+    uhc_track_end(e);
+    uhc_render_release(e);
+    uhc_video_release(e);
+    uhc_floor_release(e);
+    uhc_mesh_release(e);
+    uhc_rollout_release(e);
     for (void *p : e->allocs) cudaFree(p);
     if (e->d_expert) cudaFree(e->d_expert);
     if (e->d_shape) cudaFree(e->d_shape);

@@ -18,6 +18,7 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_track.h"
+#include "engine_slots.h"
 #include "errors.h"
 #include "eval_glue.h"
 #include "graph_cache.h"
@@ -140,10 +141,9 @@ struct TrackCtx {
     double *d_sbeta = nullptr, *d_sshape = nullptr, *d_sbf = nullptr, *d_shull = nullptr; int *d_sbad = nullptr, *d_sids = nullptr, *d_sgender = nullptr;
     int s_cap = 0;
 };
-std::vector<TrackCtx *> g_tr;
 unsigned long long g_tr_gen = 0;                   // distinct per begin: graphs never outlive the buffers they hold
 
-TrackCtx *find_ctx(UhcEngine *e) { for (TrackCtx *c : g_tr) if (c->eng == e) return c; return nullptr; }
+TrackCtx *find_ctx(UhcEngine *e) { return (TrackCtx *)engine_slot(e, SLOT_TRACK); }
 void free_ctx(TrackCtx *c) {
     cudaDeviceSynchronize();
     c->graphs.clear();
@@ -152,7 +152,7 @@ void free_ctx(TrackCtx *c) {
                     (void *)c->d_shull, (void *)c->d_sbad, (void *)c->d_sids, (void *)c->d_sgender}) if (p) cudaFree(p);
     if (c->h_ids) cudaFreeHost(c->h_ids);
     if (c->ids_done) cudaEventDestroy(c->ids_done);
-    for (size_t i = 0; i < g_tr.size(); i++) if (g_tr[i] == c) { g_tr.erase(g_tr.begin() + i); break; }
+    engine_slot(c->eng, SLOT_TRACK) = nullptr;
     delete c;
 }
 
@@ -242,7 +242,7 @@ int uhc_track_begin(UhcEngine *e, int window, int kind, int pose_dim, const int 
     if ((size_t)E * window * REC * 8 > ((size_t)1 << 40)) { uhc_err() = "uhc_track_begin: window too large"; return -2; }
     if (TrackCtx *old = find_ctx(e)) free_ctx(old);
     if (trackx::install_table(e, window, fk_model_host, shape_host)) return -1;
-    TrackCtx *c = new TrackCtx(); c->eng = e; g_tr.push_back(c);
+    TrackCtx *c = new TrackCtx(); c->eng = e; engine_slot(e, SLOT_TRACK) = c;
     c->E = E; c->H = window; c->kind = kind; c->pose_dim = pose_dim; c->row_w = kind == UHC_MOTION_SMPL ? pose_dim + 3 : UHC_NQ;
     c->table_gen = trackx::table_gen(e); c->gen = ++g_tr_gen;
     const size_t En = E;
@@ -343,8 +343,8 @@ void uhc_track_end(UhcEngine *e) {
 }
 
 int uhc_track_graph_count(const UhcEngine *e) {
-    for (const TrackCtx *c : g_tr) if (c->eng == e) return (int)c->graphs.size();
-    return 0;
+    const TrackCtx *c = e ? (const TrackCtx *)engine_slot(e, SLOT_TRACK) : nullptr;
+    return c ? (int)c->graphs.size() : 0;
 }
 
 int uhc_track_subjects_enable(UhcEngine *e, const UhcSubjectBasis *basis) {

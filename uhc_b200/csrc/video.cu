@@ -12,6 +12,7 @@
 #include <string>
 #include <vector>
 #include "../../include/uhc_video.h"
+#include "engine_slots.h"
 #include "errors.h"
 #include "video_core.h"
 
@@ -41,7 +42,6 @@ size_t frame_scratch(const Geometry &g) {
 }
 
 struct VideoCtx {
-    UhcEngine *eng = nullptr;
     int16_t *d_coef = nullptr; size_t coef_cap = 0;
     uint32_t *d_words = nullptr; size_t words_cap = 0;
     int *d_seg_raw = nullptr, *d_seg_len = nullptr; size_t *d_seg_off = nullptr; size_t seg_cap = 0;
@@ -49,21 +49,11 @@ struct VideoCtx {
     uint8_t *d_hdr = nullptr;
     unsigned char *d_stage = nullptr; size_t stage_cap = 0;         // the files of a multi-pass call that could overflow out_cap
 };
-std::vector<VideoCtx *> g_vd;
 
 VideoCtx *get_ctx(UhcEngine *e) {
-    for (VideoCtx *c : g_vd) if (c->eng == e) return c;
-    VideoCtx *c = new VideoCtx();
-    c->eng = e;
-    g_vd.push_back(c);
-    return c;
-}
-
-void free_ctx(VideoCtx *c) {
-    cudaFree(c->d_coef); cudaFree(c->d_words); cudaFree(c->d_seg_raw); cudaFree(c->d_seg_len); cudaFree(c->d_seg_off);
-    cudaFree(c->d_fsize); cudaFree(c->d_foff); cudaFreeHost(c->h_fsize); cudaFree(c->d_hdr); cudaFree(c->d_stage);
-    for (size_t i = 0; i < g_vd.size(); i++) if (g_vd[i] == c) { g_vd.erase(g_vd.begin() + i); break; }
-    delete c;
+    void *&s = engine_slot(e, SLOT_VIDEO);
+    if (!s) s = new VideoCtx();
+    return (VideoCtx *)s;
 }
 
 // grows every scratch array to hold nf frames of geometry g; the stream is synchronised first (an earlier call may still use the old arrays)
@@ -327,9 +317,11 @@ int uhc_jpeg_encode(UhcEngine *e, const unsigned char *rgb_dev, long n, int W, i
 }
 
 void uhc_video_release(UhcEngine *e) {
-    if (!e) return;
-    for (VideoCtx *c : g_vd)
-        if (c->eng == e) { free_ctx(c); return; }
+    VideoCtx *c = e ? (VideoCtx *)engine_slot(e, SLOT_VIDEO) : nullptr;
+    if (!c) return;
+    cudaFree(c->d_coef); cudaFree(c->d_words); cudaFree(c->d_seg_raw); cudaFree(c->d_seg_len); cudaFree(c->d_seg_off);
+    cudaFree(c->d_fsize); cudaFree(c->d_foff); cudaFreeHost(c->h_fsize); cudaFree(c->d_hdr); cudaFree(c->d_stage);
+    delete c; engine_slot(e, SLOT_VIDEO) = nullptr;
 }
 
 }  // extern "C"

@@ -234,13 +234,6 @@ class Engine:
 
     def close(self):
         if getattr(self, "h", None):
-            self.lib.uhc_eval_release(self.h)
-            self.lib.uhc_track_end(self.h)
-            self.lib.uhc_render_release(self.h)
-            self.lib.uhc_video_release(self.h)
-            self.lib.uhc_floor_release(self.h)
-            self.lib.uhc_mesh_release(self.h)
-            self.lib.uhc_rollout_release(self.h)
             self.lib.uhc_engine_destroy(self.h)
             self.h = None
 
