@@ -39,6 +39,7 @@ struct EngineView {
     CurView cur;
 #if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
     long long *phase_cyc;   // [E][NPHASE] cycles per phase summed over control steps (null = not collected); UHC_PHASE_CLOCKS builds only
+    long long *phase_sub_cyc;   // [E][NSUBPHASE] the same per sub-phase of PC_KIN and PC_COLLIDE
 #endif
 };
 
@@ -372,6 +373,7 @@ UHC_DEV int env_step_warp(const EngineView<Real> &ev, int env, Work<Real> &w, co
 #if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
     PCLK(true, w, PC_EPILOGUE);
     if (ev.phase_cyc && (threadIdx.x & 31) == 0) for (int i = 0; i < NPHASE; i++) ev.phase_cyc[(size_t)env * NPHASE + i] += w.pc[i];
+    if (ev.phase_sub_cyc && (threadIdx.x & 31) == 0) for (int i = 0; i < NSUBPHASE; i++) ev.phase_sub_cyc[(size_t)env * NSUBPHASE + i] += w.ps[i];
 #endif
     return fail || end;
 }

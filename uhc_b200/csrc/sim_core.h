@@ -6,12 +6,13 @@
 // debugged on a CPU-only box.  The emulation is test infrastructure; the C-ABI library only ever launches the CUDA build.
 //
 // Algorithms (all world-aligned spatial vectors about the reference point O = root position):
-//   kinematics            level-synchronous tree pass, lane = body                         (a5: mj_kinematics)
+//   kinematics            every lane composes its own chain root -> body, lane = body       (a5: mj_kinematics)
 //   bias force C(q,v)     spatial recursive Newton-Euler, lane = body / lane = dof         (a5: mj_rne)
 //   linear solves         O(n) articulated-body sweeps over a centre-rooted 7-level tree, 6 lanes per body, 3x3 block
 //                         elimination, packed fp32 pairs (replaces mj_crb + mj_factorM + cho_solve)
 //   stable PD             (M_stale + Kd dt)^-1 rhs by the articulated-body solve             (a3: humanoid_im.py:1014-1076)
-//   floor contacts        plane / convex-hull support vertex + hull-graph neighbours        (a5: collision)
+//   floor contacts        plane / convex-hull support vertex + hull-graph neighbours, all   (a5: collision)
+//                         candidate bodies in one pass (a group of lanes per candidate)
 //   constraint solve      primal Newton on the convex soft-constraint cost, Newton direction = articulated-body solve with
 //                         contact-augmented body inertias, safeguarded 1-D Newton line search (a5: solver)
 //   integration           semi-implicit Euler, quaternion exponential map for the root      (a5: mj_Euler)
@@ -118,6 +119,8 @@ constexpr int VF_BODY_DIM = 9, MAX_ACT_DIM = NU + VF_BODY_DIM * NB + 30;
 // phases of a control step for the cycle accounting of UHC_PHASE_CLOCKS builds (PCLK below, scripts/step_phase_cycles.py)
 enum { PC_LOAD, PC_PD, PC_KIN, PC_COLLIDE, PC_SMOOTH, PC_CSETUP, PC_NEWTON_ABA, PC_NEWTON_ROWS, PC_SYNC_SUBSTEP, PC_SYNC_PD, PC_SYNC_SMOOTH,
        PC_INTEGRATE, PC_EPILOGUE, NPHASE };
+// sub-phases of PC_KIN (kin_rne_forward's stages, then project_force) and PC_COLLIDE (broad phase, narrow phase, contact ranges); PSUB below
+enum { PS_KIN_SINCOS, PS_KIN_LEVELS, PS_KIN_INERTIA, PS_KIN_SUBTREE, PS_KIN_PROJECT, PS_COL_BROAD, PS_COL_NARROW, PS_COL_PREFIX, NSUBPHASE };
 
 // per-environment working set (lives in shared memory on the GPU)
 template <class Real>
@@ -163,18 +166,23 @@ struct Work {
     alignas(8) EnvCfg<Real> cfg;
 #if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
     long long pc_t, pc[NPHASE];   // clock64 of the last phase boundary, cycles per phase of this control step
+    long long ps_t, ps[NSUBPHASE];   // clock64 of the last phase or sub-phase boundary, cycles per sub-phase of this control step
 #endif
 };
 
 // Phase cycle accounting, compiled in only with -DUHC_PHASE_CLOCKS: lane 0 of a warp reads clock64() at every phase boundary of the
 // control step and adds the interval since the previous boundary to that phase; env_step_warp adds the totals to EngineView::phase_cyc.
-// PCLK(on, w, ph) closes phase ph when `on` (the in-kernel reset runs substep_dynamics without it).  Without the switch both are empty.
+// PCLK(on, w, ph) closes phase ph when `on` (the in-kernel reset runs substep_dynamics without it).  PSUB(on, w, sp) closes sub-phase sp, which
+// runs from the last PCLK or PSUB; the sub-phases of a phase end with it, so they split its cycles.  Without the switch all three are empty.
 #if defined(UHC_PHASE_CLOCKS) && !defined(UHC_EMU)
-#define PCLK_START(w) do { __syncwarp(); if ((threadIdx.x & 31) == 0) { for (int i_ = 0; i_ < NPHASE; i_++) (w).pc[i_] = 0; (w).pc_t = clock64(); } } while (0)
-#define PCLK(on, w, ph) do { if (on) { __syncwarp(); if ((threadIdx.x & 31) == 0) { const long long t_ = clock64(); (w).pc[ph] += t_ - (w).pc_t; (w).pc_t = t_; } } } while (0)
+#define PCLK_START(w) do { __syncwarp(); if ((threadIdx.x & 31) == 0) { for (int i_ = 0; i_ < NPHASE; i_++) (w).pc[i_] = 0; \
+    for (int i_ = 0; i_ < NSUBPHASE; i_++) (w).ps[i_] = 0; (w).pc_t = (w).ps_t = clock64(); } } while (0)
+#define PCLK(on, w, ph) do { if (on) { __syncwarp(); if ((threadIdx.x & 31) == 0) { const long long t_ = clock64(); (w).pc[ph] += t_ - (w).pc_t; (w).pc_t = (w).ps_t = t_; } } } while (0)
+#define PSUB(on, w, sp) do { if (on) { __syncwarp(); if ((threadIdx.x & 31) == 0) { const long long t_ = clock64(); (w).ps[sp] += t_ - (w).ps_t; (w).ps_t = t_; } } } while (0)
 #else
 #define PCLK_START(w) do { } while (0)
 #define PCLK(on, w, ph) do { (void)sizeof(on); } while (0)
+#define PSUB(on, w, sp) do { (void)sizeof(on); } while (0)
 #endif
 
 // ------------------------------------------------------------------------------------------------ scalar helpers
@@ -308,6 +316,20 @@ template <class R> UHC_DEV void warp_argmin(R &x, int &i) {
 #define WBALLOT(n) __ballot_sync(0xffffffffu, (n) != 0)
 UHC_DEV int warp_excl_scan(int x, int lane) { int p = x; for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, p, o); if (lane >= o) p += t; } return p - x; }
 #define WEXSCAN(dst, src) { dst = warp_excl_scan(src, (int)(threadIdx.x & 31)); }
+// segmented over the aligned groups of G lanes (G a power of two): every lane gets its group's warp_argmin / bitwise OR
+template <class R> UHC_DEV void warp_seg_argmin(R &x, int &i, int G) {
+#pragma unroll 1
+    for (int o = G >> 1; o; o >>= 1) { R y = __shfl_xor_sync(0xffffffffu, x, o); int j = __shfl_xor_sync(0xffffffffu, i, o); if (y < x || (y == x && j < i)) { x = y; i = j; } }
+}
+UHC_DEV unsigned warp_seg_or(unsigned x, int G) {
+#pragma unroll 1
+    for (int o = G >> 1; o; o >>= 1) x |= __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+}
+#define WSEGARGMIN(x, i, G) warp_seg_argmin(x, i, G)
+#define WSEGOR(x, G) { x = warp_seg_or(x, G); }
+// dst = src of lane SRCL (a per-lane expression of `lane`), any 32-bit type
+#define WSHFLV(dst, src, SRCL) { const int lane = (int)(threadIdx.x & 31); (void)lane; dst = __shfl_sync(0xffffffffu, src, (SRCL)); }
 // bodies are numbered depth-first, so subtree(b) = lanes [b, sub_end]: subtree sum = difference of an inclusive warp prefix sum
 // The scan steps are a rolled loop over the offsets with the K components inside: the same additions per component, a fifth of the code
 template <class R, int K> UHC_DEV void subtree_sum(R (&x)[K], int sub_end, int lane) {
@@ -352,6 +374,11 @@ template <class R> static R emu_max(const R *x) { R s = x[0]; for (int i = 1; i 
 static unsigned emu_ballot(const int *x) { unsigned m = 0; for (int i = 0; i < 32; i++) if (x[i]) m |= 1u << i; return m; }
 #define WBALLOT(n) emu_ballot(n)
 #define WEXSCAN(dst, src) { int run_ = 0; for (int l_ = 0; l_ < 32; l_++) { const int t_ = src[l_]; dst[l_] = run_; run_ += t_; } }
+#define WSEGARGMIN(x, i, G) { for (int g_ = 0; g_ < 32; g_ += (G)) { __typeof__(x[0]) ox_ = x[g_]; int oi_ = i[g_]; \
+    for (int l_ = g_ + 1; l_ < g_ + (G); l_++) if (x[l_] < ox_ || (x[l_] == ox_ && i[l_] < oi_)) { ox_ = x[l_]; oi_ = i[l_]; } \
+    for (int l_ = g_; l_ < g_ + (G); l_++) { x[l_] = ox_; i[l_] = oi_; } } }
+#define WSEGOR(x, G) { for (int g_ = 0; g_ < 32; g_ += (G)) { unsigned o_ = 0; for (int l_ = g_; l_ < g_ + (G); l_++) o_ |= x[l_]; for (int l_ = g_; l_ < g_ + (G); l_++) x[l_] = o_; } }
+#define WSHFLV(dst, src, SRCL) { __typeof__(src[0]) t_[32]; for (int l_ = 0; l_ < 32; l_++) t_[l_] = src[l_]; for (int lane = 0; lane < 32; lane++) dst[lane] = t_[(SRCL)]; }
 template <class R, int K, class TP> static void emu_subtree(R (*x)[K], const TP *tp) {
     R out[32][K];
     for (int b = 0; b < 32; b++) for (int i = 0; i < K; i++) { R s = 0; for (int c = b; c <= tp[b].sub_end && c < 32; c++) s += x[c][i]; out[b][i] = s; }
@@ -364,7 +391,14 @@ template <class R, int K, class TP> static void emu_ancestor(R (*x)[K], const TP
 #define WPREFIX(n, K) { for (int l_ = 1; l_ < 32; l_++) for (int i_ = 0; i_ < K; i_++) n[l_][i_] += n[l_ - 1][i_]; }
 #define WANCESTOR(n, K, tp) emu_ancestor<Real, K>(n, tp)
 #endif
-UHC_DEV int popc_(unsigned x) { int c = 0; while (x) { x &= x - 1; c++; } return c; }
+// population count and the position of the k-th set bit (k = 0: the lowest; -1 when m has no more than k set bits)
+#ifndef UHC_EMU
+UHC_DEV int popc32(unsigned m) { return __popc(m); }
+UHC_DEV int nth_bit(unsigned m, int k) { return (int)__fns(m, 0u, k + 1); }
+#else
+UHC_DEV int popc32(unsigned m) { return __builtin_popcount(m); }
+UHC_DEV int nth_bit(unsigned m, int k) { for (int j = 0; j < k && m; ++j) m &= m - 1; return m ? __builtin_ctz(m) : -1; }
+#endif
 
 // ================================================================================================ articulated-body solve
 // Every linear system of a substep has the form  H x = b,  H = sum_b J_b^T Ihat_b J_b + diag(arm)  with J_b x = sum_{i on chain(b)} S_i x_i:
@@ -678,13 +712,79 @@ UHC_DEVNI void aba_solve(const Model<Real> &m, Work<Real> &w, Real arm_scale, bo
 }
 
 // ================================================================================================ kinematics + RNE
-// Forward pass over tree levels, lane = body: pose, motion subspaces S (about O = root position), spatial velocity V
+// One body's step of the forward pass, from its parent's pose R / pos, spatial velocity V and velocity-product acceleration A (in place) to
+// its own.  The chain of body b applies them root -> b; the motion subspaces are stored only by the lane that owns the body (store_S).
+// The root: free joint (translation dofs along world axes, rotation dofs about the body-frame axes through O)
+template <class Real>
+UHC_DEV void kin_root_step(const Model<Real> &m, Work<Real> &w, Real *R, Real *pos, Real *V, Real *A, bool store_S) {
+    Real qn[4] = {w.q[3], w.q[4], w.q[5], w.q[6]};
+    Real n = rsqrt_(qn[0] * qn[0] + qn[1] * qn[1] + qn[2] * qn[2] + qn[3] * qn[3]);
+    for (int i = 0; i < 4; i++) qn[i] *= n;
+    q2mat(qn, R);
+    pos[0] = w.q[0]; pos[1] = w.q[1]; pos[2] = w.q[2];
+    if (store_S) {
+        for (int k = 0; k < 3; k++) {  // translation dofs, world axes
+            for (int i = 0; i < 6; i++) w.S[k][i] = 0;
+            w.S[k][3 + k] = 1;
+        }
+        for (int k = 0; k < 3; k++) {  // rotation dofs: body-frame axes through O
+            w.S[3 + k][0] = R[k]; w.S[3 + k][1] = R[3 + k]; w.S[3 + k][2] = R[6 + k];
+            w.S[3 + k][3] = w.S[3 + k][4] = w.S[3 + k][5] = 0;
+        }
+    }
+    Real wl[3] = {w.v[3], w.v[4], w.v[5]}, ww[3], t[3];
+    mv3(R, wl, ww);
+    V[0] = ww[0]; V[1] = ww[1]; V[2] = ww[2]; V[3] = w.v[0]; V[4] = w.v[1]; V[5] = w.v[2];
+    cross3(ww, V + 3, t);  // spatial acceleration of the free body with qacc = 0 is (0, -w x v); minus gravity
+    A[0] = A[1] = A[2] = 0; A[3] = -t[0]; A[4] = -t[1]; A[5] = -t[2] - m.gravz;
+}
+// Body b >= 1: body-frame offset off[3] in the parent's frame, then three hinges z, y, x, each seen in the frame produced by the previous ones
+// (sc: sin, cos of the three joint angles)
+template <class Real>
+UHC_DEV void kin_hinge_step(Work<Real> &w, int b, const Real *off, const Real *sc, Real *R, Real *pos, Real *V, Real *A, bool store_S) {
+    Real p[3];
+    mv3(R, off, p);
+    for (int i = 0; i < 3; i++) pos[i] += p[i];
+    const Real r[3] = {pos[0] - w.q[0], pos[1] - w.q[1], pos[2] - w.q[2]};
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        const int dof = 6 + 3 * (b - 1) + j, col = 2 - j;
+        Real ax[3] = {R[col], R[3 + col], R[6 + col]}, t[3]; alignas(16) Real Sj[6], Sd[6];
+        cross3(r, ax, t);
+        Sj[0] = ax[0]; Sj[1] = ax[1]; Sj[2] = ax[2]; Sj[3] = t[0]; Sj[4] = t[1]; Sj[5] = t[2];
+        cross3(V, Sj, Sd);              // Sdot = V x_m S = (w x a, w x b + v x a)
+        cross3(V, Sj + 3, Sd + 3);
+        cross3(V + 3, Sj, t);
+        Sd[3] += t[0]; Sd[4] += t[1]; Sd[5] += t[2];
+        const Real qd = w.v[dof];
+        if (store_S) for (int i = 0; i < 6; i++) w.S[dof][i] = Sj[i];
+        paxpy6(qd, reinterpret_cast<const Pr<Real> *>(Sd), reinterpret_cast<Pr<Real> *>(A));
+        paxpy6(qd, reinterpret_cast<const Pr<Real> *>(Sj), reinterpret_cast<Pr<Real> *>(V));
+        const Real sn = sc[2 * j], cs = sc[2 * j + 1];
+        // R <- R * Rot(axis col, angle): rotate the two other columns
+        const int c1 = (col + 1) % 3, c2 = (col + 2) % 3;
+        for (int i = 0; i < 3; i++) {
+            const Real u = R[3 * i + c1], v2 = R[3 * i + c2];
+            R[3 * i + c1] = cs * u + sn * v2;
+            R[3 * i + c2] = -sn * u + cs * v2;
+        }
+    }
+}
+#ifndef UHC_EMU
+#define LGET(n, i, src) __shfl_sync(0xffffffffu, n[i], (src))   // inside a lane block, every lane: element i of lane src's n
+#else
+#define LGET(n, i, src) n[src][i]
+#endif
+
+// Forward pass, lane = body: pose, motion subspaces S (about O = root position), spatial velocity V
 // and velocity-product acceleration A (gravity folded in as a base acceleration), then per-body rigid inertia and the
 // inertial wrench F = I A + V x* (I V); subtree wrenches by warp prefix sums.
+// Every lane composes its own chain root -> body with the same steps (and so the same bits) its ancestors' lanes compute for themselves:
+// no level-by-level hand-off through shared memory.
 // MuJoCo semantics: SURVEY.md Appendix B (mj_kinematics / mj_comPos / mj_rne / mj_crb).
 template <class Real, class TPT>
-UHC_DEV void kin_rne_forward(const Model<Real> &m, Work<Real> &w, const TPT &tp) {
-    // joint-angle sines / cosines of every body in one lane = body pass (the level loop below only has a few lanes active per level)
+UHC_DEV void kin_rne_forward(const Model<Real> &m, Work<Real> &w, const TPT &tp, bool clk = false) {
+    // joint-angle sines / cosines of every body in one lane = body pass; the chains fetch their ancestors' from the owning lanes
     LVARA(Real, sc, 6);
     LANES_BEGIN
     const int b = lane;
@@ -694,71 +794,37 @@ UHC_DEV void kin_rne_forward(const Model<Real> &m, Work<Real> &w, const TPT &tp)
         LVA(sc)[2 * j] = sn; LVA(sc)[2 * j + 1] = cs;
     }
     LANES_END_R
-    for (int lvl = 0; lvl <= MAXLEVEL; ++lvl) {
-        LANES_BEGIN
-        const int b = lane;
-        if (b < NB && TP.depth == lvl) {
-            const Real *bf = m.body_f + b * BODYF;
-            Real R[9], pos[3]; alignas(16) Real V[6], A[6];
-            if (b == 0) {
-                Real qn[4] = {w.q[3], w.q[4], w.q[5], w.q[6]};
-                Real n = rsqrt_(qn[0] * qn[0] + qn[1] * qn[1] + qn[2] * qn[2] + qn[3] * qn[3]);
-                for (int i = 0; i < 4; i++) qn[i] *= n;
-                q2mat(qn, R);
-                pos[0] = w.q[0]; pos[1] = w.q[1]; pos[2] = w.q[2];
-                for (int k = 0; k < 3; k++) {  // translation dofs, world axes
-                    for (int i = 0; i < 6; i++) w.S[k][i] = 0;
-                    w.S[k][3 + k] = 1;
-                }
-                for (int k = 0; k < 3; k++) {  // rotation dofs: body-frame axes through O
-                    w.S[3 + k][0] = R[k]; w.S[3 + k][1] = R[3 + k]; w.S[3 + k][2] = R[6 + k];
-                    w.S[3 + k][3] = w.S[3 + k][4] = w.S[3 + k][5] = 0;
-                }
-                Real wl[3] = {w.v[3], w.v[4], w.v[5]}, ww[3], t[3];
-                mv3(R, wl, ww);
-                V[0] = ww[0]; V[1] = ww[1]; V[2] = ww[2]; V[3] = w.v[0]; V[4] = w.v[1]; V[5] = w.v[2];
-                cross3(ww, V + 3, t);  // spatial acceleration of the free body with qacc = 0 is (0, -w x v); minus gravity
-                A[0] = A[1] = A[2] = 0; A[3] = -t[0]; A[4] = -t[1]; A[5] = -t[2] - m.gravz;
-            } else {
-                const int p = TP.parent;
-                const Real *Rp = w.xmat[p];
-                Real off[3] = {UHC_LDG(bf), UHC_LDG(bf + 1), UHC_LDG(bf + 2)};
-                mv3(Rp, off, pos);
-                for (int i = 0; i < 3; i++) pos[i] += w.xpos[p][i];
-                for (int i = 0; i < 9; i++) R[i] = Rp[i];
-                for (int i = 0; i < 6; i++) { V[i] = w.Vb[p][i]; A[i] = w.Ab[p][i]; }
-                const Real r[3] = {pos[0] - w.q[0], pos[1] - w.q[1], pos[2] - w.q[2]};
-                // three hinges z, y, x, each seen in the frame produced by the previous ones
-#pragma unroll
-                for (int j = 0; j < 3; ++j) {
-                    const int dof = 6 + 3 * (b - 1) + j, col = 2 - j;
-                    Real ax[3] = {R[col], R[3 + col], R[6 + col]}, t[3]; alignas(16) Real Sj[6], Sd[6];
-                    cross3(r, ax, t);
-                    Sj[0] = ax[0]; Sj[1] = ax[1]; Sj[2] = ax[2]; Sj[3] = t[0]; Sj[4] = t[1]; Sj[5] = t[2];
-                    cross3(V, Sj, Sd);              // Sdot = V x_m S = (w x a, w x b + v x a)
-                    cross3(V, Sj + 3, Sd + 3);
-                    cross3(V + 3, Sj, t);
-                    Sd[3] += t[0]; Sd[4] += t[1]; Sd[5] += t[2];
-                    const Real qd = w.v[dof];
-                    for (int i = 0; i < 6; i++) w.S[dof][i] = Sj[i];
-                    paxpy6(qd, reinterpret_cast<const Pr<Real> *>(Sd), reinterpret_cast<Pr<Real> *>(A));
-                    paxpy6(qd, reinterpret_cast<const Pr<Real> *>(Sj), reinterpret_cast<Pr<Real> *>(V));
-                    const Real sn = LVA(sc)[2 * j], cs = LVA(sc)[2 * j + 1];
-                    // R <- R * Rot(axis col, angle): rotate the two other columns
-                    const int c1 = (col + 1) % 3, c2 = (col + 2) % 3;
-                    for (int i = 0; i < 3; i++) {
-                        const Real u = R[3 * i + c1], v2 = R[3 * i + c2];
-                        R[3 * i + c1] = cs * u + sn * v2;
-                        R[3 * i + c2] = -sn * u + cs * v2;
-                    }
-                }
-            }
-            for (int i = 0; i < 3; i++) w.xpos[b][i] = pos[i];
-            for (int i = 0; i < 9; i++) w.xmat[b][i] = R[i];
-            for (int i = 0; i < 6; i++) { w.Vb[b][i] = V[i]; w.Ab[b][i] = A[i]; }
+    PSUB(clk, w, PS_KIN_SINCOS);
+    LANES_BEGIN
+    const int b = lane, depth = b < NB ? (int)TP.depth : 0;
+    Real R[9], pos[3]; alignas(16) Real V[6], A[6];
+    kin_root_step(m, w, R, pos, V, A, b == 0);
+    int a = 0;       // the chain's body done last (depth d - 1)
+#pragma unroll 1
+    for (int d = 1; d <= MAXLEVEL; ++d) {
+        // next on the chain: the child of a whose subtree (depth-first numbering: [child, ..]) holds b
+        const LaneTopo &ta = TP_OF(m, tp, a);
+        int c = ta.ch0;
+        if (ta.ch1 >= 0 && ta.ch1 <= b) c = ta.ch1;
+        if (ta.ch2 >= 0 && ta.ch2 <= b) c = ta.ch2;
+        const bool act = d <= depth;
+        if (!act) c = 0;
+        Real s[6];
+        for (int i = 0; i < 6; i++) s[i] = LGET(sc, i, c);      // every lane takes part in the exchange
+        if (act) {
+            const Real *bf = m.body_f + c * BODYF;
+            const Real off[3] = {UHC_LDG(bf), UHC_LDG(bf + 1), UHC_LDG(bf + 2)};
+            kin_hinge_step(w, c, off, s, R, pos, V, A, c == b);
+            a = c;
         }
-        LANES_END
     }
+    if (b < NB) {
+        for (int i = 0; i < 3; i++) w.xpos[b][i] = pos[i];
+        for (int i = 0; i < 9; i++) w.xmat[b][i] = R[i];
+        for (int i = 0; i < 6; i++) { w.Vb[b][i] = V[i]; w.Ab[b][i] = A[i]; }
+    }
+    LANES_END
+    PSUB(clk, w, PS_KIN_LEVELS);
     // rigid inertia about O in world axes, inertial wrench; then subtree sums (composite inertia, subtree wrench)
     LVARA(Real, IF, 6);
     LANES_BEGIN
@@ -792,10 +858,12 @@ UHC_DEV void kin_rne_forward(const Model<Real> &m, Work<Real> &w, const TPT &tp)
         for (int e = 0; e < 6; e++) LVA(IF)[e] = IA[e];
     }
     LANES_END
+    PSUB(clk, w, PS_KIN_INERTIA);
     WSUBTREE(IF, 6, tp);
     LANES_BEGIN
     if (lane < NB) for (int e = 0; e < 6; e++) w.Fb[lane][e] = LVA(IF)[e];
     LANES_END
+    PSUB(clk, w, PS_KIN_SUBTREE);
 }
 
 // per-body spatial vector  X_b = sum_{i on chain(b)} S_i x_i   (root -> leaves), lane = body
@@ -831,7 +899,7 @@ UHC_DEV void project_force(const Model<Real> &m, Work<Real> &w, const Real (*F)[
 // ================================================================================================ collision
 // Floor plane z = 0 against each body hull (oracle/uhc_oracle.c or_collide states the manifold rule).
 template <class Real, class TPT>
-UHC_DEV void collide(const Model<Real> &m, Work<Real> &w, const TPT &tp) {
+UHC_DEV void collide(const Model<Real> &m, Work<Real> &w, const TPT &tp, bool clk = false) {
     // broad phase for all bodies at once (lane = body): bounding sphere against the plane
     LVAR(int, near); LVAR(int, cnt); LVAR(int, adr0);
     LANES_BEGIN
@@ -841,74 +909,107 @@ UHC_DEV void collide(const Model<Real> &m, Work<Real> &w, const TPT &tp) {
         const Real cz = w.xpos[lane][2] + R[6] * UHC_LDG(bf + 14) + R[7] * UHC_LDG(bf + 15) + R[8] * UHC_LDG(bf + 16);
         f = !(cz - UHC_LDG(bf + 17) > m.margin);
     }
-    LV(near) = f; LV(cnt) = 0;
+    LV(near) = f;
     LANES_END_R
     unsigned cand_b = WBALLOT(near);
-    int ncon = 0, upper = 0;
-    while (cand_b) {     // candidate bodies in ascending order
-        int b = 0; while (!((cand_b >> b) & 1u)) b++;
-        cand_b &= cand_b - 1;
-        if (ncon + 4 > MAXCON) { w.con_overflow = 1; continue; }   // flagged: env_step_warp turns it into fail (SI_FLAGS bit 0)
+    PSUB(clk, w, PS_COL_BROAD);
+    // narrow phase for every candidate body at once: candidate k (ascending body order) gets the aligned group of G = 2^lg lanes k G .. k G + G - 1
+    const int ncand = popc32(cand_b);
+    int lg = 5; while ((ncand << lg) > 32) lg--;
+    const int G = 1 << lg;
+    LVAR(int, cb); LVAR(Real, bz); LVAR(int, bi); LVAR(unsigned, nmask); LVAR(int, nck); LVAR(int, exk); LVAR(int, acc); LVAR(int, ovf); LVAR(int, up);
+    // deepest hull vertex: every lane scans the vertices sub, sub + G, .. of its candidate in ascending order and keeps the first lowest; the
+    // group's (height, index) minimum is then today's winner of the whole hull (lowest, then lowest index)
+    LANES_BEGIN
+    const int k = lane >> lg, sub = lane & (G - 1);
+    Real best = Real(1e30); int besti = 1 << 20, b = -1;
+    if (k < ncand) {
+        b = nth_bit(cand_b, k);
         const Real *R = w.xmat[b];
         const int adr = TP_OF(m, tp, b).hadr, nvt = TP_OF(m, tp, b).hnum;
-        // deepest hull vertex: every lane keeps its best vertex (height, index, body-frame coordinates)
-        LVAR(Real, bz); LVAR(int, bi); LVARA(Real, bv, 3); LVARA(Real, nv, 3);
-        LANES_BEGIN
-        Real best = Real(1e30); int besti = 1 << 20; Real b0 = 0, b1 = 0, b2 = 0;
-        for (int i = lane; i < nvt; i += 32) {
+#pragma unroll 1
+        for (int i = sub; i < nvt; i += G) {
             const Real *vv = m.hull + 3 * (adr + i);
             const Real v0 = UHC_LDG(vv), v1 = UHC_LDG(vv + 1), v2 = UHC_LDG(vv + 2);
             const Real z = w.xpos[b][2] + R[6] * v0 + R[7] * v1 + R[8] * v2;
-            if (z < best) { best = z; besti = i; b0 = v0; b1 = v1; b2 = v2; }
+            if (z < best) { best = z; besti = i; }
         }
-        LV(bz) = best; LV(bi) = besti; LVA(bv)[0] = b0; LVA(bv)[1] = b1; LVA(bv)[2] = b2;
-        LANES_END_R
-        Real minz; int mini;
-        WARGMIN(bz, bi, minz, mini);
-        if (minz > m.margin) continue;
-        // its hull-graph neighbours (lane = neighbour): the ones within the margin join the manifold, first three in list order
-        const int g = adr + mini, n0 = UHC_LDG(m.nbradr + g), nn = UHC_LDG(m.nbradr + g + 1) - n0;
-        LVAR(int, flag);
-        LANES_BEGIN
-        int f = 0;
-        if (lane < nn) {
-            const Real *vv = m.hull + 3 * (adr + UHC_LDG(m.nbr + n0 + lane));
+    }
+    LV(cb) = b; LV(bz) = best; LV(bi) = besti;
+    LANES_END_R
+    WSEGARGMIN(LV_ALL(bz), LV_ALL(bi), G);
+    // its hull-graph neighbours within the margin, as a mask in list order (the first three join the manifold)
+    LANES_BEGIN
+    const int k = lane >> lg, sub = lane & (G - 1), b = LV(cb);
+    unsigned f = 0;
+    if (k < ncand && !(LV(bz) > m.margin)) {
+        const Real *R = w.xmat[b];
+        const int adr = TP_OF(m, tp, b).hadr, g = adr + LV(bi), n0 = UHC_LDG(m.nbradr + g), nn = min_(UHC_LDG(m.nbradr + g + 1) - n0, 32);
+#pragma unroll 1
+        for (int j = sub; j < nn; j += G) {
+            const Real *vv = m.hull + 3 * (adr + UHC_LDG(m.nbr + n0 + j));
             const Real v0 = UHC_LDG(vv), v1 = UHC_LDG(vv + 1), v2 = UHC_LDG(vv + 2);
             const Real z = w.xpos[b][2] + R[6] * v0 + R[7] * v1 + R[8] * v2;
-            f = z <= m.margin;
-            LVA(nv)[0] = v0; LVA(nv)[1] = v1; LVA(nv)[2] = v2;
+            if (z <= m.margin) f |= 1u << j;
         }
-        LV(flag) = f;
-        LANES_END_R
-        const unsigned mask = WBALLOT(flag);
-        int nsel = 0; for (unsigned t = mask; t && nsel < 3; t &= t - 1) nsel++;
-        const int nc = 1 + nsel;
-        LANES_BEGIN
-        // slot 0: the deepest vertex (held by lane mini mod 32); slots 1..: flagged neighbours in lane order
-        int below = 0; for (unsigned t = mask & ((1u << lane) - 1u); t; t &= t - 1) below++;
-        const bool is_nb = ((mask >> lane) & 1u) && below < 3, is_min = lane == (mini & 31);
-        for (int pass = 0; pass < 2; ++pass) {
-            if (pass == 0 ? is_min : is_nb) {
-                const Real v0 = pass == 0 ? LVA(bv)[0] : LVA(nv)[0], v1 = pass == 0 ? LVA(bv)[1] : LVA(nv)[1], v2 = pass == 0 ? LVA(bv)[2] : LVA(nv)[2];
-                const Real px = w.xpos[b][0] + R[0] * v0 + R[1] * v1 + R[2] * v2;
-                const Real py = w.xpos[b][1] + R[3] * v0 + R[4] * v1 + R[5] * v2;
-                const Real pz = w.xpos[b][2] + R[6] * v0 + R[7] * v1 + R[8] * v2;
-                const int c = ncon + (pass == 0 ? 0 : 1 + below);
-                w.cbody[c] = b; w.cdist[c] = pz;
-                w.cr[c][0] = px - w.q[0]; w.cr[c][1] = py - w.q[1]; w.cr[c][2] = Real(0.5) * pz - w.q[2];
-            }
-        }
-        if (lane == b) LV(cnt) = nc;
-        LANES_END
-        ncon += nc;
-        if (b >= UPPER_BODY0) upper = 1;
     }
+    LV(nmask) = f;
+    LANES_END_R
+    WSEGOR(LV_ALL(nmask), G);
+    LANES_BEGIN
+    int nc = 0;
+    if ((lane >> lg) < ncand && !(LV(bz) > m.margin)) { const int nsel = popc32(LV(nmask)); nc = 1 + (nsel < 3 ? nsel : 3); }
+    LV(nck) = nc;
+    LANES_END_R
+    // lane k <- candidate k's contact count; in body order a candidate is skipped (and the overflow flagged) when the contacts of the ones taken
+    // before it leave fewer than 4 of the MAXCON slots.  The first skipped one leaves every later one skipped, so the taken ones are the
+    // candidates whose exclusive prefix count is <= MAXCON - 4, and their slots start at that prefix.
+    WSHFLV(LV_ALL(exk), LV_ALL(nck), (lane < ncand ? lane << lg : 31));
+    LANES_BEGIN
+    if (lane >= ncand) LV(exk) = 0;
+    LV(acc) = LV(exk);
+    LANES_END_R
+    WEXSCAN(LV_ALL(exk), LV_ALL(acc));
+    LANES_BEGIN
+    const bool ok = LV(exk) + 4 <= MAXCON;
+    LV(ovf) = lane < ncand && !ok;
+    LV(up) = lane < ncand && ok && LV(acc) > 0 && nth_bit(cand_b, lane) >= UPPER_BODY0;
+    if (!ok) LV(acc) = 0;
+    LANES_END_R
+    if (WBALLOT(ovf)) w.con_overflow = 1;   // flagged: env_step_warp turns it into fail (SI_FLAGS bit 0)
+    const int upper = WBALLOT(up) != 0;
+    // per body (lane = body): its taken count; per group: its candidate's taken count and first slot
+    WSHFLV(LV_ALL(cnt), LV_ALL(acc), (((cand_b >> lane) & 1u) ? popc32(cand_b & ((1u << lane) - 1u)) : 31));
+    WSHFLV(LV_ALL(nck), LV_ALL(acc), lane >> lg);
+    WSHFLV(LV_ALL(exk), LV_ALL(exk), lane >> lg);
+    // slot 0: the deepest vertex; slots 1..: the first three neighbours within the margin, in list order (lane sub writes slots sub, sub + G, ..)
+    LANES_BEGIN
+    const int nc = LV(nck), b = LV(cb);
+    if (nc > 0) {
+        const Real *R = w.xmat[b];
+        const int adr = TP_OF(m, tp, b).hadr, g = adr + LV(bi);
+#pragma unroll 1
+        for (int c = lane & (G - 1); c < nc; c += G) {
+            const int vi = c == 0 ? g : adr + UHC_LDG(m.nbr + UHC_LDG(m.nbradr + g) + nth_bit(LV(nmask), c - 1));
+            const Real *vv = m.hull + 3 * vi;
+            const Real v0 = UHC_LDG(vv), v1 = UHC_LDG(vv + 1), v2 = UHC_LDG(vv + 2);
+            const Real px = w.xpos[b][0] + R[0] * v0 + R[1] * v1 + R[2] * v2;
+            const Real py = w.xpos[b][1] + R[3] * v0 + R[4] * v1 + R[5] * v2;
+            const Real pz = w.xpos[b][2] + R[6] * v0 + R[7] * v1 + R[8] * v2;
+            const int slot = LV(exk) + c;
+            w.cbody[slot] = b; w.cdist[slot] = pz;
+            w.cr[slot][0] = px - w.q[0]; w.cr[slot][1] = py - w.q[1]; w.cr[slot][2] = Real(0.5) * pz - w.q[2];
+        }
+    }
+    LANES_END
+    PSUB(clk, w, PS_COL_NARROW);
     // contact ranges per body: exclusive prefix sum of the per-body counts (lane = body)
     WEXSCAN(LV_ALL(adr0), LV_ALL(cnt));
     LANES_BEGIN
     if (lane <= NB) w.bcon_adr[lane] = LV(adr0);
+    if (lane == NB) w.ncon = LV(adr0);
     LANES_END
-    w.ncon = ncon; w.upper_contact = upper;
+    w.upper_contact = upper;
 #ifndef UHC_EMU
     __syncwarp();
 #endif
@@ -1376,10 +1477,12 @@ UHC_DEVNI int substep_dynamics(const Model<Real> &m, const EnvCfg<Real> &cfg, Wo
             const bool explicit_rf = with_pd && cfg.rfc_mode == 1 && act_global != nullptr;
             if (explicit_rf) rfc_explicit(m, cfg, w, tp, act_global, w.as_);        // generalized force of the per-body residual forces (stale Jacobian) -> as_
             else if (with_pd && cfg.rfc_mode == 0) rfc_implicit(cfg, w, fapp);
-            kin_rne_forward(m, w, tp);
+            kin_rne_forward(m, w, tp, cta_sync);
             project_force(m, w, w.Fb, w.C, Real(1), (const Real *)nullptr);
+            PSUB(cta_sync, w, PS_KIN_PROJECT);
             PCLK(cta_sync, w, PC_KIN);
-            collide(m, w, tp);
+            collide(m, w, tp, cta_sync);
+            PSUB(cta_sync, w, PS_COL_PREFIX);
             PCLK(cta_sync, w, PC_COLLIDE);
             LANES_BEGIN
 #pragma unroll 1

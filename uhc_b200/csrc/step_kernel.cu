@@ -294,7 +294,7 @@ template <class Real> static int build_view(UhcEngine *e, EngineView<Real> &ev, 
     ev.cur.pct = nullptr; ev.cur.start = nullptr; ev.cur.meta = nullptr; ev.cur.max_freq = 0; ev.cur.fit_clip = -1; ev.cur.prec_freq = 0.f;
     ev.state = st; ev.istate = is; ev.expert = nullptr; ev.clip_adr = nullptr; ev.clip_shape = nullptr; ev.clip_model = nullptr; ev.clip_cdf = nullptr;
 #ifdef UHC_PHASE_CLOCKS
-    ev.phase_cyc = nullptr;
+    ev.phase_cyc = nullptr; ev.phase_sub_cyc = nullptr;
 #endif
     return 0;
 }
@@ -667,6 +667,13 @@ int uhc_phase_clocks(UhcEngine *e, long long *buf) {
     e->evf.phase_cyc = buf; e->evd.phase_cyc = buf;
     e->view_gen++;
     return NPHASE;
+}
+// The same for the sub-phases of PC_KIN and PC_COLLIDE (PS_*): buf is E x NSUBPHASE int64.  Returns NSUBPHASE.
+int uhc_phase_subclocks(UhcEngine *e, long long *buf) {
+    if (!e) { uhc_err() = "uhc_phase_subclocks: bad argument"; return -2; }
+    e->evf.phase_sub_cyc = buf; e->evd.phase_sub_cyc = buf;
+    e->view_gen++;
+    return NSUBPHASE;
 }
 #endif
 
