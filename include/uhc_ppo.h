@@ -15,6 +15,7 @@
  */
 #ifndef UHC_PPO_H
 #define UHC_PPO_H
+#include <stddef.h>
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -54,19 +55,29 @@ int uhc_ppo_trainer_create(const UhcNetDesc *policy, const UhcNetDesc *value, lo
 int uhc_ppo_trainer_create_mcp(const UhcNetDesc *policy_nets, int nprim, const UhcNetDesc *value, long max_rows, int max_envs, int device, UhcPpoTrainer **out);
 void uhc_ppo_trainer_destroy(UhcPpoTrainer *t);
 
+/* The collective the trainer's updates with world > 1 call: ncclAllReduce's signature, the stream passed as a void *.  The trainer calls it in
+ * place (sendbuff == recvbuff) with datatype 7 (ncclFloat32) and op 0 (ncclSum); a non-zero return fails the update. */
+typedef int (*UhcAllReduceFn)(const void *sendbuff, void *recvbuff, size_t count, int datatype, int op, void *comm, void *stream);
+/* installs fn as this trainer's all-reduce (another process-group implementation, or an in-process one for tests); NULL restores the default,
+ * ncclAllReduce from libnccl.so.2 */
+int uhc_ppo_trainer_set_all_reduce(UhcPpoTrainer *t, UhcAllReduceFn fn);
+
 /* One PPO iteration's update on a time-major [T][E] rollout (M = T*E rows, row = t*E + e):
  *   states [M][dims[0]] normalised observations, last_states [E][dims[0]] the normalised observation after the last step (bootstrap V(s_T)),
  *   actions [M][A], rewards / masks / exps [M], log_std [A].
  *   adam_step_policy / adam_step_value (host, in/out): optimiser step counters; policy_steps_done (host, in/out): policy steps of this run so far.
  *   zfilter_stats / zfilter_sync (world > 1, may be NULL when world == 1): the running observation statistics [n, mean[D], S[D]] of this rank and
  *   the additive form [n, sum, sumsq] of what every rank agreed on last; on return every rank holds the merged statistics.
- *   nccl_comm: ncclComm_t of the training job (NULL = single GPU); world = its size.
- *   losses_out (device, 2 floats): clipped-surrogate loss and value loss of the last epoch (global means). */
+ *   nccl_comm: ncclComm_t of the training job (NULL = single GPU); world = its size.  Every rank must pass the same T and E: the value
+ *   gradient is scaled by 1 / (T E world), and ranks whose gradient tensors differ in length cannot all-reduce them.
+ *   losses_out (device, 2 floats): clipped-surrogate loss and value loss of the last epoch.  world == 1: the batch's means; world > 1: this
+ *   rank's share of the global means (their sum over the ranks is the global loss; nothing sums it). */
 int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_states, const float *actions, const float *rewards, const float *masks,
                    const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
                    int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out, void *stream);
 
-/* AgentPPO.update_policy (agent_ppo.py:16-51) alone: the epochs on caller-provided returns and (already normalised) advantages, M rows. */
+/* AgentPPO.update_policy (agent_ppo.py:16-51) alone: the epochs on caller-provided returns and (already normalised) advantages, M rows.
+ * Single GPU only: world > 1 returns -2 (the selected-row count it would divide the policy gradient by is this rank's, not the global one). */
 int uhc_ppo_update_policy(UhcPpoTrainer *t, const float *states, const float *actions, const float *returns, const float *advantages, const float *exps,
                           const float *log_std, long M, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value, int *policy_steps_done,
                           void *nccl_comm, int world, float *losses_out, void *stream);

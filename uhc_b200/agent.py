@@ -129,6 +129,8 @@ class BatchedAgent:
         self.torch = torch
         self.dev = torch.device("cuda", device)
         torch.cuda.set_device(self.dev)
+        if world > 1 and not update_tc:
+            raise ValueError("BatchedAgent: the fp32 update (update_tc=False) is single-GPU only: it has no gradient all-reduce")
         self.E, self.seed, self.rank, self.world = num_envs, seed, rank, world
         self.auto_reset = bool(env_cfg.pop("auto_reset", True))
         self.engine = Engine(num_envs, model=model, device=device, precision=precision, variants=variants, auto_reset=int(self.auto_reset), t_min=t_min, t_max=t_max,
@@ -322,7 +324,7 @@ class BatchedAgent:
             tail = self.value.gfull[self.value.nflat:]
             tail.zero_()
             nd = d.numel()
-            assert planes.numel() <= tail.numel()
+            assert planes.numel() == nn.stats_tail_floats(D) <= tail.numel()
             tail[:planes.numel()].copy_(planes.reshape(-1))
             ntot = t.zeros(1, device=self.dev, dtype=t.float64)
 

@@ -13,6 +13,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
+#include <atomic>
 #include <string>
 #include "../../include/uhc_nn.h"
 #include "errors.h"
@@ -629,11 +630,10 @@ __global__ void k_dact_bf16(const float *__restrict__ dh, const float *__restric
 typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
                              const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeFn get_encode() {
-    static EncodeFn fn = nullptr;
-    if (!fn) {
+    static const EncodeFn fn = [] {       // a function-local static: initialised once even when threads make their first GEMM calls at once
         void *p = nullptr; cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess) fn = (EncodeFn)p;
-    }
+        return cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess ? (EncodeFn)p : (EncodeFn) nullptr;
+    }();
     return fn;
 }
 int make_map(CUtensorMap *m, const void *base, int rows, int Kp, int box_rows = BM) {  // row-major [rows][Kp] bf16, box 64 x 128, 128B swizzle
@@ -658,14 +658,14 @@ int make_map_out(CUtensorMap *m, const void *base, int rows, int cols, size_t pi
     return 0;
 }
 bool tma_store_enabled() {
-    static int on = -1;
-    if (on < 0) { const char *e = getenv("UHC_TC_TMA_STORE"); on = e ? (e[0] != '0') : (UHC_TC_TMA_STORE != 0); }
-    return on != 0;
+    static const bool on = [] { const char *e = getenv("UHC_TC_TMA_STORE"); return e ? (e[0] != '0') : (UHC_TC_TMA_STORE != 0); }();
+    return on;
 }
 int sm_count(int dev) { int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); return sms; }
-// per device: the kernels' shared-memory attribute belongs to the function on the CURRENT device
+// per device: the kernels' shared-memory attribute belongs to the function on the CURRENT device.  Atomic flags: host threads may make their
+// first GEMM calls at once (one per rank of an in-process group); setting the attribute twice is harmless, a torn flag is not.
 int set_smem_attr(int dev) {
-    static bool attr_set[64] = {false};
+    static std::atomic<bool> attr_set[64] = {};
     if (dev >= 0 && dev < 64 && attr_set[dev]) return 0;
     if (cudaFuncSetAttribute(k_linear_tc<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
         cudaFuncSetAttribute(k_linear_tc<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { uhc_err() = "cudaFuncSetAttribute failed"; return -1; }
@@ -772,7 +772,7 @@ int uhc_linear_forward_tc_grouped(int G, const int *row0_host, const int *rows_h
     }
     for (int g = 0; g < G; g++) if (!W_bf16_host[g]) { uhc_err() = "uhc_linear_forward_tc_grouped: null weights"; return -2; }
     int dev = 0; cudaGetDevice(&dev);
-    static bool attr_set[64] = {false};
+    static std::atomic<bool> attr_set[64] = {};
     if (!(dev >= 0 && dev < 64 && attr_set[dev])) {
         if (cudaFuncSetAttribute(k_linear_tc_grouped, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) { uhc_err() = "cudaFuncSetAttribute failed"; return -1; }
         if (dev >= 0 && dev < 64) attr_set[dev] = true;

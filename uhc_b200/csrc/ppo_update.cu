@@ -93,14 +93,12 @@ __global__ void k_count_selected(const float *__restrict__ exps, size_t n, doubl
 __global__ void k_inv_count(const double *__restrict__ cnt, float *__restrict__ inv) { const double c = cnt[0]; inv[0] = (float)(1.0 / (c < 1.0 ? 1.0 : c)); }
 
 // ---- NCCL without a link-time dependency: the process that hands us an ncclComm_t has libnccl loaded already
-typedef int (*AllReduceFn)(const void *, void *, size_t, int, int, void *, cudaStream_t);
-AllReduceFn nccl_all_reduce() {
-    static AllReduceFn fn = nullptr;
-    if (!fn) {
+UhcAllReduceFn nccl_all_reduce() {
+    static const UhcAllReduceFn fn = [] {       // a function-local static: one lookup, however many threads update at once
         void *h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD);
         if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
-        if (h) fn = (AllReduceFn)dlsym(h, "ncclAllReduce");
-    }
+        return h ? (UhcAllReduceFn)dlsym(h, "ncclAllReduce") : (UhcAllReduceFn) nullptr;
+    }();
     return fn;
 }
 constexpr int NCCL_FLOAT32 = 7, NCCL_SUM = 0;
@@ -126,6 +124,7 @@ struct UhcPpoTrainer {
     cudaEvent_t ev_ready = nullptr, ev_v = nullptr, ev_p = nullptr;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timing; size_t timing_used = 0;
     long comm_bytes = 0; int comm_calls = 0;
+    UhcAllReduceFn all_reduce = nullptr;     // uhc_ppo_trainer_set_all_reduce; nullptr = ncclAllReduce
     long launches = 0;
     std::vector<void *> allocs;
 };
@@ -233,7 +232,7 @@ int policy_backward(UhcPpoTrainer *t, const float *dmean, long M, cudaStream_t s
     return net_backward(t, t->pnets[P], t->pbufs[P], t->dcomp, M, st);
 }
 int start_all_reduce(UhcPpoTrainer *t, void *comm, float *buf, size_t n, cudaEvent_t done, cudaStream_t st) {
-    AllReduceFn ar = nccl_all_reduce();
+    const UhcAllReduceFn ar = t->all_reduce ? t->all_reduce : nccl_all_reduce();
     if (!ar) { uhc_err() = "uhc_ppo_update: an ncclComm_t was passed but libnccl.so.2 / ncclAllReduce cannot be resolved"; return -1; }
     CK(cudaEventRecord(t->ev_ready, st));
     CK(cudaStreamWaitEvent(t->side, t->ev_ready, 0));
@@ -243,8 +242,12 @@ int start_all_reduce(UhcPpoTrainer *t, void *comm, float *buf, size_t n, cudaEve
     }
     auto &tm = t->timing[t->timing_used++];
     CK(cudaEventRecord(tm.first, t->side));
-    const int rc = ar(buf, buf, n, NCCL_FLOAT32, NCCL_SUM, comm, t->side);
-    if (rc != 0) { uhc_err() = "ncclAllReduce failed with code " + std::to_string(rc); return -1; }
+    const int rc = ar(buf, buf, n, NCCL_FLOAT32, NCCL_SUM, comm, (void *)t->side);
+    if (rc != 0) {
+        --t->timing_used;     // its end event was never recorded: uhc_ppo_comm_stats must not read the pair
+        uhc_err() = std::string("the gradient all-reduce (") + (t->all_reduce ? "the installed collective" : "ncclAllReduce") + ") failed with code " + std::to_string(rc);
+        return -1;
+    }
     CK(cudaEventRecord(tm.second, t->side));
     CK(cudaEventRecord(done, t->side));
     t->comm_bytes += (long)(n * sizeof(float)); t->comm_calls++;
@@ -369,6 +372,12 @@ void uhc_ppo_trainer_destroy(UhcPpoTrainer *t) {
     delete t;
 }
 
+int uhc_ppo_trainer_set_all_reduce(UhcPpoTrainer *t, UhcAllReduceFn fn) {
+    if (!t) { uhc_err() = "uhc_ppo_trainer_set_all_reduce: null trainer"; return -2; }
+    t->all_reduce = fn;
+    return 0;
+}
+
 long uhc_ppo_kernel_launches(const UhcPpoTrainer *t) { return t ? t->launches : 0; }
 const float *uhc_ppo_advantages(const UhcPpoTrainer *t) { return t ? t->adv : nullptr; }
 const float *uhc_ppo_returns(const UhcPpoTrainer *t) { return t ? t->ret : nullptr; }
@@ -434,7 +443,9 @@ int uhc_ppo_update_policy(UhcPpoTrainer *t, const float *states, const float *ac
     if (!t || !states || !actions || !returns || !advantages || !exps || !log_std || !cfg || !adam_step_policy || !adam_step_value || !policy_steps_done || !losses_out ||
         M <= 0 || world < 1) { uhc_err() = "uhc_ppo_update_policy: bad argument"; return -2; }
     if (M > t->cap) { uhc_err() = "uhc_ppo_update_policy: the batch exceeds the trainer's capacity"; return -2; }
-    if (world > 1 && !nccl_comm) { uhc_err() = "uhc_ppo_update_policy: world > 1 needs an ncclComm_t"; return -2; }
+    // sharded, the policy gradient would be divided by this rank's selected-row count while the value gradient is divided by the global row
+    // count; the global statistics travel only with uhc_ppo_update's collective
+    if (world > 1) { uhc_err() = "uhc_ppo_update_policy: world > 1 is not supported (the global selected-row count is unknown here): use uhc_ppo_update"; return -2; }
     CK(cudaSetDevice(t->device));
     cudaStream_t st = (cudaStream_t)stream;
     g_launches = 0;
@@ -446,8 +457,7 @@ int uhc_ppo_update_policy(UhcPpoTrainer *t, const float *states, const float *ac
     CK(cudaMemcpyAsync(t->ret, returns, (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CK(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
     ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CK(cudaGetLastError());
-    ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CK(cudaGetLastError());      // (a sharded caller passes world = 1 per shard or pre-scales exps)
-    return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, nullptr, nullptr, world > 1 ? nccl_comm : nullptr, world, false,
-                      false, losses_out, st);
+    ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CK(cudaGetLastError());
+    return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, nullptr, nullptr, nullptr, 1, false, false, losses_out, st);
 }
 }  // extern "C"

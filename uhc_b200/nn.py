@@ -27,6 +27,13 @@ def _stream(t):
     return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
 
 
+def stats_tail_floats(in_dim):
+    """floats after a net's gradients in its flat gradient tensor: a world > 1 update carries its global statistics there through the value
+    gradient's all-reduce, as split_double's 5 digit planes of [advantage sum, sum of squares, rows, selected rows, the ZFilter increment
+    (n, sum[D], sum of squares[D])], 5 (5 + 2 D) floats for an input width D (include/uhc_ppo.h UhcNetDesc.gtail)"""
+    return SPLIT_CHUNKS * (4 + 1 + 2 * in_dim)
+
+
 def linear_forward(x, W, b, act="none", save_z=False):
     import torch
     M, K = x.shape
@@ -69,6 +76,7 @@ class MLPNet:
         # gradient all-reduce (SURVEY.md section 8e) -- so Adam is one launch per net and the collective needs no flatten / copy.
         offs, o = self.flat_layout(self.dims)
         self._offs, self.nflat = offs, o
+        self.grad_tail = stats_tail_floats(in_dim)
         self._storage = storage
         if storage is None:
             self.flat = torch.zeros(o, device=device, dtype=torch.float32)
@@ -117,13 +125,11 @@ class MLPNet:
         out.net = self
         return out
 
-    GRAD_TAIL = 8192            # floats after the gradients in the flat gradient tensor (statistics riding the all-reduce)
-
     @property
     def gfull(self):
         """flat gradients + tail, allocated on first use (a net living in shared storage sees its slice of the owner's gradient tensor, no tail)"""
         if self._gfull is None:
-            self._gfull = self.torch.zeros(self.nflat + self.GRAD_TAIL, device=self.flat.device, dtype=self.torch.float32)
+            self._gfull = self.torch.zeros(self.nflat + self.grad_tail, device=self.flat.device, dtype=self.torch.float32)
         return self._gfull
 
     @property
@@ -246,17 +252,15 @@ class MCPNet:
     """PolicyMCP (uhc/models/policy_mcp.py:9-37, actor_type "mcp"): num_primitive MLPs state -> policy_hsize -> action (head weight x 0.1, bias 0) and a
     composer MLP state -> composer_dim -> num_primitive whose every layer is activated, then a softmax; action_mean = sum_k w_k prim_k(x).
     All parameters live in ONE flat tensor (and the gradients in one), the sub-nets are views: Adam and the gradient all-reduce see a single net."""
-    GRAD_TAIL = MLPNet.GRAD_TAIL
-
     def __init__(self, in_dim, hsize, out_dim, htype="relu", num_primitive=8, composer_dim=(300, 200), device="cuda", seed=None):
         import torch
         self.torch, self.htype, self.num_primitive, self.head_name = torch, htype, num_primitive, "mcp"
         self.dims = [in_dim] + list(hsize) + [out_dim]
         pd, cd = [in_dim] + list(hsize) + [out_dim], [in_dim] + list(composer_dim) + [num_primitive]
         n_p, n_c = MLPNet.flat_layout(pd)[1], MLPNet.flat_layout(cd)[1]
-        self.nflat = num_primitive * n_p + n_c
+        self.nflat, self.grad_tail = num_primitive * n_p + n_c, stats_tail_floats(in_dim)
         self.flat = torch.zeros(self.nflat, device=device, dtype=torch.float32)
-        self.gfull = torch.zeros(self.nflat + self.GRAD_TAIL, device=device, dtype=torch.float32)
+        self.gfull = torch.zeros(self.nflat + self.grad_tail, device=device, dtype=torch.float32)
         g = torch.Generator().manual_seed(seed) if seed is not None else None
         self.prims = [MLPNet(in_dim, hsize, out_dim, htype, device=device, storage=(self.flat, self.gfull, k * n_p), generator=g) for k in range(num_primitive)]
         self.composer = MLPNet(in_dim, composer_dim, num_primitive, htype, device=device, storage=(self.flat, self.gfull, num_primitive * n_p), head_act=htype,
@@ -716,6 +720,10 @@ def ppo_epochs_tc(policy, value, log_std, opt_p, opt_v, xb, xT, actions, returns
     return losses
 
 
+# include/uhc_ppo.h UhcAllReduceFn: ncclAllReduce's signature, the stream as a void *
+ALL_REDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_void_p)
+
+
 class UhcNetDesc(C.Structure):
     """include/uhc_ppo.h UhcNetDesc"""
     _fields_ = [("nlayers", C.c_int), ("act", C.c_int), ("dims", C.c_int * 10), ("flat", C.c_void_p), ("gfull", C.c_void_p), ("nflat", C.c_long), ("gtail", C.c_long),
@@ -740,7 +748,7 @@ def net_desc(net, opt, owner=None):
     d.nlayers, d.act, d.head_act = len(net.W), ACT[net.htype], ACT[net.head_act]
     for i, v in enumerate(net.dims):
         d.dims[i] = v
-    d.flat, d.gfull, d.nflat, d.gtail = top.flat.data_ptr(), top.gfull.data_ptr(), top.nflat, top.GRAD_TAIL
+    d.flat, d.gfull, d.nflat, d.gtail = top.flat.data_ptr(), top.gfull.data_ptr(), top.nflat, top.grad_tail
     for i in range(len(net.W)):
         d.w_off[i], d.b_off[i] = base + net._offs[2 * i][0], base + net._offs[2 * i + 1][0]
         d.W_bf16[i], d.kp[i] = net._bf16_store[i].data_ptr(), net._bf16_store[i].shape[1]
@@ -774,9 +782,10 @@ def make_nccl_comm(rank, world, device):
 
 class CPpoTrainer:
     """uhc_ppo_update (include/uhc_ppo.h): V(s), GAE, advantage normalisation and the PPO epochs of both nets behind ONE C-ABI call, with the
-    gradient all-reduce on the given ncclComm_t."""
+    gradient all-reduce on the given ncclComm_t.  all_reduce: an ALL_REDUCE_FN the trainer calls instead of ncclAllReduce (the `comm` passed to
+    update() reaches it unchanged); the trainer keeps a reference to it."""
 
-    def __init__(self, policy, value, opt_p, opt_v, max_rows, max_envs, device):
+    def __init__(self, policy, value, opt_p, opt_v, max_rows, max_envs, device, all_reduce=None):
         L = _lib()
         L.uhc_ppo_advantages.restype = C.c_void_p
         L.uhc_ppo_returns.restype = C.c_void_p
@@ -797,6 +806,9 @@ class CPpoTrainer:
             rc = L.uhc_ppo_trainer_create(C.byref(self.dp), C.byref(self.dv), C.c_long(max_rows), C.c_int(max_envs), C.c_int(dev or 0), C.byref(self.h))
         _check(rc, "uhc_ppo_trainer_create")
         self.max_rows, self.max_envs = max_rows, max_envs
+        self.all_reduce = all_reduce
+        if all_reduce is not None:
+            _check(L.uhc_ppo_trainer_set_all_reduce(self.h, all_reduce), "uhc_ppo_trainer_set_all_reduce")
 
     def close(self):
         if getattr(self, "h", None) is not None and self.h:
