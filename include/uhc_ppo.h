@@ -75,6 +75,14 @@ int uhc_ppo_trainer_set_all_reduce(UhcPpoTrainer *t, UhcAllReduceFn fn);
 int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_states, const float *actions, const float *rewards, const float *masks,
                    const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
                    int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out, void *stream);
+/* uhc_ppo_update with an extra payload on the same collective: the n_extra device floats at extra_in ride behind the statistics in the value
+ * gradient's tail, and right after the first value all-reduce their sum over the ranks is copied to extra_out (world == 1: extra_in itself).
+ * With world > 1 the value net's gtail must hold 5 (5 + 2 dims[0]) + n_extra floats, or the call returns -2.  The payload changes no gradient
+ * element: it only lengthens the tail.  n_extra == 0 is uhc_ppo_update (the global curriculum's payload: uhc_curriculum_stage, uhc_rollout.h). */
+int uhc_ppo_update_ex(UhcPpoTrainer *t, const float *states, const float *last_states, const float *actions, const float *rewards, const float *masks,
+                      const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
+                      int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out,
+                      const float *extra_in, float *extra_out, long n_extra, void *stream);
 
 /* AgentPPO.update_policy (agent_ppo.py:16-51) alone: the epochs on caller-provided returns and (already normalised) advantages, M rows.
  * Single GPU only: world > 1 returns -2 (the selected-row count it would divide the policy gradient by is this rank's, not the global one). */

@@ -61,6 +61,15 @@ int uhc_curriculum_enable(UhcEngine *e, int max_freq, double temp, double freq, 
  * all required), step-major then env-minor, keeps each clip's last max_freq, and rewrites the clip CDF in place from the new weights
  * (the sample_keys rule while every history is empty). */
 int uhc_curriculum_update(UhcEngine *e, const UhcRolloutBuf *buf, int T, void *stream);
+/* One history across the ranks of a data-parallel run, carried by the gradient all-reduce (uhc_ppo_update_ex's extra payload):
+ * uhc_curriculum_stage zeroes `slots` ([world][T][E][3] fp32, world * T * E * 3 floats) and writes rows 0 .. T-1 of buf (ep_clip, ep_pct, ep_start
+ * all required) into slot `rank` as (clip, percent, start), (-1, 0, 0) where no episode ended.  Summed over the ranks, the slots are every rank's
+ * log exactly (every element is one rank's value plus zeros).  uhc_curriculum_update_gathered unpacks such a sum into one log of world * T * E
+ * entries, rank-major, then step-major, then env-minor, and appends it as uhc_curriculum_update does: after it every rank holds the rings and the
+ * CDF one curriculum fed with every rank's log would hold.  Stream-ordered, no host synchronise.  Both return -2 for bad arguments and when a
+ * clip index or a start frame could exceed 2^24 (more than 2^24 clips, or a clip longer than 2^24 frames), where fp32 stops being exact. */
+int uhc_curriculum_stage(UhcEngine *e, const UhcRolloutBuf *buf, int T, int rank, int world, float *slots, void *stream);
+int uhc_curriculum_update_gathered(UhcEngine *e, const float *summed_slots, int T, int world, void *stream);
 /* host-side history: append n outcomes in order (eval results); read / replace every clip's history, oldest first:
  * len_host [C], pct_host / start_host [C][max_freq] (entries past len[c] are ignored / zero).  Each updates the CDF. */
 int uhc_curriculum_push(UhcEngine *e, int n, const int *clip_host, const float *pct_host, const int *start_host);

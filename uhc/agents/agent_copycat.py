@@ -120,7 +120,7 @@ class AgentCopycat:
             has_shape=bool(cfg.get("has_shape", False)) and bool(cfg.get("has_shape_obs", True)), actor_type=cfg.actor_type, num_primitive=int(cfg.get("num_primitive", 8)), composer_dim=tuple(cfg.get("composer_dim", [300, 200])),
             reactive_v=int(cfg.get("reactive_v", 0)), reactive_rate=float(cfg.get("reactive_rate", 0.3)),
             term_body=cfg.get("env_term_body", "body"), head_body=self.model_tables.body_names.index("Head"), reward_mul=cfg.reward_id == "world_rfc_implicit_v1_mul",
-            variants=self._subjects and self._subjects[0], subject_of=self._subjects and self._subject_of)
+            variants=self._subjects and self._subjects[0], subject_of=self._subjects and self._subject_of, curriculum_global=bool(cfg.get("curriculum_global", False)))
         self.policy_net, self.value_net, self.running_state = self.agent.policy, self.agent.value, self.agent.running_state
         self.state_dim, self.action_dim = self.agent.obs_dim, self.agent.act_dim
         self.expert_reward = reward_func[cfg.reward_id]
@@ -129,10 +129,11 @@ class AgentCopycat:
         for loader in self.test_data_loaders:                   # a separate test set: fixed here, before any evaluation reads its length
             loader.fix_floor(self.agent.engine, self.logger.info)
         # the failure-weighted curriculum (freq_dict): on the host (default) or, with curriculum_on_device, in device rings updated after
-        # every rollout (Engine.curriculum_*).  precision_mode and fit_single_key need the device curriculum and turn it on
+        # every rollout (Engine.curriculum_*).  precision_mode and fit_single_key need the device curriculum and turn it on, and so does
+        # curriculum_global: one history across the ranks of a multi-GPU run, merged from every rank's episodes in each update
         self._precision_mode = bool(cfg.get("precision_mode", False))
         self._fit_single_key = ""
-        self.curriculum_on_device = bool(cfg.get("curriculum_on_device", False)) or self._precision_mode
+        self.curriculum_on_device = bool(cfg.get("curriculum_on_device", False)) or self._precision_mode or self.agent.curriculum_global
         if self.curriculum_on_device:
             self._enable_device_curriculum()
         if checkpoint_epoch > 0:
@@ -758,7 +759,8 @@ class AgentCopycat:
     # ---------------------------------------------------------------- checkpoints (:190-260)
     def save_checkpoint(self, epoch):
         """pickle {"policy_dict", "value_dict", "running_state": ZFilter} (agent_copycat.py:190-201).  Multi-GPU: every rank holds identical
-        weights and running_state (uhc_b200/agent.py update_params), so rank 0 alone writes the file."""
+        weights and running_state (uhc_b200/agent.py update_params), so rank 0 alone writes the file; with curriculum_global its freq_dict.pt
+        is every rank's history too, otherwise rank 0's own."""
         cfg = self.cfg
         path = "%s/iter_%04d.p" % (cfg.model_dir, epoch + 1)
         if int(os.environ.get("RANK", "0")) == 0:

@@ -124,7 +124,10 @@ class BatchedAgent:
                  value_hsize=(2048, 1024, 512), htype="gelu", log_std=-2.3, policy_lr=5e-5, value_lr=3e-4, gamma=0.95, tau=0.95,
                  clip_epsilon=0.2, num_optim_epoch=10, grad_clip=40.0, t_min=5, t_max=300, noise_rate=1.0, rank=0, world=1,
                  grad_sync=None, model=None, update_tc=True, variants=None, clip_models=None, c_update=True, actor_type="gauss", num_primitive=8,
-                 composer_dim=(300, 200), subject_of=None, **env_cfg):
+                 composer_dim=(300, 200), subject_of=None, curriculum_global=False, **env_cfg):
+        """curriculum_global: one failure-weighted curriculum across the ranks of a data-parallel run (turns the device curriculum on with its
+        default parameters): every rank's episode log rides the first gradient all-reduce of update_params, and every rank merges all of them
+        into bit-identical rings.  At world 1 it is the device curriculum."""
         import torch
         self.torch = torch
         self.dev = torch.device("cuda", device)
@@ -169,6 +172,10 @@ class BatchedAgent:
         self.ep_ret = torch.zeros(num_envs, device=self.dev, dtype=torch.float32)
         self.nn_launches = 0
         self._notdone = torch.zeros(num_envs, device=self.dev, dtype=torch.bool)
+        self.curriculum_global = bool(curriculum_global)
+        self._cur_staged = None           # T of the rollout whose episode log waits in _cur_slots for the next update_params (global curriculum)
+        if self.curriculum_global:
+            self.curriculum_enable()
 
     # ---- env.reset for a subset with freshly sampled clip slices
     def reset_envs(self, ids=None):
@@ -234,6 +241,9 @@ class BatchedAgent:
         """agent.sample(): T lock-step control steps of all envs.  Returns (buffer, log).  c_loop (default: whenever auto_reset is on):
         the loop runs behind the C ABI as one CUDA graph; otherwise the Python loop over step_once (identical kernels and results)."""
         t = self.torch
+        staging = self.engine.cur_cfg is not None and self._merges_across_ranks()
+        if staging and self._cur_staged is not None:
+            raise RuntimeError("the global curriculum merges a rollout's episode log in the update that follows it: call update_params before the next sample")
         if self.obs is None:
             if self.engine.cur_cfg is not None:               # the device curriculum's sampler (fit_clip / precision starts) seeds the first episodes too
                 self.obs = self.engine.curriculum_reseed()
@@ -253,7 +263,10 @@ class BatchedAgent:
                 self.step_once(buf, k, use_tc)
         buf.last_obs.copy_(self.obs)
         if self.engine.cur_cfg is not None and c_loop:
-            self.curriculum_update(buf, T)
+            if staging:
+                self._stage_curriculum(buf, T)
+            else:
+                self.curriculum_update(buf, T)
         # episode statistics from the buffer (one sync at the end of the rollout): segment the [T][E] masks per env
         m, r = buf.masks[:T], buf.rewards[:T]
         done = m == 0
@@ -282,6 +295,7 @@ class BatchedAgent:
         L = nn._lib()
         ev = [t.cuda.Event(enable_timing=True) for _ in range(3)]
         ev[0].record()
+        staged, self._cur_staged = getattr(self, "_cur_staged", None), None    # a failed update drops the log: the rings stay as they were
         T, E = buf.T, buf.E
         N = T * E
         states = buf.flat("states")
@@ -296,7 +310,7 @@ class BatchedAgent:
             self._mlp_c = None
             return dict(update_time=time.time() - t0, surr_loss=float(losses[0]), value_loss=float(losses[1]))
         if self.c_update:
-            return self._update_params_c(buf, ev)
+            return self._update_params_c(buf, ev, staged)
         tp = getattr(self.policy, "_tc_trainer", None) or nn.TCTrainer(self.policy)
         tv = getattr(self.value, "_tc_trainer", None) or nn.TCTrainer(self.value)
         self.policy._tc_trainer, self.value._tc_trainer = tp, tv
@@ -320,16 +334,16 @@ class BatchedAgent:
             if getattr(self, "_z_sync", None) is None:                               # fresh agent: every rank starts from empty statistics
                 self._z_sync = t.zeros_like(zs)                                      # additive form of the statistics every rank agreed on last
             d = t.cat([mom, t.full((1,), float(N), device=self.dev, dtype=t.float64), cnt, nn.zfilter_to_sums(zs, D) - self._z_sync])
-            planes = nn.split_double(d)                                              # [5, nd] exact fixed-point digits (fp32)
-            tail = self.value.gfull[self.value.nflat:]
-            tail.zero_()
             nd = d.numel()
-            assert planes.numel() == nn.stats_tail_floats(D) <= tail.numel()
-            tail[:planes.numel()].copy_(planes.reshape(-1))
+            extra = self._cur_slots if staged is not None else None                  # the global curriculum's episode logs ride behind the statistics
+            self.value.ensure_grad_tail(nn.stats_tail_floats(D) + (0 if extra is None else extra.numel()))
+            nn.pack_stats_tail(self.value.gfull[self.value.nflat:], d, extra)       # [5, nd] exact fixed-point digits (fp32), then the payload
             ntot = t.zeros(1, device=self.dev, dtype=t.float64)
 
             def after(tail_r):
-                g = nn.join_double(tail_r[:nn.SPLIT_CHUNKS * nd].reshape(nn.SPLIT_CHUNKS, nd))   # summed over the ranks by the gradient all-reduce
+                g, ex = nn.unpack_stats_tail(tail_r, nd, 0 if extra is None else extra.numel())   # summed over the ranks by the gradient all-reduce
+                if extra is not None:
+                    self._cur_sum.copy_(ex)
                 ntot.copy_(g[2:3])
                 gm = g[0:2].contiguous()
                 nn._chk(L.uhc_adv_normalize(nn._p(adv), C.c_long(N), nn._p(gm), nn._p(ntot), nn._stream(adv)))
@@ -340,6 +354,8 @@ class BatchedAgent:
         losses = nn.ppo_epochs_tc(self.policy, self.value, self.log_std, self.opt_p, self.opt_v, xb, xT, buf.flat("actions"), ret, adv, exps,
                                   self.clip_epsilon, self.epochs, self.grad_clip, comm=self.comm, first_value=(v0, ctx0), after_first_reduce=after,
                                   inv_count_dev=inv_count, world=self.world)
+        if staged is not None:
+            self.engine.curriculum_update_gathered(self._cur_sum, staged, self.world)
         ev[2].record()
         t.cuda.synchronize()
         self._mlp_c = None
@@ -350,15 +366,21 @@ class BatchedAgent:
             self.comm.bytes = self.comm.calls = 0
         return out
 
-    def _update_params_c(self, buf, ev):
+    def _update_params_c(self, buf, ev, staged=None):
         """the production update: ONE call of uhc_ppo_update (include/uhc_ppo.h) -- V(s) and V(s_T), GAE, global advantage normalisation, the
-        epochs of both nets, Adam, and (world > 1) the gradient all-reduces on this job's ncclComm_t with the statistics tail."""
+        epochs of both nets, Adam, and (world > 1) the gradient all-reduces on this job's ncclComm_t with the statistics tail.  staged: T of the
+        rollout whose episode log the global curriculum carries in that tail (uhc_ppo_update_ex) and merges afterwards."""
         t = self.torch
         T, E = buf.T, buf.E
-        if self._ctrainer is None or self._ctrainer.max_rows < T * E or self._ctrainer.max_envs < E:
+        if staged is not None:
+            self.value.ensure_grad_tail(nn.stats_tail_floats(self.obs_dim) + self._cur_slots.numel())
+        if (self._ctrainer is None or self._ctrainer.max_rows < T * E or self._ctrainer.max_envs < E or self._ctrainer.dv.gtail != self.value.grad_tail
+                or self._ctrainer.dv.gfull != self.value.gfull.data_ptr()):
+            fn = None
             if self._ctrainer is not None:
+                fn = self._ctrainer.all_reduce          # an installed collective stays with the rebuilt trainer
                 self._ctrainer.close()
-            self._ctrainer = nn.CPpoTrainer(self.policy, self.value, self.opt_p, self.opt_v, T * E, E, self.dev)
+            self._ctrainer = nn.CPpoTrainer(self.policy, self.value, self.opt_p, self.opt_v, T * E, E, self.dev, all_reduce=fn)
         zs = zsync = None
         if self.world > 1:
             if self._nccl is None:
@@ -372,7 +394,10 @@ class BatchedAgent:
             self._losses = t.zeros(2, device=self.dev, dtype=t.float32)
         ev[1].record()
         self._ctrainer.update(buf.flat("states"), last_s, buf.flat("actions"), buf.rewards, buf.masks, buf.flat("exps"), self.log_std, T, E, self.gamma,
-                              self.tau, self.clip_epsilon, self.epochs, self.grad_clip, self._losses, zfilter=zs, z_sync=zsync, comm=self._nccl, world=self.world)
+                              self.tau, self.clip_epsilon, self.epochs, self.grad_clip, self._losses, zfilter=zs, z_sync=zsync, comm=self._nccl, world=self.world,
+                              extra_in=self._cur_slots if staged is not None else None, extra_out=self._cur_sum if staged is not None else None)
+        if staged is not None:
+            self.engine.curriculum_update_gathered(self._cur_sum, staged, self.world)
         ev[2].record()
         t.cuda.synchronize()
         out = dict(update_time=1e-3 * ev[0].elapsed_time(ev[2]), gae_ms=0.0, epochs_ms=ev[1].elapsed_time(ev[2]),      # GAE runs inside the call
@@ -402,6 +427,18 @@ class BatchedAgent:
 
     def curriculum_update(self, buf, T):
         self.engine.curriculum_update(buf, T)
+
+    def _merges_across_ranks(self):
+        return getattr(self, "curriculum_global", False) and self.world > 1
+
+    def _stage_curriculum(self, buf, T):
+        """the global curriculum: this rank's episode log into its slot of the payload update_params' first all-reduce sums"""
+        n = self.world * T * self.E * 3
+        if getattr(self, "_cur_slots", None) is None or self._cur_slots.numel() != n:
+            self._cur_slots = self.torch.empty(n, device=self.dev, dtype=self.torch.float32)
+            self._cur_sum = self.torch.empty_like(self._cur_slots)
+        self.engine.curriculum_stage(buf, T, self.rank, self.world, self._cur_slots)
+        self._cur_staged = T
 
     def curriculum_push(self, clips, pct, starts):
         self.engine.curriculum_push(clips, pct, starts)

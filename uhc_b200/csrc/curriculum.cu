@@ -8,6 +8,8 @@
 //   k_cur_scatter  every entry among the last max_freq of its clip goes to ring slot (head + rank) mod max_freq
 //   k_cur_weights  one block: rings advance, s_c = ewma, p = exp(-s / temp), numpy's pairwise sum, w = freq * p / sum + (1 - freq) / C
 //                  in fp32, and the CDF as a fixed-order fp64 scan, written in place into the sampler's CDF
+// The global curriculum adds k_cur_stage (this rank's log into its slot of the payload the gradient all-reduce sums) and k_cur_unpack (the
+// summed payload back into one [world T E] log, which the four launches above then take as any other log).
 #include <cuda_runtime.h>
 #include "curriculum_core.h"
 
@@ -95,6 +97,26 @@ cudaError_t launch_update(const Dev &d, const int *clip_log, const float *pct_lo
 
 cudaError_t launch_weights(const Dev &d, cudaStream_t st) {
     k_cur_weights<<<1, WT, 0, st>>>(d, 0);
+    return cudaGetLastError();
+}
+
+__global__ void k_cur_stage(const int *__restrict__ clip_log, const float *__restrict__ pct_log, const int *__restrict__ start_log, int n, float *__restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) stage_entry(clip_log[i], pct_log[i], start_log[i], out + 3 * (size_t)i);
+}
+
+__global__ void k_cur_unpack(const float *__restrict__ in, int n, int *__restrict__ clip_log, float *__restrict__ pct_log, int *__restrict__ start_log) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) unpack_entry(in + 3 * (size_t)i, clip_log + i, pct_log + i, start_log + i);
+}
+
+cudaError_t launch_stage(const int *clip_log, const float *pct_log, const int *start_log, int n, float *out, cudaStream_t st) {
+    k_cur_stage<<<(n + 255) / 256, 256, 0, st>>>(clip_log, pct_log, start_log, n, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_unpack(const float *in, int n, int *clip_log, float *pct_log, int *start_log, cudaStream_t st) {
+    k_cur_unpack<<<(n + 255) / 256, 256, 0, st>>>(in, n, clip_log, pct_log, start_log);
     return cudaGetLastError();
 }
 

@@ -121,6 +121,18 @@ UHC_CDEV int draw_start(const float *pct, const int *start, const int *meta, int
     return st;
 }
 
+// the global curriculum's payload (uhc_curriculum_stage / uhc_curriculum_update_gathered): every log entry as three fp32 values
+// (clip, percent, start), an entry without an ended episode as (-1, 0, 0).  Each rank writes its own slot of a zeroed [world][T][E][3] array,
+// so every element of the all-reduce's sum is one rank's value plus zeros, and x + 0 = x in fp32 in any order (a percent of -0 comes back as
+// +0, equal under the == the weights use).  Clip indices and start frames are integers, exact in fp32 up to 2^24.
+constexpr int STAGE_EXACT_MAX = 1 << 24;
+UHC_CDEV bool stage_exact(long long num_clips, long long longest_clip) { return num_clips <= STAGE_EXACT_MAX && longest_clip <= STAGE_EXACT_MAX; }
+UHC_CDEV void stage_entry(int clip, float pct, int start, float *out) {
+    const bool ended = clip >= 0;
+    out[0] = ended ? (float)clip : -1.f; out[1] = ended ? pct : 0.f; out[2] = ended ? (float)start : 0.f;
+}
+UHC_CDEV void unpack_entry(const float *in, int *clip, float *pct, int *start) { *clip = (int)in[0]; *pct = in[1]; *start = (int)in[2]; }
+
 #ifndef UHC_EMU
 // device state of the curriculum (owned by the engine, step_kernel.cu) and the launches of curriculum.cu
 struct Dev {
@@ -136,6 +148,9 @@ constexpr int UPD_CHUNK = 1024;         // log entries per block of the bucketin
 cudaError_t launch_update(const Dev &d, const int *clip_log, const float *pct_log, const int *start_log, int N, cudaStream_t st);
 // the weights and the CDF from the rings as they are
 cudaError_t launch_weights(const Dev &d, cudaStream_t st);
+// n log entries -> out [n][3] (stage_entry); the summed payload [n][3] -> the three logs of launch_update (unpack_entry)
+cudaError_t launch_stage(const int *clip_log, const float *pct_log, const int *start_log, int n, float *out, cudaStream_t st);
+cudaError_t launch_unpack(const float *in, int n, int *clip_log, float *pct_log, int *start_log, cudaStream_t st);
 #endif
 
 #ifdef UHC_EMU

@@ -9,7 +9,7 @@
 //   k_dact_bf16                                dz = dh act'(z) -> bf16 dz, dz^T and the bias gradient in one pass
 //   k_sqsum, k_adam                            clip_grad_norm_ scale + torch.optim.Adam, one launch per net on the flat tensors
 //   ncclAllReduce                              the one collective: each net's flat gradient tensor, on a side stream under the other net's work;
-//                                              the statistics tail (k_stats_pack / k_stats_join) rides the first one
+//                                              the statistics tail (k_stats_pack / k_stats_join) and uhc_ppo_update_ex's extra payload ride the first one
 // Per epoch the order is value forward/backward -> value all-reduce starts -> policy forward/gradient/backward -> policy all-reduce starts ->
 // value Adam -> policy Adam: the two nets are independent inside an epoch, so this equals the reference's "value step, then policy step".
 #include <cuda_runtime.h>
@@ -256,10 +256,11 @@ int start_all_reduce(UhcPpoTrainer *t, void *comm, float *buf, size_t n, cudaEve
 }  // namespace
 
 // the PPO epochs on t->xb / t->xT / t->adv / t->ret: per epoch one value step then one clipped-surrogate policy step (agent_ppo.py:46-51), see the file header
-// for the order of the collectives.  stats_tail: the first value all-reduce carries the statistics planes (uhc_ppo_update with world > 1).
+// for the order of the collectives.  stats_tail: the first value all-reduce carries the statistics planes (uhc_ppo_update with world > 1), and
+// n_extra caller floats behind them, whose sum over the ranks goes to extra_out.
 static int run_epochs(UhcPpoTrainer *t, const float *actions, const float *exps, const float *log_std, long M, const UhcPpoCfg *cfg, int *adam_step_policy,
                       int *adam_step_value, int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *comm, int world, bool stats_tail,
-                      bool value_forward_done, float *losses_out, cudaStream_t st) {
+                      long n_extra, float *extra_out, bool value_forward_done, float *losses_out, cudaStream_t st) {
     const UhcNetDesc &pol = t->pnets[0], &val = t->val;
     const int D = pol.dims[0], A = pol.dims[pol.nlayers];
     const int nd = 4 + 1 + 2 * D;
@@ -275,12 +276,13 @@ static int run_epochs(UhcPpoTrainer *t, const float *actions, const float *exps,
         CKU(uhc_value_grad_n(t->vb.out, t->ret, t->dv, losses_out + 1, (int)M, M * world, st), "value gradient");
         if (net_backward(t, val, t->vb, t->dv, M, st)) return -1;
         const bool with_tail = stats_tail && ep == 0;
-        if (comm && start_all_reduce(t, comm, val.gfull, (size_t)val.nflat + (with_tail ? (size_t)PLANES * nd : 0), t->ev_v, st)) return -1;
+        if (comm && start_all_reduce(t, comm, val.gfull, (size_t)val.nflat + (with_tail ? (size_t)PLANES * nd + n_extra : 0), t->ev_v, st)) return -1;
         if (with_tail) {    // the global statistics are needed before the first policy gradient
             CK(cudaStreamWaitEvent(st, t->ev_v, 0));
             ++g_launches; k_stats_join<<<(nd + 255) / 256, 256, 0, st>>>(tail, D, t->mom, t->ntot, t->inv_count, zfilter_sync); CK(cudaGetLastError());
             CKU(uhc_adv_normalize(t->adv, M, t->mom, t->ntot, st), "advantage normalisation (global)");
             ++g_launches; k_zfilter_from_sums<<<(2 * D + 1 + 255) / 256, 256, 0, st>>>(zfilter_sync, D, zfilter_stats); CK(cudaGetLastError());
+            if (n_extra) CK(cudaMemcpyAsync(extra_out, tail + (size_t)PLANES * nd, (size_t)n_extra * sizeof(float), cudaMemcpyDeviceToDevice, st));
         }
         if (ep > 0 && policy_forward(t, M, &pmean, st)) return -1;
         CKU(uhc_ppo_policy_grad_dev(pmean, log_std, actions, t->adv, t->fixed, exps, cfg->clip_eps, t->inv_count, t->dmean, losses_out, (int)M, A, st), "policy gradient");
@@ -394,11 +396,13 @@ int uhc_ppo_comm_stats(UhcPpoTrainer *t, double *ms, long *bytes, int *calls) {
     return 0;
 }
 
-int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_states, const float *actions, const float *rewards, const float *masks,
-                   const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
-                   int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out, void *stream) {
+int uhc_ppo_update_ex(UhcPpoTrainer *t, const float *states, const float *last_states, const float *actions, const float *rewards, const float *masks,
+                      const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
+                      int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out,
+                      const float *extra_in, float *extra_out, long n_extra, void *stream) {
     if (!t || !states || !last_states || !actions || !rewards || !masks || !exps || !log_std || !cfg || !adam_step_policy || !adam_step_value || !policy_steps_done ||
         !losses_out || T <= 0 || E <= 0 || world < 1) { uhc_err() = "uhc_ppo_update: bad argument"; return -2; }
+    if (n_extra < 0 || (n_extra > 0 && (!extra_in || !extra_out))) { uhc_err() = "uhc_ppo_update_ex: n_extra must be >= 0, with extra_in and extra_out when > 0"; return -2; }
     const long M = (long)T * E;
     if (M > t->cap || E > t->cap_envs) { uhc_err() = "uhc_ppo_update: the rollout exceeds the trainer's capacity"; return -2; }
     if (world > 1 && (!nccl_comm || !zfilter_stats || !zfilter_sync)) { uhc_err() = "uhc_ppo_update: world > 1 needs an ncclComm_t and the ZFilter statistics"; return -2; }
@@ -412,6 +416,11 @@ int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_stat
     void *comm = world > 1 ? nccl_comm : nullptr;
     const int nd = 4 + 1 + 2 * D;
     if (comm && (long)PLANES * nd > val.gtail) { uhc_err() = "uhc_ppo_update: the value net's gradient tail is too small for the statistics"; return -2; }
+    if (comm && (long)PLANES * nd + n_extra > val.gtail) {
+        uhc_err() = "uhc_ppo_update_ex: the value net's gradient tail holds " + std::to_string(val.gtail) + " floats, the statistics and the extra payload need " +
+                    std::to_string((long)PLANES * nd + n_extra);
+        return -2;
+    }
 
     // ---- V(s_T) of the state after the last step, V(s) of every row (also epoch 0's value forward), GAE
     CKU(uhc_f32_to_bf16_padded(last_states, t->lb, E, D, (int)Dp, st), "bf16 last states");
@@ -431,9 +440,18 @@ int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_stat
     } else {
         CK(cudaMemsetAsync(tail, 0, (size_t)val.gtail * sizeof(float), st));
         ++g_launches; k_stats_pack<<<(nd + 255) / 256, 256, 0, st>>>(t->mom, (double)M, t->cnt, zfilter_stats, zfilter_sync, D, tail); CK(cudaGetLastError());
+        if (n_extra) CK(cudaMemcpyAsync(tail + (size_t)PLANES * nd, extra_in, (size_t)n_extra * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
+    if (!comm && n_extra) CK(cudaMemcpyAsync(extra_out, extra_in, (size_t)n_extra * sizeof(float), cudaMemcpyDeviceToDevice, st));   // one rank: the sum is the payload
     return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, zfilter_stats, zfilter_sync, comm, world, comm != nullptr,
-                      true, losses_out, st);
+                      comm ? n_extra : 0, extra_out, true, losses_out, st);
+}
+
+int uhc_ppo_update(UhcPpoTrainer *t, const float *states, const float *last_states, const float *actions, const float *rewards, const float *masks,
+                   const float *exps, const float *log_std, int T, int E, const UhcPpoCfg *cfg, int *adam_step_policy, int *adam_step_value,
+                   int *policy_steps_done, double *zfilter_stats, double *zfilter_sync, void *nccl_comm, int world, float *losses_out, void *stream) {
+    return uhc_ppo_update_ex(t, states, last_states, actions, rewards, masks, exps, log_std, T, E, cfg, adam_step_policy, adam_step_value, policy_steps_done,
+                             zfilter_stats, zfilter_sync, nccl_comm, world, losses_out, nullptr, nullptr, 0, stream);
 }
 
 /* AgentPPO.update_policy (agent_ppo.py:16-51) alone: the epochs on caller-provided returns / (already normalised) advantages. */
@@ -458,6 +476,7 @@ int uhc_ppo_update_policy(UhcPpoTrainer *t, const float *states, const float *ac
     CK(cudaMemsetAsync(t->cnt, 0, sizeof(double), st));
     ++g_launches; k_count_selected<<<264, 256, 0, st>>>(exps, (size_t)M, t->cnt); CK(cudaGetLastError());
     ++g_launches; k_inv_count<<<1, 1, 0, st>>>(t->cnt, t->inv_count); CK(cudaGetLastError());
-    return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, nullptr, nullptr, nullptr, 1, false, false, losses_out, st);
+    return run_epochs(t, actions, exps, log_std, M, cfg, adam_step_policy, adam_step_value, policy_steps_done, nullptr, nullptr, nullptr, 1, false, 0, nullptr, false,
+                      losses_out, st);
 }
 }  // extern "C"

@@ -223,6 +223,7 @@ struct UhcEngine {
     size_t cur_cnt_cap = 0, cur_rank_cap = 0;
     int *d_reseed = nullptr;       // [4][E] ids / clip / start / len of uhc_curriculum_reseed
     int *d_push = nullptr; int push_cap = 0;   // [3][n] clip / percent bits / start of uhc_curriculum_push
+    int *d_cur_log = nullptr; size_t cur_log_cap = 0;   // [3][n] clip / percent bits / start of uhc_curriculum_update_gathered's unpacked log
     // variant 0 of the model in fp64 on the host: the base of the run-time subject builder
     std::vector<double> base_bf, base_hull, base_dof; std::vector<int> base_hull_adr, base_hull_num, base_parent, base_sub_end;
     // run-time subjects (uhc_track_subjects_enable): nslot = E once enabled, and variant nshape + env of body_f / hull / mo_model.body is env's
@@ -390,7 +391,7 @@ void uhc_engine_destroy(UhcEngine *e) {
     if (e->d_keep_t) cudaFree(e->d_keep_t);
     if (e->d_gather) cudaFree(e->d_gather);
     if (e->d_gather_i) cudaFree(e->d_gather_i);
-    for (void *p : {(void *)e->cur.pct, (void *)e->cur.start, (void *)e->cur.meta, (void *)e->cur.p, (void *)e->cur.cnt, (void *)e->cur.rank, (void *)e->cur.ncl, (void *)e->d_reseed, (void *)e->d_push}) if (p) cudaFree(p);
+    for (void *p : {(void *)e->cur.pct, (void *)e->cur.start, (void *)e->cur.meta, (void *)e->cur.p, (void *)e->cur.cnt, (void *)e->cur.rank, (void *)e->cur.ncl, (void *)e->d_reseed, (void *)e->d_push, (void *)e->d_cur_log}) if (p) cudaFree(p);
     if (e->d_slot_hull) cudaFree(e->d_slot_hull);
     subjx::builder_free(e->subj);
     delete e;
@@ -817,6 +818,8 @@ static void cur_free(UhcEngine *e) {
     for (void *p : {(void *)e->cur.pct, (void *)e->cur.start, (void *)e->cur.meta, (void *)e->cur.p, (void *)e->cur.cnt, (void *)e->cur.rank, (void *)e->cur.ncl}) if (p) cudaFree(p);
     if (e->d_push) cudaFree(e->d_push);
     e->d_push = nullptr; e->push_cap = 0;
+    if (e->d_cur_log) cudaFree(e->d_cur_log);
+    e->d_cur_log = nullptr; e->cur_log_cap = 0;
     e->cur = cur::Dev{}; e->cur_cnt_cap = e->cur_rank_cap = 0; e->fit_clip = -1; e->prec_freq = 0.f;
     // the start log is written by the curriculum's step kernel only: back to "never recorded", as on an engine that never enabled it
     int *sl = e->precision == 32 ? e->evf.ep_start_log : e->evd.ep_start_log;
@@ -891,6 +894,58 @@ int uhc_curriculum_update(UhcEngine *e, const UhcRolloutBuf *buf, int T, void *s
     cur_bind(e);
     CK(cur::launch_update(e->cur, buf->ep_clip, buf->ep_pct, buf->ep_start, (int)N, (cudaStream_t)stream));
     e->launches += 4;
+    return 0;
+}
+
+// the payload of a [world][T][E] gathered log (3 floats per entry): the length of the unpacked log fits an int, and every clip index and start
+// frame converts to fp32 exactly
+static bool cur_gather_check(UhcEngine *e, const char *who, int T, int world) {
+    if ((size_t)T * e->E * world > 0x7fffffffu) { uhc_err() = std::string(who) + ": world * T * E exceeds the log length an update takes (2^31 - 1)"; return false; }
+    int longest = 0;
+    for (int L : e->clip_len_h) longest = L > longest ? L : longest;
+    if (!cur::stage_exact(e->num_clips, longest)) {
+        uhc_err() = std::string(who) + ": " + std::to_string(e->num_clips) + " clips of up to " + std::to_string(longest) +
+                    " frames: clip indices and start frames above 2^24 are not exact in the fp32 payload";
+        return false;
+    }
+    return true;
+}
+
+int uhc_curriculum_stage(UhcEngine *e, const UhcRolloutBuf *buf, int T, int rank, int world, float *slots, void *stream) {
+    if (!cur_check(e, "uhc_curriculum_stage")) return -2;
+    if (!buf || !buf->ep_clip || !buf->ep_pct || !buf->ep_start || !slots || T <= 0 || T > buf->T_cap) {
+        uhc_err() = "uhc_curriculum_stage: needs ep_clip, ep_pct and ep_start rows, the slots and 0 < T <= T_cap"; return -2;
+    }
+    if (world < 1 || rank < 0 || rank >= world) { uhc_err() = "uhc_curriculum_stage: needs world >= 1 and 0 <= rank < world"; return -2; }
+    if (!cur_gather_check(e, "uhc_curriculum_stage", T, world)) return -2;
+    CK(cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t N = (size_t)T * e->E;
+    CK(cudaMemsetAsync(slots, 0, N * world * 3 * sizeof(float), st));
+    CK(cur::launch_stage(buf->ep_clip, buf->ep_pct, buf->ep_start, (int)N, slots + (size_t)rank * N * 3, st));
+    e->launches += 1;
+    return 0;
+}
+
+int uhc_curriculum_update_gathered(UhcEngine *e, const float *summed_slots, int T, int world, void *stream) {
+    if (!cur_check(e, "uhc_curriculum_update_gathered")) return -2;
+    if (!summed_slots || T <= 0 || world < 1) { uhc_err() = "uhc_curriculum_update_gathered: needs the summed slots, T > 0 and world >= 1"; return -2; }
+    if (!cur_gather_check(e, "uhc_curriculum_update_gathered", T, world)) return -2;
+    CK(cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t N = (size_t)T * e->E * world;
+    if (cur_scratch(e, N)) return -1;
+    if (e->cur_log_cap < N) {
+        if (e->d_cur_log) cudaFree(e->d_cur_log);
+        e->d_cur_log = nullptr; e->cur_log_cap = 0;
+        CK(cudaMalloc((void **)&e->d_cur_log, 3 * N * sizeof(int))); e->cur_log_cap = N;
+    }
+    int *clip = e->d_cur_log, *start = e->d_cur_log + 2 * N;
+    float *pct = (float *)(e->d_cur_log + N);
+    CK(cur::launch_unpack(summed_slots, (int)N, clip, pct, start, st));
+    cur_bind(e);
+    CK(cur::launch_update(e->cur, clip, pct, start, (int)N, st));
+    e->launches += 5;
     return 0;
 }
 

@@ -878,6 +878,24 @@ class Engine:
         b.ep_clip, b.ep_pct, b.ep_start, b.T_cap = buf.ep_clip.data_ptr(), buf.ep_pct.data_ptr(), buf.ep_start.data_ptr(), buf.T
         _chk(self.lib.uhc_curriculum_update(self.h, C.byref(b), C.c_int(int(T)), self._stream()), "uhc_curriculum_update", ValueError)
 
+    def curriculum_stage(self, buf, T, rank, world, slots):
+        """write the episodes that ended in rows 0 .. T-1 of a RolloutBuffer into slot `rank` of `slots` (fp32 [world][T][E][3], zeroed here):
+        summed over the ranks, the slots are every rank's log exactly.  Stream-ordered, no synchronise."""
+        from .agent import UhcRolloutBuf
+        if slots.dtype != self.torch.float32 or not slots.is_contiguous() or slots.numel() != int(world) * int(T) * self.E * 3:
+            raise ValueError(f"curriculum_stage: slots must be a contiguous float32 tensor of world * T * E * 3 = {int(world) * int(T) * self.E * 3} elements")
+        b = UhcRolloutBuf()
+        b.ep_clip, b.ep_pct, b.ep_start, b.T_cap = buf.ep_clip.data_ptr(), buf.ep_pct.data_ptr(), buf.ep_start.data_ptr(), buf.T
+        _chk(self.lib.uhc_curriculum_stage(self.h, C.byref(b), C.c_int(int(T)), C.c_int(int(rank)), C.c_int(int(world)), C.c_void_p(slots.data_ptr()),
+                                           self._stream()), "uhc_curriculum_stage", ValueError)
+
+    def curriculum_update_gathered(self, summed, T, world):
+        """append the log of every rank (the sum of their staged slots: rank-major, then step-major, then env-minor) and rewrite the clip CDF"""
+        if summed.dtype != self.torch.float32 or not summed.is_contiguous() or summed.numel() != int(world) * int(T) * self.E * 3:
+            raise ValueError(f"curriculum_update_gathered: the sum must be a contiguous float32 tensor of world * T * E * 3 = {int(world) * int(T) * self.E * 3} elements")
+        _chk(self.lib.uhc_curriculum_update_gathered(self.h, C.c_void_p(summed.data_ptr()), C.c_int(int(T)), C.c_int(int(world)), self._stream()),
+             "uhc_curriculum_update_gathered", ValueError)
+
     def curriculum_push(self, clips, pct, starts):
         clips = np.ascontiguousarray(clips, np.int32).reshape(-1)
         p = np.ascontiguousarray(pct, np.float32).reshape(-1)

@@ -136,6 +136,18 @@ class MLPNet:
     def gflat(self):
         return self.gfull[:self.nflat]
 
+    def ensure_grad_tail(self, n):
+        """grow the tail behind the gradients to at least n floats (a world > 1 update's extra payload rides there after the statistics).
+        Returns True when it grew: the gradient tensor is then a new one, and a descriptor holding its address (CPpoTrainer) must be rebuilt."""
+        if n <= self.grad_tail:
+            return False
+        assert self._storage is None, "a net in shared storage has no tail of its own"
+        g = self.torch.zeros(self.nflat + n, device=self.flat.device, dtype=self.torch.float32)
+        if self._gfull is not None:
+            g[:self._gfull.numel()].copy_(self._gfull)
+        self._gfull, self.grad_tail = g, n
+        return True
+
     def _act_of(self, i):
         return self.htype if i < len(self.W) - 1 else self.head_act
 
@@ -642,6 +654,25 @@ def join_double(planes):
     return out
 
 
+def pack_stats_tail(tail, d, extra=None):
+    """the value gradient's tail for the first all-reduce of a world > 1 update: split_double's planes of the statistics d, then the extra
+    payload (fp32, summed over the ranks as it is), then zeros"""
+    planes = split_double(d)
+    n, ne = planes.numel(), 0 if extra is None else extra.numel()
+    if n + ne > tail.numel():
+        raise ValueError(f"the gradient tail holds {tail.numel()} floats, the statistics and the extra payload need {n + ne}")
+    tail.zero_()
+    tail[:n].copy_(planes.reshape(-1))
+    if ne:
+        tail[n:n + ne].copy_(extra.reshape(-1))
+
+
+def unpack_stats_tail(tail, nd, n_extra=0):
+    """after the all-reduce: (the nd statistics summed over the ranks, fp64; the extra payload summed over the ranks, a view of the tail)"""
+    n = SPLIT_CHUNKS * nd
+    return join_double(tail[:n].reshape(SPLIT_CHUNKS, nd)), tail[n:n + n_extra]
+
+
 def zfilter_to_sums(stats, D):
     """(n, mean, S) -> additive form (n, sum, sum of squares)"""
     import torch
@@ -822,12 +853,17 @@ class CPpoTrainer:
             pass
 
     def update(self, states, last_states, actions, rewards, masks, exps, log_std, T, E, gamma, tau, clip_eps, epochs, grad_clip, losses, zfilter=None,
-               z_sync=None, comm=None, world=1):
+               z_sync=None, comm=None, world=1, extra_in=None, extra_out=None):
+        """extra_in / extra_out: fp32 device tensors of one length whose sum over the ranks rides the first value all-reduce
+        (uhc_ppo_update_ex); the value net's grad_tail must hold it behind the statistics (MLPNet.ensure_grad_tail, then a new trainer)"""
         cfg = UhcPpoCfg(gamma, tau, clip_eps, float(grad_clip or 0.0), 1, epochs)
         sp, sv = C.c_int(self.opt_p.step_n), C.c_int(self.opt_v.step_n)
         done = C.c_int(1 if getattr(self.opt_p, "_clip_consumed", False) else 0)
-        rc = self.L.uhc_ppo_update(self.h, _p(states), _p(last_states), _p(actions), _p(rewards), _p(masks), _p(exps), _p(log_std), C.c_int(T), C.c_int(E),
-                                   C.byref(cfg), C.byref(sp), C.byref(sv), C.byref(done), _p(zfilter), _p(z_sync), comm, C.c_int(world), _p(losses), _stream(states))
+        n_extra = 0 if extra_in is None else extra_in.numel()
+        assert n_extra == 0 or (extra_out is not None and extra_out.numel() == n_extra and extra_in.dtype == extra_out.dtype == self.policy.flat.dtype)
+        rc = self.L.uhc_ppo_update_ex(self.h, _p(states), _p(last_states), _p(actions), _p(rewards), _p(masks), _p(exps), _p(log_std), C.c_int(T), C.c_int(E),
+                                      C.byref(cfg), C.byref(sp), C.byref(sv), C.byref(done), _p(zfilter), _p(z_sync), comm, C.c_int(world), _p(losses),
+                                      _p(extra_in), _p(extra_out), C.c_long(n_extra), _stream(states))
         _check(rc, "uhc_ppo_update")
         self.opt_p.step_n, self.opt_v.step_n = sp.value, sv.value
         self.opt_p._clip_consumed = done.value > 0
