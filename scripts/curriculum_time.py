@@ -8,7 +8,7 @@
 The drop-in AgentCopycat's own methods run on a BatchedAgent built here (the agent's constructor would read a dataset pickle).  For each
 clip count it reports each path's wall time to a device synchronise: the bookkeeping of one rollout (`_update_freq_dict` on the host;
 `uhc_curriculum_update`, also from CUDA events, on the device), a whole training iteration (`AgentCopycat.sample` with its bookkeeping +
-`update_params`), and the eval outcomes of one `eval_policy` over every clip (`_eval_results`' appends; one `uhc_curriculum_push`), with 4096 envs, T = 32 and the production 657-(2048,1024,512)-105
+`update_params`), and the eval outcomes of one `eval_policy` over every clip (`_eval_results` + `_apply_outcomes`: the freq_dict appends; one `uhc_curriculum_push`), with 4096 envs, T = 32 and the production 657-(2048,1024,512)-105
 policy with seeded weights.  The clips are synthetic qpos motion (60-200 frames, expert tables built on the GPU); short slices
 (t_max = 12) make episodes end often.  Prints the card name and power limit, then one JSON line.
 Usage: python scripts/curriculum_time.py [--envs 4096] [--T 32] [--clips 10,3334,11000] [--iters 5]
@@ -110,14 +110,13 @@ def main():
                 if mode == "device":
                     book_ev.append(e0.elapsed_time(e1))
             # the eval outcomes of one eval_policy over every clip: C appends to freq_dict on the host, one uhc_curriculum_push on the device
-            lens_c, ids = np.asarray(ag.engine.clip_len), np.arange(C)
+            lens_c, ids = np.asarray(ag.engine.clip_len), np.arange(C, dtype=np.int32)
             torch.cuda.synchronize()
             t2 = time.perf_counter()
             pend = []
-            dropin._eval_results({}, dropin.data_loader, 0, ids, lens_c, lens_c - 1, np.zeros(C, bool), np.zeros(C), np.zeros(C, int),
+            dropin._eval_results({}, dropin.data_loader, ids, ids, lens_c, lens_c - 1, np.zeros(C, bool), np.zeros(C), np.zeros(C, int),
                                  lambda i, pct, fs: {"succ": np.array([True])}, pend)
-            if pend:
-                ag.curriculum_push([c for c, _ in pend], [o for _, o in pend], [0] * len(pend))
+            dropin._apply_outcomes(pend)
             torch.cuda.synchronize()
             row[mode] = dict(bookkeeping_ms=float(np.median(book)), iteration_ms=float(np.median(it_t)), ends_per_iter=ends / a.iters,
                              eval_outcomes_ms=(time.perf_counter() - t2) * 1e3)

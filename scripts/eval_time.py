@@ -81,7 +81,8 @@ def copycat(agent, loader, out_dir, on_device, window):
     a = object.__new__(AgentCopycat)
     a.cfg = _Cfg(fail_safe=True, eval_on_device=on_device, output_dir=out_dir)
     a.agent, a.num_envs, a.running_state, a.policy_net = agent, agent.E, agent.running_state, agent.policy
-    a.data_loader, a.test_data_loaders, a.freq_dict, a.max_freq = loader, [loader], {}, 50
+    a.data_loader, a.test_data_loaders, a.freq_dict, a.max_freq = loader, [loader], {k: [] for k in loader.data_keys}, 50
+    a.curriculum_on_device = False
     a.logger = logging.getLogger("eval_time")
     a._env_cfg = lambda test: dict(auto_reset=0 if test else 1)
     a._push_clip_weights = lambda: None

@@ -26,7 +26,7 @@ from uhc.data_loaders.dataset_amass_single import DatasetAMASSSingle
 from uhc.envs.humanoid_im import HumanoidEnv
 from uhc.losses.reward_function import reward_func
 from uhc_b200 import nn
-from uhc_b200.agent import BatchedAgent, RolloutBuffer, make_nccl_grad_sync
+from uhc_b200.agent import BatchedAgent, RolloutBuffer, make_nccl_grad_sync, shard_clips
 from uhc_b200.model import HumanoidModel
 
 
@@ -44,6 +44,72 @@ class _Batch:
 
 class _Log(dict):
     __getattr__ = dict.get
+
+
+# per-clip result keys that hold a clip's trajectory (eval_dump_motion, full_eval with dump): only rank 0, which writes the dumps, receives them
+TRAJECTORY_KEYS = frozenset(("gt", "pred", "gt_jpos", "pred_jpos", "pose_aa", "trans", "pred_vertices", "pred_joints", "gt_vertices", "gt_joints"))
+
+
+def exchange(work):
+    """this rank's share of a sharded evaluation, work() -> a picklable value, all-gathered over the job's torch.distributed group:
+    returns every rank's value in rank order.  A rank whose work raises still joins the all-gather, with its error in place of the
+    value, and then every rank raises, so no rank waits on one that stopped; the all-gather itself runs under the group's timeout."""
+    import torch.distributed as dist
+    err = None
+    try:
+        val = work()
+    except Exception as e:
+        val, err = None, e
+    out = [None] * dist.get_world_size()
+    dist.all_gather_object(out, (None if err is None else f"{type(err).__name__}: {err}", val))
+    bad = [f"rank {r}: {e}" for r, (e, _) in enumerate(out) if e is not None]
+    if bad:
+        raise RuntimeError("sharded evaluation failed on " + "; ".join(bad)) from err
+    return [v for _, v in out]
+
+
+def merge_results(parts, keys):
+    """every rank's {key: result} of one table as one dict in the table's clip order, the order world 1 builds it in"""
+    got = {}
+    for p in parts:
+        got.update(p)
+    assert len(got) == len(keys) and all(k in got for k in keys), "every clip must be evaluated by exactly one rank"
+    return {k: got[k] for k in keys}
+
+
+def merge_outcomes(parts):
+    """every rank's eval outcomes (table clip, training clip, outcome) in table clip order, the order world 1 applies them in"""
+    return sorted((o for p in parts for o in p), key=lambda o: o[0])
+
+
+def clip_betas(shapes, clips):
+    """beta[:10] of each listed clip's shape row: [len(clips)][10], also for a rank whose shard is empty"""
+    return np.array([np.asarray(shapes[c], np.float64)[:10] for c in clips], np.float64).reshape(len(clips), 10)
+
+
+def gather_to_root(local, max_bytes):
+    """every rank's {key: result} on rank 0, sent in pieces of at most max_bytes of arrays (at least one clip): rank 0 returns all of
+    them, every other rank its own `local`, and no rank other than 0 ever holds more than its own results"""
+    import torch.distributed as dist
+    rank, world = dist.get_rank(), dist.get_world_size()
+    pieces, size = [{}], 0
+    for k, r in local.items():
+        b = sum(v.nbytes for v in r.values() if isinstance(v, np.ndarray))
+        if pieces[-1] and size + b > max_bytes:
+            pieces.append({})
+            size = 0
+        pieces[-1][k] = r
+        size += b
+    counts = [None] * world
+    dist.all_gather_object(counts, 0 if rank == 0 else len(pieces))
+    out = dict(local)
+    for j in range(max(counts)):
+        got = [None] * world if rank == 0 else None
+        dist.gather_object(pieces[j] if rank and j < len(pieces) else None, got, dst=0)
+        if rank == 0:
+            for p in got:
+                out.update(p or {})
+    return out if rank == 0 else local
 
 
 def supported_variant(cfg):
@@ -273,11 +339,57 @@ class AgentCopycat:
                 pass
 
     # ---------------------------------------------------------------- evaluation (:354-494), batched: one env per clip
-    def eval_policy(self, epoch=0, dump=False):
+    def eval_policy(self, epoch=0, dump=False, max_bytes=1 << 30):
         """eval_policy / eval_seq (agent_copycat.py:354-494) for every clip at once: env i imitates clip c0 + i from frame 0 with the
         deterministic policy; per step ONE batched state read (uhc_env_get_state_batch) feeds the reference's metrics
         (smpl_eval.compute_metrics: mpjpe / pa-mpjpe / accel / vel / root distance, restated in uhc_b200/metrics.py); fail_safe re-seats a
-        failed humanoid on the expert pose with one batched set_state (humanoid_im.py:902-905)."""
+        failed humanoid on the expert pose with one batched set_state (humanoid_im.py:902-905).
+
+        With several ranks each rank evaluates its own clips (uhc_b200.agent.assign_clips), and every rank then holds every clip's metrics,
+        logs the same coverage lines, returns what one rank would return and applies every eval outcome to its curriculum in clip order.
+        Rank 0 alone writes the dumps; the trajectories they hold (eval_dump_motion, full_eval) reach it in pieces of at most max_bytes."""
+        world = self.agent.world
+        res_dicts = []
+        for loader in self.test_data_loaders:
+            if world == 1:
+                res, pending = self._eval_loader(loader, dump)
+            else:
+                local = {}
+
+                def shard(loader=loader):
+                    r, p = self._eval_loader(loader, dump)
+                    local.update(r)
+                    return {k: {m: v for m, v in d.items() if m not in TRAJECTORY_KEYS} for k, d in r.items()}, p
+                parts = exchange(shard)
+                res, pending = merge_results([p[0] for p in parts], loader.data_keys), merge_outcomes([p[1] for p in parts])
+                if dump and (self._full_eval() or self.cfg.get("eval_dump_motion", False)):
+                    full = gather_to_root(local, max_bytes)         # a collective: every rank takes part, rank 0 keeps the result
+                    if self.agent.rank == 0:
+                        res = merge_results([full], loader.data_keys)
+            self._apply_outcomes(pending)
+            res_dicts.append(self._coverage(loader, res, epoch, dump))
+        if not self.curriculum_on_device:
+            self._push_clip_weights()
+        return res_dicts
+
+    def _apply_outcomes(self, pending):
+        """eval outcomes (table clip, training clip, outcome) fed to the failure-weighted sampler like training episodes ([outcome, 0]):
+        appended to freq_dict, or pushed in one call to the device curriculum"""
+        if self.curriculum_on_device:
+            if pending:
+                self.agent.curriculum_push([i for _, i, _ in pending], [o for _, _, o in pending], [0] * len(pending))
+            return
+        keys = self.data_loader.data_keys
+        for _, i, o in pending:
+            self.freq_dict[keys[i]] = (self.freq_dict[keys[i]] + [[o, 0]])[-self.max_freq:]
+
+    def _my_clips(self):
+        """this rank's clips of the loaded table, in the order of its evaluation calls (every clip in order at world 1)"""
+        calls = shard_clips(self.agent.engine.clip_len, self.agent.world, self.agent.rank, self.num_envs)
+        return np.concatenate([np.zeros(0, np.int32)] + calls)
+
+    def _eval_loader(self, loader, dump):
+        """eval_policy's roll-out of this rank's clips of one loader: ({key: result}, [(table clip, training clip, outcome)])"""
         import torch
         from uhc_b200.metrics import compute_metrics, metrics_from_frames
         cfg = self.cfg
@@ -289,118 +401,108 @@ class AgentCopycat:
             raise ValueError("full_eval and eval_floor_metrics both write pentration / skate: enable one of them")
         if full:
             self._mesh_model()
-        res_dicts = []
         eng = self.agent.engine
         E = self.num_envs
-        pending = []        # device curriculum: this loader's eval outcomes (clip, outcome), pushed in one call once the training tables are back
-        for loader in self.test_data_loaders:
-            n = loader.get_len()
-            device_tables = self._device_tables(loader)
-            if loader is not self.data_loader:
-                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
-                self._load_tables(loader)      # invalidates every env record: only the envs reset below are stepped
-            eng.set_cfg(**self._env_cfg(test=True))
-            res = {}
-            for c0 in range(0, n, E):
-                ids = np.arange(min(E, n - c0), dtype=np.int32)
-                clips = (c0 + ids).astype(np.int32)
-                lens = eng.clip_len[clips]
-                if on_device:                                      # the same roll-out as the loop below, as CUDA-graph replays with the metrics on the device
-                    kw = dict(record_states=True, export_smpl=True) if motion else (dict(record_states=True) if full else {})
-                    dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, floor=floor, **kw)
-                    last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
-                    rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
-                    self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec,
-                                       lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs), pending)
-                    if floor:
-                        for i in ids:
-                            self._add_floor(res[loader.data_keys[c0 + i]], loader, int(clips[i]), dev[i]["floor"], np.arange(1, len(dev[i]["frames"]) + 1))
-                    if full:
-                        self._add_mesh(res, loader, c0, ids, clips, [dev[i]["states"][:, :76] for i in ids],
-                                       [np.arange(1, len(dev[i]["frames"]) + 1) for i in ids], dump)
-                    if motion:
-                        for i in ids:
-                            d = dev[i]
-                            self._add_motion(res[loader.data_keys[c0 + i]], loader, int(clips[i]), d["states"][:, :76], d["states"][:, 76:148],
-                                             d["pose_aa"], d["trans"], np.arange(1, len(d["frames"]) + 1), bool(d["fail_any"]))
-                    continue
-                if len(ids) < E:                                   # idle envs: park them on clip c0 so every record is valid (their outputs are ignored)
-                    eng.reset(np.arange(len(ids), E, dtype=np.int32), np.full(E - len(ids), c0, np.int32), 0, None)
-                obs = eng.reset(ids, clips, 0, None)
-                alive = np.ones(len(ids), bool); fail_any = np.zeros(len(ids), bool)
-                rsum = np.zeros(len(ids)); last_t = np.zeros(len(ids), np.int64)
-                traj = [dict(pred=[], pred_jpos=[], t=[]) for _ in ids]
-                gt = {}
-
-                def expert(i):
-                    """expert table of clip c0 + i: the host-built one, or the device-built one read back once (in the engine's precision)"""
-                    if not device_tables:
-                        return loader.experts[clips[i]]
-                    if i not in gt:
-                        gt[i] = eng.clip_frames(clips[i])
-                    return gt[i]
-                det = torch.ones(E, dtype=torch.uint8, device=obs.device)
-                for t in range(int(lens.max()) - 1):
-                    s = self.running_state(obs, update=False)
-                    mean = self.policy_net.forward_tc(s)
-                    a, _ = nn.gaussian_sample(mean, self.agent.log_std, 0, 0, det)
-                    obs, rew, ci, fail, end, pct = eng.step(a)
-                    f, e, r = fail.cpu().numpy()[ids] != 0, end.cpu().numpy()[ids] != 0, rew.cpu().numpy()[ids]
-                    live = np.nonzero(alive)[0]
-                    st = eng.get_states(ids[live])
-                    for j, i in enumerate(live):
-                        traj[i]["pred"].append(st["qpos"][j].copy()); traj[i]["pred_jpos"].append(st["xpos"][j].reshape(-1).copy()); traj[i]["t"].append(int(st["cur_t"][j]))
-                        last_t[i] = st["cur_t"][j]
-                    rsum[live] += r[live]
-                    failed = live[f[live]]
-                    fail_any[failed] = True
-                    if len(failed):
-                        if cfg.fail_safe:
-                            tt = [min(int(last_t[i]), expert(i)["len"] - 1) for i in failed]
-                            eng.set_states(ids[failed], np.stack([expert(i)["qpos"][k] for i, k in zip(failed, tt)]),
-                                           np.stack([expert(i)["qvel"][k] for i, k in zip(failed, tt)]))
-                        else:
-                            alive[failed] = False
-                    alive[live[e[live]]] = False
-                    if not alive.any():
-                        break
-                def host_metrics(i, pct, fs):
-                    ex = expert(i)
-                    tt = np.minimum(np.array(traj[i]["t"], dtype=np.int64), ex["len"] - 1)
-                    return compute_metrics({"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
-                                            "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": pct, "fail_safe": fs})
-                self._eval_results(res, loader, c0, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics, pending)
-                if floor:                           # the host loop's recorded qpos through the device measurement
+        pending = []        # this loader's eval outcomes, applied once the training tables are back (the device curriculum's are lost on a load)
+        device_tables = self._device_tables(loader)
+        if loader is not self.data_loader:
+            saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+            self._load_tables(loader)      # invalidates every env record: only the envs reset below are stepped
+        eng.set_cfg(**self._env_cfg(test=True))
+        res = {}
+        for clips in shard_clips(eng.clip_len, self.agent.world, self.agent.rank, E):
+            ids = np.arange(len(clips), dtype=np.int32)
+            lens = eng.clip_len[clips]
+            if on_device:                                      # the same roll-out as the loop below, as CUDA-graph replays with the metrics on the device
+                kw = dict(record_states=True, export_smpl=True) if motion else (dict(record_states=True) if full else {})
+                dev = self.agent.evaluate(clips, bool(cfg.fail_safe), window=32, floor=floor, **kw)
+                last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
+                rsum = np.array([d["reward_sum"] for d in dev]); nrec = [len(d["frames"]) for d in dev]
+                self._eval_results(res, loader, clips, ids, lens, last_t, fail_any, rsum, nrec,
+                                   lambda i, pct, fs: metrics_from_frames(dev[i]["frames"], pct, fs), pending)
+                if floor:
                     for i in ids:
-                        if traj[i]["t"]:
-                            var = None if eng.clip_models is None else int(eng.clip_models[clips[i]])
-                            rows = eng.floor_qpos(np.array(traj[i]["pred"]).reshape(-1, 76), variants=var).cpu().numpy()
-                            self._add_floor(res[loader.data_keys[c0 + i]], loader, int(clips[i]), rows, np.array(traj[i]["t"], np.int64))
+                        self._add_floor(res[loader.data_keys[clips[i]]], loader, int(clips[i]), dev[i]["floor"], np.arange(1, len(dev[i]["frames"]) + 1))
                 if full:
-                    self._add_mesh(res, loader, c0, ids, clips, [np.array(traj[i]["pred"]).reshape(-1, 76) for i in ids],
-                                   [np.array(traj[i]["t"], np.int64) for i in ids], dump)
-                if motion:                          # the host loop's recorded qpos as SMPL through the device conversion
+                    self._add_mesh(res, loader, ids, clips, [dev[i]["states"][:, :76] for i in ids],
+                                   [np.arange(1, len(dev[i]["frames"]) + 1) for i in ids], dump)
+                if motion:
                     for i in ids:
-                        pred = np.array(traj[i]["pred"]).reshape(-1, 76)
-                        pose, trans = eng.qpos_to_smpl(pred)
-                        self._add_motion(res[loader.data_keys[c0 + i]], loader, int(clips[i]), pred, np.array(traj[i]["pred_jpos"]).reshape(-1, 72),
-                                         pose.cpu().numpy(), trans.cpu().numpy(), np.array(traj[i]["t"], np.int64), bool(fail_any[i]), expert(i))
-            if loader is not self.data_loader:
-                self._load_tables(self.data_loader)
-                if saved is not None:          # a table of another clip count disabled the device curriculum: restore it
-                    self._restore_device_curriculum(saved)
-            if pending:                        # after the restore, so the outcomes of an overlapping test set stay, as on the host path
-                self.agent.curriculum_push([c for c, _ in pending], [o for _, o in pending], [0] * len(pending))
-                pending = []
-            eng.set_cfg(**self._env_cfg(test=False))
-            self.agent.obs = None
-            res_dicts.append(self._coverage(loader, res, epoch, dump))
-        if not self.curriculum_on_device:
-            self._push_clip_weights()
-        return res_dicts
+                        d = dev[i]
+                        self._add_motion(res[loader.data_keys[clips[i]]], loader, int(clips[i]), d["states"][:, :76], d["states"][:, 76:148],
+                                         d["pose_aa"], d["trans"], np.arange(1, len(d["frames"]) + 1), bool(d["fail_any"]))
+                continue
+            if len(ids) < E:                                   # idle envs: park them on the call's first clip so every record is valid (their outputs are ignored)
+                eng.reset(np.arange(len(ids), E, dtype=np.int32), np.full(E - len(ids), clips[0], np.int32), 0, None)
+            obs = eng.reset(ids, clips, 0, None)
+            alive = np.ones(len(ids), bool); fail_any = np.zeros(len(ids), bool)
+            rsum = np.zeros(len(ids)); last_t = np.zeros(len(ids), np.int64)
+            traj = [dict(pred=[], pred_jpos=[], t=[]) for _ in ids]
+            gt = {}
+
+            def expert(i):
+                """expert table of clips[i]: the host-built one, or the device-built one read back once (in the engine's precision)"""
+                if not device_tables:
+                    return loader.experts[clips[i]]
+                if i not in gt:
+                    gt[i] = eng.clip_frames(clips[i])
+                return gt[i]
+            det = torch.ones(E, dtype=torch.uint8, device=obs.device)
+            for t in range(int(lens.max()) - 1):
+                s = self.running_state(obs, update=False)
+                mean = self.policy_net.forward_tc(s)
+                a, _ = nn.gaussian_sample(mean, self.agent.log_std, 0, 0, det)
+                obs, rew, ci, fail, end, pct = eng.step(a)
+                f, e, r = fail.cpu().numpy()[ids] != 0, end.cpu().numpy()[ids] != 0, rew.cpu().numpy()[ids]
+                live = np.nonzero(alive)[0]
+                st = eng.get_states(ids[live])
+                for j, i in enumerate(live):
+                    traj[i]["pred"].append(st["qpos"][j].copy()); traj[i]["pred_jpos"].append(st["xpos"][j].reshape(-1).copy()); traj[i]["t"].append(int(st["cur_t"][j]))
+                    last_t[i] = st["cur_t"][j]
+                rsum[live] += r[live]
+                failed = live[f[live]]
+                fail_any[failed] = True
+                if len(failed):
+                    if cfg.fail_safe:
+                        tt = [min(int(last_t[i]), expert(i)["len"] - 1) for i in failed]
+                        eng.set_states(ids[failed], np.stack([expert(i)["qpos"][k] for i, k in zip(failed, tt)]),
+                                       np.stack([expert(i)["qvel"][k] for i, k in zip(failed, tt)]))
+                    else:
+                        alive[failed] = False
+                alive[live[e[live]]] = False
+                if not alive.any():
+                    break
+            def host_metrics(i, pct, fs):
+                ex = expert(i)
+                tt = np.minimum(np.array(traj[i]["t"], dtype=np.int64), ex["len"] - 1)
+                return compute_metrics({"pred": np.array(traj[i]["pred"]), "gt": np.asarray(ex["qpos"])[tt], "pred_jpos": np.array(traj[i]["pred_jpos"]),
+                                        "gt_jpos": np.asarray(ex["wbpos"])[tt], "percent": pct, "fail_safe": fs})
+            self._eval_results(res, loader, clips, ids, lens, last_t, fail_any, rsum, [len(traj[i]["t"]) for i in ids], host_metrics, pending)
+            if floor:                           # the host loop's recorded qpos through the device measurement
+                for i in ids:
+                    if traj[i]["t"]:
+                        var = None if eng.clip_models is None else int(eng.clip_models[clips[i]])
+                        rows = eng.floor_qpos(np.array(traj[i]["pred"]).reshape(-1, 76), variants=var).cpu().numpy()
+                        self._add_floor(res[loader.data_keys[clips[i]]], loader, int(clips[i]), rows, np.array(traj[i]["t"], np.int64))
+            if full:
+                self._add_mesh(res, loader, ids, clips, [np.array(traj[i]["pred"]).reshape(-1, 76) for i in ids],
+                               [np.array(traj[i]["t"], np.int64) for i in ids], dump)
+            if motion:                          # the host loop's recorded qpos as SMPL through the device conversion
+                for i in ids:
+                    pred = np.array(traj[i]["pred"]).reshape(-1, 76)
+                    pose, trans = eng.qpos_to_smpl(pred)
+                    self._add_motion(res[loader.data_keys[clips[i]]], loader, int(clips[i]), pred, np.array(traj[i]["pred_jpos"]).reshape(-1, 72),
+                                     pose.cpu().numpy(), trans.cpu().numpy(), np.array(traj[i]["t"], np.int64), bool(fail_any[i]), expert(i))
+        if loader is not self.data_loader:
+            self._load_tables(self.data_loader)
+            if saved is not None:          # a table of another clip count disabled the device curriculum: restore it
+                self._restore_device_curriculum(saved)
+        eng.set_cfg(**self._env_cfg(test=False))
+        self.agent.obs = None
+        return res, pending
 
     def _coverage(self, loader, res, epoch, dump):
-        """the coverage line and metric dict of one loader's results (and with dump its {epoch}_{loader}_coverage_full.pkl)"""
+        """the coverage line and metric dict of one loader's results (and with dump its {epoch}_{loader}_coverage_full.pkl, written by rank 0)"""
         n = loader.get_len()
         names = ("succ", "reward", "mpjpe", "mpjpe_g", "pa_mpjpe", "accel_dist", "vel_dist", "root_dist")
         if bool(self.cfg.get("eval_floor_metrics", False)):
@@ -412,7 +514,7 @@ class AgentCopycat:
         self.logger.info(f"Coverage {loader.name} of {coverage} out of {n} | " + " \t".join(f"{k}: {v:.3f}" for k, v in metrics.items()))
         metrics.update(mean_coverage=coverage / n, num_coverage=coverage, all_coverage=n)
         del metrics["succ"]
-        if dump:
+        if dump and self.agent.rank == 0:
             joblib.dump(res, osp.join(self.cfg.output_dir, f"{epoch}_{loader.name}_coverage_full.pkl"))
         return {f"coverage_{loader.name}": metrics}
 
@@ -420,7 +522,8 @@ class AgentCopycat:
         """eval_policy(eval_on_device: true) of several saved checkpoints (models/iter_%04d.p) at once: every test loader is evaluated for all
         of them in shared device calls (BatchedAgent.evaluate_policies).  Returns {epoch: res_dicts}, each what load_checkpoint(epoch) +
         eval_policy(epoch, dump) gives, and logs the same coverage lines.  Comparing checkpoints is not training: no outcome reaches freq_dict
-        or the device curriculum, and the agent's weights, log_std and running_state stay as they are."""
+        or the device curriculum, and the agent's weights, log_std and running_state stay as they are.  With several ranks each evaluates
+        its own clips and every rank returns every clip's results, as eval_policy does."""
         from uhc_b200.metrics import metrics_from_frames
         cfg, eng = self.cfg, self.agent.engine
         epochs = list(epochs)
@@ -432,28 +535,37 @@ class AgentCopycat:
                 cps.append(pickle.load(f))
         out = {epoch: [] for epoch in epochs}
         for loader in self.test_data_loaders:
-            n = loader.get_len()
-            saved = None
-            if loader is not self.data_loader:
-                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
-                self._load_tables(loader)
-            eng.set_cfg(**self._env_cfg(test=True))
-            clips = np.arange(n, dtype=np.int32)
-            lens = eng.clip_len[clips]
-            per_cp = self.agent.evaluate_policies(cps, clips, bool(cfg.fail_safe), window=32)
-            if loader is not self.data_loader:
-                self._load_tables(self.data_loader)
-                if saved is not None:
-                    self._restore_device_curriculum(saved)
-            eng.set_cfg(**self._env_cfg(test=False))
-            self.agent.obs = None
-            for epoch, dev in zip(epochs, per_cp):
-                last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
-                rsum = np.array([d["reward_sum"] for d in dev])
-                res = {}
-                for i in range(n):
-                    res[loader.data_keys[i]] = self._clip_result(lens[i], last_t[i], fail_any[i], rsum[i], len(dev[i]["frames"]),
-                                                                 lambda pct, fs, d=dev[i]: metrics_from_frames(d["frames"], pct, fs))
+            def work(loader=loader):
+                saved = None
+                if loader is not self.data_loader:
+                    saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+                    self._load_tables(loader)
+                eng.set_cfg(**self._env_cfg(test=True))
+                clips = self._my_clips()
+                lens = eng.clip_len[clips]
+                per_cp = self.agent.evaluate_policies(cps, clips, bool(cfg.fail_safe), window=32)
+                if loader is not self.data_loader:
+                    self._load_tables(self.data_loader)
+                    if saved is not None:
+                        self._restore_device_curriculum(saved)
+                eng.set_cfg(**self._env_cfg(test=False))
+                self.agent.obs = None
+                per_res = []
+                for dev in per_cp:
+                    last_t = np.array([d["last_t"] for d in dev], np.int64); fail_any = np.array([d["fail_any"] for d in dev], bool)
+                    rsum = np.array([d["reward_sum"] for d in dev])
+                    res = {}
+                    for i, c in enumerate(clips):
+                        res[loader.data_keys[c]] = self._clip_result(lens[i], last_t[i], fail_any[i], rsum[i], len(dev[i]["frames"]),
+                                                                     lambda pct, fs, d=dev[i]: metrics_from_frames(d["frames"], pct, fs))
+                    per_res.append(res)
+                return per_res
+            if self.agent.world == 1:
+                per_res = work()
+            else:
+                parts = exchange(work)
+                per_res = [merge_results([p[j] for p in parts], loader.data_keys) for j in range(len(epochs))]
+            for epoch, res in zip(epochs, per_res):
                 out[epoch].append(self._coverage(loader, res, epoch, dump))
         if not self.curriculum_on_device:
             self._push_clip_weights()          # a test table load reset the sampler's clip weights: put the training ones back
@@ -468,36 +580,49 @@ class AgentCopycat:
         r.update(gt=np.asarray(gt["qpos"])[tt], pred=np.array(pred), gt_jpos=np.asarray(gt["wbpos"])[tt].reshape(len(tt), -1), pred_jpos=np.array(pred_jpos),
                  pose_aa=np.array(pose_aa), trans=np.array(trans), fail_safe=bool(fail_any and self.cfg.fail_safe))
 
-    def export_motion(self, epoch=0, loaders=None, dump=True):
+    def export_motion(self, epoch=0, loaders=None, dump=True, max_bytes=1 << 30):
         """the simulated motion of every clip of the test loaders (or `loaders`), from the device evaluation (BatchedAgent.export_motion):
         {loader name: {key: eval_seq's dict (gt, pred, gt_jpos, pred_jpos, percent, fail_safe, reward and compute_metrics' keys with succ) plus
         pose_aa [frames][72] and trans [frames][3]}}; with dump each loader's dict goes to {epoch}_{loader}_motion.pkl.  Like eval_checkpoints
-        it is not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored."""
+        it is not training: no outcome reaches freq_dict or the device curriculum, and the training tables and cfg are restored.  max_bytes
+        bounds the host memory of one device call (BatchedAgent.export_motion).
+
+        With several ranks each rank evaluates its own clips and sends them to rank 0 in pieces of at most max_bytes: rank 0 returns
+        (and with dump writes) every clip, in clip order, and every other rank returns only its own clips."""
         from uhc_b200.metrics import metrics_from_frames
         cfg, eng = self.cfg, self.agent.engine
         out = {}
         for loader in (self.test_data_loaders if loaders is None else loaders):
-            n = loader.get_len()
-            saved = None
-            if loader is not self.data_loader:
-                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
-                self._load_tables(loader)
-            eng.set_cfg(**self._env_cfg(test=True))
-            clips = np.arange(n, dtype=np.int32)
-            lens = eng.clip_len[clips].copy()
-            mot = self.agent.export_motion(clips, bool(cfg.fail_safe), window=32)
-            res = {}
-            for i, d in enumerate(mot):
-                r = res[loader.data_keys[i]] = self._clip_result(lens[i], d["last_t"], d["fail_any"], d["reward_sum"], len(d["frames"]),
-                                                                 lambda pct, fs, d=d: metrics_from_frames(d["frames"], pct, fs))
-                self._add_motion(r, loader, i, d["pred"], d["pred_jpos"], d["pose_aa"], d["trans"], np.arange(1, len(d["frames"]) + 1), d["fail_any"])
-            if loader is not self.data_loader:
-                self._load_tables(self.data_loader)
-                if saved is not None:
-                    self._restore_device_curriculum(saved)
-            eng.set_cfg(**self._env_cfg(test=False))
-            self.agent.obs = None
-            if dump:
+            def work(loader=loader):
+                saved = None
+                if loader is not self.data_loader:
+                    saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+                    self._load_tables(loader)
+                eng.set_cfg(**self._env_cfg(test=True))
+                clips = self._my_clips()
+                lens = eng.clip_len[clips].copy()
+                mot = self.agent.export_motion(clips, bool(cfg.fail_safe), window=32, max_bytes=max_bytes)
+                res = {}
+                for c, L, d in zip(clips, lens, mot):
+                    r = res[loader.data_keys[c]] = self._clip_result(L, d["last_t"], d["fail_any"], d["reward_sum"], len(d["frames"]),
+                                                                     lambda pct, fs, d=d: metrics_from_frames(d["frames"], pct, fs))
+                    self._add_motion(r, loader, int(c), d["pred"], d["pred_jpos"], d["pose_aa"], d["trans"], np.arange(1, len(d["frames"]) + 1), d["fail_any"])
+                if loader is not self.data_loader:
+                    self._load_tables(self.data_loader)
+                    if saved is not None:
+                        self._restore_device_curriculum(saved)
+                eng.set_cfg(**self._env_cfg(test=False))
+                self.agent.obs = None
+                return res
+            if self.agent.world == 1:
+                res = work()
+            else:
+                local = {}
+                exchange(lambda: local.update(work()))
+                res = gather_to_root(local, max_bytes)
+                keys = loader.data_keys if self.agent.rank == 0 else [k for k in loader.data_keys if k in res]
+                res = merge_results([res], keys)
+            if dump and self.agent.rank == 0:
                 joblib.dump(res, osp.join(cfg.output_dir, f"{epoch}_{loader.name}_motion.pkl"))
             out[loader.name] = res
         if not self.curriculum_on_device:
@@ -514,7 +639,7 @@ class AgentCopycat:
         compresses the frames on the device (BatchedAgent.render_motion's encode="jpeg") and writes {take_key}_{cfg.id}_{epoch}_0.avi, a
         Motion-JPEG AVI (uhc_b200.video.write_mjpeg_avi), instead.  body="mesh" draws the skinned SMPL mesh instead of the body hulls:
         the neutral model data/smpl/SMPL_NEUTRAL.{pkl,npz} (as full_eval loads it, and it must hold the faces `f`), each clip shaped by its
-        beta[:10] under has_shape and zeros otherwise."""
+        beta[:10] under has_shape and zeros otherwise.  With several ranks each rank renders and writes the files of its own clips."""
         from uhc.utils.image_utils import write_frames_to_video
         from uhc_b200.video import write_mjpeg_avi
         if video not in ("mp4", "mjpeg"):
@@ -529,31 +654,37 @@ class AgentCopycat:
         cam["shift_expert"] = 1.0 if getattr(cfg, "shift_expert", False) else 0.0
         out = {}
         for loader in (self.test_data_loaders if loaders is None else loaders):
-            saved = None
-            if loader is not self.data_loader:
-                saved = self._freq_dict_from_device() if self.curriculum_on_device else None
-                self._load_tables(loader)
-            eng.set_cfg(**self._env_cfg(test=True))
             paths = {k: osp.join(out_dir, f"{k}_{cfg.id}_{epoch}_0.{ext}") for k in loader.data_keys}
 
-            def writer(i, chunks, keys=loader.data_keys, paths=paths):
-                if video == "mp4":
-                    write_frames_to_video((f for ch in chunks for f in ch), paths[keys[i]])
-                else:
-                    write_mjpeg_avi(paths[keys[i]], (f for ch in chunks for f in ch), W, H)
+            def work(loader=loader, paths=paths):
+                saved = None
+                if loader is not self.data_loader:
+                    saved = self._freq_dict_from_device() if self.curriculum_on_device else None
+                    self._load_tables(loader)
+                eng.set_cfg(**self._env_cfg(test=True))
+                ids = self._my_clips()
 
-            ids = np.arange(loader.get_len(), dtype=np.int32)
-            betas = None
-            if body == "mesh" and self.cfg.get("has_shape", False):
-                betas = np.stack([np.asarray(loader.shapes[c], np.float64)[:10] for c in ids])
-            self.agent.render_motion(ids, bool(cfg.fail_safe), size, cam, writer=writer, encode=None if video == "mp4" else "jpeg", body=body,
-                                     betas=betas)
-            if loader is not self.data_loader:
-                self._load_tables(self.data_loader)
-                if saved is not None:
-                    self._restore_device_curriculum(saved)
-            eng.set_cfg(**self._env_cfg(test=False))
-            self.agent.obs = None
+                def writer(i, chunks, keys=loader.data_keys, paths=paths):
+                    if video == "mp4":
+                        write_frames_to_video((f for ch in chunks for f in ch), paths[keys[ids[i]]])
+                    else:
+                        write_mjpeg_avi(paths[keys[ids[i]]], (f for ch in chunks for f in ch), W, H)
+
+                betas = None
+                if body == "mesh" and self.cfg.get("has_shape", False):
+                    betas = clip_betas(loader.shapes, ids)
+                self.agent.render_motion(ids, bool(cfg.fail_safe), size, cam, writer=writer, encode=None if video == "mp4" else "jpeg", body=body,
+                                         betas=betas)
+                if loader is not self.data_loader:
+                    self._load_tables(self.data_loader)
+                    if saved is not None:
+                        self._restore_device_curriculum(saved)
+                eng.set_cfg(**self._env_cfg(test=False))
+                self.agent.obs = None
+            if self.agent.world == 1:
+                work()
+            else:
+                exchange(work)           # each rank writes its own clips' files; every rank returns every path once all are written
             out[loader.name] = paths
         if not self.curriculum_on_device:
             self._push_clip_weights()
@@ -625,7 +756,7 @@ class AgentCopycat:
             self.agent.engine.render_mesh_init(path)
             self._render_mesh_ready = True
 
-    def _add_mesh(self, res, loader, c0, ids, clips, preds, ts, dump, max_bytes=1 << 30):
+    def _add_mesh(self, res, loader, ids, clips, preds, ts, dump, max_bytes=1 << 30):
         """full_eval: convert_2_smpl_params (humanoid_im.py:127-150) and compute_metrics' mesh keys (smpl_eval.py:113-121) for one evaluation
         chunk.  Every clip's simulated rows preds[k] and the expert rows min(t, len - 1) they are paired with go qpos -> SMPL -> mesh on the
         device (Engine.qpos_mesh) through the neutral model (_mesh_model), with the clip's beta[:10] when has_shape and zeros otherwise; pentration / skate (and *_gt for the expert rows)
@@ -642,7 +773,7 @@ class AgentCopycat:
             beta = np.asarray(loader.shapes[c], np.float64)[:10] if self.cfg.get("has_shape", False) else np.zeros(10)
             var = 0 if eng.clip_models is None else int(eng.clip_models[c])
             tt = np.minimum(np.asarray(t, np.int64), int(eng.clip_len[c]) - 1)
-            r = res[loader.data_keys[c0 + i]]
+            r = res[loader.data_keys[c]]
             segs += [(r, "pred", np.asarray(q, np.float64).reshape(-1, 76), beta, var), (r, "gt", np.asarray(gt["qpos"], np.float64)[tt], beta, var)]
         if not segs:
             return
@@ -680,21 +811,16 @@ class AgentCopycat:
         m["percent"] = percent
         return m
 
-    def _eval_results(self, res, loader, c0, ids, lens, last_t, fail_any, rsum, nrec, metrics_of, pending):
-        """res[key] of every clip of one evaluation chunk (_clip_result), and the eval outcome fed to the failure-weighted sampler like a
-        training episode ([percent, 0]): appended to freq_dict on the host path, collected in `pending` for one push on the device path.
-        metrics_of(i, percent, fail_safe) -> compute_metrics' dict."""
+    def _eval_results(self, res, loader, clips, ids, lens, last_t, fail_any, rsum, nrec, metrics_of, pending):
+        """res[key] of every clip of one evaluation call (_clip_result), and the eval outcome of every clip the training table holds,
+        collected in `pending` as (table clip, training clip, outcome) for _apply_outcomes.  metrics_of(i, percent, fail_safe) -> compute_metrics' dict."""
         index = {k: c for c, k in enumerate(self.data_loader.data_keys)}
         for i in ids:
-            k = loader.data_keys[c0 + i]
+            k = loader.data_keys[clips[i]]
             m = res[k] = self._clip_result(lens[i], last_t[i], fail_any[i], rsum[i], nrec[i], lambda pct, fs: metrics_of(i, pct, fs))
             if k not in index:
                 continue
-            outcome = 1.0 if m["succ"][0] else min(m["percent"], 0.999)
-            if self.curriculum_on_device:
-                pending.append((index[k], outcome))
-            else:
-                self.freq_dict[k] = (self.freq_dict[k] + [[outcome, 0]])[-self.max_freq:]
+            pending.append((int(clips[i]), index[k], 1.0 if m["succ"][0] else min(m["percent"], 0.999)))
 
     @staticmethod
     def _device_tables(loader):

@@ -66,6 +66,39 @@ def pack_groups(K, n, E, max_groups=MAX_EVAL_GROUPS):
     return calls
 
 
+def call_env_steps(lens):
+    """env-steps of one evaluation call over clips of these lengths: every env of the call steps until its longest clip ends"""
+    lens = np.asarray(lens, np.int64).reshape(-1)
+    return int(len(lens) * (lens.max() - 1)) if len(lens) else 0
+
+
+def assign_clips(clip_len, world, E):
+    """the evaluation's clips of every rank, each split into its device calls of at most E clips: [[clips of one call, ...] per rank].
+    World 1 keeps the contiguous chunks c0 .. c0 + E - 1.  Otherwise the clips, longest first, are cut into calls of
+    min(E, ceil(n / world)) consecutive clips, so the clips of a call have similar lengths and few padded steps, and each call in turn goes to
+    the rank with the fewest env-steps (call_env_steps) so far, the lower rank on a tie.  Every env's roll-out is independent of the others
+    and of its slot, so a clip's result does not depend on where it runs.  A caller that hands a rank's clips to a method which re-chunks them
+    (evaluate_policies, export_motion) gets the same clips per rank, but not these calls."""
+    lens = np.asarray(clip_len, np.int64).reshape(-1)
+    n = len(lens)
+    assert world >= 1 and E >= 1
+    if world == 1:
+        return [[np.arange(c0, min(n, c0 + E), dtype=np.int32) for c0 in range(0, n, E)]]
+    order = np.argsort(-lens, kind="stable").astype(np.int32)
+    b = max(1, min(E, -(-n // world)))
+    calls, load = [[] for _ in range(world)], [0] * world
+    for k in range(0, n, b):
+        r = load.index(min(load))
+        calls[r].append(order[k:k + b])
+        load[r] += call_env_steps(lens[order[k:k + b]])
+    return calls
+
+
+def shard_clips(clip_len, world, rank, E):
+    """this rank's calls of assign_clips"""
+    return assign_clips(clip_len, world, E)[rank]
+
+
 class ClipSampler:
     """DatasetAMASSSingle.sample_seq / get_sample_from_key (dataset_amass_single.py:172-253): uniform clip choice (or
     failure-weighted when freq stats are given), start ~ U[0, len - t_min), slice length min(t_max, len - start)."""
